@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the FIRA hot path: commits/s of one TRAINING step (forward + backward + Adam) on
 synthetic commits that follow the DataSet's node/edge distribution (BASELINE.json metric, config
-"run_model.py train, 1xB200, batch 64"; N GPUs -> global batch 64*N, weak scaling).
+"run_model.py train, 1 GPU, batch 64"; N GPUs -> global batch 64*N, weak scaling).
 
     python bench.py --gpus N --steps K --warmup W            # our CUDA path
     python bench.py --impl reference --steps K --warmup W    # reference algorithm on the host CPU cores
@@ -12,6 +12,12 @@ D2H read of the loss inside the timed region).  `roofline` is the GNN scatter ke
 (fira_gcn_aggregate) timed live with CUDA events against the measured HBM peak; `cpu_baseline` is
 the CPU oracle port (oracle/fira_oracle.py, the reference algorithm as the reference executes it)
 timed on this box's host cores on a bounded sample.
+
+    python bench.py ... --dump-outputs DIR
+
+writes, after the timed steps, what the timed training step computed in its last step as DIR/<name>.npy
+(loss, a fixed seeded sample of the updated parameters and of their gradients), so that two builds can
+be compared output for output on identical inputs.
 """
 import argparse
 import json
@@ -27,7 +33,7 @@ sys.path.insert(0, ROOT)
 PER_GPU_BATCH = 64
 VOCAB, AST_VOCAB = 24650, 71
 N_POOL = 4                      # distinct synthetic batches rotated through the timed region
-WORKLOAD = ("run_model.py train, 1xB200 per-GPU batch 64 (BASELINE.json configs[1]), "
+WORKLOAD = ("run_model.py train, per-GPU batch 64 (BASELINE.json configs[1]), "
             "synthetic commits with the DataSet node/edge distribution")
 
 
@@ -47,7 +53,7 @@ def measured_peaks():
     if os.path.exists(path):
         p = json.load(open(path))
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data-sheet HBM3 bandwidth, not measured)"
 
 
 # ------------------------------------------------------------------------------------------------ clocks
@@ -269,7 +275,7 @@ def spmm_roofline(dev, hb, B, bf16=False, label=None):
             "launches_timed": n, "rows": R, "nnz": pe.nnz, "commits": B, "peak_source": how,
             "dtype": "bf16" if bf16 else "f32", "shape": label or f"{B} commits x 650 padded node rows",
             "timing": TIMING_NOTE,
-            "l2": f"cold: {n_pairs} rotating buffer pairs ({n_pairs * 2 * R * 256 * esz / 1e6:.0f} MB > 126 MB L2)"}
+            "l2": f"cold: {n_pairs} rotating buffer pairs ({n_pairs * 2 * R * 256 * esz / 1e6:.0f} MB > 50 MB L2)"}
 
 
 def spmm_packed_roofline(dev, pb):
@@ -299,8 +305,8 @@ def spmm_packed_roofline(dev, pb):
 
 # ------------------------------------------------------------------------------------------------ fused GCN roofline
 def gcn_fused_roofline(dev, pb):
-    """The fused GCN layer kernel (fira_gcn_layer_fwd: gather -> tcgen05 -> bias/rowsum/dropout/residual/LayerNorm out of
-    TMEM, ONE launch) on the node rows / adjacency of a packed bench batch `pb` (device), cold L2.  Algorithmic bytes =
+    """The fused GCN layer kernel (fira_gcn_layer_fwd: gather -> wgmma -> bias/rowsum/dropout/residual/LayerNorm on the
+    register accumulators, ONE launch) on the node rows / adjacency of a packed bench batch `pb` (device), cold L2.  Algorithmic bytes =
     SURVEY.md 8d's fused formula: read H once + write the layer output once + rowptr + (col, val) + the weight once per
     launch; the kernel also writes Z (the pre-LayerNorm rows the backward needs) -- reported separately."""
     import torch
@@ -332,18 +338,18 @@ def gcn_fused_roofline(dev, pb):
     tpath = os.path.join(ROOT, "profiles", "roofline_traffic.json")
     if os.path.exists(tpath):
         traffic = json.load(open(tpath)).get("fira_gcn_layer_fwd_dram_bytes_per_launch")
-    return {"bound": "hbm", "kernel": "gcn_fused_kernel<0> (fira_gcn_layer_fwd: gather -> tcgen05.mma -> LayerNorm epilogue)",
+    return {"bound": "hbm", "kernel": "gcn_fused_kernel<0> (fira_gcn_layer_fwd: gather -> wgmma -> LayerNorm epilogue)",
             "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
             "algorithmic_bytes_per_launch": alg_bytes, "bytes_incl_saved_z": alg_bytes + R * 256 * 2,
             "avg_launch_ms": avg_ms, "median_launch_ms": med_ms, "launches_timed": n, "rows": R, "nnz": nnz,
             "peak_source": how, "dtype": "bf16", "timing": TIMING_NOTE,
             "shape": "node rows / adjacency of one packed bench batch (per-commit packed layout)",
-            "l2": f"cold: {n_sets} rotating buffer sets ({n_sets * 4 * R * 256 * 2 / 1e6:.0f} MB > 126 MB L2)"}
+            "l2": f"cold: {n_sets} rotating buffer sets ({n_sets * 4 * R * 256 * 2 / 1e6:.0f} MB > 50 MB L2)"}
 
 
 # ------------------------------------------------------------------------------------------------ GEMM roofline
 def gemm_roofline(dev, M, N=256, K=256, what="GCN layer product of a padded batch"):
-    """The kernel family with the largest share of the bf16 step is the tcgen05 GEMM: time one shape live (bf16 in /
+    """The kernel family with the largest share of the bf16 step is the wgmma GEMM: time one shape live (bf16 in /
     out, bias) on rotating buffers (> L2) and report it against BOTH measured peaks (N = K = 256: HBM-bound by
     arithmetic intensity)."""
     import torch
@@ -360,22 +366,49 @@ def gemm_roofline(dev, M, N=256, K=256, what="GCN layer product of a padded batc
     alg_bytes = (M * K + N * K + M * N) * 2 + N * 4
     flops = 2.0 * M * N * K
     hbm, how = measured_peaks()
-    tf_peak = 1645.8
+    tf_peak, tf_how = 989.0, "H100 SXM data-sheet dense bf16 rate, not measured"
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        tf_peak = float(json.load(open(path)).get("bf16_tflops", tf_peak))
+    if os.path.exists(path) and "bf16_tflops" in json.load(open(path)):
+        tf_peak, tf_how = float(json.load(open(path))["bf16_tflops"]), "measured (MEASURED_PEAKS.json)"
     gbs = alg_bytes / (avg * 1e-3) / 1e9
     tfs = flops / (avg * 1e-3) / 1e12
     del xs, ys
     return {"kernel": "gemm_tc_kernel (fira_gemm_bf16_tc): " + what, "shape": [M, N, K],
             "bound": "hbm", "achieved": gbs, "peak": hbm, "unit": "GB/s", "frac": gbs / hbm,
-            "achieved_tflops": tfs, "peak_tflops": tf_peak, "frac_tensor": tfs / tf_peak,
+            "achieved_tflops": tfs, "peak_tflops": tf_peak, "peak_tflops_source": tf_how, "frac_tensor": tfs / tf_peak,
             "algorithmic_bytes_per_launch": alg_bytes, "flops_per_launch": flops, "avg_launch_ms": avg,
             "median_launch_ms": med, "launches_timed": n, "peak_source": how, "timing": TIMING_NOTE,
             "note": "arithmetic intensity 2*256/(2+2+~0) ~ 128 FLOP/B < ridge ~250: the HBM roofline applies"}
 
 
 # ------------------------------------------------------------------------------------------------ GPU arm
+DUMP_SAMPLE = 4 << 20              # elements per dumped array (16 MB of float32): three arrays stay below 64 MB
+
+
+def dump_outputs(out_dir, loss_sum, n_tok, model):
+    """The timed step's results: its loss, and the parameters after its Adam update with the gradients it computed
+    (state-dict order, flattened; a fixed seeded sample when larger than DUMP_SAMPLE)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    ls, nt = float(loss_sum.item() if torch.is_tensor(loss_sum) else loss_sum), float(n_tok.item() if torch.is_tensor(n_tok) else n_tok)
+    np.save(os.path.join(out_dir, "loss_sum.npy"), np.array([ls], dtype=np.float64))
+    np.save(os.path.join(out_dir, "n_tokens.npy"), np.array([nt], dtype=np.float64))
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([ls / nt], dtype=np.float64))
+
+    def sample(flat):
+        if flat.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randperm(flat.numel(), generator=g)[:DUMP_SAMPLE].sort().values
+            flat = flat[idx]
+        return flat.numpy().astype(np.float32)
+    params = [p for _, p in sorted(model.named_parameters())]
+    np.save(os.path.join(out_dir, "params.npy"), sample(torch.cat([p.detach().float().reshape(-1).cpu() for p in params])))
+    grads = [p.grad for p in params if p.grad is not None]
+    if grads:
+        np.save(os.path.join(out_dir, "grads.npy"), sample(torch.cat([g.detach().float().reshape(-1).cpu() for g in grads])))
+
+
 def run_gpu_arm(args):
     import torch
     import torch.distributed as dist
@@ -454,6 +487,7 @@ def run_gpu_arm(args):
         return ms.item()
 
     last_loss = [0.0]
+    last_res = [None]                                                # (loss_sum, n_tok) of the last eager resident step
     if args.graph:
         # whole step captured in a CUDA graph (fira_icse_b200/engine.py): one cudaGraphLaunch per step
         eng = GraphedTrainStep(model, B, adam_factory(model),
@@ -482,7 +516,7 @@ def run_gpu_arm(args):
         launches_per_step = None
 
         def resident_step(i):
-            dp.step(pool_dev[i % N_POOL])
+            last_res[0] = dp.step(pool_dev[i % N_POOL])
 
         def e2e_step(i):
             loss, _ = dp.step(device_batch(pool_host[i % N_POOL], dev, B))
@@ -499,6 +533,13 @@ def run_gpu_arm(args):
     launches = (_lib.LAUNCH_COUNT - launches0) if launches_per_step is None else launches_per_step * args.steps
     clocks = sampler.stop() if rank == 0 else None
     value = world * B * args.steps / (ms * 1e-3)
+    if args.dump_outputs and rank == 0:
+        if args.graph:
+            loss_sum, n_tok = eng.loss_sum, eng.n_local
+        else:
+            loss, n_tok = last_res[0]                                # DataParallelStep.step returns the mean loss
+            loss_sum = loss.double() * n_tok.double()
+        dump_outputs(args.dump_outputs, loss_sum, n_tok, model)
 
     if args.timeline:
         from torch.profiler import ProfilerActivity, profile
@@ -656,7 +697,7 @@ def run_gpu_arm(args):
             "scaling": "weak", "vs_baseline": None, "dtype": "bf16" if args.precision == "bf16" else "f32",
             "data": "synthetic",
             "config": {"workload": WORKLOAD, "per_gpu_batch": B, "global_batch": B * world, "parallelism": f"dp{world}",
-                       "precision_mode": ("bf16 throughput (bf16 activations, tcgen05 GEMMs with fp32 TMEM accumulators, "
+                       "precision_mode": ("bf16 throughput (bf16 activations, wgmma GEMMs with fp32 register accumulators, "
                                           "fp32 parameters/statistics/gradients)" if args.precision == "bf16" else
                                           "fp32 parity (fp32 storage, fp32 FFMA accumulate)"),
                        "optimizer": ("Adam lr 1e-4 (torch.optim.Adam fused)" if os.environ.get("FIRA_TORCH_ADAM", "0") != "0" else "Adam lr 1e-4 (fira_adam_flat: one launch over the flat parameter buffer)") + ", dropout on (0.1 / GCN 0.2)",
@@ -669,7 +710,7 @@ def run_gpu_arm(args):
                        "batch_shapes": (sorted({pb.shape_key for pb in pool_host}) if packed else
                                         sorted({(hb[0]["sou"].shape[1], hb[0]["sub_token"].shape[1],
                                                  hb[0]["ast_change"].shape[1]) for hb in pool_host})),
-                       "l2": f"{N_POOL} distinct batches rotated; one step touches >1 GB of activations (> 126 MB L2)"},
+                       "l2": f"{N_POOL} distinct batches rotated; one step touches >1 GB of activations (> 50 MB L2)"},
             "e2e": {"value": e2e_value, "unit": "commits/s",
                     "h2d_bytes_per_step": int(pool_host[0].h2d_bytes() if packed else h2d_bytes(pool_host[0])),
                     "d2h_bytes_per_step": 4, "ms_per_step": ms_e2e / args.steps,
@@ -707,6 +748,9 @@ def main():
                     help="profiling runs only: after the timed region, 3 more steps under torch.profiler (CUPTI kernel "
                          "activity); writes the chrome trace to this path and its summary (tools/timeline_summary.py) "
                          "next to it, then exits")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last step's loss and a fixed seeded sample of the updated "
+                         "parameters and their gradients as DIR/<name>.npy (at most 64 MB)")
     ap.add_argument("--profile-step", action="store_true",
                     help="profiling runs only (ncu --profile-from-start off): after the timed region, ONE more step "
                          "between cudaProfilerStart/Stop, then exit without the extra legs")

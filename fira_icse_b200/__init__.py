@@ -1,4 +1,4 @@
-"""fira_icse_b200 -- B200-native (sm_100a) hot path of FIRA behind the reference's nn.Module surface.
+"""fira_icse_b200 -- H100-native (sm_90a) hot path of FIRA behind the reference's nn.Module surface.
 
 The directory is `fira_icse_b200` (an importable identifier) for the package the task text calls
 `fira-icse_b200`.  Importing the package does not need a GPU; running anything does, and fails

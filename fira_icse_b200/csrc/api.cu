@@ -33,7 +33,22 @@ void fira_set_error(int code, const char* fmt, ...) {
 extern "C" {
 int fira_version(void) { return 3; }
 const char* fira_last_error_string(void) { return g_err; }
-int fira_built_arch(void) { return 100; }
+int fira_built_arch(void) { return 90; }
+int fira_num_sms(void) {
+  static std::atomic<int> cache[64];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0) dev = 0;
+  const int slot = dev < 64 ? dev : 63;
+  int n = dev < 64 ? cache[slot].load(std::memory_order_relaxed) : 0;
+  if (n <= 0) {
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
+      cudaGetLastError();
+      n = 132;                                   // no device to ask: the H100 SXM
+    }
+    if (dev < 64) cache[slot].store(n, std::memory_order_relaxed);
+  }
+  return n;
+}
 int fira_set_pdl(int on) { g_pdl.store(on ? 1 : 0, std::memory_order_relaxed); return 0; }
 int fira_get_pdl(void) { return fira_pdl_on(); }
 }

@@ -15,7 +15,7 @@
 #include "common.cuh"
 #include "fira_b200.h"
 
-// tcgen05 path of the bf16 mode (attention_tc.cu)
+// wgmma path of the bf16 mode (attention_tc.cu)
 int fira_attn_tc_fwd(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
                      const unsigned char* key_mask, const int* ranges, long kv_rows, int causal, void* ctx, long ldo,
                      float* stats, int B, int H, int Lq, int Lk, void* stream);

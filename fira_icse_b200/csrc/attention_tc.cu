@@ -1,9 +1,9 @@
-// Multi-head attention core on the 5th-generation tensor cores (bf16 throughput mode), gnn_transformer.py:144-156:
+// Multi-head attention core on the Hopper tensor cores (wgmma, bf16 throughput mode), gnn_transformer.py:144-156:
 //     S = Q K^T / sqrt(32);  S[mask == 0] = -1e9;  P = softmax(S);  ctx = P V          (+ the backward of exactly that)
 //
-// The per-head problem (30 x Lk x 32) is far below a tcgen05.mma tile (M = 128), and every head has its own K/V slice,
-// so the kernel works on a HEAD GROUP: one CTA per (commit, 4 heads).  The 128 rows of the UMMA tile are
-// (head hl, query t) = hl*32 + t, and the A operand is the query block REPLICATED and MASKED per head:
+// The per-head problem (30 x Lk x 32) is far below a 128-row tile, and every head has its own K/V slice, so the kernel
+// works on a HEAD GROUP: one CTA per (commit, 4 heads).  The 128 rows of the tile are (head hl, query t) = hl*32 + t,
+// two m64 warpgroups of 64 rows each, and the A operand is the query block REPLICATED and MASKED per head:
 //     A'[(hl,t), f] = Q[t, 128 g + f]  if feature f belongs to head hl (f / 32 == hl), else 0          (128 x 128)
 // With that operand one M128 x N128 x K128 product against the K rows AS THEY LIE IN MEMORY (K-major, 128 features of
 // the group) yields all four heads' score rows at once; the zeros make the cross-head terms vanish, the tensor core
@@ -12,10 +12,10 @@
 //     dP' = dO' V^T ,  dQ' = dS K ,  dK = dS^T A'(Q) ,  dV = P^T A'(dO)      (A' as MN-major B: cross-head terms are 0)
 // K and V tiles arrive by TMA (SWIZZLE_128B); one [128 keys x 64 features] box serves as K-major B (scores) and as
 // MN-major B (P V, dS K) -- the bytes are the same, only the descriptor differs.  P and dS are written by the softmax
-// threads (thread = row) into the same swizzled layout, where they serve as K-major A (P V, dS K) and as MN-major A
-// (P^T dO, dS^T Q).  Accumulators live in TMEM (512 columns); softmax statistics are thread-local (lane = row).
-// Keys are processed in chunks of 128; forward keeps all score chunks in TMEM (Lk <= 384) and makes two passes
-// (max, then exp / sum / P), so no online rescaling is needed.
+// threads into the same swizzled layout, where they serve as K-major A (P V, dS K) and as MN-major A (P^T dO, dS^T Q).
+// Accumulators live in registers (wgmma fragments: a row's columns are spread over the 4 threads of a lane quad).
+// Keys are processed in chunks of 128 (Lk <= 384).  The forward makes two passes over the score chunks -- row maximum,
+// then the scores are recomputed for exp / sum / P -- so no online rescaling is needed.
 //
 // Semantics kept from the FFMA kernels (attention.cu): scale before mask, -1e9 fill (a fully masked row is uniform
 // over all Lk keys), masked keys get exactly zero dK / dV unless the whole row is masked, statistics = (row max, row
@@ -32,7 +32,7 @@ constexpr int KC = 128;                              // keys per chunk
 constexpr int MAX_CH = 3;                            // Lk <= 384
 constexpr int TILE = 128 * 128 * 2;                  // one [128 rows x 128 cols] bf16 tile = two 16 KB panels
 constexpr int PANEL = 16384;
-constexpr int THREADS = 192;                         // warps 0-3: softmax / epilogue (TMEM lane quarters), 4: TMA + MMA, 5: helper
+constexpr int THREADS = 256;                         // two warpgroups: tile rows [0, 64) and [64, 128)
 
 struct Args {
   const __nv_bfloat16* q; long ldq;
@@ -141,230 +141,215 @@ __device__ __forceinline__ float fast_exp2(float x) {
 }
 constexpr float kLog2e = 1.4426950408889634f;
 
+// rows of this thread's accumulator fragments: mr[h] = tile row (hl, t), h = 0 / 1
+struct FragRows { int mr[2], t[2]; int hl; };
+__device__ __forceinline__ FragRows frag_rows(int warp, int lane) {
+  FragRows f;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) { f.mr[h] = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h; f.t[h] = f.mr[h] & 31; }
+  f.hl = f.mr[0] >> 5;                               // both rows of a thread belong to the same head
+  return f;
+}
+// bf16 pair (keys key, key + 1) into a P / dS tile: 2 panels of 64 keys x [128 rows x 128 B], SWIZZLE_128B
+__device__ __forceinline__ uint32_t pair_off(int m, int key) {
+  return (key >> 6) * PANEL + sw128_offset(m, (key & 63) >> 3) + (key & 7) * 2;
+}
+
+// S (64 rows of warpgroup wg x 128 keys of a chunk) = A'(Q) K^T
+__device__ __forceinline__ void scores(float* s, uint32_t aq, uint32_t kt, int wg) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) s[i] = 0.f;
+  wgmma_fence();
+#pragma unroll
+  for (int kb_ = 0; kb_ < 2; ++kb_)
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      wgmma<128, 0, 0>(s, make_desc(aq + kb_ * PANEL + wg * 8192 + k * 32, 16, 1024), make_desc(kt + kb_ * PANEL + k * 32, 16, 1024));
+  wgmma_commit();
+  wgmma_wait<0>();
+  reg_fence<64>(s);
+}
+
 // =================================================================================================== forward
-// smem: A'(Q) 32 KB | KV[3] 96 KB | P[2] 64 KB
+// smem: A'(Q) 32 KB | K[3] 96 KB | V[2] 64 KB | P 32 KB   (V of chunk 2 reuses the V slot of chunk 0)
 __global__ void __launch_bounds__(THREADS, 1)
 attn_tc_fwd_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, Args a) {
   extern __shared__ unsigned char smem_raw[];
-  __shared__ __align__(8) unsigned long long kv_full[MAX_CH], v_full[MAX_CH], s_full, p_full[2], p_empty[2], o_full;
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) unsigned long long k_full[MAX_CH], v_full[MAX_CH], v_free;
   __shared__ unsigned char s_mask[MAX_CH * KC];
   __shared__ Chunks ch, rm;
   __shared__ KeyBits kb;
   const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;
   unsigned char* sm = smem_raw + (base - smem_addr(smem_raw));
-  constexpr uint32_t OFF_AQ = 0, OFF_KV = TILE, OFF_P = OFF_KV + MAX_CH * TILE;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  constexpr uint32_t OFF_AQ = 0, OFF_K = TILE, OFF_V = OFF_K + MAX_CH * TILE, OFF_P = OFF_V + 2 * TILE;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2, q4 = lane & 3;
   const int b = blockIdx.x >> 1, g = blockIdx.x & 1;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < MAX_CH; ++i) { mbar_init(smem_addr(&kv_full[i]), 1); mbar_init(smem_addr(&v_full[i]), 1); }
-    mbar_init(smem_addr(&s_full), 1);
-    mbar_init(smem_addr(&o_full), 1);
-    for (int i = 0; i < 2; ++i) { mbar_init(smem_addr(&p_full[i]), 128); mbar_init(smem_addr(&p_empty[i]), 1); }
+    for (int i = 0; i < MAX_CH; ++i) { mbar_init(smem_addr(&k_full[i]), 1); mbar_init(smem_addr(&v_full[i]), 1); }
+    mbar_init(smem_addr(&v_free), THREADS);
     mbar_init_fence();
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
   }
-  if (warp == 4) tmem_alloc(smem_addr(&tmem_slot), 512);
   pdl_wait(); pdl_trigger();       // PDL: the prologue above overlapped the previous kernel's tail (common.cuh)
   if (threadIdx.x == 0) make_chunks(ch, a.ranges, b, a.Lk);
   for (int i = threadIdx.x; i < MAX_CH * KC; i += THREADS)
     s_mask[i] = i < a.Lk ? (a.key_mask ? a.key_mask[(long)b * a.Lk + i] : (unsigned char)1) : (unsigned char)0;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
   prepare_keys(ch, rm, kb, s_mask, a.causal, warp, lane);
   const int nch = ch.nch;
-  if (warp == 4 && lane == 0) {                      // K chunks can fly while the A' tile is built
-    for (int c = 0; c < nch; ++c) {
-      const uint32_t dst = base + OFF_KV + c * TILE, bar = smem_addr(&kv_full[c]);
-      mbar_expect_tx(bar, TILE);
-      tma_load_2d(dst, &tmK, g * GF, ch.row[c], bar);
-      tma_load_2d(dst + PANEL, &tmK, g * GF + 64, ch.row[c], bar);
-    }
+  auto load = [&](const CUtensorMap* map, uint32_t dst, int c, unsigned long long* bar) {
+    mbar_expect_tx(smem_addr(bar), TILE);
+    tma_load_2d(dst, map, g * GF, ch.row[c], smem_addr(bar));
+    tma_load_2d(dst + PANEL, map, g * GF + 64, ch.row[c], smem_addr(bar));
+  };
+  if (threadIdx.x == 0) {                            // K and the first two V chunks fly while the A' tile is built
+    for (int c = 0; c < nch; ++c) load(&tmK, base + OFF_K + c * TILE, c, &k_full[c]);
+    for (int c = 0; c < nch && c < 2; ++c) load(&tmV, base + OFF_V + c * TILE, c, &v_full[c]);
   }
   build_masked_tile(sm + OFF_AQ, a.q, a.ldq, b, g, a.Lq, threadIdx.x, THREADS);
   fence_proxy_async();
   __syncthreads();
 
-  if (warp == 4) {
-    if (lane == 0) {
-      // ---- S chunks = A'(Q) K^T : K-major A (2 k-blocks of 64 features), K-major B (key rows)
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, KC, false, false);
-      for (int c = 0; c < nch; ++c) {
-        mbar_wait(smem_addr(&kv_full[c]), 0);
-        tc_fence_after();
+  const FragRows fr = frag_rows(warp, lane);
+  bool live[2], rowfilled[2];
 #pragma unroll
-        for (int kb_ = 0; kb_ < 2; ++kb_)
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16(tmem + c * KC, make_desc(base + OFF_AQ + kb_ * PANEL + k * 32, 16, 1024),
-                      make_desc(base + OFF_KV + c * TILE + kb_ * PANEL + k * 32, 16, 1024), idesc_s, (kb_ | k) ? 1u : 0u);
-      }
-      umma_commit(smem_addr(&s_full));
-      mbar_wait(smem_addr(&s_full), 0);               // the K tiles have been read: reuse their buffers for V
-      for (int c = 0; c < nch; ++c) {
-        const uint32_t dst = base + OFF_KV + c * TILE, bar = smem_addr(&v_full[c]);
-        mbar_expect_tx(bar, TILE);
-        tma_load_2d(dst, &tmV, g * GF, ch.row[c], bar);
-        tma_load_2d(dst + PANEL, &tmV, g * GF + 64, ch.row[c], bar);
-      }
-      // ---- O' += P_c V_c : K-major A (P, 2 k-blocks of 64 keys), MN-major B (V: K = key rows, N = 128 features)
-      constexpr uint32_t idesc_o = make_idesc_bf16(128, GF, false, true);
-      for (int c = 0; c < nch; ++c) {
-        mbar_wait(smem_addr(&v_full[c]), 0);
-        mbar_wait(smem_addr(&p_full[c & 1]), (c >> 1) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < 8; ++k)                    // 8 steps of 16 keys
-          umma_bf16(tmem + MAX_CH * KC,
-                    make_desc(base + OFF_P + (c & 1) * TILE + (k >> 2) * PANEL + (k & 3) * 32, 16, 1024),
-                    make_desc(base + OFF_KV + c * TILE + k * 2048, PANEL, 1024), idesc_o, (c | k) ? 1u : 0u);
-        umma_commit(smem_addr(&p_empty[c & 1]));
-      }
-      umma_commit(smem_addr(&o_full));
-    }
-  } else if (warp < 4) {
-    // ---- softmax + epilogue: thread = row (hl = warp, t = lane)
-    const int t = lane;
-    const bool live = t < a.Lq;
-    const uint32_t trow = tmem + ((uint32_t)(warp * 32) << 16);
+  for (int h = 0; h < 2; ++h) {
+    live[h] = fr.t[h] < a.Lq;
     // does this row see any valid key at all?  (no: every score is -1e9 -> uniform over all existing keys)
     uint32_t any = 0;
     for (int c = 0; c < nch; ++c)
 #pragma unroll
-      for (int j = 0; j < 4; ++j) any |= row_bits(kb, ch, c, j, t, a.causal);
-    const bool rowfilled = any == 0;
-    if (lane == 0) mbar_wait(smem_addr(&s_full), 0);
-    __syncwarp();
-    tc_fence_after();
-    // pass A: row maximum of the raw scores over the valid keys (the scale is positive)
-    float mraw = -INFINITY;
-    for (int c = 0; c < nch; ++c)
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {
-        const uint32_t vb = row_bits(kb, ch, c, j, t, a.causal);
-        if (__any_sync(0xffffffffu, vb != 0)) {       // warp-uniform: tcgen05.ld is .sync.aligned
-          uint32_t r[32];
-          tmem_ld32(trow + c * KC + j * 32, r);
+      for (int j = 0; j < 4; ++j) any |= row_bits(kb, ch, c, j, fr.t[h], a.causal);
+    rowfilled[h] = any == 0;
+  }
+  float s[64];
+  // pass A: row maximum of the raw scores over the valid keys (the scale is positive)
+  float mraw[2] = {-INFINITY, -INFINITY};
+  for (int c = 0; c < nch; ++c) {
+    mbar_wait(smem_addr(&k_full[c]), 0);
+    scores(s, base + OFF_AQ, base + OFF_K + c * TILE, wg);
 #pragma unroll
-          for (int i = 0; i < 32; ++i) if ((vb >> i) & 1) mraw = fmaxf(mraw, __uint_as_float(r[i]));
-        }
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+        const uint32_t vb = row_bits(kb, ch, c, jj >> 2, fr.t[h], a.causal) >> (8 * (jj & 3) + 2 * q4);
+        if (vb & 1) mraw[h] = fmaxf(mraw[h], s[4 * jj + 2 * h]);
+        if (vb & 2) mraw[h] = fmaxf(mraw[h], s[4 * jj + 2 * h + 1]);
       }
-    const float mx = rowfilled ? kMaskFill : mraw * a.scale;            // what the reference's softmax subtracts
-    const float k2 = a.scale * kLog2e, m2 = mraw * k2;
-    float sum = 0.f;
-    const int m = warp * 32 + lane;
-    for (int c = 0; c < nch; ++c) {
-      if (c >= 2) { if (lane == 0) mbar_wait(smem_addr(&p_empty[c & 1]), ((c >> 1) - 1) & 1); __syncwarp(); }
-      unsigned char* ptile = sm + OFF_P + (c & 1) * TILE;
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {
-        const uint32_t vb = row_bits(kb, ch, c, j, t, a.causal), eb = kb.exist[c * 4 + j];
-        float e[32];
-        if (__any_sync(0xffffffffu, vb != 0 && !rowfilled)) {
-          uint32_t r[32];
-          tmem_ld32(trow + c * KC + j * 32, r);
+  }
+  const float k2 = a.scale * kLog2e;
+  float m2[2], sum[2] = {0.f, 0.f};
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            // the MMA consumes bf16(e): sum the ROUNDED values so that P rows are normalised exactly
-            const float x = rowfilled ? (((eb >> i) & 1) ? 1.f : 0.f)
-                                      : (((vb >> i) & 1) ? fast_exp2(fmaf(__uint_as_float(r[i]), k2, -m2)) : 0.f);
-            e[i] = live ? __bfloat162float(__float2bfloat16_rn(x)) : 0.f;
-            sum += e[i];
-          }
-        } else {
+  for (int h = 0; h < 2; ++h) {
+    mraw[h] = fmaxf(mraw[h], __shfl_xor_sync(0xffffffffu, mraw[h], 1));
+    mraw[h] = fmaxf(mraw[h], __shfl_xor_sync(0xffffffffu, mraw[h], 2));
+    m2[h] = mraw[h] * k2;
+  }
+  // pass B: scores again, P = bf16(exp) into shared memory, O' += P V
+  float o[64];
 #pragma unroll
-          for (int i = 0; i < 32; ++i) { e[i] = (live && rowfilled && ((eb >> i) & 1)) ? 1.f : 0.f; sum += e[i]; }
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  for (int c = 0; c < nch; ++c) {
+    scores(s, base + OFF_AQ, base + OFF_K + c * TILE, wg);
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+      const uint32_t eb = kb.exist[c * 4 + (jj >> 2)] >> (8 * (jj & 3) + 2 * q4);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t vb = row_bits(kb, ch, c, jj >> 2, fr.t[h], a.causal) >> (8 * (jj & 3) + 2 * q4);
+        float e[2];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          // the MMA consumes bf16(e): sum the ROUNDED values so that P rows are normalised exactly
+          const float x = rowfilled[h] ? (((eb >> i) & 1) ? 1.f : 0.f)
+                                       : (((vb >> i) & 1) ? fast_exp2(fmaf(s[4 * jj + 2 * h + i], k2, -m2[h])) : 0.f);
+          e[i] = live[h] ? __bfloat162float(__float2bfloat16_rn(x)) : 0.f;
+          sum[h] += e[i];
         }
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 v;
-          __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&v);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) h[i] = __floats2bfloat162_rn(e[q * 8 + 2 * i], e[q * 8 + 2 * i + 1]);
-          const int key = j * 32 + q * 8;             // key within the chunk
-          *reinterpret_cast<uint4*>(ptile + (key >> 6) * PANEL + sw128_offset(m, (key & 63) >> 3)) = v;
-        }
+        *reinterpret_cast<__nv_bfloat162*>(sm + OFF_P + pair_off(fr.mr[h], 8 * jj + 2 * q4)) = __floats2bfloat162_rn(e[0], e[1]);
       }
-      fence_proxy_async();
-      mbar_arrive(smem_addr(&p_full[c & 1]));
     }
-    if (lane == 0) mbar_wait(smem_addr(&o_full), 0);
-    __syncwarp();
-    tc_fence_after();
-    uint32_t r[32];
-    tmem_ld32(trow + MAX_CH * KC + warp * DH, r);      // own head's 32 output columns
-    if (live) {
-      const float inv = 1.f / sum;
-      __nv_bfloat16* dst = a.ctx + ((long)b * a.Lq + t) * a.ldo + g * GF + warp * DH;
+    fence_proxy_async();
+    named_bar(2 + wg, 128);                          // the warpgroup's P rows are complete
+    mbar_wait(smem_addr(&v_full[c]), 0);
+    const uint32_t vt = base + OFF_V + (c & 1) * TILE;
+    wgmma_fence();
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        float o[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) o[i] = __uint_as_float(r[q * 8 + i]) * inv;
-        Act<__nv_bfloat16>::store8(dst + q * 8, o);
-      }
-      if (a.stats) {
-        float* st = a.stats + (((long)b * a.H + g * HG + warp) * a.Lq + t) * 2;
-        st[0] = mx; st[1] = sum;
+    for (int k = 0; k < 8; ++k)                      // 8 steps of 16 keys
+      wgmma<128, 0, 1>(o, make_desc(base + OFF_P + (k >> 2) * PANEL + wg * 8192 + (k & 3) * 32, 16, 1024),
+                       make_desc(vt + k * 2048, PANEL, 1024));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence<64>(o);
+    if (c == 0 && nch == 3) {                        // V slot 0 is free: chunk 2's V goes there
+      mbar_arrive(smem_addr(&v_free));
+      if (threadIdx.x == 0) {
+        mbar_wait(smem_addr(&v_free), 0);
+        load(&tmV, base + OFF_V, 2, &v_full[2]);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) { tc_fence_after(); tmem_dealloc(tmem, 512); }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 1);
+    sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 2);
+    if (!live[h]) continue;
+    const int t = fr.t[h];
+    const float inv = 1.f / sum[h];
+    __nv_bfloat16* dst = a.ctx + ((long)b * a.Lq + t) * a.ldo + g * GF;
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj)                  // own head's 32 output columns
+      if ((jj >> 2) == fr.hl)
+        *reinterpret_cast<__nv_bfloat162*>(dst + 8 * jj + 2 * q4) =
+            __floats2bfloat162_rn(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
+    if (a.stats && q4 == 0) {
+      float* st = a.stats + (((long)b * a.H + g * HG + fr.hl) * a.Lq + t) * 2;
+      st[0] = rowfilled[h] ? kMaskFill : mraw[h] * a.scale;          // what the reference's softmax subtracts
+      st[1] = sum[h];
+    }
+  }
 }
 
 // =================================================================================================== backward
-// smem: A'(Q) | A'(dO) | K | V | P | dS  (6 x 32 KB).  TMEM: S [0,128) dP [128,256) dQ [256,384) dK [384,512), dV reuses [0,128).
+// smem: A'(Q) | A'(dO) | K | V | P | dS  (6 x 32 KB)
 __global__ void __launch_bounds__(THREADS, 1)
 attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, Args a) {
   extern __shared__ unsigned char smem_raw[];
-  __shared__ __align__(8) unsigned long long kv_full, s_full, ds_full, g_full, epi_done;
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) unsigned long long kv_full;
   __shared__ unsigned char s_mask[MAX_CH * KC];
   __shared__ Chunks ch, rm;
   __shared__ KeyBits kb;
   const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;
   unsigned char* sm = smem_raw + (base - smem_addr(smem_raw));
   constexpr uint32_t OFF_AQ = 0, OFF_ADO = TILE, OFF_K = 2 * TILE, OFF_V = 3 * TILE, OFF_P = 4 * TILE, OFF_DS = 5 * TILE;
-  constexpr uint32_t T_S = 0, T_DP = 128, T_DQ = 256, T_DK = 384, T_DV = 0;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2, q4 = lane & 3;
   const int b = blockIdx.x >> 1, g = blockIdx.x & 1;
 
   if (threadIdx.x == 0) {
     rm.nch = 0;
     mbar_init(smem_addr(&kv_full), 1);
-    mbar_init(smem_addr(&s_full), 1);
-    mbar_init(smem_addr(&ds_full), 128);
-    mbar_init(smem_addr(&g_full), 1);
-    mbar_init(smem_addr(&epi_done), 128);
     mbar_init_fence();
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
   }
-  if (warp == 4) tmem_alloc(smem_addr(&tmem_slot), 512);
   pdl_wait(); pdl_trigger();       // PDL: the prologue above overlapped the previous kernel's tail (common.cuh)
   if (threadIdx.x == 0) make_chunks(ch, a.ranges, b, a.Lk);
   for (int i = threadIdx.x; i < MAX_CH * KC; i += THREADS)
     s_mask[i] = i < a.Lk ? (a.key_mask ? a.key_mask[(long)b * a.Lk + i] : (unsigned char)1) : (unsigned char)0;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
   prepare_keys(ch, rm, kb, s_mask, a.causal, warp, lane);
   const int nch = ch.nch;
-  if (warp == 4 && lane == 0 && nch > 0) {           // the first K / V chunk flies while the A' tiles are built
+  auto load_kv = [&](int c) {
     const uint32_t bar = smem_addr(&kv_full);
     mbar_expect_tx(bar, 2 * TILE);
-    tma_load_2d(base + OFF_K, &tmK, g * GF, ch.row[0], bar);
-    tma_load_2d(base + OFF_K + PANEL, &tmK, g * GF + 64, ch.row[0], bar);
-    tma_load_2d(base + OFF_V, &tmV, g * GF, ch.row[0], bar);
-    tma_load_2d(base + OFF_V + PANEL, &tmV, g * GF + 64, ch.row[0], bar);
-  }
+    tma_load_2d(base + OFF_K, &tmK, g * GF, ch.row[c], bar);
+    tma_load_2d(base + OFF_K + PANEL, &tmK, g * GF + 64, ch.row[c], bar);
+    tma_load_2d(base + OFF_V, &tmV, g * GF, ch.row[c], bar);
+    tma_load_2d(base + OFF_V + PANEL, &tmV, g * GF + 64, ch.row[c], bar);
+  };
+  if (threadIdx.x == 0 && nch > 0) load_kv(0);       // the first K / V chunk flies while the A' tiles are built
   // dropped chunks (no valid key, the commit has valid keys elsewhere): their dK / dV rows are exactly zero
   for (int c = 0; c < rm.nch; ++c)
     for (int i = threadIdx.x; i < rm.n[c] * (GF / 8); i += THREADS) {
@@ -379,162 +364,141 @@ attn_tc_bwd_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
   fence_proxy_async();
   __syncthreads();
 
-  if (warp == 4) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_kk = make_idesc_bf16(128, KC, false, false);      // S, dP : K-major A, K-major B
-      constexpr uint32_t idesc_kn = make_idesc_bf16(128, GF, false, true);       // dQ     : K-major A (dS), MN-major B (K)
-      constexpr uint32_t idesc_nn = make_idesc_bf16(128, GF, true, true);        // dK, dV : MN-major A (dS^T / P^T), MN-major B (A')
-      for (int c = 0; c < nch; ++c) {
-        const uint32_t bar = smem_addr(&kv_full);
-        if (c >= 1) {
-          mbar_wait(smem_addr(&epi_done), (c - 1) & 1); // dK/dV of the previous chunk read out; K/V/P/dS free
-          mbar_expect_tx(bar, 2 * TILE);
-          tma_load_2d(base + OFF_K, &tmK, g * GF, ch.row[c], bar);
-          tma_load_2d(base + OFF_K + PANEL, &tmK, g * GF + 64, ch.row[c], bar);
-          tma_load_2d(base + OFF_V, &tmV, g * GF, ch.row[c], bar);
-          tma_load_2d(base + OFF_V + PANEL, &tmV, g * GF + 64, ch.row[c], bar);
-        }
-        mbar_wait(bar, c & 1);
-        tc_fence_after();
+  const FragRows fr = frag_rows(warp, lane);
+  bool live[2], rowfilled[2];
+  // delta = dO . O over the own head's 32 features; row statistics
+  float delta[2], m2[2], inv[2];
 #pragma unroll
-        for (int kb_ = 0; kb_ < 2; ++kb_)
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            umma_bf16(tmem + T_S, make_desc(base + OFF_AQ + kb_ * PANEL + k * 32, 16, 1024),
-                      make_desc(base + OFF_K + kb_ * PANEL + k * 32, 16, 1024), idesc_kk, (kb_ | k) ? 1u : 0u);
-            umma_bf16(tmem + T_DP, make_desc(base + OFF_ADO + kb_ * PANEL + k * 32, 16, 1024),
-                      make_desc(base + OFF_V + kb_ * PANEL + k * 32, 16, 1024), idesc_kk, (kb_ | k) ? 1u : 0u);
-          }
-        umma_commit(smem_addr(&s_full));
-        mbar_wait(smem_addr(&ds_full), c & 1);         // P and dS of this chunk are in shared memory, S / dP consumed
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {                   // K dim = 128 keys (dQ) / 128 (hl,t) rows (dK, dV), 16 per step
-          // dQ' += dS K       A: dS K-major (k-block = k>>2, 32 B per step)      B: K tile MN-major (16 key rows per step)
-          umma_bf16(tmem + T_DQ, make_desc(base + OFF_DS + (k >> 2) * PANEL + (k & 3) * 32, 16, 1024),
-                    make_desc(base + OFF_K + k * 2048, PANEL, 1024), idesc_kn, (c | k) ? 1u : 0u);
-          // dK = dS^T A'(Q)   A: dS MN-major (M = keys: panels of 64 keys, K = rows)   B: A'(Q) MN-major (K = rows, N = features)
-          umma_bf16(tmem + T_DK, make_desc(base + OFF_DS + k * 2048, PANEL, 1024),
-                    make_desc(base + OFF_AQ + k * 2048, PANEL, 1024), idesc_nn, k ? 1u : 0u);
-          // dV = P^T A'(dO)
-          umma_bf16(tmem + T_DV, make_desc(base + OFF_P + k * 2048, PANEL, 1024),
-                    make_desc(base + OFF_ADO + k * 2048, PANEL, 1024), idesc_nn, k ? 1u : 0u);
-        }
-        umma_commit(smem_addr(&g_full));
-      }
-    }
-  } else if (warp < 4) {
-    const int t = lane, m = warp * 32 + lane;
-    const bool live = t < a.Lq;
-    const uint32_t trow = tmem + ((uint32_t)(warp * 32) << 16);
+  for (int h = 0; h < 2; ++h) {
+    const int t = fr.t[h];
+    live[h] = t < a.Lq;
     uint32_t any = 0;
     for (int c = 0; c < nch; ++c)
 #pragma unroll
       for (int j = 0; j < 4; ++j) any |= row_bits(kb, ch, c, j, t, a.causal);
-    const bool rowfilled = any == 0;
-    // delta = dO . O over the own head's 32 features; row statistics
-    float delta = 0.f, mx = 0.f, inv = 0.f;
-    if (live) {
-      const __nv_bfloat16* orow = a.ctx + ((long)b * a.Lq + t) * a.ldo + g * GF + warp * DH;
-      const __nv_bfloat16* grow = a.d_ctx + ((long)b * a.Lq + t) * a.ldo + g * GF + warp * DH;
+    rowfilled[h] = any == 0;
+    delta[h] = 0.f; m2[h] = 0.f; inv[h] = 0.f;
+    if (live[h]) {
+      const __nv_bfloat16* orow = a.ctx + ((long)b * a.Lq + t) * a.ldo + g * GF + fr.hl * DH;
+      const __nv_bfloat16* grow = a.d_ctx + ((long)b * a.Lq + t) * a.ldo + g * GF + fr.hl * DH;
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         float o[8], d[8];
         Act<__nv_bfloat16>::load8(orow + q * 8, o);
         Act<__nv_bfloat16>::load8(grow + q * 8, d);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) delta = fmaf(o[i], d[i], delta);
+        for (int i = 0; i < 8; ++i) delta[h] = fmaf(o[i], d[i], delta[h]);
       }
-      const float* st = a.stats + (((long)b * a.H + g * HG + warp) * a.Lq + t) * 2;
-      mx = st[0]; inv = 1.f / st[1];
-    }
-    const float k2 = a.scale * kLog2e, m2 = mx * kLog2e;
-    for (int c = 0; c < nch; ++c) {
-      if (lane == 0) mbar_wait(smem_addr(&s_full), c & 1);
-      __syncwarp();
-      tc_fence_after();
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {
-        const uint32_t vb = row_bits(kb, ch, c, j, t, a.causal), eb = kb.exist[c * 4 + j];
-        float pv[32], dsv[32];
-        if (__any_sync(0xffffffffu, vb != 0 && !rowfilled)) {
-          uint32_t rs[32], rp[32];
-          tmem_ld32(trow + T_S + j * 32, rs);
-          tmem_ld32(trow + T_DP + j * 32, rp);
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const bool ok = live && !rowfilled && ((vb >> i) & 1);
-            const float p = ok ? fast_exp2(fmaf(__uint_as_float(rs[i]), k2, -m2)) * inv
-                               : ((live && rowfilled && ((eb >> i) & 1)) ? inv : 0.f);
-            pv[i] = p;
-            dsv[i] = ok ? p * (__uint_as_float(rp[i]) - delta) * a.scale : 0.f;      // masked_fill blocks the gradient
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) { pv[i] = (live && rowfilled && ((eb >> i) & 1)) ? inv : 0.f; dsv[i] = 0.f; }
-        }
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 v, w;
-          __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&v);
-          __nv_bfloat162* hw = reinterpret_cast<__nv_bfloat162*>(&w);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            h[i] = __floats2bfloat162_rn(pv[q * 8 + 2 * i], pv[q * 8 + 2 * i + 1]);
-            hw[i] = __floats2bfloat162_rn(dsv[q * 8 + 2 * i], dsv[q * 8 + 2 * i + 1]);
-          }
-          const int key = j * 32 + q * 8;
-          const uint32_t off = (key >> 6) * PANEL + sw128_offset(m, (key & 63) >> 3);
-          *reinterpret_cast<uint4*>(sm + OFF_P + off) = v;
-          *reinterpret_cast<uint4*>(sm + OFF_DS + off) = w;
-        }
-      }
-      tc_fence_before();
-      fence_proxy_async();
-      mbar_arrive(smem_addr(&ds_full));
-      // ---- dK, dV rows of this chunk: thread = key row (warp*32 + lane), 128 features of the group
-      if (lane == 0) mbar_wait(smem_addr(&g_full), c & 1);
-      __syncwarp();
-      tc_fence_after();
-      const int ki = warp * 32 + lane;                 // key row of this chunk
-#pragma unroll 1
-      for (int j = 0; j < GF / 32; ++j) {
-        uint32_t rk[32], rv[32];
-        tmem_ld32(trow + T_DK + j * 32, rk);
-        tmem_ld32(trow + T_DV + j * 32, rv);
-        if (ki < ch.n[c]) {
-          __nv_bfloat16* kd = a.dk + (long)(ch.row[c] + ki) * a.lddk + g * GF + j * 32;
-          __nv_bfloat16* vd = a.dv + (long)(ch.row[c] + ki) * a.lddv + g * GF + j * 32;
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            float x[8], y[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) { x[i] = __uint_as_float(rk[q * 8 + i]); y[i] = __uint_as_float(rv[q * 8 + i]); }
-            Act<__nv_bfloat16>::store8(kd + q * 8, x);
-            Act<__nv_bfloat16>::store8(vd + q * 8, y);
-          }
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(smem_addr(&epi_done));
-    }
-    // ---- dQ: own head's 32 columns (the scale is already folded into dS)
-    uint32_t r[32];
-    if (nch > 0) tmem_ld32(trow + T_DQ + warp * DH, r);
-    if (live) {
-      __nv_bfloat16* dst = a.dq + ((long)b * a.Lq + t) * a.lddq + g * GF + warp * DH;
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        float o[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) o[i] = nch > 0 ? __uint_as_float(r[q * 8 + i]) : 0.f;
-        Act<__nv_bfloat16>::store8(dst + q * 8, o);
-      }
+      const float* st = a.stats + (((long)b * a.H + g * HG + fr.hl) * a.Lq + t) * 2;
+      m2[h] = st[0] * kLog2e; inv[h] = 1.f / st[1];
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) { tc_fence_after(); tmem_dealloc(tmem, 512); }
+  const float k2 = a.scale * kLog2e;
+  float dq[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) dq[i] = 0.f;
+  for (int c = 0; c < nch; ++c) {
+    if (c >= 1 && threadIdx.x == 0) load_kv(c);      // every warpgroup is done with the previous chunk (barrier below)
+    mbar_wait(smem_addr(&kv_full), c & 1);
+    // ---- S and dP, 64 keys at a time -> P and dS (bf16) into shared memory
+#pragma unroll 1
+    for (int kh = 0; kh < 2; ++kh) {
+      float sv[32], dp[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) { sv[i] = 0.f; dp[i] = 0.f; }
+      wgmma_fence();
+#pragma unroll
+      for (int kb_ = 0; kb_ < 2; ++kb_)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          wgmma<64, 0, 0>(sv, make_desc(base + OFF_AQ + kb_ * PANEL + wg * 8192 + k * 32, 16, 1024),
+                          make_desc(base + OFF_K + kb_ * PANEL + kh * 8192 + k * 32, 16, 1024));
+          wgmma<64, 0, 0>(dp, make_desc(base + OFF_ADO + kb_ * PANEL + wg * 8192 + k * 32, 16, 1024),
+                          make_desc(base + OFF_V + kb_ * PANEL + kh * 8192 + k * 32, 16, 1024));
+        }
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence<32>(sv);
+      reg_fence<32>(dp);
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        const int key = kh * 64 + 8 * jj + 2 * q4, grp = key >> 5, sh = key & 31;
+        const uint32_t eb = kb.exist[c * 4 + grp] >> sh;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t vb = row_bits(kb, ch, c, grp, fr.t[h], a.causal) >> sh;
+          float pv[2], dsv[2];
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const bool ok = live[h] && !rowfilled[h] && ((vb >> i) & 1);
+            const float p = ok ? fast_exp2(fmaf(sv[4 * jj + 2 * h + i], k2, -m2[h])) * inv[h]
+                               : ((live[h] && rowfilled[h] && ((eb >> i) & 1)) ? inv[h] : 0.f);
+            pv[i] = p;
+            dsv[i] = ok ? p * (dp[4 * jj + 2 * h + i] - delta[h]) * a.scale : 0.f;      // masked_fill blocks the gradient
+          }
+          const uint32_t off = pair_off(fr.mr[h], key);
+          *reinterpret_cast<__nv_bfloat162*>(sm + OFF_P + off) = __floats2bfloat162_rn(pv[0], pv[1]);
+          *reinterpret_cast<__nv_bfloat162*>(sm + OFF_DS + off) = __floats2bfloat162_rn(dsv[0], dsv[1]);
+        }
+      }
+    }
+    fence_proxy_async();
+    named_bar(1, THREADS);                           // all 128 rows of P / dS are in shared memory
+    // ---- dQ' += dS K     A: dS K-major (k-block = k>>2, 32 B per step)      B: K tile MN-major (16 key rows per step)
+    // ---- dK = dS^T A'(Q)  A: dS MN-major (M = this warpgroup's 64 keys, K = rows)   B: A'(Q) MN-major (K = rows, N = features)
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      wgmma<128, 0, 1>(dq, make_desc(base + OFF_DS + (k >> 2) * PANEL + wg * 8192 + (k & 3) * 32, 16, 1024),
+                       make_desc(base + OFF_K + k * 2048, PANEL, 1024));
+      wgmma<128, 1, 1>(acc, make_desc(base + OFF_DS + wg * PANEL + k * 2048, PANEL, 1024),
+                       make_desc(base + OFF_AQ + k * 2048, PANEL, 1024));
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence<64>(dq);
+    reg_fence<64>(acc);
+    // dK / dV rows of this chunk: fragment row = key of the chunk, 128 features of the group
+    auto store_rows = [&](__nv_bfloat16* dst, long ld) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int ki = fr.mr[h];
+        if (ki < ch.n[c]) {
+          __nv_bfloat16* row = dst + (long)(ch.row[c] + ki) * ld + g * GF;
+#pragma unroll
+          for (int jj = 0; jj < 16; ++jj)
+            *reinterpret_cast<__nv_bfloat162*>(row + 8 * jj + 2 * q4) = __floats2bfloat162_rn(acc[4 * jj + 2 * h], acc[4 * jj + 2 * h + 1]);
+        }
+      }
+    };
+    store_rows(a.dk, a.lddk);
+    // ---- dV = P^T A'(dO)
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+      wgmma<128, 1, 1>(acc, make_desc(base + OFF_P + wg * PANEL + k * 2048, PANEL, 1024),
+                       make_desc(base + OFF_ADO + k * 2048, PANEL, 1024));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence<64>(acc);
+    store_rows(a.dv, a.lddv);
+    named_bar(1, THREADS);                           // K / V / P / dS free for the next chunk
+  }
+  // ---- dQ: own head's 32 columns (the scale is already folded into dS)
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (!live[h]) continue;
+    __nv_bfloat16* dst = a.dq + ((long)b * a.Lq + fr.t[h]) * a.lddq + g * GF;
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj)
+      if ((jj >> 2) == fr.hl)
+        *reinterpret_cast<__nv_bfloat162*>(dst + 8 * jj + 2 * q4) = __floats2bfloat162_rn(dq[4 * jj + 2 * h], dq[4 * jj + 2 * h + 1]);
+  }
 }
 
 // max_chunks: 128-key chunks a commit needs (padded batches ceil(Lk / 128); packed batches every range starts its own
@@ -558,11 +522,11 @@ int fira_attn_tc_fwd(const void* q, long ldq, const void* k, long ldk, const voi
   Args a{};
   a.q = (const __nv_bfloat16*)q; a.ldq = ldq; a.key_mask = key_mask; a.ranges = ranges; a.causal = causal; a.B = B; a.H = H; a.Lq = Lq;
   a.Lk = Lk; a.scale = 1.f / sqrtf((float)DH); a.ctx = (__nv_bfloat16*)ctx; a.ldo = ldo; a.stats = stats;
-  const size_t smem = (1 + MAX_CH + 2) * (size_t)TILE + 1024;
+  const size_t smem = (1 + MAX_CH + 2 + 1) * (size_t)TILE + 1024;
   cudaError_t e = cudaFuncSetAttribute(attn_tc_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) { fira_set_error(FIRA_ERR_CUDA, "attn_tc_fwd attr: %s", cudaGetErrorString(e)); return FIRA_ERR_CUDA; }
   launch_k(attn_tc_fwd_kernel, dim3(B * 2), dim3(THREADS), smem, (cudaStream_t)stream, tk, tv, a);
-  FIRA_CHECK_LAUNCH("fira_attn_fwd (tcgen05)");
+  FIRA_CHECK_LAUNCH("fira_attn_fwd (wgmma)");
   return FIRA_OK;
 }
 
@@ -584,7 +548,7 @@ int fira_attn_tc_bwd(const void* q, long ldq, const void* k, long ldk, const voi
   cudaError_t e = cudaFuncSetAttribute(attn_tc_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) { fira_set_error(FIRA_ERR_CUDA, "attn_tc_bwd attr: %s", cudaGetErrorString(e)); return FIRA_ERR_CUDA; }
   launch_k(attn_tc_bwd_kernel, dim3(B * 2), dim3(THREADS), smem, (cudaStream_t)stream, tk, tv, a);
-  FIRA_CHECK_LAUNCH("fira_attn_bwd (tcgen05)");
+  FIRA_CHECK_LAUNCH("fira_attn_bwd (wgmma)");
   return FIRA_OK;
 }
 

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libfira_b200 (sm_100a only).
+// Shared device/host helpers for libfira_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -35,6 +35,10 @@ void fira_set_error(int code, const char* fmt, ...);
     }                                                                             \
   } while (0)
 
+// streaming multiprocessors of the current device (api.cu, cached per device): every grid of the library is sized
+// from this one query
+extern "C" int fira_num_sms(void);
+
 static inline bool fira_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // launch mode of every kernel of the library (api.cu; fira_set_pdl / FIRA_PDL): 1 = programmatic dependent launch
@@ -45,7 +49,7 @@ int fira_pdl_on();
 // ---- programmatic dependent launch (PDL).  Every kernel of the library starts with pdl_wait() -- before its first
 //      global-memory access -- and pdl_trigger(): launched with the programmatic-serialization attribute (launch_k
 //      below), its CTAs are scheduled while the previous kernel of the stream drains, run their on-chip prologue
-//      (barrier init, TMEM allocation, tensor-map prefetch), and block in griddepcontrol.wait until that kernel has
+//      (barrier init, tensor-map prefetch), and block in griddepcontrol.wait until that kernel has
 //      completed and flushed.  Because EVERY kernel waits before touching memory, completion is transitive along the
 //      stream.  Inside a captured CUDA graph the attribute becomes a programmatic edge; after a non-kernel node or a
 //      cross-stream join it degrades to a full dependency.  Without the attribute both instructions are no-ops.

@@ -4,17 +4,17 @@
 //   backward (MODE 1):  AdZ = A^T dZ (side output for dWc = AdZ^T H) ;  dH = AdZ Wc + d_resid
 //
 // gather -> transform -> epilogue without a round trip through HBM between them:
-//   * 8 gather warps build the aggregated 128-row tile (A H)[rows, 0:256] straight in shared memory, in the
-//     K-major SWIZZLE_128B layout tcgen05.mma reads (the tile IS the A operand): a quarter warp per destination row,
+//   * 4 gather warps build the aggregated 128-row tile (A H)[rows, 0:256] straight in shared memory, in the
+//     K-major SWIZZLE_128B layout wgmma reads (the tile IS the A operand): a quarter warp per destination row,
 //     16-byte loads, 8 x 128 B of neighbour rows in flight per lane group, fp32 accumulation in CSR order, the tile's
 //     rowptr / (col, val) metadata prefetched into shared memory first (one dependent latency per row, not three);
 //   * the 256 x 256 weight (128 KB bf16) is loaded ONCE per CTA by TMA and stays resident (persistent CTAs, one per SM);
-//   * one elected thread issues 16 tcgen05.mma (M128 N256 K16) per tile into one of TWO 256-column TMEM accumulators,
-//     so the epilogue of tile t overlaps the gather of tile t+1;
-//   * 4 epilogue warps read the accumulator (tcgen05.ld: lane = row), add bias + rowsum*c1, write Z, apply dropout +
-//     residual + LayerNorm (row statistics are thread-local: a thread owns a whole row) and write the normalised rows;
-//     all global traffic of the epilogue goes through a small per-warp staging block so loads/stores are 64-B row
-//     segments instead of one row per lane.
+//   * two consumer warpgroups (rows 0-63 / 64-127 of the tile) issue 16 wgmma m64 n256 k16 each per tile, fp32
+//     accumulator in registers; the A tile is handed back as soon as they complete, so the gather of tile t+1
+//     overlaps the epilogue of tile t;
+//   * the epilogue works on the register fragments: add bias + rowsum*c1, write Z, apply dropout + residual +
+//     LayerNorm (a row's 256 columns live in the 4 threads of a lane quad: two shuffles for the row statistics) and
+//     write the normalised rows.
 // Rows are addressed through a CSR in BUFFER order (rowptr[r], col = buffer row; fira_csr_to_rows builds it from the
 // (graph, node)-ordered CSR), so the kernel does not care whether the node buffer is padded segment-major or packed.
 #include "tc_common.cuh"
@@ -25,20 +25,16 @@ namespace {
 using namespace tc;
 
 constexpr int D = 256;
-constexpr int TM = 128;                    // rows per tile = UMMA M
-constexpr int N_EPI = 8, N_GATHER = 8;     // epilogue warp w: TMEM lane quarter w & 3, column half w >> 2
-constexpr int WARP_MMA = N_EPI;            // warps 0-7 epilogue, 8 = TMA + MMA, 9-16 gather
-constexpr int THREADS = (N_EPI + 1 + N_GATHER) * 32;
+constexpr int TM = 128;                    // rows per tile: two m64 warpgroups
+constexpr int N_CONSUMER = 256;            // warps 0-7
+constexpr int N_GATHER = 4;                // warps 8-11
+constexpr int THREADS = N_CONSUMER + N_GATHER * 32;
 constexpr int EC = 1024;                   // edges of a tile staged in shared memory (larger tiles read col/val from global)
-constexpr int STG_PITCH = 80;              // bytes per staged row of 32 bf16 (64 B) + 16 B pad: conflict-free 16-B accesses
 constexpr uint32_t B_BYTES = D * D * 2;    // 131072: 4 k-blocks x [256 n-rows x 128 B]
 constexpr uint32_t A_BYTES = TM * D * 2;   // 65536:  4 k-blocks x [128 rows x 128 B]
-constexpr uint32_t STG_BYTES = N_EPI * 32 * STG_PITCH;          // per epilogue warp: one [32 x 32] bf16 block (in, then out)
-constexpr uint32_t OFF_A = B_BYTES, OFF_STG = OFF_A + A_BYTES, OFF_ROWPTR = OFF_STG + STG_BYTES,
-                   OFF_COL = OFF_ROWPTR + 544, OFF_VAL = OFF_COL + EC * 4, OFF_RS = OFF_VAL + EC * 4,
-                   OFF_ST = OFF_RS + 4 * TM * 4, SMEM_BYTES = OFF_ST + 2 * TM * 2 * 4;
+constexpr uint32_t OFF_A = B_BYTES, OFF_ROWPTR = OFF_A + A_BYTES, OFF_COL = OFF_ROWPTR + 544, OFF_VAL = OFF_COL + EC * 4,
+                   OFF_RS = OFF_VAL + EC * 4, SMEM_BYTES = OFF_RS + 4 * TM * 4;
 constexpr int GATHER_BAR = 1;              // named barrier of the gather warps
-constexpr int EPI_BAR = 2;                 // named barrier of the epilogue warps (row statistics exchange)
 
 struct Params {
   const int* rowptr; const int* col; const float* val;      // buffer-order CSR
@@ -80,24 +76,13 @@ __device__ __forceinline__ void unpack8(const uint4& raw, float* v) {
 #pragma unroll
   for (int i = 0; i < 4; ++i) { const float2 f = __bfloat1622float2(h[i]); v[2 * i] = f.x; v[2 * i + 1] = f.y; }
 }
-// 32 lanes x 32 consecutive fp32 columns back into TMEM (the layout tmem_ld32 reads)
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
+// 12 warps cap the kernel at 168 registers: the LayerNorm epilogue over the 128-register accumulator spills (ptxas -v: up
+// to 1.2 KB); the kernel is opt-in (FIRA_GCN_FUSED) and has not been timed on the H100
 template <int MODE>
 __global__ void __launch_bounds__(THREADS, 1) gcn_fused_kernel(const __grid_constant__ CUtensorMap tmW, Params p) {
   extern __shared__ unsigned char smem_raw[];
-  __shared__ __align__(8) unsigned long long b_full, a_full, a_empty, tmem_full[2], tmem_empty[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) unsigned long long b_full, a_full, a_empty;
   const uint32_t base = (smem_addr(smem_raw) + 1023u) & ~1023u;
   unsigned char* sm = smem_raw + (base - smem_addr(smem_raw));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -108,47 +93,17 @@ __global__ void __launch_bounds__(THREADS, 1) gcn_fused_kernel(const __grid_cons
   if (threadIdx.x == 0) {
     mbar_init(smem_addr(&b_full), 1);
     mbar_init(smem_addr(&a_full), N_GATHER * 32);
-    mbar_init(smem_addr(&a_empty), 1);
-    for (int i = 0; i < 2; ++i) { mbar_init(smem_addr(&tmem_full[i]), 1); mbar_init(smem_addr(&tmem_empty[i]), N_EPI * 32); }
+    mbar_init(smem_addr(&a_empty), N_CONSUMER);
     mbar_init_fence();
     tma_prefetch_desc(&tmW);
   }
-  if (warp == WARP_MMA) tmem_alloc(smem_addr(&tmem_slot), 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
   pdl_wait(); pdl_trigger();       // PDL: the prologue above overlapped the previous kernel's tail (common.cuh)
 
-  if (warp == WARP_MMA) {
-    if (lane == 0 && ntiles > 0) {
-      // ---- weight: resident B operand, 4 k-blocks of [256 n x 64 k]
-      mbar_expect_tx(smem_addr(&b_full), B_BYTES);
-#pragma unroll
-      for (int kb = 0; kb < 4; ++kb) tma_load_2d(base + kb * 32768, &tmW, kb * 64, 0, smem_addr(&b_full));
-      mbar_wait(smem_addr(&b_full), 0);
-      constexpr uint32_t idesc = make_idesc_bf16(TM, D, false, false);
-      for (int t = 0; t < ntiles; ++t) {
-        const int buf = t & 1;
-        if (t >= 2) mbar_wait(smem_addr(&tmem_empty[buf]), ((t >> 1) - 1) & 1);      // epilogue of tile t-2 drained it
-        mbar_wait(smem_addr(&a_full), t & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int kb = 0; kb < 4; ++kb)
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t da = make_desc(base + OFF_A + kb * 16384 + k * 32, 16, 1024);
-            const uint64_t db = make_desc(base + kb * 32768 + k * 32, 16, 1024);
-            umma_bf16(tmem_base + buf * D, da, db, idesc, (kb | k) ? 1u : 0u);
-          }
-        umma_commit(smem_addr(&a_empty));            // A tile may be overwritten
-        umma_commit(smem_addr(&tmem_full[buf]));     // accumulator ready
-      }
-    }
-  } else if (warp > WARP_MMA) {
+  if (warp >= N_CONSUMER / 32) {
     // ======================================================= gather warps: A tile = (A_hat X)[tile rows, :]
-    const int gw = warp - WARP_MMA - 1;              // 0..7
-    const int gtid = gw * 32 + lane;                 // 0..255
+    const int gw = warp - N_CONSUMER / 32;           // 0..3
+    const int gtid = gw * 32 + lane;                 // 0..127
     const int q = lane >> 3, ql = lane & 7;          // quarter-warp (row slot) / lane within it
     int* s_rowptr = reinterpret_cast<int*>(sm + OFF_ROWPTR);
     int* s_col = reinterpret_cast<int*>(sm + OFF_COL);
@@ -158,22 +113,22 @@ __global__ void __launch_bounds__(THREADS, 1) gcn_fused_kernel(const __grid_cons
       long r0; int rows, nt_;
       tile_range(p.R, cta, ncta, t, r0, rows, nt_);
       // ---- tile metadata -> shared memory (every gather warp is done with the previous tile's metadata first)
-      if (t >= 1) asm volatile("bar.sync %0, %1;" ::"n"(GATHER_BAR), "n"(N_GATHER * 32) : "memory");
+      if (t >= 1) named_bar(GATHER_BAR, N_GATHER * 32);
       for (int i = gtid; i <= rows; i += N_GATHER * 32) s_rowptr[i] = p.rowptr[r0 + i];
-      asm volatile("bar.sync %0, %1;" ::"n"(GATHER_BAR), "n"(N_GATHER * 32) : "memory");
+      named_bar(GATHER_BAR, N_GATHER * 32);
       const int e_lo = s_rowptr[0], e_hi = s_rowptr[rows];
       const int nE = e_hi - e_lo;
       const bool staged = nE <= EC;
       if (staged)
         for (int i = gtid; i < nE; i += N_GATHER * 32) { s_col[i] = p.col[e_lo + i]; s_val[i] = p.val[e_lo + i]; }
-      if (t >= 1 && gtid == 0) mbar_wait(smem_addr(&a_empty), (t - 1) & 1);   // MMAs of tile t-1 have read the A tile
-      asm volatile("bar.sync %0, %1;" ::"n"(GATHER_BAR), "n"(N_GATHER * 32) : "memory");
+      if (t >= 1 && gtid == 0) mbar_wait(smem_addr(&a_empty), (t - 1) & 1);   // wgmma of tile t-1 have read the A tile
+      named_bar(GATHER_BAR, N_GATHER * 32);
       const int* cp = staged ? s_col : p.col + e_lo;
       const float* vp = staged ? s_val : p.val + e_lo;
-      // each warp: rows gw*16 + it*4 + q
+      // each warp: rows gw*32 + it*4 + q
 #pragma unroll 1
-      for (int it = 0; it < 4; ++it) {
-        const int r = gw * 16 + it * 4 + q;
+      for (int it = 0; it < 8; ++it) {
+        const int r = gw * 32 + it * 4 + q;
         if (r < rows) {
           const int e0 = s_rowptr[r] - e_lo, e1 = s_rowptr[r + 1] - e_lo;
           float acc[4][8];
@@ -231,175 +186,119 @@ __global__ void __launch_bounds__(THREADS, 1) gcn_fused_kernel(const __grid_cons
           if (MODE == 0 && ql == 0) s_rs[(t & 3) * TM + r] = rsum;
         }
       }
-      fence_proxy_async();                           // my generic-proxy writes -> visible to the UMMA (async proxy) reads
+      fence_proxy_async();                           // my generic-proxy writes -> visible to the wgmma (async proxy) reads
       mbar_arrive(smem_addr(&a_full));
     }
-  } else {
-    // ======================================================= epilogue warps: TMEM lanes 32*(warp & 3), columns 128*(warp >> 2)
-    // Per warp and 32-column chunk: the residual / addend block [32 rows x 32 cols] is fetched one chunk AHEAD into
-    // registers (coalesced 64-B row segments), handed over through a staging block (lane = row afterwards); results go
-    // back through a second staging block so that global stores are 64-B row segments too.  MODE 0 keeps
-    // y = dropout(z) + h in TMEM (tcgen05.st) between the statistics pass and the normalisation pass.
-    const int quarter = warp & 3, half = warp >> 2;
-    unsigned char* stg = sm + OFF_STG + warp * 32 * STG_PITCH;
-    const float* s_rs = reinterpret_cast<const float*>(sm + OFF_RS);
-    float* s_st = reinterpret_cast<float*>(sm + OFF_ST);                 // [2 halves][128 rows][sum, sumsq]
-    uint64_t seed = p.seed;
-    if (MODE == 0 && p.seed_ctr) seed += *p.seed_ctr;
-    const float keep_scale = (MODE == 0 && p.p_drop > 0.f) ? 1.f / (1.f - p.p_drop) : 1.f;
-    const int lrow = lane >> 2, lch = lane & 3;      // cooperative 64-B row segments: 8 rows x 4 chunks per instruction
-    const __nv_bfloat16* resid = MODE == 0 ? p.x : p.addend;
-    for (int t = 0; t < ntiles; ++t) {
-      long r0; int rows, nt_;
-      tile_range(p.R, cta, ncta, t, r0, rows, nt_);
-      const int buf = t & 1;
-      const int wrow0 = quarter * 32;                // first tile row of this warp
-      const int my = wrow0 + lane;                   // this thread's tile row
-      const bool live = my < rows;
-      const long grow = r0 + my;
-      const uint32_t tacc = tmem_base + buf * D + ((uint32_t)wrow0 << 16) + half * 128;
-      const int col0 = half * 128;
-      // residual / addend: every thread reads ITS row directly (16-B loads, two 32-column chunks ahead in registers);
-      // the first two chunks are requested before the accumulator is ready, so their latency hides behind the MMAs
-      uint4 hq[2][4];
-      auto fetch = [&](int k, uint4* dst) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          dst[j] = make_uint4(0, 0, 0, 0);
-          if (live && resid != nullptr) dst[j] = __ldg(reinterpret_cast<const uint4*>(resid + grow * D + col0 + k * 32 + j * 8));
-        }
-      };
-      fetch(0, hq[0]);
-      fetch(1, hq[1]);
-      if (lane == 0) mbar_wait(smem_addr(&tmem_full[buf]), (t >> 1) & 1);
-      __syncwarp();
-      tc_fence_after();
-      float rs = 0.f, sum = 0.f, sq = 0.f;
-      if (MODE == 0 && live) rs = s_rs[(t & 3) * TM + my];
-      auto chunk = [&](int k, const uint4* hp) {
-        const int c = col0 + k * 32;
-        uint32_t acc[32];
-        tmem_ld32(tacc + k * 32, acc);
-        float y[32];
-        if (MODE == 0) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 bv = __ldg(reinterpret_cast<const float4*>(p.bias + c + j));
-            const float4 cv = __ldg(reinterpret_cast<const float4*>(p.c1 + c + j));
-            y[j + 0] = fmaf(rs, cv.x, __uint_as_float(acc[j + 0]) + bv.x);
-            y[j + 1] = fmaf(rs, cv.y, __uint_as_float(acc[j + 1]) + bv.y);
-            y[j + 2] = fmaf(rs, cv.z, __uint_as_float(acc[j + 2]) + bv.z);
-            y[j + 3] = fmaf(rs, cv.w, __uint_as_float(acc[j + 3]) + bv.w);
-          }
-          // Z is stored as bf16 and the LayerNorm backward recomputes from the stored value: normalise the same value
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const uint4 zp = pack8(y + j * 8);
-            *reinterpret_cast<uint4*>(stg + lane * STG_PITCH + j * 16) = zp;
-            unpack8(zp, y + j * 8);
-          }
-          if (p.p_drop > 0.f) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const uint32_t m = dropout_keep8(seed, p.stream_id, (uint64_t)grow * 32 + (c >> 3) + j, p.p_drop);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) y[j * 8 + i] = ((m >> i) & 1) ? y[j * 8 + i] * keep_scale : 0.f;
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            float h[8];
-            unpack8(hp[j], h);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) { const float v = y[j * 8 + i] + h[i]; y[j * 8 + i] = v; sum += v; sq = fmaf(v, v, sq); }
-          }
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] = __float_as_uint(y[j]);
-          tmem_st32(tacc + k * 32, acc);             // y stays in TMEM for the normalisation pass
-        } else {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            float h[8];
-            unpack8(hp[j], h);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) y[j * 8 + i] = __uint_as_float(acc[j * 8 + i]) + h[i];
-            *reinterpret_cast<uint4*>(stg + lane * STG_PITCH + j * 16) = pack8(y + j * 8);
-          }
-        }
-        __syncwarp();
-        // staged [32 x 32] bf16 block (Z, or dH) -> global, 64-B row segments
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int rr = i * 8 + lrow;
-          if (wrow0 + rr < rows) {
-            const uint4 v = *reinterpret_cast<const uint4*>(stg + rr * STG_PITCH + lch * 16);
-            __nv_bfloat16* dst = MODE == 0 ? p.z : p.y;
-            *reinterpret_cast<uint4*>(dst + (r0 + wrow0 + rr) * D + c + lch * 8) = v;
-          }
-        }
-        __syncwarp();
-      };
-#pragma unroll 1
-      for (int k = 0; k < 4; k += 2) {
-        chunk(k, hq[0]);
-        if (k + 2 < 4) fetch(k + 2, hq[0]);
-        chunk(k + 1, hq[1]);
-        if (k + 3 < 4) fetch(k + 3, hq[1]);
-      }
-      if (MODE == 0) {
-        tmem_st_wait();
-        // row statistics over all 256 columns: the two warps of a lane quarter exchange their halves
-        s_st[(half * TM + my) * 2] = sum;
-        s_st[(half * TM + my) * 2 + 1] = sq;
-        asm volatile("bar.sync %0, %1;" ::"n"(EPI_BAR), "n"(N_EPI * 32) : "memory");
-        const float tsum = sum + s_st[((half ^ 1) * TM + my) * 2];
-        const float tsq = sq + s_st[((half ^ 1) * TM + my) * 2 + 1];
-        const float mean = tsum * (1.f / D);
-        const float var = fmaxf(tsq * (1.f / D) - mean * mean, 0.f);
-        const float rstd = rsqrtf(var + kLnEps);
-        if (live && half == 0 && p.mean) { p.mean[grow] = mean; p.rstd[grow] = rstd; }
-#pragma unroll 1
-        for (int k = 0; k < 4; ++k) {
-          const int c = col0 + k * 32;
-          uint32_t acc[32];
-          tmem_ld32(tacc + k * 32, acc);
-          float o[32];
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 gv = __ldg(reinterpret_cast<const float4*>(p.gamma + c + j));
-            const float4 bt = __ldg(reinterpret_cast<const float4*>(p.beta + c + j));
-            o[j + 0] = fmaf((__uint_as_float(acc[j + 0]) - mean) * rstd, gv.x, bt.x);
-            o[j + 1] = fmaf((__uint_as_float(acc[j + 1]) - mean) * rstd, gv.y, bt.y);
-            o[j + 2] = fmaf((__uint_as_float(acc[j + 2]) - mean) * rstd, gv.z, bt.z);
-            o[j + 3] = fmaf((__uint_as_float(acc[j + 3]) - mean) * rstd, gv.w, bt.w);
-          }
-#pragma unroll
-          for (int j = 0; j < 4; ++j) *reinterpret_cast<uint4*>(stg + lane * STG_PITCH + j * 16) = pack8(o + j * 8);
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int rr = i * 8 + lrow;
-            if (wrow0 + rr < rows) {
-              const long gr = r0 + wrow0 + rr;
-              const uint4 v = *reinterpret_cast<const uint4*>(stg + rr * STG_PITCH + lch * 16);
-              __nv_bfloat16* dst = gr < p.split ? p.outA : p.outB;
-              *reinterpret_cast<uint4*>(dst + gr * D + c + lch * 8) = v;
-            }
-          }
-          __syncwarp();
-        }
-        // the partner warp must have read s_st before the next tile overwrites it
-        asm volatile("bar.sync %0, %1;" ::"n"(EPI_BAR), "n"(N_EPI * 32) : "memory");
-      }
-      tc_fence_before();
-      mbar_arrive(smem_addr(&tmem_empty[buf]));
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == WARP_MMA) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+
+  // ======================================================= consumers: warpgroup wg = tile rows [64 wg, +64)
+  const int wg = warp >> 2, q4 = lane & 3;
+  if (threadIdx.x == 0 && ntiles > 0) {
+    // ---- weight: resident B operand, 4 k-blocks of [256 n x 64 k]
+    mbar_expect_tx(smem_addr(&b_full), B_BYTES);
+#pragma unroll
+    for (int kb = 0; kb < 4; ++kb) tma_load_2d(base + kb * 32768, &tmW, kb * 64, 0, smem_addr(&b_full));
+  }
+  if (ntiles > 0) mbar_wait(smem_addr(&b_full), 0);
+  const float* s_rs = reinterpret_cast<const float*>(sm + OFF_RS);
+  uint64_t seed = p.seed;
+  if (MODE == 0 && p.seed_ctr) seed += *p.seed_ctr;
+  const float keep_scale = (MODE == 0 && p.p_drop > 0.f) ? 1.f / (1.f - p.p_drop) : 1.f;
+  const __nv_bfloat16* resid = MODE == 0 ? p.x : p.addend;
+  for (int t = 0; t < ntiles; ++t) {
+    long r0; int rows, nt_;
+    tile_range(p.R, cta, ncta, t, r0, rows, nt_);
+    float acc[D / 2];
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) acc[i] = 0.f;
+    mbar_wait(smem_addr(&a_full), t & 1);
+    wgmma_fence();
+#pragma unroll
+    for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma<D, 0, 0>(acc, make_desc(base + OFF_A + kb * 16384 + wg * 8192 + k * 32, 16, 1024),
+                       make_desc(base + kb * 32768 + k * 32, 16, 1024));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence<D / 2>(acc);
+    mbar_arrive(smem_addr(&a_empty));                // the A tile may be overwritten
+    // fragment rows tr[h] (tile), h = 0/1: acc[4j + 2h], acc[4j + 2h + 1] are columns 8j + 2 (lane & 3) + {0, 1}
+    int tr[2];
+    bool live[2];
+    long grow[2];
+    float rs[2], sum[2] = {0.f, 0.f}, sq[2] = {0.f, 0.f};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      tr[h] = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+      live[h] = tr[h] < rows;
+      grow[h] = r0 + tr[h];
+      rs[h] = (MODE == 0 && live[h]) ? s_rs[(t & 3) * TM + tr[h]] : 0.f;
+    }
+#pragma unroll
+    for (int j = 0; j < D / 8; ++j) {
+      const int c = 8 * j + 2 * q4;
+      float2 bv = make_float2(0.f, 0.f), cv = make_float2(0.f, 0.f);
+      if (MODE == 0) {
+        bv = __ldg(reinterpret_cast<const float2*>(p.bias + c));
+        cv = __ldg(reinterpret_cast<const float2*>(p.c1 + c));
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float2 hv = make_float2(0.f, 0.f);
+        if (live[h] && resid != nullptr) hv = __bfloat1622float2(__ldg(reinterpret_cast<const __nv_bfloat162*>(resid + grow[h] * D + c)));
+        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (MODE == 0) {
+          v0 = fmaf(rs[h], cv.x, v0 + bv.x);
+          v1 = fmaf(rs[h], cv.y, v1 + bv.y);
+          // Z is stored as bf16 and the LayerNorm backward recomputes from the stored value: normalise the same value
+          const __nv_bfloat162 zb = __floats2bfloat162_rn(v0, v1);
+          if (live[h]) *reinterpret_cast<__nv_bfloat162*>(p.z + grow[h] * D + c) = zb;
+          const float2 zf = __bfloat1622float2(zb);
+          v0 = zf.x; v1 = zf.y;
+          if (p.p_drop > 0.f) {
+            const uint32_t m = dropout_keep8(seed, p.stream_id, (uint64_t)grow[h] * 32 + j, p.p_drop) >> (2 * q4);
+            v0 = (m & 1) ? v0 * keep_scale : 0.f;
+            v1 = (m & 2) ? v1 * keep_scale : 0.f;
+          }
+          v0 += hv.x; v1 += hv.y;
+          acc[4 * j + 2 * h] = v0; acc[4 * j + 2 * h + 1] = v1;   // y stays in registers for the normalisation pass
+          sum[h] += v0 + v1;
+          sq[h] = fmaf(v0, v0, fmaf(v1, v1, sq[h]));
+        } else if (live[h]) {
+          *reinterpret_cast<__nv_bfloat162*>(p.y + grow[h] * D + c) = __floats2bfloat162_rn(v0 + hv.x, v1 + hv.y);
+        }
+      }
+    }
+    if (MODE == 0) {
+      float mean[2], rstd[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 1);
+        sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 2);
+        sq[h] += __shfl_xor_sync(0xffffffffu, sq[h], 1);
+        sq[h] += __shfl_xor_sync(0xffffffffu, sq[h], 2);
+        mean[h] = sum[h] * (1.f / D);
+        const float var = fmaxf(sq[h] * (1.f / D) - mean[h] * mean[h], 0.f);
+        rstd[h] = rsqrtf(var + kLnEps);
+        if (live[h] && q4 == 0 && p.mean) { p.mean[grow[h]] = mean[h]; p.rstd[grow[h]] = rstd[h]; }
+      }
+#pragma unroll
+      for (int j = 0; j < D / 8; ++j) {
+        const int c = 8 * j + 2 * q4;
+        const float2 gv = __ldg(reinterpret_cast<const float2*>(p.gamma + c));
+        const float2 bt = __ldg(reinterpret_cast<const float2*>(p.beta + c));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!live[h]) continue;
+          const float o0 = fmaf((acc[4 * j + 2 * h] - mean[h]) * rstd[h], gv.x, bt.x);
+          const float o1 = fmaf((acc[4 * j + 2 * h + 1] - mean[h]) * rstd[h], gv.y, bt.y);
+          __nv_bfloat16* dst = grow[h] < p.split ? p.outA : p.outB;
+          *reinterpret_cast<__nv_bfloat162*>(dst + grow[h] * D + c) = __floats2bfloat162_rn(o0, o1);
+        }
+      }
+    }
   }
 }
 
@@ -481,7 +380,7 @@ int launch_fused(int mode, const CUtensorMap& tm, const Params& p, cudaStream_t 
       : cudaFuncSetAttribute(gcn_fused_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) { fira_set_error(FIRA_ERR_CUDA, "gcn_layer attr: %s", cudaGetErrorString(e)); return FIRA_ERR_CUDA; }
   long want = (p.R + 31) / 32;
-  const int grid = (int)(want < 148 ? (want < 1 ? 1 : want) : 148);
+  const int grid = (int)(want < fira_num_sms() ? (want < 1 ? 1 : want) : fira_num_sms());
   if (mode == 0) launch_k(gcn_fused_kernel<0>, dim3(grid), dim3(THREADS), smem, st, tm, p);
   else launch_k(gcn_fused_kernel<1>, dim3(grid), dim3(THREADS), smem, st, tm, p);
   return FIRA_OK;
@@ -499,10 +398,10 @@ int fira_csr_to_rows(const int* rowptr, const int* col, const float* val, int B,
   const int N = n_code + n_sub + n_ast;
   const long R = (long)B * N;
   cudaStream_t st = (cudaStream_t)stream;
-  int grid = (int)((R + 255) / 256 < 148 * 4 ? (R + 255) / 256 : 148 * 4);
+  int grid = (int)((R + 255) / 256 < fira_num_sms() * 4 ? (R + 255) / 256 : fira_num_sms() * 4);
   launch_k(rows_count_kernel, dim3(grid), dim3(256), 0, st, rowptr, s, N, counts);
   launch_k(rows_scan_kernel, dim3(1), dim3(1024), 0, st, counts, rowptr_rows, R);
-  grid = (int)((R + 7) / 8 < 148 * 8 ? (R + 7) / 8 : 148 * 8);
+  grid = (int)((R + 7) / 8 < fira_num_sms() * 8 ? (R + 7) / 8 : fira_num_sms() * 8);
   launch_k(rows_fill_kernel, dim3(grid), dim3(256), 0, st, rowptr, col, val, s, N, rowptr_rows, col_rows, val_rows);
   FIRA_CHECK_LAUNCH("fira_csr_to_rows");
   return FIRA_OK;

@@ -3,7 +3,7 @@
 // The reference runs every nn.Linear in fp32 (gnn_transformer.py:78,82,141-143,158,171-173,
 // 200-204; Model.py:16-19,54).  "logits within 1e-4 rel" cannot be met through 12 post-LN
 // layers with TF32/bf16 operands, so the parity mode keeps true fp32 products on the CUDA
-// cores; the throughput mode uses the tcgen05 kernels in gemm_tc.cu instead.
+// cores; the throughput mode uses the wgmma kernels in gemm_tc.cu instead.
 //
 // One generic kernel covers the three shapes a Linear needs:
 //   forward      Y[M,N]  = X[M,K]  * W[N,K]^T (+bias, +relu, + rs[m]*rc[n])     A k-contig, B k-contig

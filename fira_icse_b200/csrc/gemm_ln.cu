@@ -4,13 +4,14 @@
 //     z   = x W^T + bias (+ rs[m] * rc[n])                   [M, 256]   (stored: the backward recomputes from it)
 //     out = LayerNorm(dropout_p(z) + resid) * gamma + beta               (rows < split -> outA[r], else outB[r])
 //
-// A 128-row tile owns whole 256-wide rows, so the row statistics are thread-local in the epilogue (lane = TMEM lane =
-// row).  Pipeline: warp 0 = TMA producer (x and W k-blocks through a 3-stage ring, the residual tile in one go), warp 1
-// = tcgen05.mma issuer (M128 x N256 x K16, fp32 accumulator in TMEM), warps 2-5 = epilogue.  The epilogue makes two
-// passes over the accumulator: (1) z -> bf16 -> staging tile -> TMA store; y = dropout(z) + resid kept in TMEM
-// (tcgen05.st), row sum / sum of squares; (2) normalise, scale, -> staging tile -> TMA store.  All global traffic of the
-// epilogue is TMA (swizzled [32 x 64] boxes): no per-lane row stores.  Replaces fira_gemm_bf16_tc + fira_ln_residual_fwd
-// (two launches, one round trip of z through L2) on the forward critical path.
+// A 128-row tile owns whole 256-wide rows.  Pipeline: warps 0-7 = two consumer warpgroups (wgmma m64 x n256 x k16, fp32
+// accumulator in registers, rows 0-63 / 64-127 of the tile), warp 8 = TMA producer (x and W k-blocks through a 3-stage
+// ring, the residual tile in one go).  The epilogue works on the accumulator fragments in registers: a row's 256 columns
+// are spread over the 4 threads of a lane quad, so the row statistics take two shuffles.  Two passes: (1) z -> bf16 ->
+// staging boxes -> TMA store; y = dropout(z) + resid kept in the accumulator registers, row sum / sum of squares;
+// (2) normalise, scale, -> staging boxes -> TMA store.  All global traffic of the epilogue is TMA (swizzled [64 x 64]
+// boxes): no per-lane row stores.  Replaces fira_gemm_bf16_tc + fira_ln_residual_fwd (two launches, one round trip of
+// z through L2) on the forward critical path.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include "tc_common.cuh"
@@ -21,11 +22,14 @@ namespace {
 using namespace tc;
 
 constexpr int BM = 128, BN = 256, BK = 64, STAGES = 3;
-constexpr int THREADS = 192;
+constexpr int N_CONSUMER = 256;                      // warps 0-7
+constexpr int THREADS = N_CONSUMER + 32;             // + warp 8: TMA producer
 constexpr uint32_t A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2, STAGE_BYTES = A_BYTES + B_BYTES;   // 16 KB + 32 KB
 constexpr uint32_t RING_BYTES = STAGES * STAGE_BYTES;                                                // 144 KB
 constexpr uint32_t RES_BYTES = BM * BN * 2;                                                          // 64 KB: 4 boxes [128 x 64]
 constexpr uint32_t SMEM_BYTES = RING_BYTES + RES_BYTES + 1024;
+constexpr uint32_t BOX = 64 * 64 * 2;                // one [64 rows x 64 cols] bf16 staging box
+constexpr uint32_t OFF_OUT = 8 * BOX;                // z staging: ring [0, 64 KB), output staging: ring [64 KB, 128 KB)
 
 struct LnParams {
   int M, K;
@@ -36,28 +40,14 @@ struct LnParams {
   int has_b;
 };
 
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(map), "r"(src), "r"(c0), "r"(c1) : "memory");
-}
-
+// 9 warps: 3 share an SM sub-partition's 16K registers -> <= 168 each, so the 128-register accumulator epilogue spills a
+// little (ptxas -v: 584 B); the kernel is opt-in (FIRA_GEMM_LN) and has not been timed on the H100
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_ln_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
                const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmZ,
                const __grid_constant__ CUtensorMap tmOA, const __grid_constant__ CUtensorMap tmOB, LnParams p) {
   extern __shared__ unsigned char smem_dyn[];
-  __shared__ __align__(8) unsigned long long full_bar[STAGES], empty_bar[STAGES], res_bar, tmem_full_bar;
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) unsigned long long full_bar[STAGES], empty_bar[STAGES], res_bar;
   __shared__ __align__(16) float s_bias[BN], s_rc[BN], s_gamma[BN], s_beta[BN];
   const uint32_t base = (smem_addr(smem_dyn) + 1023u) & ~1023u;
   unsigned char* sm = smem_dyn + (base - smem_addr(smem_dyn));
@@ -66,181 +56,160 @@ gemm_ln_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ 
   const int nkb = (p.K + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(smem_addr(&full_bar[s]), 1); mbar_init(smem_addr(&empty_bar[s]), 1); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(smem_addr(&full_bar[s]), 1); mbar_init(smem_addr(&empty_bar[s]), N_CONSUMER); }
     mbar_init(smem_addr(&res_bar), 1);
-    mbar_init(smem_addr(&tmem_full_bar), 1);
     mbar_init_fence();
     tma_prefetch_desc(&tmX); tma_prefetch_desc(&tmW); tma_prefetch_desc(&tmR); tma_prefetch_desc(&tmZ);
     tma_prefetch_desc(&tmOA);
     if (p.has_b) tma_prefetch_desc(&tmOB);
   }
-  if (warp == 1) tmem_alloc(smem_addr(&tmem_slot), BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = tmem_slot;
   pdl_wait(); pdl_trigger();       // PDL: the prologue above overlapped the previous kernel's tail (common.cuh)
 
-  if (warp == 0 && lane == 0) {
+  if (warp == N_CONSUMER / 32) {
     // ===================== TMA producer: k-blocks of x and W, then the residual tile =====================
-    for (int i = 0; i < nkb; ++i) {
-      const int s = i % STAGES;
-      mbar_wait(smem_addr(&empty_bar[s]), ((i / STAGES) & 1) ^ 1);
-      const uint32_t sa = base + s * STAGE_BYTES, sb = sa + A_BYTES, fb = smem_addr(&full_bar[s]);
-      mbar_expect_tx(fb, STAGE_BYTES);
-      const int kb = (i + (int)blockIdx.x) % nkb;                      // rotated k order: see gemm_tc.cu
-      tma_load_2d(sa, &tmX, kb * BK, m0, fb);                          // box {64 k, 128 m}
-      tma_load_2d(sb, &tmW, kb * BK, 0, fb);                           // box {64 k, 256 n}
-      if (i == 0) {                                                    // residual rows: 4 boxes {64 cols, 128 rows}
-        const uint32_t rb = smem_addr(&res_bar);
-        mbar_expect_tx(rb, RES_BYTES);
-#pragma unroll
-        for (int g = 0; g < 4; ++g) tma_load_2d(base + RING_BYTES + g * 16384, &tmR, g * 64, m0, rb);
-      }
-    }
-  } else if (warp == 1 && lane == 0) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc = make_idesc_bf16(BM, BN, false, false);
-    for (int i = 0; i < nkb; ++i) {
-      const int s = i % STAGES;
-      mbar_wait(smem_addr(&full_bar[s]), (i / STAGES) & 1);
-      tc_fence_after();
-      const uint32_t sa = base + s * STAGE_BYTES, sb = sa + A_BYTES;
-#pragma unroll
-      for (int k = 0; k < BK / 16; ++k)
-        umma_bf16(tmem_acc, make_desc(sa + k * 32, 16, 1024), make_desc(sb + k * 32, 16, 1024), idesc, (i | k) ? 1u : 0u);
-      umma_commit(smem_addr(&empty_bar[s]));
-    }
-    umma_commit(smem_addr(&tmem_full_bar));
-  } else if (warp >= 2) {
-    // ===================== epilogue: lane = row, 8 chunks of 32 columns, two passes =====================
-    const int quarter = warp & 3;                    // TMEM lanes [32*quarter, +32)
-    const int row0 = m0 + quarter * 32;              // first global row of this warp
-    const int m = row0 + lane;
-    const bool live = m < p.M;
-    for (int c = quarter * 32 + lane; c < BN; c += 128) {
-      s_bias[c] = p.bias ? p.bias[c] : 0.f;
-      s_rc[c] = p.rs ? p.rc[c] : 0.f;
-      s_gamma[c] = p.gamma[c];
-      s_beta[c] = p.beta[c];
-    }
-    const float rsm = (p.rs && live) ? p.rs[m] : 0.f;
-    uint64_t seed = p.seed;
-    if (p.seed_ctr) seed += *p.seed_ctr;
-    const float keep_scale = p.p_drop > 0.f ? 1.f / (1.f - p.p_drop) : 1.f;
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    mbar_wait(smem_addr(&tmem_full_bar), 0);         // every MMA done: the ring is free -> staging tiles live there
-    tc_fence_after();
-    mbar_wait(smem_addr(&res_bar), 0);
-    const uint32_t tacc = tmem_acc + ((uint32_t)(quarter * 32) << 16);
-    unsigned char* stg = sm + (size_t)quarter * 4 * 4096;            // this warp: 4 boxes [32 rows x 64 cols] bf16
-    const unsigned char* res = sm + RING_BYTES;
-    const int tr = quarter * 32 + lane;              // tile row
-    float sum = 0.f, sq = 0.f;
-    // ---- pass 1: z (stored), y = dropout(z) + resid (kept in TMEM), row statistics
-#pragma unroll 1
-    for (int g = 0; g < 4; ++g) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int c0 = g * 64 + h * 32;
-        uint32_t r[32];
-        tmem_ld32(tacc + c0, r);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          float v[8];
-          const float4 b0 = *reinterpret_cast<const float4*>(s_bias + c0 + q * 8), b1 = *reinterpret_cast<const float4*>(s_bias + c0 + q * 8 + 4);
-          const float4 k0 = *reinterpret_cast<const float4*>(s_rc + c0 + q * 8), k1 = *reinterpret_cast<const float4*>(s_rc + c0 + q * 8 + 4);
-          const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-          const float kk[8] = {k0.x, k0.y, k0.z, k0.w, k1.x, k1.y, k1.z, k1.w};
-#pragma unroll
-          for (int j = 0; j < 8; ++j) v[j] = fmaf(rsm, kk[j], __uint_as_float(r[q * 8 + j]) + bb[j]);
-          // z is stored as bf16 and the LayerNorm backward recomputes from the stored value: normalise that value
-          uint4 zp;
-          __nv_bfloat162* hp = reinterpret_cast<__nv_bfloat162*>(&zp);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) hp[j] = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-          const int chunk = h * 4 + q;
-          const uint32_t so = (uint32_t)(lane * 128 + ((chunk ^ (lane & 7)) << 4));
-          *reinterpret_cast<uint4*>(stg + g * 4096 + so) = zp;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) { const float2 f = __bfloat1622float2(hp[j]); v[2 * j] = f.x; v[2 * j + 1] = f.y; }
-          if (p.p_drop > 0.f) {
-            const uint32_t mk = dropout_keep8(seed, p.stream_id, (uint64_t)m * 32 + (c0 >> 3) + q, p.p_drop);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = ((mk >> j) & 1) ? v[j] * keep_scale : 0.f;
-          }
-          // residual: box g of the tile, row tr, 16-byte chunk `chunk` (same swizzle as the staging tile)
-          const uint4 rq = *reinterpret_cast<const uint4*>(res + g * 16384 + tr * 128 + ((chunk ^ (tr & 7)) << 4));
-          const __nv_bfloat162* rp = reinterpret_cast<const __nv_bfloat162*>(&rq);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float2 f = __bfloat1622float2(rp[j]);
-            v[2 * j] += f.x; v[2 * j + 1] += f.y;
-          }
-#pragma unroll
-          for (int j = 0; j < 8; ++j) { sum += v[j]; sq = fmaf(v[j], v[j], sq); r[q * 8 + j] = __float_as_uint(v[j]); }
-        }
-        tmem_st32(tacc + c0, r);
-      }
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0 && row0 < p.M) tma_store_2d(&tmZ, smem_addr(stg + g * 4096), g * 64, row0);
-    }
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-    const float mean = sum * (1.f / BN);
-    const float var = fmaxf(sq * (1.f / BN) - mean * mean, 0.f);
-    const float rstd = rsqrtf(var + kLnEps);
-    if (live) { p.mean[m] = mean; p.rstd[m] = rstd; }
-    if (lane == 0) {                                 // the z boxes have been read out of the staging tiles
-      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-      asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    }
-    __syncwarp();
-    // ---- pass 2: normalise, scale, store.  Rows below `split` go to outA[r], the others to outB[r].  Map A ends at
-    // `split` (TMA clips the rest of a slab that straddles it); map B covers all rows of outB, so the one straddling slab
-    // also writes its rows below `split` into outB -- storage the callers leave unused (see fira_b200.h).
-#pragma unroll 1
-    for (int g = 0; g < 4; ++g) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int c0 = g * 64 + h * 32;
-        uint32_t r[32];
-        tmem_ld32(tacc + c0, r);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float4 g0 = *reinterpret_cast<const float4*>(s_gamma + c0 + q * 8), g1 = *reinterpret_cast<const float4*>(s_gamma + c0 + q * 8 + 4);
-          const float4 e0 = *reinterpret_cast<const float4*>(s_beta + c0 + q * 8), e1 = *reinterpret_cast<const float4*>(s_beta + c0 + q * 8 + 4);
-          const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-          const float ee[8] = {e0.x, e0.y, e0.z, e0.w, e1.x, e1.y, e1.z, e1.w};
-          float o[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) o[j] = fmaf((__uint_as_float(r[q * 8 + j]) - mean) * rstd, gg[j], ee[j]);
-          uint4 op;
-          __nv_bfloat162* hp = reinterpret_cast<__nv_bfloat162*>(&op);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) hp[j] = __floats2bfloat162_rn(o[2 * j], o[2 * j + 1]);
-          const int chunk = h * 4 + q;
-          *reinterpret_cast<uint4*>(stg + g * 4096 + lane * 128 + ((chunk ^ (lane & 7)) << 4)) = op;
-        }
-      }
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0 && row0 < p.M) {
-        if (row0 < p.split) tma_store_2d(&tmOA, smem_addr(stg + g * 4096), g * 64, row0);
-        if (p.has_b && row0 + 32 > p.split) tma_store_2d(&tmOB, smem_addr(stg + g * 4096), g * 64, row0);
-      }
-    }
     if (lane == 0) {
-      asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-      asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+      for (int i = 0; i < nkb; ++i) {
+        const int s = i % STAGES;
+        mbar_wait(smem_addr(&empty_bar[s]), ((i / STAGES) & 1) ^ 1);
+        const uint32_t sa = base + s * STAGE_BYTES, sb = sa + A_BYTES, fb = smem_addr(&full_bar[s]);
+        mbar_expect_tx(fb, STAGE_BYTES);
+        const int kb = (i + (int)blockIdx.x) % nkb;                      // rotated k order: see gemm_tc.cu
+        tma_load_2d(sa, &tmX, kb * BK, m0, fb);                          // box {64 k, 128 m}
+        tma_load_2d(sb, &tmW, kb * BK, 0, fb);                           // box {64 k, 256 n}
+        if (i == 0) {                                                    // residual rows: 4 boxes {64 cols, 128 rows}
+          const uint32_t rb = smem_addr(&res_bar);
+          mbar_expect_tx(rb, RES_BYTES);
+#pragma unroll
+          for (int g = 0; g < 4; ++g) tma_load_2d(base + RING_BYTES + g * 16384, &tmR, g * 64, m0, rb);
+        }
+      }
     }
-    __syncwarp();
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_acc, BN);
+
+  // ===================== consumers: warpgroup wg = tile rows [64 wg, +64) =====================
+  const int wg = warp >> 2;
+  for (int c = threadIdx.x; c < BN; c += N_CONSUMER) {
+    s_bias[c] = p.bias ? p.bias[c] : 0.f;
+    s_rc[c] = p.rs ? p.rc[c] : 0.f;
+    s_gamma[c] = p.gamma[c];
+    s_beta[c] = p.beta[c];
+  }
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  for (int i = 0; i < nkb; ++i) {
+    const int s = i % STAGES;
+    mbar_wait(smem_addr(&full_bar[s]), (i / STAGES) & 1);
+    const uint32_t sa = base + s * STAGE_BYTES + wg * 8192, sb = base + s * STAGE_BYTES + A_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) wgmma<BN, 0, 0>(acc, make_desc(sa + k * 32, 16, 1024), make_desc(sb + k * 32, 16, 1024));
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (i > 0) mbar_arrive(smem_addr(&empty_bar[(i - 1) % STAGES]));
+  }
+  wgmma_wait<0>();
+  reg_fence<BN / 2>(acc);
+  named_bar(1, N_CONSUMER);                          // both warpgroups are done with the ring: staging boxes live there now
+  mbar_wait(smem_addr(&res_bar), 0);
+
+  // fragment rows (tile) tr[h], h = 0/1: acc[4j + 2h], acc[4j + 2h + 1] are columns 8j + 2 (lane & 3) + {0, 1}
+  const int q4 = lane & 3;
+  int tr[2], br[2], m[2];
+  float rsm[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    tr[h] = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+    br[h] = tr[h] - wg * 64;                         // row inside this warpgroup's [64 x 64] staging boxes
+    m[h] = m0 + tr[h];
+    rsm[h] = (p.rs && m[h] < p.M) ? p.rs[m[h]] : 0.f;
+  }
+  uint64_t seed = p.seed;
+  if (p.seed_ctr) seed += *p.seed_ctr;
+  const float keep_scale = p.p_drop > 0.f ? 1.f / (1.f - p.p_drop) : 1.f;
+  const unsigned char* res = sm + RING_BYTES;
+  unsigned char* zst = sm + wg * 4 * BOX;
+  unsigned char* ost = sm + OFF_OUT + wg * 4 * BOX;
+  const int row0 = m0 + wg * 64;                     // first global row of this warpgroup
+  float sum[2] = {0.f, 0.f}, sq[2] = {0.f, 0.f};
+  // ---- pass 1: z (stored), y = dropout(z) + resid (kept in registers), row statistics
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int c = 8 * j + 2 * q4, g = j >> 3, chunk = j & 7;
+    const float2 bb = *reinterpret_cast<const float2*>(s_bias + c), kk = *reinterpret_cast<const float2*>(s_rc + c);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float v0 = fmaf(rsm[h], kk.x, acc[4 * j + 2 * h] + bb.x), v1 = fmaf(rsm[h], kk.y, acc[4 * j + 2 * h + 1] + bb.y);
+      // z is stored as bf16 and the LayerNorm backward recomputes from the stored value: normalise that value
+      const __nv_bfloat162 zb = __floats2bfloat162_rn(v0, v1);
+      *reinterpret_cast<__nv_bfloat162*>(zst + g * BOX + br[h] * 128 + ((chunk ^ (br[h] & 7)) << 4) + q4 * 4) = zb;
+      const float2 zf = __bfloat1622float2(zb);
+      v0 = zf.x; v1 = zf.y;
+      if (p.p_drop > 0.f) {
+        const uint32_t mk = dropout_keep8(seed, p.stream_id, (uint64_t)m[h] * 32 + j, p.p_drop) >> (2 * q4);
+        v0 = (mk & 1) ? v0 * keep_scale : 0.f;
+        v1 = (mk & 2) ? v1 * keep_scale : 0.f;
+      }
+      const float2 rf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(
+          res + g * 16384 + tr[h] * 128 + ((chunk ^ (tr[h] & 7)) << 4) + q4 * 4));
+      v0 += rf.x; v1 += rf.y;
+      acc[4 * j + 2 * h] = v0; acc[4 * j + 2 * h + 1] = v1;
+      sum[h] += v0 + v1;
+      sq[h] = fmaf(v0, v0, fmaf(v1, v1, sq[h]));
+    }
+  }
+  fence_proxy_async();
+  named_bar(2 + wg, 128);
+  if ((threadIdx.x & 127) == 0 && row0 < p.M) {
+#pragma unroll
+    for (int g = 0; g < 4; ++g) tma_store_2d(&tmZ, smem_addr(zst + g * BOX), g * 64, row0);
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+  }
+  float mean[2], rstd[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 1);
+    sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 2);
+    sq[h] += __shfl_xor_sync(0xffffffffu, sq[h], 1);
+    sq[h] += __shfl_xor_sync(0xffffffffu, sq[h], 2);
+    mean[h] = sum[h] * (1.f / BN);
+    const float var = fmaxf(sq[h] * (1.f / BN) - mean[h] * mean[h], 0.f);
+    rstd[h] = rsqrtf(var + kLnEps);
+    if (q4 == 0 && m[h] < p.M) { p.mean[m[h]] = mean[h]; p.rstd[m[h]] = rstd[h]; }
+  }
+  // ---- pass 2: normalise, scale, store.  Rows below `split` go to outA[r], the others to outB[r].  Map A ends at
+  // `split` (TMA clips the rest of a box that straddles it); map B covers all rows of outB and is written in 32-row
+  // slabs, so the one straddling slab also writes its rows below `split` into outB -- storage the callers leave unused
+  // (see fira_b200.h).
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int c = 8 * j + 2 * q4, g = j >> 3, chunk = j & 7;
+    const float2 gg = *reinterpret_cast<const float2*>(s_gamma + c), ee = *reinterpret_cast<const float2*>(s_beta + c);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float o0 = fmaf((acc[4 * j + 2 * h] - mean[h]) * rstd[h], gg.x, ee.x);
+      const float o1 = fmaf((acc[4 * j + 2 * h + 1] - mean[h]) * rstd[h], gg.y, ee.y);
+      *reinterpret_cast<__nv_bfloat162*>(ost + g * BOX + br[h] * 128 + ((chunk ^ (br[h] & 7)) << 4) + q4 * 4) =
+          __floats2bfloat162_rn(o0, o1);
+    }
+  }
+  fence_proxy_async();
+  named_bar(2 + wg, 128);
+  if ((threadIdx.x & 127) == 0) {
+    if (row0 < p.M) {
+#pragma unroll
+      for (int g = 0; g < 4; ++g) {
+        if (row0 < p.split) tma_store_2d(&tmOA, smem_addr(ost + g * BOX), g * 64, row0);
+        // outB in [32 x 64] halves of the box: only the 32-row slab that straddles `split` writes rows below it
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+          if (p.has_b && row0 + 32 * hh < p.M && row0 + 32 * hh + 32 > p.split)
+            tma_store_2d(&tmOB, smem_addr(ost + g * BOX + hh * 4096), g * 64, row0 + 32 * hh);
+      }
+    }
+    tma_store_commit_wait_read();                    // the staging boxes must stay valid until TMA has read them
   }
 }
 
@@ -265,11 +234,11 @@ extern "C" int fira_gemm_ln_fwd(const void* x, long ldx, const void* w, const fl
   if ((rc_ = make_map_bf16(&tx, x, M, K, ldx, BK, BM, "gemm_ln_fwd"))) return rc_;
   if ((rc_ = make_map_bf16(&tw, w, BN, K, K, BK, BN, "gemm_ln_fwd"))) return rc_;
   if ((rc_ = make_map_bf16(&tr, resid, M, BN, BN, 64, BM, "gemm_ln_fwd"))) return rc_;
-  if ((rc_ = make_map_bf16(&tz, z, M, BN, BN, 64, 32, "gemm_ln_fwd"))) return rc_;
+  if ((rc_ = make_map_bf16(&tz, z, M, BN, BN, 64, 64, "gemm_ln_fwd"))) return rc_;
   const bool has_a = split > 0, has_b = split < rows;
   // map A: rows [0, split) of outA; map B: all rows of outB (indexed by the global row; only slabs reaching `split` or
   // beyond are stored through it)
-  if ((rc_ = make_map_bf16(&toa, outA, has_a ? split : 1, BN, BN, 64, 32, "gemm_ln_fwd"))) return rc_;
+  if ((rc_ = make_map_bf16(&toa, outA, has_a ? split : 1, BN, BN, 64, 64, "gemm_ln_fwd"))) return rc_;
   tob = toa;
   if (has_b && (rc_ = make_map_bf16(&tob, outB, rows, BN, BN, 64, 32, "gemm_ln_fwd"))) return rc_;
   LnParams p{M, K, has_a ? split : 0, bias, rs, rc, gamma, beta, mean, rstd, p_drop, seed, seed_ctr, stream_id, has_b ? 1 : 0};

@@ -1,8 +1,7 @@
-// bf16 tensor-core GEMM for the throughput path: tcgen05.mma (UMMA, SASS UTCHMMA) with the fp32
-// accumulator in TMEM, operands staged in shared memory by TMA (cp.async.bulk.tensor, SASS UTMALDG)
-// through a 2-3 stage mbarrier ring (two CTAs per SM), warp-specialised: warp 0 = TMA producer, warp 1 = MMA issuer
-// (one elected thread) + TMEM allocator, warps 2-5 = epilogue (tcgen05.ld -> bias / rank-1 / relu ->
-// global).  One 128 x BN output tile per CTA, cta_group::1.
+// bf16 tensor-core GEMM for the throughput path: wgmma.mma_async (SASS HGMMA) with the fp32 accumulator in
+// registers, operands staged in shared memory by TMA (cp.async.bulk.tensor, SASS UTMALDG) through a 2-4 stage mbarrier
+// ring, warp-specialised: warps 0-7 = two consumer warpgroups (rows 0-63 / 64-127 of the tile: wgmma issue, then the
+// epilogue), warp 8 = TMA producer.  One 128 x BN output tile per CTA.
 //
 //   C[M,N] = A (M x K) * B (K x N) + bias[n] + rs[m]*rc[n]      (optional relu; fp32 or bf16 output)
 //
@@ -10,22 +9,25 @@
 //   a_kmajor = 1 : A[m*lda + k]   (activations as they are)        a_kmajor = 0 : A[k*lda + m]  (dY^T, X^T)
 //   b_kmajor = 1 : B[n*ldb + k]   (nn.Linear weight [out,in])      b_kmajor = 0 : B[k*ldb + n]
 // The MN-major forms let the weight-gradient GEMM dW = dY^T X read dY and X in place (no transpose
-// pass): TMA fetches [64 k-rows x 64 mn] boxes and the UMMA descriptor carries the MN-major
-// canonical SWIZZLE_128B layout (instruction-descriptor bits 15/16).
+// pass): TMA fetches [64 k-rows x 64 mn] boxes and the wgmma descriptor carries the MN-major
+// canonical SWIZZLE_128B layout (transpose bits of the instruction).
 // splits > 1: split-K across blockIdx.z, fp32 partials atomically added into a zero-filled C.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <atomic>
 #include <stdlib.h>
-#include "common.cuh"
+#include "tc_common.cuh"
 #include "fira_b200.h"
 
 namespace {
 
-constexpr int BM = 128;          // UMMA M (cta_group::1)
+using namespace tc;
+
+constexpr int BM = 128;          // two m64 warpgroups
 constexpr int BK = 64;           // 64 bf16 = 128 B = one SWIZZLE_128B atom row
-constexpr int UMMA_K = 16;
-constexpr int NUM_THREADS = 192; // 6 warps
+constexpr int N_CONSUMER = 256;  // warps 0-7
+constexpr int NUM_THREADS = N_CONSUMER + 32;   // + warp 8: TMA producer
+constexpr int CONSUMER_BAR = 1;  // named barrier of the consumer warps
 
 struct TcParams {
   void* C; long ldc; int c_is_bf16;
@@ -51,66 +53,66 @@ __device__ __forceinline__ void stamp(const TcParams& p, int slot) {
   }
 }
 
-__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok = 0, spins = 0;
-  while (true) {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-    if (ok) break;
-    if (++spins > (1u << 26)) __trap();      // never hang the GPU on a protocol bug
+// Mainloop of one consumer warpgroup: wait for a stage, 4 x wgmma m64 x BN x k16 on it, fold the A column sums in while
+// they run, hand the previous stage back.  TA / TB = 1: A / B MN-major (the transpose bits are immediates of the
+// instruction, so each operand-major combination is its own instantiation).
+template <int BN, int STAGES, int TA, int TB>
+__device__ __forceinline__ void mainloop(float* acc, float& cs, bool do_cs, int nkb, uint32_t base, const unsigned char* sm,
+                                         unsigned long long* full_bar, unsigned long long* empty_bar, int wg, const TcParams& p) {
+  constexpr uint32_t A_BYTES = BM * BK * 2, STAGE_BYTES = A_BYTES + BN * BK * 2;
+  // column sums (MN-major A, [m/64][64 k][64 m] panels): thread <-> m column (t & 63) of its warpgroup's panel, half of k
+  const int cs_m = threadIdx.x & 63, cs_k0 = ((threadIdx.x >> 6) & 1) * 32;
+  for (int i = 0; i < nkb; ++i) {
+    const int s = i % STAGES;
+    mbar_wait(smem_addr(&full_bar[s]), (i / STAGES) & 1);
+    if (i == 0 && threadIdx.x == 0) stamp(p, 4);     // first operand stage landed
+    const uint32_t sa = base + s * STAGE_BYTES + wg * 8192, sb = base + s * STAGE_BYTES + A_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+      // K-major: step 16 k = 32 B inside the 128-B swizzle row; MN-major: step 16 k-rows = 2048 B
+      const uint64_t da = TA ? make_desc(sa + k * 2048, 8192, 1024) : make_desc(sa + k * 32, 16, 1024);
+      const uint64_t db = TB ? make_desc(sb + k * 2048, 8192, 1024) : make_desc(sb + k * 32, 16, 1024);
+      wgmma<BN, TA, TB>(acc, da, db);
+    }
+    wgmma_commit();
+    if (do_cs) {
+      const unsigned char* a = sm + (size_t)s * STAGE_BYTES + wg * 8192 + (cs_m & 7) * 2;
+#pragma unroll 8
+      for (int k = cs_k0; k < cs_k0 + 32; ++k)
+        cs += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(a + (k >> 3) * 1024 + (k & 7) * 128 + (((cs_m >> 3) ^ (k & 7)) << 4)));
+    }
+    wgmma_wait<1>();                                 // the previous stage's wgmma are complete: hand it back
+    if (i > 0) mbar_arrive(smem_addr(&empty_bar[(i - 1) % STAGES]));
   }
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
+  wgmma_wait<0>();
+  reg_fence<BN / 2>(acc);
 }
 
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, SM100): start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout SWIZZLE_128B=2 [61,64).
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
+template <int BN, int STAGES>
+__host__ __device__ constexpr uint32_t acc_region_bytes() {
+  constexpr uint32_t ring = STAGES * (BM * BK * 2 + BN * BK * 2), acc = BM * (BN + 4) * 4;
+  return ring > acc ? ring : acc;
 }
 
 // Stage layout in shared memory (1024-B aligned, SWIZZLE_128B):
 //   K-major operand  : [rows][64 k]          rows x 128 B, 8-row groups 1024 B apart (SBO = 1024)
 //   MN-major operand : [mn/64][64 k][64 mn]  each 64-mn panel is 64 k-rows x 128 B = 8 KB (LBO = 8192 between
 //                      panels, SBO = 1024 between 8-k groups); one TMA box per panel.
+// Once the last k-block has been consumed, the ring holds the fp32 accumulator tile [128][BN + 4] (row pitch + 16 B:
+// conflict-free 16-byte reads with lane = row); the TMA-store staging boxes follow the ring.
 template <int BN, int STAGES>
-__global__ void __launch_bounds__(NUM_THREADS, 2)
+__global__ void __launch_bounds__(NUM_THREADS, BN == 256 ? 1 : 2)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmC, TcParams p) {
   extern __shared__ unsigned char smem_dyn[];
   __shared__ __align__(16) float s_bias[BN], s_rc[BN];   // per-column epilogue constants of this tile (TMA-store path)
   constexpr uint32_t A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2, STAGE_BYTES = A_BYTES + B_BYTES;
-  __shared__ __align__(8) unsigned long long full_bar[STAGES], empty_bar[STAGES], tmem_full_bar;
-  __shared__ uint32_t tmem_base_slot;
+  constexpr int PITCH = BN + 4;                                        // floats per row of the accumulator tile
+  __shared__ __align__(8) unsigned long long full_bar[STAGES], empty_bar[STAGES];
 
   const uint32_t base = (smem_addr(smem_dyn) + 1023u) & ~1023u;
+  unsigned char* sm = smem_dyn + (base - smem_addr(smem_dyn));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
   const int kb_total = (p.K + BK - 1) / BK;
@@ -120,252 +122,176 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (threadIdx.x == 0) stamp(p, 0);                 // kernel entry
 
   // bias gradient folded into the weight-gradient product: the CTAs of the first column tile also sum the A tile
-  // (= dY^T) over k as it passes through shared memory; a stage is then released by the MMAs AND the four summing warps
+  // (= dY^T) over k as it passes through shared memory, while the wgmma of the stage runs
   const bool do_cs = p.colsum != nullptr && blockIdx.x == 0;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(smem_addr(&full_bar[s]), 1); mbar_init(smem_addr(&empty_bar[s]), do_cs ? 5 : 1); }
-    mbar_init(smem_addr(&tmem_full_bar), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-    if (p.tma_store) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmC) : "memory");
+    for (int s = 0; s < STAGES; ++s) { mbar_init(smem_addr(&full_bar[s]), 1); mbar_init(smem_addr(&empty_bar[s]), N_CONSUMER); }
+    mbar_init_fence();
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    if (p.tma_store) tma_prefetch_desc(&tmC);
   }
-  if (warp == 1) {   // TMEM: BN fp32 accumulator columns (power of two >= 32)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_addr(&tmem_base_slot)), "r"(BN));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = tmem_base_slot;
-  if (threadIdx.x == 0) stamp(p, 1);                 // prologue done (barriers, TMEM)
+  if (threadIdx.x == 0) stamp(p, 1);                 // prologue done (barriers)
   pdl_wait(); pdl_trigger();       // PDL: the prologue above overlapped the previous kernel's tail (common.cuh)
   if (threadIdx.x == 0) stamp(p, 2);                 // previous kernel complete
 
-  if (warp == 0 && lane == 0) {
+  if (warp == N_CONSUMER / 32) {
     // ===================== TMA producer =====================
-    for (int i = 0; i < nkb; ++i) {
-      const int s = i % STAGES;
-      const uint32_t ph = (i / STAGES) & 1;
-      mbar_wait(smem_addr(&empty_bar[s]), ph ^ 1);
-      const uint32_t sa = base + s * STAGE_BYTES, sb = sa + A_BYTES;
-      const uint32_t fb = smem_addr(&full_bar[s]);
-      mbar_expect_tx(fb, STAGE_BYTES);
-      // The CTAs of one tile row all read the same A tile and those of one tile column the same B tile, at the same
-      // moment: the phase probe showed the load phase growing with the number of CTAs that share a tile (1.1 us with 4
-      // sharers, 5.1 us with 8) -- same-line contention in L2.  Rotating the k-block order by the tile coordinates makes
-      // the sharers ask for different lines at any one time; the fp32 sum over k-blocks is order-independent up to
-      // rounding.
-      const int kb = p.rotate ? kb_begin + (i + (int)(blockIdx.x + blockIdx.y)) % nkb : kb_begin + i;
-      const int k0 = kb * BK;
-      if (p.a_kmajor) {
-        tma_load_2d(sa, &tmA, k0, m0, fb);                        // box {64 k, 128 m}
-      } else {
-        tma_load_2d(sa, &tmA, m0, k0, fb);                        // two boxes {64 m, 64 k}
-        tma_load_2d(sa + 8192, &tmA, m0 + 64, k0, fb);
-      }
-      if (p.b_kmajor) {
-        tma_load_2d(sb, &tmB, k0, n0, fb);                        // box {64 k, BN n}
-      } else {
-#pragma unroll
-        for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * 8192, &tmB, n0 + j * 64, k0, fb);
-      }
-    }
-    stamp(p, 3);                                     // every TMA load issued
-  } else if (warp == 1 && lane == 0) {
-    // ===================== MMA issuer =====================
-    // instruction descriptor (cute::UMMA::InstrDescriptor): D=f32 [4,6)=1, A=bf16 [7,10)=1, B=bf16 [10,13)=1,
-    // a_major bit 15, b_major bit 16 (1 = MN-major), N>>3 [17,23), M>>4 [24,29)
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((p.a_kmajor ? 0u : 1u) << 15) |
-                           ((p.b_kmajor ? 0u : 1u) << 16) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-    for (int i = 0; i < nkb; ++i) {
-      const int s = i % STAGES;
-      const uint32_t ph = (i / STAGES) & 1;
-      mbar_wait(smem_addr(&full_bar[s]), ph);
-      tc_fence_after();
-      if (i == 0) stamp(p, 4);                       // first operand stage landed
-      const uint32_t sa = base + s * STAGE_BYTES, sb = sa + A_BYTES;
-#pragma unroll
-      for (int k = 0; k < BK / UMMA_K; ++k) {
-        // K-major: step 16 k = 32 B inside the 128-B swizzle row; MN-major: step 16 k-rows = 2048 B
-        const uint64_t da = p.a_kmajor ? make_desc(sa + k * 32, 16, 1024) : make_desc(sa + k * 2048, 8192, 1024);
-        const uint64_t db = p.b_kmajor ? make_desc(sb + k * 32, 16, 1024) : make_desc(sb + k * 2048, 8192, 1024);
-        umma_bf16(tmem_acc, da, db, idesc, (i > 0 || k > 0) ? 1u : 0u);
-      }
-      umma_commit(smem_addr(&empty_bar[s]));        // frees the stage when these MMAs have read it
-    }
-    umma_commit(smem_addr(&tmem_full_bar));         // accumulator complete
-    stamp(p, 5);                                     // every MMA issued
-  } else if (warp >= 2) {
-    // ===================== epilogue: TMEM -> registers -> smem (lane = row) -> global (lane = column) =====
-    // tcgen05.ld hands every lane ONE accumulator row; storing that straight to global makes each warp
-    // store touch 32 different rows (32 sectors per instruction: measured ~30 us per tile, round 1).  So the
-    // warp parks a 32 x HB fp32 block in the (now idle) pipeline stages with a +16 B row pitch
-    // (conflict-free float4 writes), then streams it out with lanes across the columns of a row:
-    // contiguous 256-512 B (bf16) / 512 B-1 KB (fp32) per store; bias / rank-1 / relu / accumulate /
-    // split-K atomics are applied on the way out with per-lane column constants.  HB = 128 columns at a
-    // time keeps the staging area inside two pipeline stages, so two CTAs fit per SM and one CTA's
-    // epilogue overlaps the other's TMA/MMA phase.
-    const int quarter = warp & 3;                   // TMEM lanes [32*quarter, +32) are this warp's
-    constexpr int HB = BN < 128 ? BN : 128;         // columns staged per pass
-    constexpr int PITCH = HB + 4;                   // floats
-    constexpr int LPR = HB / 8;                     // lanes per row on the way out (8 columns per lane)
-    constexpr int RPI = 32 / LPR;                   // rows per store iteration
-    float* stg = reinterpret_cast<float*>(smem_dyn + (base - smem_addr(smem_dyn))) + (size_t)quarter * 32 * PITCH;
-    if (do_cs) {
-      // thread <-> one of the 128 m columns of the MN-major A tile: [m/64][64 k][64 m] bf16, 128-B rows, SWIZZLE_128B
-      const int t = quarter * 32 + lane;
-      const unsigned char* a_base = smem_dyn + (base - smem_addr(smem_dyn)) + (t >> 6) * 8192 + (t & 7) * 2;
-      const int chunk = (t & 63) >> 3;
-      float cs = 0.f;
+    if (lane == 0) {
       for (int i = 0; i < nkb; ++i) {
         const int s = i % STAGES;
-        mbar_wait(smem_addr(&full_bar[s]), (i / STAGES) & 1);
-        const unsigned char* a = a_base + (size_t)s * STAGE_BYTES;
-#pragma unroll 8
-        for (int k = 0; k < BK; ++k)
-          cs += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(a + (k >> 3) * 1024 + (k & 7) * 128 + ((chunk ^ (k & 7)) << 4)));
-        __syncwarp();
-        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(&empty_bar[s])) : "memory");
-      }
-      if (m0 + t < p.M) atomicAdd(p.colsum + m0 + t, cs);
-      asm volatile("bar.sync 1, 128;" ::: "memory");   // every summing warp is done with the stages before one is reused for staging
-    }
-    const int mrow0 = m0 + quarter * 32;
-    if (p.tma_store) {                               // per-column constants -> shared memory while the MMAs run
-      for (int c = quarter * 32 + lane; c < BN; c += 128) {
-        const int n = n0 + c;
-        s_bias[c] = (p.bias && n < p.N) ? p.bias[n] : 0.f;
-        s_rc[c] = (p.rs && n < p.N) ? p.rc[n] : 0.f;
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-    }
-    if (nkb > 0) {
-      mbar_wait(smem_addr(&tmem_full_bar), 0);
-      tc_fence_after();
-    }
-    if (p.tma_store) {
-      // ---- bf16 output through TMA: each warp converts its 32 rows, 64 columns at a time, into a [32 x 64] bf16 box in
-      // the SWIZZLE_128B layout (conflict-free 16-byte st.shared: lane = row, chunk slot = chunk ^ (row & 7)) and one
-      // elected lane hands the box to the TMA engine; rows / columns past M / N are clipped by the tensor map.  The
-      // per-column constants were staged in shared memory while the MMAs ran.  (probe: 1.7 us -> for the 128 x 64 tile
-      // of the smem-staged path below, 6.7 us for 128 x 256.)
-      unsigned char* cst = smem_dyn + (base - smem_addr(smem_dyn)) + (size_t)quarter * (BN / 64) * 4096;
-      const int m = mrow0 + lane;
-      const float rsm = (p.rs && m < p.M) ? p.rs[m] : 0.f;
-      if (warp == 2 && lane == 0) stamp(p, 6);
-      const __nv_bfloat16* mrow = nullptr;          // relu-backward mask: this lane's row of the forward activations
-      if (p.relu_mask && m < p.M) {
-        mrow = p.relu_mask + (long)m * p.ldc + n0;
-#pragma unroll
-        for (int g = 0; g < BN / 64; ++g)
-          if (n0 + g * 64 < p.N) asm volatile("prefetch.global.L2 [%0];" ::"l"(mrow + g * 64));
-      }
-#pragma unroll 1
-      for (int g = 0; g < BN / 64; ++g) {
-        uint4 mk[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) mk[j] = make_uint4(0x3f803f80u, 0x3f803f80u, 0x3f803f80u, 0x3f803f80u);   // 1.0: keep
-        if (mrow != nullptr && n0 + g * 64 + 63 < p.N) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) mk[j] = *reinterpret_cast<const uint4*>(mrow + g * 64 + j * 8);
-        } else if (mrow != nullptr) {
-          __nv_bfloat16* me = reinterpret_cast<__nv_bfloat16*>(mk);
-          for (int j = 0; j < 64; ++j) if (n0 + g * 64 + j < p.N) me[j] = mrow[g * 64 + j];
+        const uint32_t ph = (i / STAGES) & 1;
+        mbar_wait(smem_addr(&empty_bar[s]), ph ^ 1);
+        const uint32_t sa = base + s * STAGE_BYTES, sb = sa + A_BYTES;
+        const uint32_t fb = smem_addr(&full_bar[s]);
+        mbar_expect_tx(fb, STAGE_BYTES);
+        // The CTAs of one tile row all read the same A tile and those of one tile column the same B tile, at the same
+        // moment.  Rotating the k-block order by the tile coordinates makes the sharers ask for different L2 lines at
+        // any one time; the fp32 sum over k-blocks is order-independent up to rounding.
+        const int kb = p.rotate ? kb_begin + (i + (int)(blockIdx.x + blockIdx.y)) % nkb : kb_begin + i;
+        const int k0 = kb * BK;
+        if (p.a_kmajor) {
+          tma_load_2d(sa, &tmA, k0, m0, fb);                        // box {64 k, 128 m}
+        } else {
+          tma_load_2d(sa, &tmA, m0, k0, fb);                        // two boxes {64 m, 64 k}
+          tma_load_2d(sa + 8192, &tmA, m0 + 64, k0, fb);
         }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          uint32_t r[32];
-          const int c0 = g * 64 + h * 32;
-          if (nkb > 0) {
-            const uint32_t taddr = tmem_acc + ((uint32_t)(quarter * 32) << 16) + (uint32_t)c0;
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                  "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-                  "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-                  "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                : "r"(taddr));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) r[j] = 0u;
-          }
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            float v[8];
-            const float4 b0 = *reinterpret_cast<const float4*>(s_bias + c0 + q * 8), b1 = *reinterpret_cast<const float4*>(s_bias + c0 + q * 8 + 4);
-            const float4 k0 = *reinterpret_cast<const float4*>(s_rc + c0 + q * 8), k1 = *reinterpret_cast<const float4*>(s_rc + c0 + q * 8 + 4);
-            const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-            const float kk[8] = {k0.x, k0.y, k0.z, k0.w, k1.x, k1.y, k1.z, k1.w};
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              v[j] = fmaf(rsm, kk[j], __uint_as_float(r[q * 8 + j]) + bb[j]);
-              if (p.relu) v[j] = fmaxf(v[j], 0.f);
-            }
-            {
-              const __nv_bfloat162* mp = reinterpret_cast<const __nv_bfloat162*>(&mk[h * 4 + q]);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const float2 f = __bfloat1622float2(mp[j]);
-                if (!(f.x > 0.f)) v[2 * j] = 0.f;
-                if (!(f.y > 0.f)) v[2 * j + 1] = 0.f;
-              }
-            }
-            uint4 o;
-            __nv_bfloat162* hp = reinterpret_cast<__nv_bfloat162*>(&o);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) hp[j] = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
-            const int chunk = h * 4 + q;
-            *reinterpret_cast<uint4*>(cst + g * 4096 + lane * 128 + ((chunk ^ (lane & 7)) << 4)) = o;
-          }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0 && n0 + g * 64 < p.N && mrow0 < p.M)
-          asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                       ::"l"(&tmC), "r"(smem_addr(cst + g * 4096)), "r"(n0 + g * 64), "r"(mrow0) : "memory");
-      }
-      if (lane == 0) {
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-      }
-      __syncwarp();
-    } else {
-    if (warp == 2 && lane == 0) stamp(p, 6);         // accumulator visible to the epilogue
-    const bool first = blockIdx.z == 0;
-#pragma unroll 1
-    for (int hb = 0; hb < BN; hb += HB) {
-#pragma unroll 1
-      for (int c = 0; c < HB / 32; ++c) {
-        uint32_t r[32];
-        if (nkb > 0) {
-          const uint32_t taddr = tmem_acc + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(hb + c * 32);
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-              "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-              : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-                "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-                "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-              : "r"(taddr));
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        if (p.b_kmajor) {
+          tma_load_2d(sb, &tmB, k0, n0, fb);                        // box {64 k, BN n}
         } else {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) r[j] = 0u;
+          for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * 8192, &tmB, n0 + j * 64, k0, fb);
         }
-        float* dst = stg + (size_t)lane * PITCH + c * 32;
-#pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          *reinterpret_cast<uint4*>(dst + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
       }
+      stamp(p, 3);                                   // every TMA load issued
+    }
+    return;
+  }
+
+  // ===================== consumers: warpgroup wg owns rows [64 wg, +64) of the tile =====================
+  const int wg = warp >> 2;
+  if (p.tma_store) {                                 // per-column constants -> shared memory
+    for (int c = threadIdx.x; c < BN; c += N_CONSUMER) {
+      const int n = n0 + c;
+      s_bias[c] = (p.bias && n < p.N) ? p.bias[n] : 0.f;
+      s_rc[c] = (p.rs && n < p.N) ? p.rc[n] : 0.f;
+    }
+  }
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  float cs = 0.f;
+  if (p.a_kmajor) {
+    if (p.b_kmajor) mainloop<BN, STAGES, 0, 0>(acc, cs, do_cs, nkb, base, sm, full_bar, empty_bar, wg, p);
+    else mainloop<BN, STAGES, 0, 1>(acc, cs, do_cs, nkb, base, sm, full_bar, empty_bar, wg, p);
+  } else {
+    if (p.b_kmajor) mainloop<BN, STAGES, 1, 0>(acc, cs, do_cs, nkb, base, sm, full_bar, empty_bar, wg, p);
+    else mainloop<BN, STAGES, 1, 1>(acc, cs, do_cs, nkb, base, sm, full_bar, empty_bar, wg, p);
+  }
+  if (threadIdx.x == 0) stamp(p, 5);                 // every wgmma complete
+  if (do_cs && m0 + wg * 64 + (threadIdx.x & 63) < p.M) atomicAdd(p.colsum + m0 + wg * 64 + (threadIdx.x & 63), cs);
+  named_bar(CONSUMER_BAR, N_CONSUMER);               // both warpgroups are done with the ring: it becomes the accumulator tile
+  float* accs = reinterpret_cast<float*>(sm);
+  {
+    const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      *reinterpret_cast<float2*>(accs + (size_t)r * PITCH + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(accs + (size_t)(r + 8) * PITCH + 8 * j + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+  }
+  named_bar(CONSUMER_BAR, N_CONSUMER);
+
+  // ===================== epilogue: smem tile (lane = row) -> global (lane = column) =====================
+  // warp -> 32 rows (quarter) and every other 64 / HB column group (colhalf).  Stores go out with lanes across the
+  // columns of a row: contiguous 256-512 B (bf16) / 512 B-1 KB (fp32) per store; bias / rank-1 / relu / accumulate /
+  // split-K atomics are applied on the way out with per-lane column constants.
+  const int quarter = warp & 3, colhalf = warp >> 2;
+  constexpr int HB = BN < 128 ? BN : 128;           // columns per pass
+  constexpr int LPR = HB / 8;                       // lanes per row on the way out (8 columns per lane)
+  constexpr int RPI = 32 / LPR;                     // rows per store iteration
+  const int mrow0 = m0 + quarter * 32;
+  auto ld32 = [&](int c0, uint32_t* r) {            // this lane's row, 32 consecutive accumulator columns
+    const float* src = accs + (size_t)(quarter * 32 + lane) * PITCH + c0;
+#pragma unroll
+    for (int j = 0; j < 32; j += 4) *reinterpret_cast<uint4*>(r + j) = *reinterpret_cast<const uint4*>(src + j);
+  };
+  if (p.tma_store) {
+    // ---- bf16 output through TMA: each warp converts its 32 rows, 64 columns at a time, into a [32 x 64] bf16 box in
+    // the SWIZZLE_128B layout (conflict-free 16-byte st.shared: lane = row, chunk slot = chunk ^ (row & 7)) and one
+    // elected lane hands the box to the TMA engine; rows / columns past M / N are clipped by the tensor map.
+    unsigned char* cst = sm + acc_region_bytes<BN, STAGES>() + (size_t)quarter * (BN / 64) * 4096;
+    const int m = mrow0 + lane;
+    const float rsm = (p.rs && m < p.M) ? p.rs[m] : 0.f;
+    if (warp == 0 && lane == 0) stamp(p, 6);
+    const __nv_bfloat16* mrow = nullptr;            // relu-backward mask: this lane's row of the forward activations
+    if (p.relu_mask && m < p.M) {
+      mrow = p.relu_mask + (long)m * p.ldc + n0;
+      for (int g = colhalf; g < BN / 64; g += 2)
+        if (n0 + g * 64 < p.N) asm volatile("prefetch.global.L2 [%0];" ::"l"(mrow + g * 64));
+    }
+#pragma unroll 1
+    for (int g = colhalf; g < BN / 64; g += 2) {
+      uint4 mk[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) mk[j] = make_uint4(0x3f803f80u, 0x3f803f80u, 0x3f803f80u, 0x3f803f80u);   // 1.0: keep
+      if (mrow != nullptr && n0 + g * 64 + 63 < p.N) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) mk[j] = *reinterpret_cast<const uint4*>(mrow + g * 64 + j * 8);
+      } else if (mrow != nullptr) {
+        __nv_bfloat16* me = reinterpret_cast<__nv_bfloat16*>(mk);
+        for (int j = 0; j < 64; ++j) if (n0 + g * 64 + j < p.N) me[j] = mrow[g * 64 + j];
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        uint32_t r[32];
+        const int c0 = g * 64 + h * 32;
+        ld32(c0, r);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          float v[8];
+          const float4 b0 = *reinterpret_cast<const float4*>(s_bias + c0 + q * 8), b1 = *reinterpret_cast<const float4*>(s_bias + c0 + q * 8 + 4);
+          const float4 k0 = *reinterpret_cast<const float4*>(s_rc + c0 + q * 8), k1 = *reinterpret_cast<const float4*>(s_rc + c0 + q * 8 + 4);
+          const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+          const float kk[8] = {k0.x, k0.y, k0.z, k0.w, k1.x, k1.y, k1.z, k1.w};
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            v[j] = fmaf(rsm, kk[j], __uint_as_float(r[q * 8 + j]) + bb[j]);
+            if (p.relu) v[j] = fmaxf(v[j], 0.f);
+          }
+          {
+            const __nv_bfloat162* mp = reinterpret_cast<const __nv_bfloat162*>(&mk[h * 4 + q]);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const float2 f = __bfloat1622float2(mp[j]);
+              if (!(f.x > 0.f)) v[2 * j] = 0.f;
+              if (!(f.y > 0.f)) v[2 * j + 1] = 0.f;
+            }
+          }
+          uint4 o;
+          __nv_bfloat162* hp = reinterpret_cast<__nv_bfloat162*>(&o);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) hp[j] = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
+          const int chunk = h * 4 + q;
+          *reinterpret_cast<uint4*>(cst + g * 4096 + lane * 128 + ((chunk ^ (lane & 7)) << 4)) = o;
+        }
+      }
+      fence_proxy_async();
       __syncwarp();
+      if (lane == 0 && n0 + g * 64 < p.N && mrow0 < p.M) tma_store_2d(&tmC, smem_addr(cst + g * 4096), n0 + g * 64, mrow0);
+    }
+    if (lane == 0) tma_store_commit_wait_read();
+    __syncwarp();
+  } else {
+    if (warp == 0 && lane == 0) stamp(p, 6);         // accumulator visible to the epilogue
+    const bool first = blockIdx.z == 0;
+#pragma unroll 1
+    for (int hb = colhalf * HB; hb < BN; hb += 2 * HB) {
+      const float* stg = accs + (size_t)(quarter * 32) * PITCH + hb;
       if (p.splits > 1) {
-        // split-K partials: lane <-> consecutive columns, so every RED.ADD of a warp covers one 128-B line
-        // 16-byte vector reductions (red.global.add.v4.f32, sm_90+): a lane owns 4 consecutive columns, so a row of the
-        // 128-column pass is ONE warp instruction instead of four -- the split-K weight-gradient products issue ~1 M
-        // fp32 reductions per launch
+        // split-K partials: 16-byte vector reductions (red.global.add.v4.f32, sm_90+): a lane owns 4 consecutive
+        // columns, so a row of the 128-column pass is ONE warp instruction instead of four
         const bool vec = (p.ldc & 3) == 0;
         for (int rr = 0; rr < 32; ++rr) {
           const int m = mrow0 + rr;
@@ -453,17 +379,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           }
         }
       }
-      __syncwarp();                                 // staging block free for the next column pass
     }
-    }   // smem-staged epilogue
   }
-  if (warp == 2 && lane == 0) stamp(p, 7);           // this warp's stores issued
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_acc), "r"(BN));
-  }
+  if (warp == 0 && lane == 0) stamp(p, 7);           // this warp's stores issued
   if (threadIdx.x == 0) stamp(p, 8);                 // exit
 }
 
@@ -478,37 +396,15 @@ bool rotate_on() {             // FIRA_GEMM_ROTATE=0: every CTA walks k in the s
   return on;
 }
 
-PFN_cuTensorMapEncodeTiled get_encode() {
-  static PFN_cuTensorMapEncodeTiled fn = [] {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess) f = nullptr;
-    return (PFN_cuTensorMapEncodeTiled)f;
-  }();
-  return fn;
-}
-
-// 2-D bf16 tensor map over a row-major [rows, cols] matrix (cols contiguous), box {box_cols, box_rows}, SW128
 int make_map(CUtensorMap* map, const void* ptr, long rows, long cols, long ld, int box_cols, int box_rows) {
-  PFN_cuTensorMapEncodeTiled enc = get_encode();
-  if (!enc) { fira_set_error(FIRA_ERR_CUDA, "gemm_tc: cuTensorMapEncodeTiled unavailable"); return FIRA_ERR_CUDA; }
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    fira_set_error(FIRA_ERR_CUDA, "gemm_tc: cuTensorMapEncodeTiled failed (%d) rows=%ld cols=%ld ld=%ld", (int)r, rows, cols, ld);
-    return FIRA_ERR_CUDA;
-  }
-  return FIRA_OK;
+  return make_map_bf16(map, ptr, rows, cols, ld, box_cols, box_rows, "gemm_tc");
 }
 
 template <int BN, int STAGES>
 int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const TcParams& p, cudaStream_t st) {
-  const size_t smem = (size_t)STAGES * (BM * BK * 2 + BN * BK * 2) + 1024;
+  // ring / accumulator tile, then the TMA-store staging boxes ([4 x 32 rows] x BN bf16), + 1 KB for the alignment
+  constexpr size_t smem = acc_region_bytes<BN, STAGES>() + (size_t)BN * 256 + 1024;
+  static_assert(smem + 2 * BN * 4 + 2 * STAGES * 8 <= 227 * 1024, "gemm_tc: shared-memory budget");
   // per launch, not cached in a static: the attribute is per device, and a static flag would be shared state
   cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) { fira_set_error(FIRA_ERR_CUDA, "gemm_tc attr: %s", cudaGetErrorString(e)); return FIRA_ERR_CUDA; }
@@ -517,16 +413,21 @@ int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& 
   return FIRA_OK;
 }
 
-// Two launch shapes per tile width (measured, profiles/ + DESIGN.md):
-//   more CTAs than SMs -> shallow ring (2 x 48 KB for the 128x256 tile), TWO CTAs per SM: one CTA's epilogue
-//                         overlaps the other's TMA/MMA phase (GCN 325-CTA GEMM 30 -> 24 us, KV 145 -> 98 us);
-//   at most one wave   -> 4-stage ring, one CTA per SM: all four k-blocks of a K = 256 product are in flight at
-//                         once, which is what the latency-bound 15-105 CTA launches of the decoder need.
+// Two launch shapes per tile width:
+//   more CTAs than SMs -> shallow ring, TWO CTAs per SM where the tile allows it (BN <= 128): one CTA's epilogue
+//                         overlaps the other's TMA / wgmma phase;
+//   at most one wave   -> 4-stage ring (3 for BN = 256: the fp32 accumulator tile and the staging boxes must fit too),
+//                         one CTA per SM: the k-blocks of a K = 256 product are in flight at once, which is what the
+//                         latency-bound 15-105 CTA launches of the decoder need.
 template <int BN>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc, const TcParams& p, cudaStream_t st) {
   const long ctas = (long)((p.N + BN - 1) / BN) * ((p.M + BM - 1) / BM) * p.splits;
-  if (ctas > 148) return launch_cfg<BN, (BN == 256 ? 2 : 3)>(ta, tb, tc, p, st);
-  return launch_cfg<BN, 4>(ta, tb, tc, p, st);
+  if constexpr (BN == 256) {
+    return launch_cfg<BN, 3>(ta, tb, tc, p, st);
+  } else {
+    if (ctas > fira_num_sms()) return launch_cfg<BN, (BN == 128 ? 2 : 3)>(ta, tb, tc, p, st);
+    return launch_cfg<BN, 4>(ta, tb, tc, p, st);
+  }
 }
 
 }  // namespace
@@ -552,13 +453,13 @@ int gemm_tc_impl(const void* A, long lda, int a_kmajor, const void* B, long ldb,
   cudaStream_t st = (cudaStream_t)stream;
   // Tile width: 256 columns per CTA amortise the A tile best, but a product with few row tiles (the decoder's
   // M = B*30 = 15 tiles) then runs on 15-60 SMs and each CTA carries a 128 x 256 epilogue.  Narrower tiles spread such
-  // products over more SMs: the smallest width whose grid still fits one wave (148 CTAs) wins.
+  // products over more SMs: the smallest width whose grid still fits one wave (one CTA per SM) wins.
   int BN = N > 128 ? 256 : (N > 64 ? 128 : 64);
   {
     const long mt = (M + BM - 1) / BM;
     const int sp = splits < 1 ? 1 : splits;
     for (int cand = 64; cand < BN; cand *= 2)
-      if (mt * ((N + cand - 1) / cand) * sp <= 148) { BN = cand; break; }
+      if (mt * ((N + cand - 1) / cand) * sp <= fira_num_sms()) { BN = cand; break; }
   }
   CUtensorMap ta, tb;
   int rc_;

@@ -252,11 +252,10 @@ __global__ void __launch_bounds__(256) csr_spmm_part_kernel(const int* __restric
   }
 }
 
-// Version 6 (opt-in, FIRA_SPMM_VARIANT=6; written after the last GPU minutes of round 1, NOT YET MEASURED): the v4
-// row mapping on a persistent one-wave grid with the metadata software-pipelined two rows ahead.  ncu on v4
-// (profiles/spmm_bf16_r1_ncu_details.txt): 4.39 waves of CTAs, each living exactly one dependent chain
-// rowptr -> (col,val) -> neighbour rows (three DRAM latencies), 54 % of stall cycles on that chain.  Here a row group
-// walks ~R / (148 * 4 * 16) rows; while the neighbour rows of row k are gathered, the first (col,val) chunk of row
+// Version 6 (opt-in, FIRA_SPMM_VARIANT=6, not measured): the v4 row mapping on a persistent one-wave grid with the
+// metadata software-pipelined two rows ahead.  In v4 every CTA lives exactly one dependent chain
+// rowptr -> (col,val) -> neighbour rows (three DRAM latencies).  Here a row group
+// walks ~R / (SMs * 4 * 16) rows; while the neighbour rows of row k are gathered, the first (col,val) chunk of row
 // k+1 and the rowptr pair of row k+2 are already in flight, so a row costs ~one latency instead of three.
 template <typename T, int LPR>
 __global__ void __launch_bounds__(256) csr_spmm_pipe_kernel(const int* __restrict__ rowptr, const int* __restrict__ col,
@@ -338,7 +337,7 @@ __global__ void __launch_bounds__(256) csr_spmm_pipe_kernel(const int* __restric
 }
 
 // Version 3: bulk-async (TMA engine, SASS UBLKCP) staging of the neighbour rows in shared memory.
-// Little's law on B200 asks for ~45 KB of reads in flight per SM; v1/v2 hold the gathered rows in
+// Little's law asks for tens of KB of reads in flight per SM; v1/v2 hold the gathered rows in
 // registers and spend most of a row's life on the two dependent metadata round trips, so they sit at
 // ~13 KB/SM.  Here a warp takes a group of GR consecutive destination rows, builds their edge list
 // once (one rowptr round trip, one col/val round trip), then every lane fires ONE
@@ -472,7 +471,7 @@ int fira_csr_count_dense(const void* edge, int edge_dtype, long stride_b, long s
   FIRA_CHECK_ARG(B > 0 && N > 0, FIRA_ERR_SHAPE, "csr_count_dense: B=%d N=%d", B, N);
   cudaStream_t st = (cudaStream_t)stream;
   const long rows = (long)B * N;
-  int grid = (int)((rows + 7) / 8 < 148 * 8 ? (rows + 7) / 8 : 148 * 8);
+  int grid = (int)((rows + 7) / 8 < fira_num_sms() * 8 ? (rows + 7) / 8 : fira_num_sms() * 8);
   if (edge_dtype == 0) launch_k(dense_count_kernel<float>, dim3(grid), dim3(256), 0, st, (const float*)edge, stride_b, stride_i, stride_j, B, N, counts);
   else if (edge_dtype == 2) launch_k(dense_count_kernel<double>, dim3(grid), dim3(256), 0, st, (const double*)edge, stride_b, stride_i, stride_j, B, N, counts);
   else if (edge_dtype == 1) launch_k(dense_count_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, st, (const __nv_bfloat16*)edge, stride_b, stride_i, stride_j, B, N, counts);
@@ -487,7 +486,7 @@ int fira_csr_fill_dense(const void* edge, int edge_dtype, long stride_b, long st
                         const int* rowptr, int* col, float* val, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const long rows = (long)B * N;
-  int grid = (int)((rows + 7) / 8 < 148 * 8 ? (rows + 7) / 8 : 148 * 8);
+  int grid = (int)((rows + 7) / 8 < fira_num_sms() * 8 ? (rows + 7) / 8 : fira_num_sms() * 8);
   if (edge_dtype == 0) launch_k(dense_fill_kernel<float>, dim3(grid), dim3(256), 0, st, (const float*)edge, stride_b, stride_i, stride_j, B, N, rowptr, col, val);
   else if (edge_dtype == 2) launch_k(dense_fill_kernel<double>, dim3(grid), dim3(256), 0, st, (const double*)edge, stride_b, stride_i, stride_j, B, N, rowptr, col, val);
   else if (edge_dtype == 1) launch_k(dense_fill_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, st, (const __nv_bfloat16*)edge, stride_b, stride_i, stride_j, B, N, rowptr, col, val);
@@ -517,22 +516,20 @@ int fira_gcn_aggregate(const int* rowptr, const int* col, const float* val, cons
   Segs s{B, n_code, n_sub, n_ast};
   const int N = n_code + n_sub + n_ast;
   const long R = (long)B * N;
-  // measured default (profiles/scatter_variants_r2.jsonl, graph-replayed launches, 64 / 512 commits): a QUARTER warp per
-  // destination row (variant 8: four independent rowptr -> (col,val) -> neighbour-row chains per warp, 32 features =
-  // 64-128 B per lane and neighbour row) -- 0.52 / 0.65 of the measured HBM peak in bf16 and 0.70 in fp32, against 0.46 /
-  // 0.58 / 0.62 for half a warp per row (variant 4) and 0.38 / 0.44 / 0.59 for a whole warp (variant 1).
-  // FIRA_SPMM_VARIANT overrides (A/B runs).
+  // default: a QUARTER warp per destination row (variant 8: four independent rowptr -> (col,val) -> neighbour-row chains
+  // per warp, 32 features = 64-128 B per lane and neighbour row), more independent chains in flight than half a warp
+  // (variant 4) or a whole warp (variant 1) per row.  FIRA_SPMM_VARIANT overrides (A/B runs).
   static const int forced = [] { const char* e = getenv("FIRA_SPMM_VARIANT"); return e ? atoi(e) : 0; }();
   const int variant = forced ? forced : 8;
   if (variant == 1) {                      // round-1 baseline kernel, kept for A/B profiling
     long ctas = (R + 7) / 8;
-    const long cap = 148L * 8 * 4;
+    const long cap = (long)fira_num_sms() * 8 * 4;
     int grid = (int)(ctas < cap ? ctas : cap);
     DISPATCH_T(dtype, launch_k(csr_spmm_kernel<T>, dim3(grid), dim3(256), 0, (cudaStream_t)stream, rowptr, col, val, (const T*)x,
                                                                                    (const T*)addend, (T*)y, s, N);)
   } else if (variant == 4) {
     long ctas = (R + 15) / 16;               // 8 warps x 2 rows
-    const long cap = 148L * 8 * 4;
+    const long cap = (long)fira_num_sms() * 8 * 4;
     int grid = (int)(ctas < cap ? ctas : cap);
     DISPATCH_T(dtype, launch_k(csr_spmm_part_kernel<T, 16>, dim3(grid), dim3(256), 0, (cudaStream_t)stream, 
         rowptr, col, val, (const T*)x, (const T*)addend, (T*)y, s, N);)
@@ -541,7 +538,7 @@ int fira_gcn_aggregate(const int* rowptr, const int* col, const float* val, cons
     // row (bf16); 10: a quarter warp per row, two neighbour rows in flight
     const int rows_per_cta = variant == 7 ? 16 : (variant == 9 ? 64 : 32);
     long ctas = (R + rows_per_cta - 1) / rows_per_cta;
-    const long cap = 148L * 8 * 4;
+    const long cap = (long)fira_num_sms() * 8 * 4;
     int grid = (int)(ctas < cap ? ctas : cap);
     if (variant == 7) {
       DISPATCH_T(dtype, launch_k(csr_spmm_part_kernel<T, 16, 2>, dim3(grid), dim3(256), 0, (cudaStream_t)stream,
@@ -559,7 +556,7 @@ int fira_gcn_aggregate(const int* rowptr, const int* col, const float* val, cons
   } else if (variant == 6) {                 // persistent one-wave grid, metadata pipelined two rows ahead (unmeasured)
     const int rows_per_cta = dtype == FIRA_BF16 ? 16 : 8;
     long ctas = (R + rows_per_cta - 1) / rows_per_cta;
-    const long cap = 148L * 4;               // 64 registers/thread -> 4 CTAs of 256 threads per SM
+    const long cap = (long)fira_num_sms() * 4;               // 64 registers/thread -> 4 CTAs of 256 threads per SM
     int grid = (int)(ctas < cap ? ctas : cap);
     if (dtype == FIRA_BF16) {
       launch_k(csr_spmm_pipe_kernel<__nv_bfloat16, 16>, dim3(grid), dim3(256), 0, (cudaStream_t)stream, 
@@ -580,7 +577,7 @@ int fira_gcn_aggregate(const int* rowptr, const int* col, const float* val, cons
       attr_done = true;
     }
     long ctas = (R + (long)GR * WARPS - 1) / ((long)GR * WARPS);
-    const long cap = 148L * 8;
+    const long cap = (long)fira_num_sms() * 8;
     int grid = (int)(ctas < cap ? ctas : cap);
     DISPATCH_T(dtype, launch_k(csr_spmm_bulk_kernel<T, WARPS>, dim3(grid), dim3(WARPS * 32), smem, (cudaStream_t)stream, 
         rowptr, col, val, (const T*)x, (const T*)addend, (T*)y, s, N);)

@@ -222,7 +222,7 @@ __global__ void __launch_bounds__(256) head_fwd_kernel(const T* __restrict__ log
   MaxSum v{-INFINITY, 0.f};
   if (need_vocab) {
     // 8 logits per 16-byte (bf16) / 32-byte (fp32) load; the running (max, sum) is rescaled once per group instead of
-    // once per element (one 2-byte load and two expf per element made this kernel 61 us for 95 MB)
+    // once per element (instead of one 2-byte load and two expf per element)
     const int V8 = V >> 3;
     for (int g = threadIdx.x; g < V8; g += blockDim.x) {
       float x[8];

@@ -2,7 +2,7 @@
 //   embeddings (+position table), dropout+residual+LayerNorm fwd/bwd, Combination gate fwd/bwd,
 //   column sums (bias gradients), encoder-memory pack/unpack.
 // All are HBM-bound: every lane moves 32 B (fp32) / 16 B (bf16) per row access, a warp moves one
-// whole contiguous row, grids are sized as multiples of the 148 SMs.
+// whole contiguous row, grids are sized as multiples of the SM count.
 #include "common.cuh"
 #include "fira_b200.h"
 
@@ -14,7 +14,7 @@ constexpr int CTA = ROWS_PER_CTA * kWarp;
 
 __host__ inline int row_grid(long rows) {
   long g = (rows + ROWS_PER_CTA - 1) / ROWS_PER_CTA;
-  const long cap = 148L * 16;   // grid-stride beyond 16 CTAs/SM
+  const long cap = (long)fira_num_sms() * 16;   // grid-stride beyond 16 CTAs/SM
   return (int)(g < cap ? (g > 0 ? g : 1) : cap);
 }
 
@@ -104,7 +104,7 @@ __global__ void embed_rows_bwd_kernel(const int* __restrict__ ids, const T* __re
     float v[8];
     Act<T>::load8(g + r * D + lane * 8, v);
     // rows whose gradient is exactly zero (padded target positions: no loss, masked as keys) add nothing; skipping
-    // them avoids ~1,000 rows of atomics serialising on the <pad> row of the table (measured 105 us -> a few us)
+    // them avoids ~1,000 rows of atomics serialising on the <pad> row of the table
     bool nz = false;
 #pragma unroll
     for (int i = 0; i < 8; ++i) nz |= v[i] != 0.f;
@@ -544,7 +544,7 @@ int fira_embed_nodes_pos_fwd(const int* sou, const int* pos, const int* sub_toke
 int fira_zero_pad_rows(void* x, long ld, int width, const int* off, int B, int Rc, int Rs, int dtype, void* stream) {
   FIRA_CHECK_ARG(x && off && B > 0 && width > 0 && width % 8 == 0 && ld >= width, FIRA_ERR_ARG, "zero_pad_rows: arguments");
   FIRA_CHECK_ARG(fira_aligned16(x) && (ld % 8) == 0, FIRA_ERR_ALIGN, "zero_pad_rows: 16-B alignment");
-  DISPATCH_T(dtype, launch_k(zero_pad_rows_kernel<T>, dim3(148), dim3(256), 0, (cudaStream_t)stream, (T*)x, ld, width, off, B, Rc, Rs);)
+  DISPATCH_T(dtype, launch_k(zero_pad_rows_kernel<T>, dim3(fira_num_sms()), dim3(256), 0, (cudaStream_t)stream, (T*)x, ld, width, off, B, Rc, Rs);)
   FIRA_CHECK_LAUNCH("fira_zero_pad_rows");
   return FIRA_OK;
 }
@@ -599,7 +599,7 @@ int fira_ln_residual_bwd(const void* d_outA, const void* d_outB, long split, con
   FIRA_CHECK_ARG(dim == D, FIRA_ERR_SHAPE, "ln_residual_bwd: dim %d != 256", dim);
   if (rows == 0) return FIRA_OK;
   long g = (rows + ROWS_PER_CTA - 1) / ROWS_PER_CTA;
-  int grid = (int)(g < 148L * 4 ? g : 148L * 4);   // few CTAs -> few d_gamma/d_beta atomics
+  int grid = (int)(g < (long)fira_num_sms() * 4 ? g : (long)fira_num_sms() * 4);   // few CTAs -> few d_gamma/d_beta atomics
   DISPATCH_T(dtype, launch_k(ln_bwd_kernel<T>, dim3(grid), dim3(CTA), 0, (cudaStream_t)stream, 
       (const T*)d_outA, (const T*)d_outB, split, (const T*)z, (const T*)resid, mean, rstd, gamma, (T*)d_z,
       (T*)d_resid, d_resid_accum, d_gamma, d_beta, rows, p_drop, seed, seed_ctr, stream_id);)
@@ -626,7 +626,7 @@ int fira_comb_gate_bwd(const void* qk, long ld_qk, const float* vtab, const int*
   if (rows == 0) return FIRA_OK;
   const float scale = 1.f / sqrtf((float)d_head);
   long g = (rows + ROWS_PER_CTA - 1) / ROWS_PER_CTA;
-  int grid = (int)(g < 148L * 4 ? g : 148L * 4);
+  int grid = (int)(g < (long)fira_num_sms() * 4 ? g : (long)fira_num_sms() * 4);
   DISPATCH_T(dtype, launch_k(comb_gate_bwd_kernel<T>, dim3(grid), dim3(CTA), 0, (cudaStream_t)stream, 
       (const T*)qk, ld_qk, vtab, mark, (const T*)d_out, (T*)d_qk, d_vtab, rows, scale, p_drop, seed, seed_ctr, stream_id);)
   FIRA_CHECK_LAUNCH("fira_comb_gate_bwd");
@@ -678,7 +678,7 @@ int fira_relu_bwd(const void* h, void* d, long n, int dtype, void* stream) {
   FIRA_CHECK_ARG(n % 8 == 0, FIRA_ERR_SHAPE, "relu_bwd: n %ld not a multiple of 8", n);
   if (n == 0) return FIRA_OK;
   long blocks = (n / 8 + 255) / 256;
-  if (blocks > 148L * 16) blocks = 148L * 16;
+  if (blocks > (long)fira_num_sms() * 16) blocks = (long)fira_num_sms() * 16;
   DISPATCH_T(dtype, launch_k(relu_bwd_kernel<T>, dim3((int)blocks), dim3(256), 0, (cudaStream_t)stream, (const T*)h, (T*)d, n / 8);)
   FIRA_CHECK_LAUNCH("fira_relu_bwd");
   return FIRA_OK;

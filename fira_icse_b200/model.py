@@ -1,4 +1,4 @@
-"""`Model.py` surface of the reference (CopyNet, TransModel) on the B200 CUDA path.
+"""`Model.py` surface of the reference (CopyNet, TransModel) on the CUDA path.
 
     model = TransModel(args)                  # args as run_model.py:27-56
     loss_sum, n_tok = model(sou, tar, attr, mark, ast_change, edge, tar_label, sub_token, 'train')
@@ -67,7 +67,7 @@ class TransModel(nn.Module):
         self.set_precision(os.environ.get("FIRA_PRECISION", "fp32"))
 
     def set_precision(self, precision):
-        """'fp32' (parity mode, default) or 'bf16' (throughput mode: bf16 activations, tcgen05 GEMMs)."""
+        """'fp32' (parity mode, default) or 'bf16' (throughput mode: bf16 activations, wgmma GEMMs)."""
         if precision not in ("fp32", "bf16"):
             raise ValueError("precision must be 'fp32' or 'bf16'")
         self.precision = precision

@@ -5,7 +5,7 @@ stream.  No torch compute op sits on the path (torch supplies memory, streams, a
 Precision modes (cfg["bf16"]):
   * fp32 parity mode  : fp32 activations, every Linear on fira_gemm_f32 (fp32 FFMA) -- logits within
                         1e-4 of the reference.
-  * bf16 throughput   : bf16 activations, every large Linear on fira_gemm_bf16_tc (tcgen05.mma, TMEM
+  * bf16 throughput   : bf16 activations, every large Linear on fira_gemm_bf16_tc (wgmma, register
                         fp32 accumulators, TMA operands); statistics, parameters, parameter gradients
                         and the handful of tiny products (4 x 256 value table, 256^3 weight merges,
                         2-wide gate) stay fp32.
@@ -65,14 +65,19 @@ def _gdest(ts, shape, zero=False):
     return (torch.zeros if zero else torch.empty)(shape, dtype=torch.float32, device=ts[0].device)
 
 
+def _num_sms():
+    """SMs of the current device, as the library sizes its own grids (fira_num_sms)"""
+    return _lib.lib().fira_num_sms()
+
+
 # ----------------------------------------------------------------------------- fp32 GEMM (parity mode)
 def _pick_splits(M, N, K, relu):
     if relu:
         return 1
-    if _ceil(M, 128) * _ceil(N, 128) >= 148:
+    if _ceil(M, 128) * _ceil(N, 128) >= _num_sms():
         return 1
     tiles = _ceil(M, 64) * _ceil(N, 64)
-    want = _ceil(296, tiles)
+    want = _ceil(2 * _num_sms(), tiles)
     return max(1, min(want, _ceil(K, 16) // 8))
 
 
@@ -113,10 +118,10 @@ def linear_dw(dy, ld_dy, x, ldx, M, N, K, dy_off=0, x_off=0, out=None):
     return dW
 
 
-# ----------------------------------------------------------------------------- bf16 tcgen05 GEMM
+# ----------------------------------------------------------------------------- bf16 wgmma GEMM
 def gemm_tc(A, lda, a_kmajor, Bm, ldb, b_kmajor, C, ldc, M, N, K, bias=None, rs=None, rc=None, relu=False,
             accumulate=False, splits=1, a_off=0, b_off=0, c_off=0):
-    """C[M,N] = A(MxK) B(KxN) (+bias, +rs*rc, relu) on tcgen05; A/B bf16, C fp32 or bf16 (by C.dtype)."""
+    """C[M,N] = A(MxK) B(KxN) (+bias, +rs*rc, relu) on wgmma; A/B bf16, C fp32 or bf16 (by C.dtype)."""
     call("fira_gemm_bf16_tc", _ptr(A, a_off), lda, int(a_kmajor), _ptr(Bm, b_off), ldb, int(b_kmajor), _ptr(C, c_off),
          ldc, int(C.dtype == torch.bfloat16), M, N, K, _ptr(bias), _ptr(rs), _ptr(rc), int(relu), int(accumulate),
          splits, _stream())
@@ -124,16 +129,21 @@ def gemm_tc(A, lda, a_kmajor, Bm, ldb, b_kmajor, C, ldc, M, N, K, bias=None, rs=
 
 
 # CTAs a split-K weight-gradient product may spread over.  These products run on the side streams NEXT TO the main
-# chain: filling all 148 SMs shortens the product itself but takes the SMs (and, through the fp32 atomics of split-K,
+# chain: filling all 132 SMs shortens the product itself but takes the SMs (and, through the fp32 atomics of split-K,
 # the L2 atomic throughput) away from the critical path.
-WGRAD_CTAS = max(1, int(os.environ.get("FIRA_WGRAD_CTAS", "148")))
+_WGRAD_CTAS_ENV = os.environ.get("FIRA_WGRAD_CTAS")
+
+
+def _wgrad_ctas():
+    return max(1, int(_WGRAD_CTAS_ENV)) if _WGRAD_CTAS_ENV else _num_sms()
 
 
 def _tc_splits(tiles, kblocks):
-    """split-K factor of a small-output GEMM: at least 8 k-blocks per split, at most WGRAD_CTAS CTAs in all"""
-    if tiles >= WGRAD_CTAS:
+    """split-K factor of a small-output GEMM: at least 8 k-blocks per split, at most _wgrad_ctas() CTAs in all"""
+    wgrad_ctas = _wgrad_ctas()
+    if tiles >= wgrad_ctas:
         return 1
-    return max(1, min(kblocks // 8 if kblocks >= 16 else 1, _ceil(WGRAD_CTAS, tiles)))
+    return max(1, min(kblocks // 8 if kblocks >= 16 else 1, _ceil(wgrad_ctas, tiles)))
 
 
 def colsum(x, ld, M, N, weight=None, x_off=0, dtype=None, out=None):
@@ -276,11 +286,10 @@ _SIDE_STREAMS = {}
 # groups rotate over several streams = parallel branches of the captured graph
 N_SIDE = max(1, int(os.environ.get("FIRA_SIDE_STREAMS", "8")))
 # the 256^3 fp32 products of the GCN weight merge (W2 W1 and its two adjoints) are 16 CTAs of the 64 x 64 tile: split-K
-# spreads them over 64 CTAs (15.9 us per product in the step timeline); bf16 mode only -- the fp32 parity mode keeps the
-# deterministic single-pass sum
+# spreads them over 64 CTAs; bf16 mode only -- the fp32 parity mode keeps the deterministic single-pass sum
 # fira_gemm_ln_fwd (Linear + dropout + residual + LayerNorm in one launch) is OPT-IN: a 128-row tile owns whole rows, so a
-# decoder product runs on 15 CTAs that each pull 256 KB and make two passes over the accumulator -- measured 0.09 ms per
-# step SLOWER than the 60-CTA product followed by the LayerNorm kernel (profiles/bench_r2_ab_run_l.jsonl)
+# decoder product runs on 15 CTAs that each pull 256 KB instead of the 60 CTAs of the product followed by the LayerNorm
+# kernel
 FUSE_GEMM_LN = os.environ.get("FIRA_GEMM_LN", "0") != "0"
 FUSE_DX_RELU = os.environ.get("FIRA_DX_RELU", "1") != "0" and os.environ.get("FIRA_GEMM_TMA_STORE", "1") != "0"
 MERGE_SPLITS = max(1, int(os.environ.get("FIRA_MERGE_SPLITS", "4")))
@@ -452,9 +461,9 @@ class EncoderFn(torch.autograd.Function):
         else:
             call("fira_embed_nodes_fwd", _ptr(sou), _ptr(sub_token), _ptr(ast_change), _ptr(emb), _ptr(ast_emb),
                  _ptr(pos_table), _ptr(Xc), _ptr(Gin), B, n_code, n_sub, n_ast, D, pr.code, st)
-        # GCN layer: scatter (fira_gcn_aggregate) -> tcgen05 GEMM -> LayerNorm.  FIRA_GCN_FUSED=1 (bf16 mode) runs the whole
-        # layer as ONE kernel instead (gather -> tcgen05 -> LayerNorm epilogue, csrc/gcn_fused.cu): validated, but measured
-        # 33 us against 22 us for the three launches on the packed rows of a 64-commit batch, so it is opt-in
+        # GCN layer: scatter (fira_gcn_aggregate) -> wgmma GEMM -> LayerNorm.  FIRA_GCN_FUSED=1 (bf16 mode) runs the whole
+        # layer as ONE kernel instead (gather -> wgmma -> LayerNorm epilogue, csrc/gcn_fused.cu): validated by the tests,
+        # opt-in (its speed against the three launches has not been measured on the H100)
         fused = pr.bf16 and os.environ.get("FIRA_GCN_FUSED", "0") != "0"
         rs = None if fused else edges.rowsum(n_code, n_sub, n_ast)
         erows = edges.rows_csr(n_code, n_sub, n_ast) if fused else None
@@ -555,8 +564,8 @@ class EncoderFn(torch.autograd.Function):
                 ev_dwc = torch.cuda.Event()
                 ev_dwc.record()
                 fork.keep.extend((dWc, d_c1))
-            # the three fp32 adjoints of the weight merge are independent of each other: two more side streams (the
-            # last layer's chain dWc -> d_W2 -> d_W1 -> d_b1 used to end 60 us after the main stream)
+            # the three fp32 adjoints of the weight merge are independent of each other: two more side streams, so the
+            # last layer's chain dWc -> d_W2 -> d_W1 -> d_b1 does not trail the main stream
             with fork():
                 torch.cuda.current_stream().wait_event(ev_dwc)
                 d_W2 = _gdest(W2, (D, D))               # dWc W1^T + d_c1 b1^T

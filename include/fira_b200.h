@@ -1,4 +1,4 @@
-/* libfira_b200 -- C ABI of the B200-native FIRA hot path.
+/* libfira_b200 -- C ABI of the H100-native (sm_90a) FIRA hot path.
  *
  * The reference (DJjjjhao/FIRA-ICSE) has no FFI of its own: its hot path is PyTorch library
  * calls issued from Model.py / gnn_transformer.py / combination_layer.py.  The drop-in boundary
@@ -38,12 +38,12 @@ extern "C" {
 
 int fira_version(void);                    /* ABI version, bumped on any signature change */
 const char* fira_last_error_string(void);
-int fira_built_arch(void);                 /* 100 when compiled for sm_100a */
+int fira_built_arch(void);                 /* 90 when compiled for sm_90a */
+int fira_num_sms(void);                    /* SMs of the current device; every launch shape is sized from it */
 /* Launch mode of every kernel of the library (the one process-wide switch, atomic): on = programmatic dependent
  * launch -- a kernel's CTAs are scheduled while the previous kernel of the stream drains and block in
  * griddepcontrol.wait before their first global-memory access (results are identical).
- * Default: on (FIRA_PDL=0 in the environment turns it off).  Measured on the captured training step (profiles/):
- * 3.23 -> 3.05 ms once the side work runs on several streams; with ONE side stream it was 3% slower. */
+ * Default: on (FIRA_PDL=0 in the environment turns it off). */
 int fira_set_pdl(int on);
 int fira_get_pdl(void);
 
@@ -57,7 +57,7 @@ int fira_gemm_f32(const float* A, long lda, int a_kcontig, const float* B, long 
                   long ldc, int M, int N, int K, const float* bias, const float* rs, const float* rc, int relu,
                   int accumulate, int splits, void* stream);
 
-/* ---- bf16 tensor-core Linear (throughput mode): tcgen05.mma with TMEM accumulators, TMA-staged
+/* ---- bf16 tensor-core Linear (throughput mode): wgmma with register accumulators, TMA-staged
  *      operands.  Same contraction as fira_gemm_f32 on bf16 operands (fp32 accumulate):
  *      A(m,k) = a_kmajor ? A[m*lda+k] : A[k*lda+m];  B(k,n) = b_kmajor ? B[n*ldb+k] : B[k*ldb+n];
  *      lda/ldb multiples of 8; C fp32 or bf16 (c_is_bf16); accumulate: C += result;
@@ -181,7 +181,7 @@ int fira_gcn_aggregate(const int* rowptr, const int* col, const float* val, cons
                        void* y, int B, int n_code, int n_sub, int n_ast, int dim, int dtype, void* stream);
 
 /* ---- fused GCN layer, bf16 throughput mode (gnn_transformer.py:74-86 as ONE kernel per direction): gather the
- *      neighbour rows into the shared-memory A tile -> tcgen05.mma with the merged weight -> epilogue out of TMEM.
+ *      neighbour rows into the shared-memory A tile -> wgmma with the merged weight -> epilogue on the register accumulators.
  *      The CSR is in BUFFER order: rowptr_rows[r] indexes the rows of the node buffer, col_rows are buffer rows
  *      (fira_csr_to_rows converts the (graph, node)-ordered CSR; counts is an int32[rows] workspace).
  *   fwd:  z = (A h) w_merged^T + rowsum(A) (x) c1 + bias ;  out = LN(dropout(z) + h)   (w_merged = fc2.W fc1.W [out,in]
@@ -213,7 +213,7 @@ int fira_attn_bwd(const void* q, long ldq, const void* k, long ldk, const void* 
  * k / v, ranges[b] = {first row, rows, first row, rows} (code rows, sub-token rows; GLOBAL row ids, kv_rows = rows of
  * k / v), key_mask [B, mask_pitch] over the commit's own key positions (NULL: all valid), mask_pitch >= rows of any
  * commit; max_chunks = an upper bound the caller guarantees on ceil(rows0 / 128) + ceil(rows1 / 128) of any commit
- * (fira_host_packed_dims reports it; <= 3 lets bf16 run on the tcgen05 kernels).  Rows of dk / dv outside every range
+ * (fira_host_packed_dims reports it; <= 3 lets bf16 run on the wgmma kernels).  Rows of dk / dv outside every range
  * are not written (fira_zero_pad_rows clears the segment padding). */
 int fira_attn_packed_fwd(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv, const int* ranges,
                          long kv_rows, const unsigned char* key_mask, int mask_pitch, int max_chunks, void* ctx, long ldo,

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""`python run_model.py train|test` -- the reference's CLI (run_model.py:417-425) on the B200 path.
+"""`python run_model.py train|test` -- the reference's CLI (run_model.py:417-425) on the CUDA path.
 
 Same CWD-relative files (DataSet/*.json, all_index, VOCAB_UPPER_CASE, best_model.pt,
 OUTPUT/{output_fira,train_process,dev_output}), same hyper-parameters (run_model.py:27-46), same

@@ -1,4 +1,4 @@
-"""Whole-path parity on the B200: the CUDA TransModel against (a) the committed outputs of the
+"""Whole-path parity on the GPU: the CUDA TransModel against (a) the committed outputs of the
 unmodified reference (tests/golden/model_first128.npz) and (b) the CPU oracle, on real DataSet
 commits; fp32 parity mode, tolerance 1e-4 relative (BASELINE.json north_star)."""
 import numpy as np
@@ -170,7 +170,7 @@ def test_empty_and_ragged_inputs(model):
     assert int(n_tok) == 0 and loss_sum.item() == 0.0
 
 
-# ------------------------------------------------------------------ bf16 throughput mode (tcgen05 GEMMs)
+# ------------------------------------------------------------------ bf16 throughput mode (wgmma GEMMs)
 BF16_LOGP_EPS = 5e-2     # bound on |log p_bf16 - log p_fp32| through 12 post-LN layers of bf16 activations
 
 

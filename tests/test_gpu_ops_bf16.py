@@ -4,7 +4,7 @@ evaluated on those rounded inputs.  The kernels accumulate in fp32 and round the
 the bound is one bf16 rounding of the result (2^-8 relative, element-wise) plus the fp32 round-off of the
 reduction; where an op consumes a bf16-rounded intermediate of its own forward (attention / LayerNorm
 backward) the bound is stated relative to the largest reference element.  The fp32 instantiations are
-checked in tests/test_gpu_ops.py; the tcgen05 GEMM in tests/test_gpu_tc.py."""
+checked in tests/test_gpu_ops.py; the wgmma GEMM in tests/test_gpu_tc.py."""
 import math
 
 import pytest

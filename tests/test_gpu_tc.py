@@ -1,4 +1,4 @@
-"""tcgen05 / TMEM / TMA GEMM (fira_gemm_bf16_tc) against torch on the same bf16-rounded operands.
+"""wgmma / TMA GEMM (fira_gemm_bf16_tc) against torch on the same bf16-rounded operands.
 bf16 x bf16 products are exact in fp32, so only the fp32 summation order differs: tolerance 1e-4."""
 import pytest
 import torch

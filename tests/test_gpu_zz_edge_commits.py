@@ -1,4 +1,4 @@
-"""Whole-path parity on the B200 for the edge-case fixture (tests/golden/make_golden_edge.py): the DataSet's extreme
+"""Whole-path parity on the GPU for the edge-case fixture (tests/golden/make_golden_edge.py): the DataSet's extreme
 commits and crafted commits that reach the truncation branches, against the outputs of the unmodified reference
 (tests/golden/model_edge.npz); fp32 parity mode, 1e-4 relative."""
 import numpy as np

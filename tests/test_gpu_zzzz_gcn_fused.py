@@ -1,6 +1,6 @@
-"""The fused GCN layer kernels (csrc/gcn_fused.cu: gather -> tcgen05.mma -> LayerNorm epilogue in ONE launch per
+"""The fused GCN layer kernels (csrc/gcn_fused.cu: gather -> wgmma -> LayerNorm epilogue in ONE launch per
 direction) against a float64 restatement of gnn_transformer.py:74-86 on the bf16-rounded operands, and against the
-three-launch CUDA sequence they replace.  Runs last (file name): a protocol bug in a tcgen05 kernel traps the context."""
+three-launch CUDA sequence they replace.  Runs last (file name): a protocol bug in an mbarrier pipeline traps the context."""
 import os
 
 import numpy as np
@@ -85,7 +85,7 @@ def st():
 CASES = [
     dict(B=3, n=(96, 40, 56), seed=1, extra=2.0),            # a few CTAs, one tile each, 192 rows / graph
     dict(B=4, n=(210, 160, 280), seed=2, extra=1.2),         # the reference's 650-node layout
-    dict(B=48, n=(200, 104, 136), seed=3, extra=1.5),        # 21,120 rows: two tiles per CTA on 148 SMs (TMEM double buffer)
+    dict(B=48, n=(200, 104, 136), seed=3, extra=1.5),        # 21,120 rows: two tiles per CTA on 132 SMs (gather of one tile overlaps the epilogue of the other)
     dict(B=2, n=(64, 32, 32), seed=4, extra=40.0),           # dense tiles: > 1024 edges per tile (metadata read from global)
 ]
 
@@ -131,7 +131,7 @@ def test_gcn_layer_fwd(case):
     mean, var = y.mean(1), y.var(1, unbiased=False)
     check(stats[0], mean, 1e-4, 1e-4, "mean")
     check(stats[1], (var + 1e-5).rsqrt(), 1e-3, 1e-4, "rstd")
-    # against the three-launch CUDA sequence (scatter -> tcgen05 GEMM -> LayerNorm kernel)
+    # against the three-launch CUDA sequence (scatter -> wgmma GEMM -> LayerNorm kernel)
     pr = ops.Prec(True)
     G3 = torch.empty(R, 256, device=DEV, dtype=BF)
     _lib.call("fira_gcn_aggregate", pe.rowptr.data_ptr(), pe.col.data_ptr(), pe.val.data_ptr(), H.data_ptr(), None,

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """A/B timings of single kernels with CUDA events (warm L2 like inside a training step, 20 launches after 5 warm-ups),
-at the shapes the bf16 bench step launches: attention forward/backward (FFMA vs tcgen05, FIRA_ATTN_TC) and the GCN layer
+at the shapes the bf16 bench step launches: attention forward/backward (FFMA vs wgmma, FIRA_ATTN_TC) and the GCN layer
 (scatter + GEMM + LayerNorm vs the fused kernel, forward and backward).  One JSON line per measurement.
 
     python tools/bench_kernels.py [--batch 64]
@@ -78,8 +78,8 @@ def attention(B, out):
         for tc in ("0", "1"):
             os.environ["FIRA_ATTN_TC"] = tc
             fwd()
-            out({"kernel": "attention fwd", "case": name, "tcgen05": tc == "1", **timeit(fwd)})
-            out({"kernel": "attention bwd", "case": name, "tcgen05": tc == "1", **timeit(bwd)})
+            out({"kernel": "attention fwd", "case": name, "wgmma": tc == "1", **timeit(fwd)})
+            out({"kernel": "attention bwd", "case": name, "wgmma": tc == "1", **timeit(bwd)})
     os.environ.pop("FIRA_ATTN_TC", None)
 
 
@@ -130,7 +130,7 @@ def gcn(B, out):
         _lib.call("fira_gcn_layer_bwd", er[0].data_ptr(), er[1].data_ptr(), er[2].data_ptr(), dZ.data_ptr(),
                   WcT16.data_ptr(), dRes.data_ptr(), AdZ.data_ptr(), dH.data_ptr(), R, 256, st())
     info = {"rows": R, "segments": n, "nnz": pe.nnz}
-    out({"kernel": "GCN layer fwd: scatter + tcgen05 GEMM + LayerNorm (3 launches)", **info, **timeit(unfused_fwd)})
+    out({"kernel": "GCN layer fwd: scatter + wgmma GEMM + LayerNorm (3 launches)", **info, **timeit(unfused_fwd)})
     out({"kernel": "GCN layer fwd: fused (1 launch)", **info, **timeit(fused_fwd)})
     out({"kernel": "GCN layer bwd (dX path): GEMM + scatter (2 launches)", **info, **timeit(unfused_bwd)})
     out({"kernel": "GCN layer bwd (dX path): fused (1 launch)", **info, **timeit(fused_bwd)})

@@ -48,7 +48,7 @@ def run(name, coo, N, segs, dtype_code=0):
     copy_avg = sum(copy_ms) / len(copy_ms)
     alg = 2 * R * 256 * esz + (R + 1) * 4 + pe.nnz * 8
     peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(
-        os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+        os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0     # H100 SXM data-sheet HBM3 bandwidth
     print(json.dumps({"workload": name, "variant": os.environ.get("FIRA_SPMM_VARIANT", "2"),
                       "dtype": "f32" if dtype_code == 0 else "bf16", "rows": R, "nnz": pe.nnz,
                       "avg_us": round(avg * 1e3, 2), "min_us": round(ms[0] * 1e3, 2),

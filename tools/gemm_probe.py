@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Where does a small tcgen05 GEMM launch spend its time?  fira_debug_set_probe makes CTA (0,0,0) of fira_gemm_bf16_tc
+"""Where does a small wgmma GEMM launch spend its time?  fira_debug_set_probe makes CTA (0,0,0) of fira_gemm_bf16_tc
 stamp %globaltimer at its phase boundaries; this tool replays a CUDA graph of 8 dependent launches (each reads the previous
 output, like the decoder's chain) and prints the phase deltas of the LAST one, plus the per-launch time of the chain.
 

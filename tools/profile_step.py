@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Per-kernel GPU time of one eager training step via torch.profiler (CUPTI) -- the cheap iteration tool;
-the ncu launch lists under profiles/ are the evidence.  usage: python tools/profile_step.py [bf16|fp32] [B]"""
+"""Per-kernel GPU time of one eager training step via torch.profiler (CUPTI) -- the cheap iteration tool.
+usage: python tools/profile_step.py [bf16|fp32] [B]"""
 import collections
 import os
 import sys

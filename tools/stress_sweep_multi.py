@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""BASELINE.json config 5 on N GPUs: "synthetic stress: 2048-node graphs, 16k edges/relation, batch 256, 8xB200
+"""BASELINE.json config 5 on N GPUs: "synthetic stress: 2048-node graphs, 16k edges/relation, batch 256, 8xH100
 roofline sweep".  Graphs shard by rank (no data-path collective: message passing never crosses a graph); every rank
 times the GNN scatter (fira_gcn_aggregate, fp32 and bf16) and the fused GCN layer (fira_gcn_layer_fwd, bf16) on ITS
 shard for per-GPU batches 32 ... 256, cold L2 (rotating buffers), CUDA events; the time of a configuration is the MAX
@@ -30,7 +30,7 @@ def main():
     from fira_icse_b200 import _lib
     from fira_icse_b200.graph import PackedEdges
     from fira_icse_b200.synth import synth_stress_graphs
-    peak = 6650.0
+    peak = 3350.0                        # H100 SXM data-sheet HBM3 bandwidth unless MEASURED_PEAKS.json says otherwise
     pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pk):
         peak = float(json.load(open(pk))["hbm_gbs"])
@@ -92,7 +92,7 @@ def main():
                 alg = 3 * R * 256 * 2 + (R + 1) * 4 + pe.nnz * 8 + 256 * 256 * 2
                 if rank == 0:
                     print(json.dumps({"config": "stress N=2048, 4 x 16,384 edges/relation",
-                                      "kernel": "fira_gcn_layer_fwd (gather -> tcgen05 -> LayerNorm, one launch)",
+                                      "kernel": "fira_gcn_layer_fwd (gather -> wgmma -> LayerNorm, one launch)",
                                       "dtype": "bf16", "n_gpus": world, "per_gpu_batch": B, "rows_per_gpu": R,
                                       "ms_max_over_ranks": round(ms, 4),
                                       "graph_layers_per_s_all_gpus": round(world * B / (ms * 1e-3), 1),
