@@ -362,6 +362,200 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(const T* __restrict__ log
   }
 }
 
+// ------------------------------------------------------------------ seeded sampling from the mixture
+// One CTA per row (commit b, sample n).  Candidates are the j of [vocab || copy positions] with mem_mask set and
+// P_j > 0 in fp32; s_j = log P_j / T.  The rank order (s descending, then index ascending) is a strict total order,
+// encoded as a 47-bit key (32 order-preserving bits of s, 15 bits of 0x7fff - j), so every cut is "key >= threshold":
+//   top-k: the largest threshold that still keeps k candidates; top-p: the largest threshold whose kept weight
+//   sum(exp(s - s_max)) reaches p times the weight left after top-k.  Both are bisections over the key with
+//   fixed-order block reductions (integer counts / fp32 sums), so a row's draw is a pure function of its inputs.
+// Draw: u * Z against the kept weights in index order.  The scores are staged once in dynamic shared memory.
+constexpr int kSampleThreads = 256;                   // = head_fwd_kernel's block: the same row statistics, bit for bit
+constexpr uint32_t kSampleStream = 0x53414D50u;       // Philox stream id of the draw; dropout sites use ids < 256
+constexpr uint64_t kKeyEnd = 1ull << 47;
+
+__device__ __forceinline__ bool is_cand(float s) { return s == s; }          // NaN marks a non-candidate
+__device__ __forceinline__ uint64_t rank_key(float s, int j) {
+  uint32_t b = __float_as_uint(s);
+  b = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+  return ((uint64_t)b << 15) | (uint32_t)(0x7FFF - j);
+}
+
+// fixed-order reduction: xor butterfly inside each warp, then the 8 warp results in warp order (every thread gets it)
+template <typename V, typename Op>
+__device__ __forceinline__ V block_reduce(V v, V* sh, Op op) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = op(v, __shfl_xor_sync(0xffffffffu, v, o));
+  __syncthreads();                                    // `sh` may still be read by the previous reduction
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  V r = sh[0];
+#pragma unroll
+  for (int w = 1; w < kSampleThreads / 32; ++w) r = op(r, sh[w]);
+  return r;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kSampleThreads) pointer_mix_sample_kernel(
+    const T* __restrict__ logits, long ldl, const float* __restrict__ sc, const float* __restrict__ gate_logit,
+    const unsigned char* __restrict__ mem_mask, const int* __restrict__ copy_src, const uint64_t* __restrict__ seed_p,
+    const int* __restrict__ first_index_p, const float* __restrict__ uniforms, float temp, int top_k, float top_p,
+    int eos_id, int pad_id, int* __restrict__ next_tok, int* __restrict__ seq, int* __restrict__ raw,
+    float* __restrict__ tok_lp, unsigned char* __restrict__ tok_mask, long ld_out, int pos,
+    unsigned char* __restrict__ finished, int* __restrict__ length, float* __restrict__ lp_sum, int N, int V, int S) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  extern __shared__ float s_sc[];                     // [V + S] tempered scores, NaN = not a candidate
+  __shared__ MaxSum sh_ms[8];
+  __shared__ float bc[4];
+  __shared__ float shf[8];
+  __shared__ unsigned shu[8];
+  __shared__ int shi[8];
+  __shared__ float part[kSampleThreads];
+  __shared__ float sh_target;
+  __shared__ int sh_pick;
+  const long row = blockIdx.x;
+  const int b = (int)(row / N), n = (int)(row % N);
+  const long o = row * ld_out + pos + 1;
+  if (finished[row]) {                                // after <eos>: pad, no log-probability, length kept
+    if (threadIdx.x == 0) { next_tok[row] = pad_id; seq[o] = pad_id; raw[o] = pad_id; tok_lp[o] = 0.f; tok_mask[o] = 0; }
+    return;
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const T* lrow = logits + row * ldl;
+  const float* srow = sc + row * S;
+  const unsigned char* mrow = mem_mask + (long)b * S;
+
+  // row statistics exactly as head_fwd_kernel forms them (same loop, same reduction order), so the emitted
+  // log-probability is the one fira_pointer_mix_nll_fwd gives the same label
+  MaxSum v{-INFINITY, 0.f};
+  const int V8 = V >> 3;
+  for (int g = threadIdx.x; g < V8; g += blockDim.x) {
+    float x[8];
+    Act<T>::load8(lrow + (long)g * 8, x);
+    float m8 = x[0];
+#pragma unroll
+    for (int i = 1; i < 8; ++i) m8 = fmaxf(m8, x[i]);
+    if (m8 > v.m) { v.s *= expf(v.m - m8); v.m = m8; }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) v.s += expf(x[i] - v.m);
+  }
+  for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) { MaxSum u{Act<T>::ld(lrow + j), 1.f}; v = ms_merge(v, u); }
+  v = ms_warp(v);
+  if (lane == 0) sh_ms[warp] = v;
+  __syncthreads();
+  if (warp == 0) { MaxSum u = lane < 8 ? sh_ms[lane] : MaxSum{-INFINITY, 0.f}; u = ms_warp(u); if (lane == 0) { bc[0] = u.m; bc[1] = u.s; } }
+  __syncthreads();
+  MaxSum c{-INFINITY, 0.f};
+  for (int j = threadIdx.x; j < S; j += blockDim.x) { MaxSum u{mrow[j] ? srow[j] : kMaskFill, 1.f}; c = ms_merge(c, u); }
+  c = ms_warp(c);
+  if (lane == 0) sh_ms[warp] = c;
+  __syncthreads();
+  if (warp == 0) { MaxSum u = lane < 8 ? sh_ms[lane] : MaxSum{-INFINITY, 0.f}; u = ms_warp(u); if (lane == 0) { bc[2] = u.m; bc[3] = u.s; } }
+  __syncthreads();
+  const float vmax = bc[0], vsum = bc[1], cmax = bc[2], csum = bc[3];
+  const float gl0 = gate_logit[row * 2], gl1 = gate_logit[row * 2 + 1];
+  const float gm = fmaxf(gl0, gl1);
+  const float e0 = expf(gl0 - gm), e1 = expf(gl1 - gm);
+  const float g0 = e0 / (e0 + e1), g1 = e1 / (e0 + e1);
+  // P_j as head_fwd_kernel forms the probability of label j
+  auto prob = [&](int j) {
+    if (j < V) return g0 * (expf(Act<T>::ld(lrow + j) - vmax) / vsum);
+    const int s = j - V;
+    return g1 * (expf((mrow[s] ? srow[s] : kMaskFill) - cmax) / csum);
+  };
+
+  const int C = V + S;
+  for (int j = threadIdx.x; j < C; j += blockDim.x) {
+    const float p = prob(j);
+    s_sc[j] = ((j < V || mrow[j - V]) && p > 0.f) ? logf(fminf(p, 1.f)) / temp : __int_as_float(0x7fffffff);
+  }
+  __syncthreads();
+
+  // every pass below walks a contiguous index range per thread (index order is what the draw needs)
+  const int chunk = (C + kSampleThreads - 1) / kSampleThreads;
+  const int j0 = min(C, (int)threadIdx.x * chunk), j1 = min(C, j0 + chunk);
+  auto add_u = [](unsigned a, unsigned x) { return a + x; };
+  auto add_f = [](float a, float x) { return a + x; };
+  float smax = -INFINITY;
+  unsigned cnt = 0;
+  for (int j = j0; j < j1; ++j) { const float s = s_sc[j]; if (is_cand(s)) { smax = fmaxf(smax, s); ++cnt; } }
+  smax = block_reduce(smax, shf, [](float a, float x) { return fmaxf(a, x); });
+  const unsigned n_cand = block_reduce(cnt, shu, add_u);
+  auto weight = [&](float s) { return s == smax ? 1.f : expf(s - smax); };
+  auto count_ge = [&](uint64_t th) {
+    unsigned k = 0;
+    for (int j = j0; j < j1; ++j) { const float s = s_sc[j]; k += (is_cand(s) && rank_key(s, j) >= th) ? 1u : 0u; }
+    return block_reduce(k, shu, add_u);
+  };
+  auto weight_ge = [&](uint64_t th) {
+    float a = 0.f;
+    for (int j = j0; j < j1; ++j) { const float s = s_sc[j]; if (is_cand(s) && rank_key(s, j) >= th) a += weight(s); }
+    return block_reduce(a, shf, add_f);
+  };
+  uint64_t cut = 1;                                   // kept <=> candidate with rank_key >= cut
+  if (top_k > 0 && (unsigned)top_k < n_cand) {
+    uint64_t lo = cut, hi = kKeyEnd;                  // count_ge(lo) >= k, count_ge(hi) < k
+    while (hi - lo > 1) { const uint64_t mid = lo + (hi - lo) / 2; if (count_ge(mid) >= (unsigned)top_k) lo = mid; else hi = mid; }
+    cut = lo;
+  }
+  if (top_p < 1.f && n_cand > 1) {
+    const float target = top_p * weight_ge(cut);
+    uint64_t lo = cut, hi = kKeyEnd;                  // the top candidate alone has weight 1 > 0: lo stays at or below it
+    while (hi - lo > 1) { const uint64_t mid = lo + (hi - lo) / 2; if (weight_ge(mid) >= target) lo = mid; else hi = mid; }
+    cut = lo;
+  }
+
+  // draw: prefix sums of the kept weights in index order (one fixed-order scan of the per-thread sums)
+  float a = 0.f;
+  int last = -1;
+  for (int j = j0; j < j1; ++j) {
+    const float s = s_sc[j];
+    if (is_cand(s) && rank_key(s, j) >= cut) { const float w = weight(s); a += w; if (w > 0.f) last = j; }
+  }
+  last = block_reduce(last, shi, [](int x, int y) { return max(x, y); });   // fallback when u * Z rounds to Z
+  part[threadIdx.x] = a;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float acc = 0.f;
+    for (int i = 0; i < kSampleThreads; ++i) { acc += part[i]; part[i] = acc; }
+    float u;
+    if (uniforms) {
+      u = uniforms[row];
+    } else {
+      const uint64_t seed = *seed_p;
+      const uint4 r = philox4((uint32_t)(*first_index_p + b), (uint32_t)n, kSampleStream, (uint32_t)pos,
+                              (uint32_t)seed, (uint32_t)(seed >> 32));
+      u = (float)(r.x >> 8) * 0x1p-24f;
+    }
+    sh_target = u * acc;
+    sh_pick = last >= 0 ? last : 0;
+  }
+  __syncthreads();
+  const float target = sh_target;
+  const float excl = threadIdx.x ? part[threadIdx.x - 1] : 0.f;
+  if (excl <= target && target < part[threadIdx.x]) {   // at most one thread: the one whose range crosses u * Z
+    float r = excl;
+    int pick = -1;
+    for (int j = j0; j < j1; ++j) {
+      const float s = s_sc[j];
+      if (!is_cand(s) || rank_key(s, j) < cut) continue;
+      const float w = weight(s);
+      if (w > 0.f) { r += w; pick = j; if (r > target) break; }
+    }
+    sh_pick = pick;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const int j = sh_pick;
+    const float lp = logf(fminf(fmaxf(prob(j), 1e-10f), 1.f));        // = -nll of fira_pointer_mix_nll_fwd for label j
+    const int tok = j < V ? j : copy_src[(long)b * S + (j - V)];
+    next_tok[row] = tok; seq[o] = tok; raw[o] = j; tok_lp[o] = lp; tok_mask[o] = tok != pad_id;
+    length[row] += 1;
+    lp_sum[row] += lp;
+    if (tok == eos_id) finished[row] = 1;
+  }
+}
+
 }  // namespace
 
 #define DISPATCH_T(dtype, ...)                                                            \
@@ -458,6 +652,36 @@ int fira_pointer_mix_nll_bwd(const void* logits, long ld_logits, const float* co
       (const T*)logits, ld_logits, copy_scores, mem_mask, label, stats, upstream, (T*)d_logits, d_copy_scores,
       d_gate_logits, row_active, T_len, V, S);)
   FIRA_CHECK_LAUNCH("fira_pointer_mix_nll_bwd");
+  return FIRA_OK;
+}
+
+int fira_pointer_mix_sample(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                            const unsigned char* mem_mask, const int* copy_src, const uint64_t* seed,
+                            const int* first_index, const float* uniforms, float temperature, int top_k, float top_p,
+                            int eos_id, int pad_id, int* next_tok, int* seq, int* raw, float* token_logprob,
+                            unsigned char* tok_mask, long ld_out, int pos, unsigned char* finished, int* length,
+                            float* logprob, int B, int N, int V, int S, int dtype, void* stream) {
+  FIRA_CHECK_ARG(B >= 0 && N > 0 && V > 0 && S > 0 && V + S <= 0x7FFF, FIRA_ERR_SHAPE,
+                 "pointer_mix_sample: shape (B %d, N %d, V %d, S %d; V + S must be <= 32767)", B, N, V, S);
+  FIRA_CHECK_ARG(pos >= 0 && ld_out >= pos + 2, FIRA_ERR_SHAPE, "pointer_mix_sample: pos %d, ld_out %ld", pos, ld_out);
+  FIRA_CHECK_ARG(temperature > 0.f && temperature <= 3.4e38f, FIRA_ERR_ARG, "pointer_mix_sample: temperature %g",
+                 (double)temperature);
+  FIRA_CHECK_ARG(top_k >= 0, FIRA_ERR_ARG, "pointer_mix_sample: top_k %d < 0", top_k);
+  FIRA_CHECK_ARG(top_p > 0.f && top_p <= 1.f, FIRA_ERR_ARG, "pointer_mix_sample: top_p %g not in (0, 1]", (double)top_p);
+  FIRA_CHECK_ARG(uniforms || (seed && first_index), FIRA_ERR_ARG, "pointer_mix_sample: seed / first_index missing");
+  FIRA_CHECK_ARG(fira_aligned16(logits) && ld_logits % 8 == 0, FIRA_ERR_ALIGN,
+                 "pointer_mix_sample: logits must be 16-byte aligned with a leading dimension that is a multiple of 8");
+  if (B == 0) return FIRA_OK;
+  const int smem = (int)sizeof(float) * (V + S);
+  cudaError_t e = dtype == FIRA_F32
+      ? cudaFuncSetAttribute(pointer_mix_sample_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)
+      : cudaFuncSetAttribute(pointer_mix_sample_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e != cudaSuccess) { fira_set_error(FIRA_ERR_CUDA, "pointer_mix_sample attr: %s", cudaGetErrorString(e)); return FIRA_ERR_CUDA; }
+  DISPATCH_T(dtype, launch_k(pointer_mix_sample_kernel<T>, dim3((unsigned)(B * N)), dim3(kSampleThreads), smem,
+      (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, seed, first_index,
+      uniforms, temperature, top_k, top_p, eos_id, pad_id, next_tok, seq, raw, token_logprob, tok_mask, ld_out, pos,
+      finished, length, logprob, N, V, S);)
+  FIRA_CHECK_LAUNCH("fira_pointer_mix_sample");
   return FIRA_OK;
 }
 

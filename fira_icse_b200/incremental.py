@@ -187,6 +187,11 @@ class IncrementalDecoder:
         (a view of a static buffer: consume it before the next step)."""
         self.tok[:self.R].copy_(tokens)
         self.tok_mask[:, t].copy_(tokens != pad_id)
+        return self.advance(t)
+
+    def advance(self, t):
+        """Decoder output row t for the tokens already in `tok[:B*K]` and `tok_mask[:, t]` (step() fills them from the
+        host side; the sampler's kernel writes them on the device)."""
         if not self.use_graphs:
             self._layers(t)
         elif t in self.graphs:

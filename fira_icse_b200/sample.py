@@ -1,0 +1,192 @@
+"""Seeded sampling decoding: temperature, top-k and top-p draws from the dual-copy mixture (Model.py:54-86).
+
+Where beam search keeps the most probable continuations, `sample` draws N independent messages per commit from the
+model's distribution and reports the model's own log-probability of every drawn token:
+
+    P_j = g0 * softmax(vocab logits)_j  (j < V)   ||   g1 * softmax(masked copy scores)_s  (j = V + s)
+    candidates: P_j > 0 in fp32 and, for copies, mem_mask[b, s] != 0;  s_j = log P_j / temperature
+    top_k > 0 keeps the top_k highest s_j (ties: smaller j first); top_p < 1 then keeps the shortest such rank prefix
+    whose weight sum(exp(s_j - max s)) reaches top_p of the kept weight; the draw u in [0, 1) picks the smallest kept
+    j whose running weight in index order exceeds u * (total kept weight).
+
+u comes from Philox4x32-7 keyed by `seed` with the counter (first_index + b, n, position), so a commit's samples depend
+on its position in the dataset, not on the batch it was decoded in or the GPU count.  The emitted log-probability is
+log(clamp(P_j, 1e-10, 1)) whatever temperature, top_k and top_p are: it is -nll of the training loss for label j.
+
+Per batch the encoder, the cross-attention K/V of the memory and LinearSource(memory) run once.  The N samples of a
+commit are the N query rows of an incremental.IncrementalDecoder.  Per position: newest decoder row -> out_fc ->
+target projection and gate -> copy scores -> fira_pointer_mix_sample, which also writes the next input token
+straight into the decoder's token buffer and keeps each row's finished flag, length and log-probability sum.  A
+position is captured once into a CUDA graph and replayed for every later batch of the same shape; the loop reads
+back nothing but an all-finished flag, once every 8 positions.
+"""
+import ctypes
+import weakref
+from typing import NamedTuple
+
+import torch
+
+from . import ops
+from ._lib import call
+from .incremental import IncrementalDecoder
+
+D = ops.D
+MAX_SAMPLES = 32          # the N samples of a commit are its query rows in fira_attn_fwd / fira_copy_scores_fwd (<= 32)
+POLL_EVERY = 8            # positions between two reads of the all-finished flag
+
+
+class Samples(NamedTuple):
+    seq: torch.Tensor             # [B, N, T] int64 vocabulary ids: <start>, the drawn tokens, pad after <eos>
+    raw: torch.Tensor             # [B, N, T] int64 raw indices (label encoding: V + memory position for a copy)
+    length: torch.Tensor          # [B, N] int64 tokens including <start> and <eos>
+    logprob: torch.Tensor         # [B, N] fp32 sum of token_logprob
+    token_logprob: torch.Tensor   # [B, N, T] fp32 log(clamp(P, 1e-10, 1)) of each drawn token, 0 at 0 and after <eos>
+
+
+def _f32(x):
+    return ctypes.c_float(x).value
+
+
+def check_args(num_samples, temperature, top_k, top_p, seed, first_index, tar_len):
+    """ValueError for any parameter the sampler cannot honour (called before any device work)."""
+    def is_int(v):
+        return isinstance(v, int) and not isinstance(v, bool)
+    if not is_int(num_samples) or not 1 <= num_samples <= MAX_SAMPLES:
+        raise ValueError(f"num_samples must be an integer in [1, {MAX_SAMPLES}], got {num_samples!r}")
+    if not isinstance(temperature, (int, float)) or not 0.0 < _f32(temperature) < float("inf"):
+        raise ValueError(f"temperature must be a positive finite number (in fp32), got {temperature!r}")
+    if not is_int(top_k) or top_k < 0:
+        raise ValueError(f"top_k must be an integer >= 0 (0 = off), got {top_k!r}")
+    if not isinstance(top_p, (int, float)) or not 0.0 < _f32(top_p) <= 1.0:
+        raise ValueError(f"top_p must be in (0, 1] (1 = off), got {top_p!r}")
+    if not is_int(seed) or not 0 <= seed < 2 ** 64:
+        raise ValueError(f"seed must be an integer in [0, 2**64), got {seed!r}")
+    if not is_int(first_index) or not 0 <= first_index < 2 ** 31:
+        raise ValueError(f"first_index must be an integer in [0, 2**31), got {first_index!r}")
+    if not is_int(tar_len) or tar_len < 2:
+        raise ValueError(f"tar_len must be an integer >= 2, got {tar_len!r}")
+
+
+def _weights_key(model):
+    ps = list(model.parameters())
+    return (getattr(model.decoder, "weights_epoch", 0),) + tuple(p._version for p in ps) + tuple(p.data_ptr() for p in ps)
+
+
+class _Sampler:
+    """Static buffers and captured position graphs of one (model, B, N, tar_len, S, precision)."""
+
+    def __init__(self, model, B, N, T, S):
+        self.model, self.B, self.N, self.T, self.S = model, B, N, T, S
+        self.inc = IncrementalDecoder(model.decoder, B, N, T, S, graphs=False)   # its launches go into our graphs
+        self.pr = ops.Prec(self.inc.be.bf16)
+        dev = model.out_fc.weight.device
+        R = self.R = B * N
+        tdt = self.inc.be.tdt
+        i32 = dict(dtype=torch.int32, device=dev)
+        f32 = dict(dtype=torch.float32, device=dev)
+        self.V = model.vocab_size
+        self.ldl = ops._ld_logits(self.V)
+        self.seed = torch.zeros(1, dtype=torch.int64, device=dev)      # read by the kernel as uint64
+        self.first = torch.zeros(1, **i32)
+        self.mem_mask = torch.zeros((B, S), dtype=torch.uint8, device=dev)
+        self.copy_src = torch.zeros((B, S), **i32)
+        self.src = torch.empty((B * S, D), dtype=tdt, device=dev)
+        self.logits = torch.empty((R, self.ldl), dtype=tdt, device=dev)
+        self.tgt = torch.empty((R, D), dtype=tdt, device=dev)
+        self.gl = torch.empty((R, 2), **f32)
+        self.sc = torch.empty((B, N, S), **f32)
+        self.seq = torch.empty((R, T), **i32)
+        self.raw = torch.empty((R, T), **i32)
+        self.tlp = torch.empty((R, T), **f32)
+        self.finished = torch.empty(R, dtype=torch.uint8, device=dev)
+        self.length = torch.empty(R, **i32)
+        self.lp = torch.empty(R, **f32)
+        self.graphs = {}
+
+    def start(self, memory, mem_mask, copy_src, seed, first_index, start_id, pad_id):
+        inc = self.inc
+        inc.start(memory, mem_mask)
+        mem2 = memory.contiguous().to(inc.be.tdt).view(self.B * self.S, D)
+        self.pr.linear(mem2, self.model.copy_net.LinearSource.weight, out=self.src)     # once per batch, not per row
+        self.mem_mask.copy_(mem_mask)
+        self.copy_src.copy_(copy_src)
+        self.seed.fill_(seed - 2 ** 64 if seed >= 2 ** 63 else seed)
+        self.first.fill_(first_index)
+        self.seq.fill_(pad_id)
+        self.seq[:, 0] = start_id
+        self.raw.fill_(pad_id)
+        self.raw[:, 0] = start_id
+        self.tlp.zero_()
+        self.finished.zero_()
+        self.length.fill_(1)
+        self.lp.zero_()
+        inc.tok[:self.R].fill_(start_id)
+        inc.tok_mask[:, 0].fill_(int(start_id != pad_id))
+
+    def position(self, t, temperature, top_k, top_p, eos_id, pad_id):
+        """Draw position t + 1 from decoder row t (every launch on the current stream: capturable)."""
+        m, pr, B, N, S, R = self.model, self.pr, self.B, self.N, self.S, self.R
+        cn = m.copy_net
+        x = self.inc.advance(t)                                                  # [R, D]
+        pr.linear(x, m.out_fc.weight, m.out_fc.bias, out=self.logits, ld_out=self.ldl)
+        pr.linear(x, cn.LinearTarget.weight, out=self.tgt)
+        ops.linear(x.float() if pr.bf16 else x, cn.LinearProb.weight, cn.LinearProb.bias, out=self.gl)   # fp32 gate
+        st = ops._stream()
+        p = ops._ptr
+        call("fira_copy_scores_fwd", p(self.src), p(self.tgt), p(cn.LinearRes.weight), p(cn.LinearRes.bias),
+             p(self.mem_mask), None, p(self.sc), B, N, S, D, pr.code, st)
+        call("fira_pointer_mix_sample", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
+             p(self.copy_src), p(self.seed), p(self.first), None, float(temperature), int(top_k), float(top_p),
+             int(eos_id), int(pad_id), p(self.inc.tok), p(self.seq), p(self.raw), p(self.tlp), p(self.inc.tok_mask),
+             self.T, t, p(self.finished), p(self.length), p(self.lp), B, N, self.V, S, pr.code, st)
+
+
+_SAMPLERS = weakref.WeakKeyDictionary()          # model -> {(B, N, T, S, precision): (weights key, _Sampler)}
+
+
+def _sampler(model, B, N, T, S):
+    store = _SAMPLERS.setdefault(model, {})
+    key = (B, N, T, S, model.precision)
+    wkey = _weights_key(model)
+    if key not in store or store[key][0] != wkey:       # changed weights: fresh operand copies and graphs
+        store[key] = (wkey, _Sampler(model, B, N, T, S))
+    return store[key][1]
+
+
+@torch.no_grad()
+def sample(model, sou, mark, ast_change, edge, sub_token, *, num_samples=1, temperature=1.0, top_k=0, top_p=1.0,
+           seed=0, first_index=0, tar_len=30, start_id, eos_id, pad_id=0):
+    """Draw `num_samples` messages per commit -> Samples(seq, raw, length, logprob, token_logprob).
+
+    first_index: dataset position of the batch's first commit (the Philox counter uses first_index + b)."""
+    check_args(num_samples, temperature, top_k, top_p, seed, first_index, tar_len)
+    if tar_len > model.decoder.pos_encode.shape[0]:
+        raise ValueError(f"tar_len {tar_len} exceeds the decoder's {model.decoder.pos_encode.shape[0]} positions")
+    if first_index + sou.shape[0] > 2 ** 31:
+        raise ValueError("first_index + batch size must stay below 2**31")
+    dev = model.out_fc.weight.device
+    sou, mark, ast_change, sub_token = (t.to(dev) for t in (sou, mark, ast_change, sub_token))
+    B, N, T = sou.shape[0], num_samples, tar_len
+    memory = model.encoder.encode_memory(sou, mark, ast_change, edge, sub_token)        # once per batch
+    S = memory.shape[1]
+    mem_mask = torch.cat((sou != pad_id, sub_token != 0), dim=1)
+    copy_src = torch.cat((sou, sub_token), dim=1)                                       # copy position -> vocabulary id
+    st = _sampler(model, B, N, T, S)
+    st.start(memory, mem_mask, copy_src, seed, first_index, start_id, pad_id)
+    cfg = (float(temperature), int(top_k), float(top_p), int(eos_id), int(pad_id))
+    for t in range(T - 1):
+        if t and t % POLL_EVERY == 0 and not bool(st.finished.eq(0).any()):
+            break
+        g = st.graphs.get((cfg, t))
+        if g is not None:
+            g.replay()
+            continue
+        st.position(t, *cfg)                               # this batch's result (and the warm-up of a capture) ...
+        torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):                          # ... and the same launches recorded for later batches
+            st.position(t, *cfg)
+        st.graphs[(cfg, t)] = g
+    shape = (B, N, T)
+    return Samples(st.seq.view(shape).long(), st.raw.view(shape).long(), st.length.view(B, N).long(),
+                   st.lp.view(B, N).clone(), st.tlp.view(shape).clone())

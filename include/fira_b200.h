@@ -253,6 +253,27 @@ int fira_pointer_mix_nll_bwd(const void* logits, long ld_logits, const float* co
                              const float* upstream, void* d_logits, float* d_copy_scores, float* d_gate_logits,
                              unsigned char* row_active, long rows, int T_len, int V, int S, int dtype, void* stream);
 
+/* ---- one seeded sampling step from the same mixture (fira_icse_b200/sample.py).  Rows are (commit b, sample n),
+ *      B*N of them: logits [B*N, ld_logits], copy_scores [B, N, S], gate_logits [B*N, 2], mem_mask / copy_src [B, S]
+ *      (copy_src: the vocabulary id behind each memory position).  Candidates: vocabulary entries and unmasked copy
+ *      positions whose mixture probability P_j is > 0 in fp32; s_j = log P_j / temperature, ranked by s descending then
+ *      index ascending; top_k > 0 keeps the first top_k ranks; top_p < 1 then keeps the shortest rank prefix whose
+ *      weight sum(exp(s_j - max s)) reaches top_p times the kept weight; the draw picks the smallest kept index whose
+ *      running weight in index order exceeds u * (total kept weight).  u in [0, 1): uniforms[row] when uniforms is
+ *      not NULL, else 24 bits of Philox4x32-7 keyed by *seed with counter (*first_index + b, n, stream, pos) --
+ *      seed / first_index are device scalars, so one captured graph per position serves every batch.
+ *      A row not yet finished writes, at column pos + 1 of seq / raw / token_logprob / tok_mask ([B*N, ld_out]):
+ *      the next input token (j, or copy_src[b, j - V] for a copy), the raw index j, log(clamp(P_j, 1e-10, 1)) (=
+ *      -nll of fira_pointer_mix_nll_fwd for label j), token != pad_id; also next_tok[row] = the token, length[row] += 1,
+ *      logprob[row] += the log-probability, finished[row] = 1 on eos_id.  A finished row writes pad_id / 0 and keeps
+ *      length and logprob.  V + S <= 32767; temperature > 0, top_k >= 0, 0 < top_p <= 1. */
+int fira_pointer_mix_sample(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                            const unsigned char* mem_mask, const int* copy_src, const uint64_t* seed,
+                            const int* first_index, const float* uniforms, float temperature, int top_k, float top_p,
+                            int eos_id, int pad_id, int* next_tok, int* seq, int* raw, float* token_logprob,
+                            unsigned char* tok_mask, long ld_out, int pos, unsigned char* finished, int* length,
+                            float* logprob, int B, int N, int V, int S, int dtype, void* stream);
+
 /* ---- HOST-side batch preparation (CPU only: every pointer below is HOST memory, there is no stream).
  *
  * fira_host_build_adjacency: the commit graph of Dataset.py:220-294 + process_edge (Dataset.py:346-357).

@@ -16,6 +16,11 @@ beam search ranking.  Differences, all below the module surface:
     FIRA_MAX_BATCHES (smoke runs), FIRA_WORKERS, FIRA_PRECISION (fp32 parity mode | bf16 throughput mode),
     FIRA_MAX_SHAPES (bound on distinct trimmed batch shapes = captured graphs, default 24), FIRA_BUCKET (0 = the
     reference's uniform batching; K > 1 = size-bucketed batches within windows of K batches, see PackedBatchLoader).
+  * `test` decoding: FIRA_DECODE=beam (default, the reference's beam search -> OUTPUT/output_fira) or sample (seeded
+    sampling, fira_icse_b200.sample -> OUTPUT/output_fira_samples: FIRA_SAMPLES consecutive lines per commit in test
+    order, `<log-probability>\\t<message>`; prints the mean sentence BLEU over all samples).  Sampling parameters:
+    FIRA_SAMPLES (default 3), FIRA_TEMPERATURE (1.0), FIRA_TOP_K (0 = off), FIRA_TOP_P (1.0 = off), FIRA_SEED (0).
+    A commit's samples depend on the seed and its position in the test split only, so sharded runs draw the same.
 """
 import json
 import os
@@ -34,6 +39,7 @@ from fira_icse_b200.bleu import sentence_bleu_method2
 from fira_icse_b200.data import PackedBatchLoader, TransDataset, batch_to_device, collate_packed
 from fira_icse_b200.engine import GraphedTrainStep
 from fira_icse_b200.parallel import DataParallelStep, shard_range
+from fira_icse_b200.sample import sample
 
 
 class DotDict(dict):
@@ -234,6 +240,37 @@ def test(model, test_loader, g, test_index, dev_, out_path="OUTPUT/output_fira")
     return bleus / max(1, total)
 
 
+def sample_test(model, test_loader, g, test_index, dev_, first_index, out_path="OUTPUT/output_fira_samples"):
+    """Seeded sampling over the test split: FIRA_SAMPLES lines `<log-prob>\\t<message>` per commit, in test order."""
+    vocab, r_vocab, var_maps = g["vocab"], g["r_vocab"], g["var_maps"]
+    n = int(os.environ.get("FIRA_SAMPLES", 3))
+    opts = dict(num_samples=n, temperature=float(os.environ.get("FIRA_TEMPERATURE", 1.0)),
+                top_k=int(os.environ.get("FIRA_TOP_K", 0)), top_p=float(os.environ.get("FIRA_TOP_P", 1.0)),
+                seed=int(os.environ.get("FIRA_SEED", 0)))
+    model.eval()
+    total, bleus = 0, 0.0
+    with open(out_path, 'w') as f:
+        for batch in test_loader:
+            b = batch_to_device(batch, dev_)
+            out = sample(model, b[0], b[3], b[4], b[5], b[7], first_index=first_index + total, tar_len=args.tar_len,
+                         start_id=vocab['<start>'], eos_id=vocab['<eos>'], pad_id=vocab['<pad>'], **opts)
+            seq, length, logprob = out.seq.cpu().numpy(), out.length.cpu().numpy(), out.logprob.cpu().numpy()
+            tar = batch[1].numpy()
+            bleu_batch = 0.0
+            for i in range(len(seq)):
+                ref = tar[i].tolist()
+                ref = [r_vocab[x] for x in ref[1:ref.index(vocab['<eos>'])]]
+                for k in range(n):
+                    hyp = ids_to_text(seq[i, k][:length[i, k]].tolist(), r_vocab)
+                    bl = sentence_bleu_method2([ref], hyp)
+                    bleus += bl; bleu_batch += bl
+                    f.write('%.6f\t%s\n' % (logprob[i, k], ' '.join(deanonymise(hyp, var_maps[test_index[total + i]]))))
+            f.flush()
+            total += len(seq)
+            print("data: %d/%d bleu: %f" % (total, len(test_loader.dataset), bleu_batch / (len(seq) * n)))
+    return bleus / max(1, total * n)
+
+
 def main_test():
     dev_ = device()
     g = load_globals()
@@ -245,8 +282,15 @@ def main_test():
     lo, hi = shard_range(len(test_set), RANK, WORLD)                # replicas only: index ranges, files concatenated
     idx = list(range(lo, hi)) if WORLD > 1 else None
     test_loader = loader(test_set, args.test_batch_size, False, idx)
-    out = "OUTPUT/output_fira" if WORLD == 1 else f"OUTPUT/output_fira.part{RANK:02d}"
-    bleu = test(model, test_loader, g, all_index['test'][lo:hi], dev_, out)
+    decode = os.environ.get("FIRA_DECODE", "beam")
+    if decode == "beam":
+        out = "OUTPUT/output_fira" if WORLD == 1 else f"OUTPUT/output_fira.part{RANK:02d}"
+        bleu = test(model, test_loader, g, all_index['test'][lo:hi], dev_, out)
+    elif decode == "sample":
+        out = "OUTPUT/output_fira_samples" if WORLD == 1 else f"OUTPUT/output_fira_samples.part{RANK:02d}"
+        bleu = sample_test(model, test_loader, g, all_index['test'][lo:hi], dev_, lo, out)
+    else:
+        raise SystemExit("FIRA_DECODE must be 'beam' or 'sample'")
     print("mean sentence bleu: %f" % bleu)
 
 

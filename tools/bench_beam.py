@@ -7,6 +7,7 @@ reference's own loop was timed on in BASELINE.md (72 s for 32 commits on CPU).  
 (batch, beam) configuration; timing with CUDA events around whole batches, inputs resident on the device.
 
     python tools/bench_beam.py [--batches 20,128] [--beams 3,5] [--precision fp32|bf16] [--reps 3]
+                               [--modes full,incremental,graph,sample]   (sample: N = the beam width)
 """
 import argparse
 import json
@@ -33,6 +34,7 @@ def main():
     import fira_icse_b200 as F
     from fira_icse_b200 import _lib
     from fira_icse_b200.beam import beam_search
+    from fira_icse_b200.sample import sample
     dev = torch.device("cuda", 0)
     torch.manual_seed(0)
     model = F.TransModel(bench.model_args()).to(dev)
@@ -43,28 +45,33 @@ def main():
         b = bench.device_batch(hb, dev, B)
         for K, mode in ((int(x), m) for x in a.beams.split(",") for m in a.modes.split(",")):
             def run():
+                if mode == "sample":                                 # N = the beam width, default T / k / p
+                    return sample(model, b[0], b[3], b[4], b[5], b[7], num_samples=K, tar_len=30, start_id=1, eos_id=2,
+                                  pad_id=0)
                 return beam_search(model, b[0], b[3], b[4], b[5], b[7], beam_size=K, tar_len=30, start_id=1, eos_id=2,
                                    pad_id=0, mode=mode)
             ref = run()                                              # warm-up (lazy CUDA state, graph capture)
             if mode == "full":
                 ref_full = ref
-            same = bool(torch.equal(ref[0], ref_full[0])) if "full" in a.modes.split(",") else None
+            same = bool(torch.equal(ref[0], ref_full[0])) if "full" in a.modes.split(",") and mode != "sample" else None
             torch.cuda.synchronize()
             n0 = _lib.LAUNCH_COUNT
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             for _ in range(a.reps):
-                seq, length, prob = run()
+                out = run()
+            length = out[2] if mode == "sample" else out[1]
             e1.record()
             torch.cuda.synchronize()
             ms = e0.elapsed_time(e1) / a.reps
             print(json.dumps({
-                "metric": "beam-search inference throughput", "unit": "commits/s", "value": B / ms * 1e3,
+                "metric": "sampling inference throughput" if mode == "sample" else "beam-search inference throughput", "unit": "commits/s", "value": B / ms * 1e3,
                 "ms_per_batch": ms, "batch": B, "beam": K, "decoded_steps": int(length.max().item()) - 1,
                 "precision": a.precision, "mode": mode, "ids_equal_full_mode": same, "trimmed": bool(a.trim), "data": "synthetic (DataSet distribution), random weights",
                 "c_abi_calls_per_batch": (_lib.LAUNCH_COUNT - n0) // a.reps,
                 "note": "encoder once per batch; full = 30-position decoder re-run per step over all live beams, "
-                        "incremental = newest row against K/V caches, graph = the same as CUDA-graph replays"}),
+                        "incremental = newest row against K/V caches, graph = the same as CUDA-graph replays, "
+                        "sample = beam-width seeded samples per commit (T = 1, no top-k / top-p), one graph per position"}),
                   flush=True)
 
 
