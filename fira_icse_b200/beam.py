@@ -14,13 +14,42 @@ only the newest decoder row per step against cached keys/values (incremental.Inc
 replays each step's kernels as a CUDA graph); mode="full" re-runs the 30-position decoder every step.
 The default comes from FIRA_BEAM_MODE (default "graph").  Ranking keeps the reference's candidate layout; only
 the first `beam_size` entries of its descending sort are ever used, so the sort is a device top-k.
+
+`nbest` is beam search in log space with length normalisation, decoded on the device, returning every commit's K
+hypotheses with their scores (`beam_search` stays the reference-exact default):
+
+    lp_j = log(clamp(P_j, 1e-10, 1))   (P_j the dual-copy mixture; = -nll of the training loss for label j)
+    candidates: every vocabulary entry and every unmasked copy position (masked copy positions never)
+    position 0: only slot 0 is live (L = 0); slots 1..K-1 are inactive and propose nothing
+    a live slot i (log-probability sum L_i, n_i generated tokens) proposes (i, j): L = L_i + lp_j (fp32), n = n_i + 1;
+    a finished slot (its last token <eos>) proposes itself unchanged, once, as j = C = V + S
+    score = L / ((5 + n) / 6) ** length_penalty (fp32, powf): length_penalty = 0 ranks by L, the reference's
+    ranking in log space, so it cannot underflow to 0 the way products of probabilities do
+    the K best by (score descending, then i * (C + 1) + j ascending) become the new slots, in that order
+    copies become vocabulary ids through the commit's own sou / sub_token; stop when every slot of every commit has
+    finished, or after tar_len - 1 positions.
+A vocabulary candidate and a copy candidate that spell the same word stay two candidates (as in the reference), so an
+n-best list can hold the same message twice.
+
+The loop is decode_loop.PositionLoop (the sampler's): per position the head, then fira_pointer_mix_beam_step (per
+live slot row its top K, then per commit the merge, writing the new slots, their parents and the next tokens), the
+KV-cache reorder to the parents and the pad mask of the next tokens, all in one captured CUDA graph.  Slot state is
+double-buffered by the parity of the position (a slot's new history comes from another row).
 """
+import ctypes
+import math
 import os
 import weakref
+from typing import NamedTuple
 
 import torch
 
+from . import ops
+from ._lib import call
+from .decode_loop import PositionLoop, loop_for
 from .incremental import IncrementalDecoder
+
+MAX_BEAM = 16             # the row stage keeps a per-thread top K in registers
 
 
 _DECODERS = weakref.WeakKeyDictionary()          # model -> {(B, K, ...): IncrementalDecoder}
@@ -114,3 +143,102 @@ def best_sequences(seq, length, prob):
     best = torch.argmax(prob, dim=1)
     ar = torch.arange(seq.shape[0], device=seq.device)
     return seq[ar, best], length[ar, best]
+
+
+class Hypotheses(NamedTuple):
+    seq: torch.Tensor             # [B, K, T] int64 vocabulary ids: <start>, the tokens, pad after <eos>; best first
+    raw: torch.Tensor             # [B, K, T] int64 raw indices (label encoding: V + memory position for a copy)
+    length: torch.Tensor          # [B, K] int64 tokens including <start> and <eos>
+    logprob: torch.Tensor         # [B, K] fp32 sum of token_logprob
+    score: torch.Tensor           # [B, K] fp32 logprob / ((5 + length - 1) / 6) ** length_penalty, non-increasing
+    token_logprob: torch.Tensor   # [B, K, T] fp32 log(clamp(P, 1e-10, 1)) of each token, 0 at 0 and after <eos>
+    finished: torch.Tensor        # [B, K] bool: the hypothesis ends with <eos>
+
+
+def _f32(x):
+    return ctypes.c_float(x).value
+
+
+def check_nbest_args(beam_size, length_penalty, tar_len):
+    """ValueError for any parameter nbest cannot honour (called before any device work)."""
+    def is_int(v):
+        return isinstance(v, int) and not isinstance(v, bool)
+    if not is_int(beam_size) or not 1 <= beam_size <= MAX_BEAM:
+        raise ValueError(f"beam_size must be an integer in [1, {MAX_BEAM}], got {beam_size!r}")
+    if (isinstance(length_penalty, bool) or not isinstance(length_penalty, (int, float))
+            or not 0.0 <= _f32(length_penalty) < math.inf):
+        raise ValueError(f"length_penalty must be a finite number >= 0 (in fp32), got {length_penalty!r}")
+    if not is_int(tar_len) or tar_len < 2:
+        raise ValueError(f"tar_len must be an integer >= 2, got {tar_len!r}")
+
+
+class _NBest(PositionLoop):
+    """Double-buffered slot state ([2, B*K, ...], half t & 1 read at position t) on top of the shared position loop."""
+
+    def __init__(self, model, B, K, T, S):
+        super().__init__(model, B, K, T, S)
+        R, dev = self.R, self.dev
+        i32 = dict(dtype=torch.int32, device=dev)
+        f32 = dict(dtype=torch.float32, device=dev)
+        self.seq = torch.empty((2, R, T), **i32)
+        self.raw = torch.empty((2, R, T), **i32)
+        self.tlp = torch.empty((2, R, T), **f32)
+        self.length = torch.empty((2, R), **i32)
+        self.lp = torch.empty((2, R), **f32)
+        self.score = torch.empty((2, R), **f32)
+        self.status = torch.empty((2, R), dtype=torch.uint8, device=dev)      # 0 live, 1 finished, 2 inactive
+        self.parent = torch.empty(R, dtype=torch.int64, device=dev)
+        self.work = torch.empty(R * K, dtype=torch.int64, device=dev)         # per-row top K rank keys (uint64)
+
+    def start(self, memory, mem_mask, copy_src, start_id, pad_id):
+        super().start(memory, mem_mask, copy_src, start_id, pad_id)
+        for x in (self.seq, self.raw):           # half 1 is written whole at position 0 (its columns > 1 from half 0)
+            x[0].fill_(pad_id)
+            x[0, :, 0] = start_id
+        self.tlp[0].zero_()
+        self.length[0].fill_(1)
+        self.lp[0].zero_()
+        self.score[0].zero_()
+        self.status[0].view(self.B, self.N).fill_(2)
+        self.status[0].view(self.B, self.N)[:, 0] = 0          # beam 0 has probability 1, the others 0
+
+    def unfinished(self, t):
+        return self.status[t & 1].eq(0).any()
+
+    def position(self, t, length_penalty, eos_id, pad_id):
+        """Slots of position t + 1 from decoder row t (every launch on the current stream: capturable)."""
+        self.head(t)
+        p = ops._ptr
+        inc = self.inc
+        call("fira_pointer_mix_beam_step", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
+             p(self.copy_src), float(length_penalty), int(eos_id), int(pad_id), p(self.work), p(self.seq), p(self.raw),
+             p(self.tlp), p(self.length), p(self.lp), p(self.score), p(self.status), p(self.parent), p(inc.tok),
+             self.T, t, self.B, self.N, self.V, self.S, self.pr.code, ops._stream())
+        # caches follow the parents BEFORE the pad mask of the new tokens is written (reorder moves tok_mask rows too)
+        inc.reorder(self.parent)
+        inc.tok_mask[:, t + 1].copy_(inc.tok[:self.R] != pad_id)
+
+
+@torch.no_grad()
+def nbest(model, sou, mark, ast_change, edge, sub_token, *, beam_size=3, length_penalty=0.0, tar_len=30, start_id,
+          eos_id, pad_id=0):
+    """Log-space beam search with length normalisation -> Hypotheses, each commit's K best first (module docstring)."""
+    check_nbest_args(beam_size, length_penalty, tar_len)
+    if beam_size > model.vocab_size:
+        raise ValueError(f"beam_size {beam_size} exceeds the vocabulary ({model.vocab_size})")
+    if tar_len > model.decoder.pos_encode.shape[0]:
+        raise ValueError(f"tar_len {tar_len} exceeds the decoder's {model.decoder.pos_encode.shape[0]} positions")
+    dev = model.out_fc.weight.device
+    sou, mark, ast_change, sub_token = (t.to(dev) for t in (sou, mark, ast_change, sub_token))
+    B, K, T = sou.shape[0], beam_size, tar_len
+    memory = model.encoder.encode_memory(sou, mark, ast_change, edge, sub_token)        # once per batch
+    S = memory.shape[1]
+    mem_mask = torch.cat((sou != pad_id, sub_token != 0), dim=1)
+    copy_src = torch.cat((sou, sub_token), dim=1)                                       # copy position -> vocabulary id
+    st = loop_for(_NBest, model, B, K, T, S)
+    st.start(memory, mem_mask, copy_src, start_id, pad_id)
+    h = st.run((float(length_penalty), int(eos_id), int(pad_id))) & 1
+    shape = (B, K, T)
+    return Hypotheses(st.seq[h].view(shape).long(), st.raw[h].view(shape).long(), st.length[h].view(B, K).long(),
+                      st.lp[h].view(B, K).clone(), st.score[h].view(B, K).clone(), st.tlp[h].view(shape).clone(),
+                      st.status[h].view(B, K) == 1)

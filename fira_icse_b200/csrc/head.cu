@@ -375,10 +375,12 @@ constexpr uint32_t kSampleStream = 0x53414D50u;       // Philox stream id of the
 constexpr uint64_t kKeyEnd = 1ull << 47;
 
 __device__ __forceinline__ bool is_cand(float s) { return s == s; }          // NaN marks a non-candidate
+__device__ __forceinline__ uint32_t order_bits(float s) {      // unsigned order = float order (no NaN)
+  const uint32_t b = __float_as_uint(s);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
 __device__ __forceinline__ uint64_t rank_key(float s, int j) {
-  uint32_t b = __float_as_uint(s);
-  b = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-  return ((uint64_t)b << 15) | (uint32_t)(0x7FFF - j);
+  return ((uint64_t)order_bits(s) << 15) | (uint32_t)(0x7FFF - j);
 }
 
 // fixed-order reduction: xor butterfly inside each warp, then the 8 warp results in warp order (every thread gets it)
@@ -393,6 +395,48 @@ __device__ __forceinline__ V block_reduce(V v, V* sh, Op op) {
 #pragma unroll
   for (int w = 1; w < kSampleThreads / 32; ++w) r = op(r, sh[w]);
   return r;
+}
+
+// Row statistics of the mixture exactly as head_fwd_kernel forms them when the vocabulary pass runs (same loops, same
+// reduction order): with them, g0 * (expf(x_j - vmax) / vsum) and g1 * (expf(c_s - cmax) / csum) are bit for bit the
+// probabilities fira_pointer_mix_nll_fwd gives labels j and V + s.  Block-wide: every thread of the 256 calls it.
+struct MixRow { float vmax, vsum, cmax, csum, g0, g1; };
+template <typename T>
+__device__ __forceinline__ MixRow mix_row_stats(const T* __restrict__ lrow, const float* __restrict__ srow,
+                                                const unsigned char* __restrict__ mrow, const float* __restrict__ gl,
+                                                int V, int S, MaxSum* sh_ms, float* bc) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  MaxSum v{-INFINITY, 0.f};
+  const int V8 = V >> 3;
+  for (int g = threadIdx.x; g < V8; g += blockDim.x) {
+    float x[8];
+    Act<T>::load8(lrow + (long)g * 8, x);
+    float m8 = x[0];
+#pragma unroll
+    for (int i = 1; i < 8; ++i) m8 = fmaxf(m8, x[i]);
+    if (m8 > v.m) { v.s *= expf(v.m - m8); v.m = m8; }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) v.s += expf(x[i] - v.m);
+  }
+  for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) { MaxSum u{Act<T>::ld(lrow + j), 1.f}; v = ms_merge(v, u); }
+  v = ms_warp(v);
+  if (lane == 0) sh_ms[warp] = v;
+  __syncthreads();
+  if (warp == 0) { MaxSum u = lane < 8 ? sh_ms[lane] : MaxSum{-INFINITY, 0.f}; u = ms_warp(u); if (lane == 0) { bc[0] = u.m; bc[1] = u.s; } }
+  __syncthreads();
+  MaxSum c{-INFINITY, 0.f};
+  for (int j = threadIdx.x; j < S; j += blockDim.x) { MaxSum u{mrow[j] ? srow[j] : kMaskFill, 1.f}; c = ms_merge(c, u); }
+  c = ms_warp(c);
+  if (lane == 0) sh_ms[warp] = c;
+  __syncthreads();
+  if (warp == 0) { MaxSum u = lane < 8 ? sh_ms[lane] : MaxSum{-INFINITY, 0.f}; u = ms_warp(u); if (lane == 0) { bc[2] = u.m; bc[3] = u.s; } }
+  __syncthreads();
+  const float vmax = bc[0], vsum = bc[1], cmax = bc[2], csum = bc[3];
+  const float gl0 = gl[0], gl1 = gl[1];
+  const float gm = fmaxf(gl0, gl1);
+  const float e0 = expf(gl0 - gm), e1 = expf(gl1 - gm);
+  const float g0 = e0 / (e0 + e1), g1 = e1 / (e0 + e1);
+  return MixRow{vmax, vsum, cmax, csum, g0, g1};
 }
 
 template <typename T>
@@ -420,43 +464,14 @@ __global__ void __launch_bounds__(kSampleThreads) pointer_mix_sample_kernel(
     if (threadIdx.x == 0) { next_tok[row] = pad_id; seq[o] = pad_id; raw[o] = pad_id; tok_lp[o] = 0.f; tok_mask[o] = 0; }
     return;
   }
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const T* lrow = logits + row * ldl;
   const float* srow = sc + row * S;
   const unsigned char* mrow = mem_mask + (long)b * S;
 
   // row statistics exactly as head_fwd_kernel forms them (same loop, same reduction order), so the emitted
   // log-probability is the one fira_pointer_mix_nll_fwd gives the same label
-  MaxSum v{-INFINITY, 0.f};
-  const int V8 = V >> 3;
-  for (int g = threadIdx.x; g < V8; g += blockDim.x) {
-    float x[8];
-    Act<T>::load8(lrow + (long)g * 8, x);
-    float m8 = x[0];
-#pragma unroll
-    for (int i = 1; i < 8; ++i) m8 = fmaxf(m8, x[i]);
-    if (m8 > v.m) { v.s *= expf(v.m - m8); v.m = m8; }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v.s += expf(x[i] - v.m);
-  }
-  for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) { MaxSum u{Act<T>::ld(lrow + j), 1.f}; v = ms_merge(v, u); }
-  v = ms_warp(v);
-  if (lane == 0) sh_ms[warp] = v;
-  __syncthreads();
-  if (warp == 0) { MaxSum u = lane < 8 ? sh_ms[lane] : MaxSum{-INFINITY, 0.f}; u = ms_warp(u); if (lane == 0) { bc[0] = u.m; bc[1] = u.s; } }
-  __syncthreads();
-  MaxSum c{-INFINITY, 0.f};
-  for (int j = threadIdx.x; j < S; j += blockDim.x) { MaxSum u{mrow[j] ? srow[j] : kMaskFill, 1.f}; c = ms_merge(c, u); }
-  c = ms_warp(c);
-  if (lane == 0) sh_ms[warp] = c;
-  __syncthreads();
-  if (warp == 0) { MaxSum u = lane < 8 ? sh_ms[lane] : MaxSum{-INFINITY, 0.f}; u = ms_warp(u); if (lane == 0) { bc[2] = u.m; bc[3] = u.s; } }
-  __syncthreads();
-  const float vmax = bc[0], vsum = bc[1], cmax = bc[2], csum = bc[3];
-  const float gl0 = gate_logit[row * 2], gl1 = gate_logit[row * 2 + 1];
-  const float gm = fmaxf(gl0, gl1);
-  const float e0 = expf(gl0 - gm), e1 = expf(gl1 - gm);
-  const float g0 = e0 / (e0 + e1), g1 = e1 / (e0 + e1);
+  const MixRow ms = mix_row_stats(lrow, srow, mrow, gate_logit + row * 2, V, S, sh_ms, bc);
+  const float vmax = ms.vmax, vsum = ms.vsum, cmax = ms.cmax, csum = ms.csum, g0 = ms.g0, g1 = ms.g1;
   // P_j as head_fwd_kernel forms the probability of label j
   auto prob = [&](int j) {
     if (j < V) return g0 * (expf(Act<T>::ld(lrow + j) - vmax) / vsum);
@@ -553,6 +568,161 @@ __global__ void __launch_bounds__(kSampleThreads) pointer_mix_sample_kernel(
     length[row] += 1;
     lp_sum[row] += lp;
     if (tok == eos_id) finished[row] = 1;
+  }
+}
+
+// ------------------------------------------------------------------ one n-best beam step from the mixture
+// Slot rows r = b * K + k.  The slot state is double-buffered ([2][B*K] scalars, [2][B*K][T] histories): position
+// `pos` reads half pos & 1 and writes the other half, since a new slot's history is copied from a parent row that
+// another CTA may be rewriting.  status: 0 live, 1 finished (its token was <eos>), 2 inactive (before position 0).
+//   row stage     one CTA per live slot row: lp_j = log(clamp(P_j, 1e-10, 1)) of every vocabulary entry and unmasked
+//                 copy position; the row's K best by rank_key(lp, j) (lp descending, then j ascending) -> workspace.
+//                 Each thread keeps a sorted top K in registers over its strided indices, then K fixed-order block
+//                 maxima pop the heads, so the result is a pure function of the row.
+//   select stage  one CTA per commit: live slot i proposes its K row winners (i, j) with L = L_i + lp and n = n_i + 1,
+//                 finished slot i proposes itself once as j = C = V + S; score = L / powf((5 + n) / 6, alpha); the K
+//                 best by (score descending, then i * (C + 1) + j ascending) become new slots 0..K-1 in that order.
+// Within one parent row the score rises with lp (n is the same for every extension), so every winner of the select
+// stage is among its parent's row top K.
+constexpr int kBeamThreads = 256;   // = head_fwd_kernel's block (the same row statistics); >= kMaxBeam^2 candidates
+constexpr int kMaxBeam = 16;
+
+__device__ __forceinline__ float key_lp(uint64_t key) {          // inverse of rank_key's score bits
+  const uint32_t b = (uint32_t)(key >> 15);
+  return __uint_as_float((b & 0x80000000u) ? (b & 0x7FFFFFFFu) : ~b);
+}
+__device__ __forceinline__ int key_index(uint64_t key) { return 0x7FFF - (int)(key & 0x7FFFu); }
+__device__ __forceinline__ uint64_t key_max(uint64_t a, uint64_t b) { return a > b ? a : b; }
+__device__ __forceinline__ uint64_t key_min(uint64_t a, uint64_t b) { return a < b ? a : b; }
+// insert `x` into the descending list top[0..K) (entries from K on stay 0) -> the new top[K - 1]
+__device__ __forceinline__ uint64_t topk_insert(uint64_t (&top)[kMaxBeam], uint64_t x, int K) {
+  uint64_t last = ~0ull;                              // min over top[0..K) = top[K - 1], without a dynamic index
+#pragma unroll
+  for (int i = 0; i < kMaxBeam; ++i)
+    if (i < K) { const uint64_t hi = key_max(top[i], x); x = key_min(top[i], x); top[i] = hi; last = key_min(last, hi); }
+  return last;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kBeamThreads, 1) beam_row_kernel(
+    const T* __restrict__ logits, long ldl, const float* __restrict__ sc, const float* __restrict__ gate_logit,
+    const unsigned char* __restrict__ mem_mask, const unsigned char* __restrict__ status, uint64_t* __restrict__ row_top,
+    int K, int V, int S) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  __shared__ MaxSum sh_ms[8];
+  __shared__ float bc[4];
+  __shared__ uint64_t shk[8];
+  const long row = blockIdx.x;
+  if (status[row] != 0) return;                       // finished or inactive: the select stage reads nothing of it
+  const int b = (int)(row / K);
+  const T* lrow = logits + row * ldl;
+  const float* srow = sc + row * S;
+  const unsigned char* mrow = mem_mask + (long)b * S;
+  const MixRow ms = mix_row_stats(lrow, srow, mrow, gate_logit + row * 2, V, S, sh_ms, bc);
+
+  uint64_t top[kMaxBeam];                             // this thread's best keys, descending; 0 = empty
+#pragma unroll
+  for (int i = 0; i < kMaxBeam; ++i) top[i] = 0;
+  uint64_t thr = 0;                                   // top[K - 1]: the key a candidate has to beat
+  auto offer = [&](float p, int j) {
+    const uint64_t key = rank_key(logf(fminf(fmaxf(p, 1e-10f), 1.f)), j);   // lp = -nll of fira_pointer_mix_nll_fwd
+    if (key > thr) thr = topk_insert(top, key, K);
+  };
+  const int V8 = V >> 3;
+  for (int g = threadIdx.x; g < V8; g += blockDim.x) {
+    float x[8];
+    Act<T>::load8(lrow + (long)g * 8, x);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) offer(ms.g0 * (expf(x[i] - ms.vmax) / ms.vsum), g * 8 + i);
+  }
+  for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) offer(ms.g0 * (expf(Act<T>::ld(lrow + j) - ms.vmax) / ms.vsum), j);
+  for (int s = threadIdx.x; s < S; s += blockDim.x)
+    if (mrow[s]) offer(ms.g1 * (expf(srow[s] - ms.cmax) / ms.csum), V + s);
+
+  // block top K: K fixed-order maxima over the list heads; keys are distinct, so exactly one thread owns each maximum
+  for (int k = 0; k < K; ++k) {
+    const uint64_t m = block_reduce(top[0], shk, key_max);
+    if (m != 0 && top[0] == m) {
+#pragma unroll
+      for (int i = 0; i + 1 < kMaxBeam; ++i) top[i] = top[i + 1];
+      top[kMaxBeam - 1] = 0;
+    }
+    if (threadIdx.x == 0) row_top[row * K + k] = m;
+  }
+}
+
+__global__ void __launch_bounds__(kBeamThreads) beam_select_kernel(
+    const uint64_t* __restrict__ row_top, const int* __restrict__ copy_src, float alpha, int eos_id, int pad_id,
+    int* __restrict__ seq, int* __restrict__ raw, float* __restrict__ tok_lp, int* __restrict__ length,
+    float* __restrict__ lp_sum, float* __restrict__ score, unsigned char* __restrict__ status,
+    long* __restrict__ parent, int* __restrict__ next_tok, int Tn, int pos, int B, int K, int V, int S) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  __shared__ uint64_t sh_key[kBeamThreads];
+  __shared__ int s_from[kMaxBeam], s_j[kMaxBeam], s_tok[kMaxBeam];
+  __shared__ float s_lp[kMaxBeam], s_L[kMaxBeam], s_score[kMaxBeam];
+  const int b = blockIdx.x, C = V + S;
+  const long R = (long)B * K;
+  const long in = (pos & 1) ? R : 0, out = (pos & 1) ? 0 : R;     // row offsets of the read and the written half
+  const long base = (long)b * K;
+  if (threadIdx.x < K) { s_from[threadIdx.x] = threadIdx.x; s_j[threadIdx.x] = C; }   // unfilled slot: keeps itself
+
+  // candidate threadIdx.x = i * K + q: the q-th row winner of live slot i, or (q = 0) finished slot i itself
+  uint64_t mine = 0;
+  int i = 0, j = C;
+  float lp = 0.f, L = 0.f, sco = 0.f;
+  if (threadIdx.x < K * K) {
+    i = threadIdx.x / K;
+    const int q = threadIdx.x % K;
+    const long pr = in + base + i;
+    if (status[pr] == 0) {
+      const uint64_t c = row_top[(base + i) * K + q];
+      if (c != 0) {
+        lp = key_lp(c);
+        j = key_index(c);
+        L = lp_sum[pr] + lp;
+        const int n = length[pr];                     // tokens generated with this one: (length - 1) + 1
+        sco = L / powf((5.f + (float)n) / 6.f, alpha) + 0.f;           // + 0: -0 and +0 rank as one value
+        mine = 1;
+      }
+    } else if (status[pr] == 1 && q == 0) {
+      L = lp_sum[pr];
+      sco = score[pr] + 0.f;
+      mine = 1;
+    }
+    if (mine) mine = ((uint64_t)order_bits(sco) << 32) | (0xFFFFFFFFu - (uint32_t)(i * (C + 1) + j));
+  }
+  sh_key[threadIdx.x] = mine;
+  __syncthreads();
+  if (mine) {
+    int rank = 0;
+    for (int u = 0; u < K * K; ++u) rank += sh_key[u] > mine ? 1 : 0;
+    if (rank < K) {
+      s_from[rank] = i; s_j[rank] = j; s_lp[rank] = lp; s_L[rank] = L; s_score[rank] = sco;
+      s_tok[rank] = j < V ? j : (j < C ? copy_src[(long)b * S + (j - V)] : pad_id);
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < K) {
+    const int k = threadIdx.x;
+    const long pr = in + base + s_from[k], nr = out + base + k;
+    parent[base + k] = base + s_from[k];
+    if (s_j[k] == C) {                                // a finished slot carried unchanged
+      length[nr] = length[pr]; lp_sum[nr] = lp_sum[pr]; score[nr] = score[pr]; status[nr] = status[pr];
+      next_tok[base + k] = pad_id;
+    } else {
+      length[nr] = length[pr] + 1; lp_sum[nr] = s_L[k]; score[nr] = s_score[k];
+      status[nr] = s_tok[k] == eos_id ? 1 : 0;
+      next_tok[base + k] = s_tok[k];
+    }
+  }
+  // histories follow their parents; a grown slot gets its new token at column pos + 1
+  for (int e = threadIdx.x; e < K * Tn; e += blockDim.x) {
+    const int k = e / Tn, c = e % Tn;
+    const long src = (in + base + s_from[k]) * Tn + c, dst = (out + base + k) * Tn + c;
+    const bool grow = s_j[k] != C && c == pos + 1;
+    seq[dst] = grow ? s_tok[k] : seq[src];
+    raw[dst] = grow ? s_j[k] : raw[src];
+    tok_lp[dst] = grow ? s_lp[k] : tok_lp[src];
   }
 }
 
@@ -682,6 +852,31 @@ int fira_pointer_mix_sample(const void* logits, long ld_logits, const float* cop
       uniforms, temperature, top_k, top_p, eos_id, pad_id, next_tok, seq, raw, token_logprob, tok_mask, ld_out, pos,
       finished, length, logprob, N, V, S);)
   FIRA_CHECK_LAUNCH("fira_pointer_mix_sample");
+  return FIRA_OK;
+}
+
+int fira_pointer_mix_beam_step(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                               const unsigned char* mem_mask, const int* copy_src, float length_penalty, int eos_id,
+                               int pad_id, uint64_t* workspace, int* seq, int* raw, float* token_logprob, int* length,
+                               float* logprob, float* score, unsigned char* status, long* parent, int* next_tok,
+                               int T_len, int pos, int B, int K, int V, int S, int dtype, void* stream) {
+  FIRA_CHECK_ARG(B >= 0 && K >= 1 && K <= kMaxBeam && V >= K && S > 0 && V + S <= 0x7FFF, FIRA_ERR_SHAPE,
+                 "pointer_mix_beam_step: shape (B %d, K %d, V %d, S %d; 1 <= K <= 16, K <= V, V + S <= 32767)",
+                 B, K, V, S);
+  FIRA_CHECK_ARG(pos >= 0 && pos + 2 <= T_len, FIRA_ERR_SHAPE, "pointer_mix_beam_step: pos %d, T_len %d", pos, T_len);
+  FIRA_CHECK_ARG(length_penalty >= 0.f && length_penalty <= 3.4e38f, FIRA_ERR_ARG,
+                 "pointer_mix_beam_step: length_penalty %g", (double)length_penalty);
+  FIRA_CHECK_ARG(fira_aligned16(logits) && ld_logits % 8 == 0, FIRA_ERR_ALIGN,
+                 "pointer_mix_beam_step: logits must be 16-byte aligned with a leading dimension that is a multiple of 8");
+  if (B == 0) return FIRA_OK;
+  DISPATCH_T(dtype, launch_k(beam_row_kernel<T>, dim3((unsigned)(B * K)), dim3(kBeamThreads), 0, (cudaStream_t)stream,
+      (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, (const unsigned char*)status + (pos & 1) * (long)B * K,
+      workspace, K, V, S);)
+  FIRA_CHECK_LAUNCH("fira_pointer_mix_beam_step (rows)");
+  launch_k(beam_select_kernel, dim3((unsigned)B), dim3(kBeamThreads), 0, (cudaStream_t)stream, (const uint64_t*)workspace,
+           copy_src, length_penalty, eos_id, pad_id, seq, raw, token_logprob, length, logprob, score, status, parent,
+           next_tok, T_len, pos, B, K, V, S);
+  FIRA_CHECK_LAUNCH("fira_pointer_mix_beam_step (select)");
   return FIRA_OK;
 }
 

@@ -13,26 +13,23 @@ u comes from Philox4x32-7 keyed by `seed` with the counter (first_index + b, n, 
 on its position in the dataset, not on the batch it was decoded in or the GPU count.  The emitted log-probability is
 log(clamp(P_j, 1e-10, 1)) whatever temperature, top_k and top_p are: it is -nll of the training loss for label j.
 
-Per batch the encoder, the cross-attention K/V of the memory and LinearSource(memory) run once.  The N samples of a
-commit are the N query rows of an incremental.IncrementalDecoder.  Per position: newest decoder row -> out_fc ->
-target projection and gate -> copy scores -> fira_pointer_mix_sample, which also writes the next input token
-straight into the decoder's token buffer and keeps each row's finished flag, length and log-probability sum.  A
-position is captured once into a CUDA graph and replayed for every later batch of the same shape; the loop reads
-back nothing but an all-finished flag, once every 8 positions.
+The loop is decode_loop.PositionLoop: per batch the encoder, the cross-attention K/V of the memory and
+LinearSource(memory) run once, and the N samples of a commit are the N query rows of an incremental.IncrementalDecoder.
+Per position: newest decoder row -> out_fc -> target projection and gate -> copy scores -> fira_pointer_mix_sample,
+which also writes the next input token straight into the decoder's token buffer and keeps each row's finished flag,
+length and log-probability sum.  A position is captured once into a CUDA graph and replayed for every later batch of
+the same shape; the loop reads back nothing but an all-finished flag, once every 8 positions.
 """
 import ctypes
-import weakref
 from typing import NamedTuple
 
 import torch
 
 from . import ops
 from ._lib import call
-from .incremental import IncrementalDecoder
+from .decode_loop import PositionLoop, loop_for
 
-D = ops.D
 MAX_SAMPLES = 32          # the N samples of a commit are its query rows in fira_attn_fwd / fira_copy_scores_fwd (<= 32)
-POLL_EVERY = 8            # positions between two reads of the all-finished flag
 
 
 class Samples(NamedTuple):
@@ -67,49 +64,25 @@ def check_args(num_samples, temperature, top_k, top_p, seed, first_index, tar_le
         raise ValueError(f"tar_len must be an integer >= 2, got {tar_len!r}")
 
 
-def _weights_key(model):
-    ps = list(model.parameters())
-    return (getattr(model.decoder, "weights_epoch", 0),) + tuple(p._version for p in ps) + tuple(p.data_ptr() for p in ps)
-
-
-class _Sampler:
-    """Static buffers and captured position graphs of one (model, B, N, tar_len, S, precision)."""
+class _Sampler(PositionLoop):
+    """The sampler's state on top of the shared position loop: seed, first index and every row's draws."""
 
     def __init__(self, model, B, N, T, S):
-        self.model, self.B, self.N, self.T, self.S = model, B, N, T, S
-        self.inc = IncrementalDecoder(model.decoder, B, N, T, S, graphs=False)   # its launches go into our graphs
-        self.pr = ops.Prec(self.inc.be.bf16)
-        dev = model.out_fc.weight.device
-        R = self.R = B * N
-        tdt = self.inc.be.tdt
+        super().__init__(model, B, N, T, S)
+        R, dev = self.R, self.dev
         i32 = dict(dtype=torch.int32, device=dev)
         f32 = dict(dtype=torch.float32, device=dev)
-        self.V = model.vocab_size
-        self.ldl = ops._ld_logits(self.V)
         self.seed = torch.zeros(1, dtype=torch.int64, device=dev)      # read by the kernel as uint64
         self.first = torch.zeros(1, **i32)
-        self.mem_mask = torch.zeros((B, S), dtype=torch.uint8, device=dev)
-        self.copy_src = torch.zeros((B, S), **i32)
-        self.src = torch.empty((B * S, D), dtype=tdt, device=dev)
-        self.logits = torch.empty((R, self.ldl), dtype=tdt, device=dev)
-        self.tgt = torch.empty((R, D), dtype=tdt, device=dev)
-        self.gl = torch.empty((R, 2), **f32)
-        self.sc = torch.empty((B, N, S), **f32)
         self.seq = torch.empty((R, T), **i32)
         self.raw = torch.empty((R, T), **i32)
         self.tlp = torch.empty((R, T), **f32)
         self.finished = torch.empty(R, dtype=torch.uint8, device=dev)
         self.length = torch.empty(R, **i32)
         self.lp = torch.empty(R, **f32)
-        self.graphs = {}
 
     def start(self, memory, mem_mask, copy_src, seed, first_index, start_id, pad_id):
-        inc = self.inc
-        inc.start(memory, mem_mask)
-        mem2 = memory.contiguous().to(inc.be.tdt).view(self.B * self.S, D)
-        self.pr.linear(mem2, self.model.copy_net.LinearSource.weight, out=self.src)     # once per batch, not per row
-        self.mem_mask.copy_(mem_mask)
-        self.copy_src.copy_(copy_src)
+        super().start(memory, mem_mask, copy_src, start_id, pad_id)
         self.seed.fill_(seed - 2 ** 64 if seed >= 2 ** 63 else seed)
         self.first.fill_(first_index)
         self.seq.fill_(pad_id)
@@ -120,37 +93,19 @@ class _Sampler:
         self.finished.zero_()
         self.length.fill_(1)
         self.lp.zero_()
-        inc.tok[:self.R].fill_(start_id)
-        inc.tok_mask[:, 0].fill_(int(start_id != pad_id))
+
+    def unfinished(self, t):
+        return self.finished.eq(0).any()
 
     def position(self, t, temperature, top_k, top_p, eos_id, pad_id):
         """Draw position t + 1 from decoder row t (every launch on the current stream: capturable)."""
-        m, pr, B, N, S, R = self.model, self.pr, self.B, self.N, self.S, self.R
-        cn = m.copy_net
-        x = self.inc.advance(t)                                                  # [R, D]
-        pr.linear(x, m.out_fc.weight, m.out_fc.bias, out=self.logits, ld_out=self.ldl)
-        pr.linear(x, cn.LinearTarget.weight, out=self.tgt)
-        ops.linear(x.float() if pr.bf16 else x, cn.LinearProb.weight, cn.LinearProb.bias, out=self.gl)   # fp32 gate
-        st = ops._stream()
+        self.head(t)
         p = ops._ptr
-        call("fira_copy_scores_fwd", p(self.src), p(self.tgt), p(cn.LinearRes.weight), p(cn.LinearRes.bias),
-             p(self.mem_mask), None, p(self.sc), B, N, S, D, pr.code, st)
         call("fira_pointer_mix_sample", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
              p(self.copy_src), p(self.seed), p(self.first), None, float(temperature), int(top_k), float(top_p),
              int(eos_id), int(pad_id), p(self.inc.tok), p(self.seq), p(self.raw), p(self.tlp), p(self.inc.tok_mask),
-             self.T, t, p(self.finished), p(self.length), p(self.lp), B, N, self.V, S, pr.code, st)
-
-
-_SAMPLERS = weakref.WeakKeyDictionary()          # model -> {(B, N, T, S, precision): (weights key, _Sampler)}
-
-
-def _sampler(model, B, N, T, S):
-    store = _SAMPLERS.setdefault(model, {})
-    key = (B, N, T, S, model.precision)
-    wkey = _weights_key(model)
-    if key not in store or store[key][0] != wkey:       # changed weights: fresh operand copies and graphs
-        store[key] = (wkey, _Sampler(model, B, N, T, S))
-    return store[key][1]
+             self.T, t, p(self.finished), p(self.length), p(self.lp), self.B, self.N, self.V, self.S, self.pr.code,
+             ops._stream())
 
 
 @torch.no_grad()
@@ -171,22 +126,9 @@ def sample(model, sou, mark, ast_change, edge, sub_token, *, num_samples=1, temp
     S = memory.shape[1]
     mem_mask = torch.cat((sou != pad_id, sub_token != 0), dim=1)
     copy_src = torch.cat((sou, sub_token), dim=1)                                       # copy position -> vocabulary id
-    st = _sampler(model, B, N, T, S)
+    st = loop_for(_Sampler, model, B, N, T, S)
     st.start(memory, mem_mask, copy_src, seed, first_index, start_id, pad_id)
-    cfg = (float(temperature), int(top_k), float(top_p), int(eos_id), int(pad_id))
-    for t in range(T - 1):
-        if t and t % POLL_EVERY == 0 and not bool(st.finished.eq(0).any()):
-            break
-        g = st.graphs.get((cfg, t))
-        if g is not None:
-            g.replay()
-            continue
-        st.position(t, *cfg)                               # this batch's result (and the warm-up of a capture) ...
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):                          # ... and the same launches recorded for later batches
-            st.position(t, *cfg)
-        st.graphs[(cfg, t)] = g
+    st.run((float(temperature), int(top_k), float(top_p), int(eos_id), int(pad_id)))
     shape = (B, N, T)
     return Samples(st.seq.view(shape).long(), st.raw.view(shape).long(), st.length.view(B, N).long(),
                    st.lp.view(B, N).clone(), st.tlp.view(shape).clone())

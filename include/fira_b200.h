@@ -274,6 +274,27 @@ int fira_pointer_mix_sample(const void* logits, long ld_logits, const float* cop
                             unsigned char* tok_mask, long ld_out, int pos, unsigned char* finished, int* length,
                             float* logprob, int B, int N, int V, int S, int dtype, void* stream);
 
+/* ---- one n-best beam step from the same mixture (fira_icse_b200/beam.py nbest).  Rows are (commit b, slot k), B*K
+ *      of them: logits [B*K, ld_logits], copy_scores [B, K, S], gate_logits [B*K, 2], mem_mask / copy_src [B, S].
+ *      Slot state is double-buffered: seq / raw / token_logprob [2, B*K, T_len], length / logprob / score / status
+ *      [2, B*K]; position `pos` reads half pos & 1 and writes half 1 - (pos & 1) (a slot's new history comes from
+ *      another row).  status: 0 live, 1 finished, 2 inactive (slots 1..K-1 before position 0).  length counts <start>.
+ *      Rule: lp_j = log(clamp(P_j, 1e-10, 1)) (= -nll of fira_pointer_mix_nll_fwd for label j) for every vocabulary
+ *      entry and every unmasked copy position; a live slot i proposes (i, j) with L = logprob_i + lp_j (fp32) and
+ *      n = length_i tokens generated, a finished slot proposes itself once as j = C = V + S, an inactive slot nothing;
+ *      score = L / powf((5 + n) / 6, length_penalty); the K best by (score descending, then i * (C + 1) + j
+ *      ascending) become slots 0..K-1 in that order.  Two launches: per live row its top K (lp, j) into workspace
+ *      [B*K, K] (uint64 rank keys, caller-owned), then per commit the merge.  A grown slot writes its parent's history
+ *      with column pos + 1 = (token, j, lp_j) (token = j, or copy_src[b, j - V] for a copy), length + 1, logprob L,
+ *      its score, status 1 on eos_id; a carried finished slot copies its state unchanged.  Every slot writes
+ *      parent[b*K + k] = b*K + i (int64, for the caller's cache reorder) and next_tok[b*K + k] = its token (pad_id
+ *      when carried).  1 <= K <= 16, K <= V, V + S <= 32767, length_penalty >= 0, 0 <= pos <= T_len - 2. */
+int fira_pointer_mix_beam_step(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                               const unsigned char* mem_mask, const int* copy_src, float length_penalty, int eos_id,
+                               int pad_id, uint64_t* workspace, int* seq, int* raw, float* token_logprob, int* length,
+                               float* logprob, float* score, unsigned char* status, long* parent, int* next_tok,
+                               int T_len, int pos, int B, int K, int V, int S, int dtype, void* stream);
+
 /* ---- HOST-side batch preparation (CPU only: every pointer below is HOST memory, there is no stream).
  *
  * fira_host_build_adjacency: the commit graph of Dataset.py:220-294 + process_edge (Dataset.py:346-357).

@@ -21,6 +21,10 @@ beam search ranking.  Differences, all below the module surface:
     order, `<log-probability>\\t<message>`; prints the mean sentence BLEU over all samples).  Sampling parameters:
     FIRA_SAMPLES (default 3), FIRA_TEMPERATURE (1.0), FIRA_TOP_K (0 = off), FIRA_TOP_P (1.0 = off), FIRA_SEED (0).
     A commit's samples depend on the seed and its position in the test split only, so sharded runs draw the same.
+    FIRA_DECODE=nbest: log-space beam search with length normalisation (fira_icse_b200.beam.nbest) ->
+    OUTPUT/output_fira_nbest: FIRA_BEAM consecutive lines per commit in test order, best first,
+    `<score>\t<log-probability>\t<message>`; FIRA_LENGTH_PENALTY (default 0 = rank by log-probability) sets the
+    penalty alpha of score = logprob / ((5 + n) / 6) ** alpha; prints the mean sentence BLEU of the top hypothesis.
 """
 import json
 import os
@@ -34,7 +38,7 @@ from torch.optim import Adam
 from torch.utils.data import DataLoader
 
 from fira_icse_b200 import TransModel
-from fira_icse_b200.beam import beam_search, best_sequences
+from fira_icse_b200.beam import beam_search, best_sequences, nbest
 from fira_icse_b200.bleu import sentence_bleu_method2
 from fira_icse_b200.data import PackedBatchLoader, TransDataset, batch_to_device, collate_packed
 from fira_icse_b200.engine import GraphedTrainStep
@@ -271,6 +275,38 @@ def sample_test(model, test_loader, g, test_index, dev_, first_index, out_path="
     return bleus / max(1, total * n)
 
 
+def nbest_test(model, test_loader, g, test_index, dev_, out_path="OUTPUT/output_fira_nbest"):
+    """n-best beam search over the test split: FIRA_BEAM lines `<score>\t<log-prob>\t<message>` per commit, best first."""
+    vocab, r_vocab, var_maps = g["vocab"], g["r_vocab"], g["var_maps"]
+    K = args.beam_size
+    alpha = float(os.environ.get("FIRA_LENGTH_PENALTY", 0.0))
+    model.eval()
+    total, bleus = 0, 0.0
+    with open(out_path, 'w') as f:
+        for batch in test_loader:
+            b = batch_to_device(batch, dev_)
+            out = nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=K, length_penalty=alpha, tar_len=args.tar_len,
+                        start_id=vocab['<start>'], eos_id=vocab['<eos>'], pad_id=vocab['<pad>'])
+            seq, length = out.seq.cpu().numpy(), out.length.cpu().numpy()
+            score, logprob = out.score.cpu().numpy(), out.logprob.cpu().numpy()
+            tar = batch[1].numpy()
+            bleu_batch = 0.0
+            for i in range(len(seq)):
+                ref = tar[i].tolist()
+                ref = [r_vocab[x] for x in ref[1:ref.index(vocab['<eos>'])]]
+                for k in range(K):
+                    hyp = ids_to_text(seq[i, k][:length[i, k]].tolist(), r_vocab)
+                    if k == 0:
+                        bl = sentence_bleu_method2([ref], hyp)
+                        bleus += bl; bleu_batch += bl
+                    f.write('%.6f\t%.6f\t%s\n' % (score[i, k], logprob[i, k],
+                                                   ' '.join(deanonymise(hyp, var_maps[test_index[total + i]]))))
+            f.flush()
+            total += len(seq)
+            print("data: %d/%d bleu: %f" % (total, len(test_loader.dataset), bleu_batch / len(seq)))
+    return bleus / max(1, total)
+
+
 def main_test():
     dev_ = device()
     g = load_globals()
@@ -289,8 +325,11 @@ def main_test():
     elif decode == "sample":
         out = "OUTPUT/output_fira_samples" if WORLD == 1 else f"OUTPUT/output_fira_samples.part{RANK:02d}"
         bleu = sample_test(model, test_loader, g, all_index['test'][lo:hi], dev_, lo, out)
+    elif decode == "nbest":
+        out = "OUTPUT/output_fira_nbest" if WORLD == 1 else f"OUTPUT/output_fira_nbest.part{RANK:02d}"
+        bleu = nbest_test(model, test_loader, g, all_index['test'][lo:hi], dev_, out)
     else:
-        raise SystemExit("FIRA_DECODE must be 'beam' or 'sample'")
+        raise SystemExit("FIRA_DECODE must be 'beam', 'sample' or 'nbest'")
     print("mean sentence bleu: %f" % bleu)
 
 

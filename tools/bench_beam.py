@@ -7,7 +7,8 @@ reference's own loop was timed on in BASELINE.md (72 s for 32 commits on CPU).  
 (batch, beam) configuration; timing with CUDA events around whole batches, inputs resident on the device.
 
     python tools/bench_beam.py [--batches 20,128] [--beams 3,5] [--precision fp32|bf16] [--reps 3]
-                               [--modes full,incremental,graph,sample]   (sample: N = the beam width)
+                               [--modes full,incremental,graph,sample,nbest]   (sample: N = the beam width;
+                               nbest: beam.nbest, log-space n-best beam search with length_penalty 0)
 """
 import argparse
 import json
@@ -33,7 +34,7 @@ def main():
     import bench
     import fira_icse_b200 as F
     from fira_icse_b200 import _lib
-    from fira_icse_b200.beam import beam_search
+    from fira_icse_b200.beam import beam_search, nbest
     from fira_icse_b200.sample import sample
     dev = torch.device("cuda", 0)
     torch.manual_seed(0)
@@ -48,19 +49,22 @@ def main():
                 if mode == "sample":                                 # N = the beam width, default T / k / p
                     return sample(model, b[0], b[3], b[4], b[5], b[7], num_samples=K, tar_len=30, start_id=1, eos_id=2,
                                   pad_id=0)
+                if mode == "nbest":
+                    return nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=K, tar_len=30, start_id=1, eos_id=2,
+                                 pad_id=0)
                 return beam_search(model, b[0], b[3], b[4], b[5], b[7], beam_size=K, tar_len=30, start_id=1, eos_id=2,
                                    pad_id=0, mode=mode)
             ref = run()                                              # warm-up (lazy CUDA state, graph capture)
             if mode == "full":
                 ref_full = ref
-            same = bool(torch.equal(ref[0], ref_full[0])) if "full" in a.modes.split(",") and mode != "sample" else None
+            same = bool(torch.equal(ref[0], ref_full[0])) if "full" in a.modes.split(",") and mode not in ("sample", "nbest") else None
             torch.cuda.synchronize()
             n0 = _lib.LAUNCH_COUNT
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             for _ in range(a.reps):
                 out = run()
-            length = out[2] if mode == "sample" else out[1]
+            length = out.length if mode in ("sample", "nbest") else out[1]
             e1.record()
             torch.cuda.synchronize()
             ms = e0.elapsed_time(e1) / a.reps
@@ -71,7 +75,8 @@ def main():
                 "c_abi_calls_per_batch": (_lib.LAUNCH_COUNT - n0) // a.reps,
                 "note": "encoder once per batch; full = 30-position decoder re-run per step over all live beams, "
                         "incremental = newest row against K/V caches, graph = the same as CUDA-graph replays, "
-                        "sample = beam-width seeded samples per commit (T = 1, no top-k / top-p), one graph per position"}),
+                        "sample = beam-width seeded samples per commit (T = 1, no top-k / top-p), one graph per position, "
+                        "nbest = log-space n-best beam search (length_penalty 0), one graph per position"}),
                   flush=True)
 
 
