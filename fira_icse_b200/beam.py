@@ -9,9 +9,10 @@ What is kept from the reference:
     through the commit's own diff / sub-token ids; the loop stops when every beam of every sample ended.
 What changes: the encoder memory is computed once, ALL live beams go through the decoder in one
 batched call, and only position `step` is pushed through the output head (the reference recomputes the
-full 30 x 25,020 distribution per beam and reads one row of it).  mode="incremental" / "graph" evaluates
-only the newest decoder row per step against cached keys/values (incremental.IncrementalDecoder; "graph"
-replays each step's kernels as a CUDA graph); mode="full" re-runs the 30-position decoder every step.
+full 30 x 25,020 distribution per beam and reads one row of it).  mode="graph" evaluates only the newest decoder row
+per step against cached keys/values (incremental.IncrementalDecoder), replaying each step's kernels as a CUDA graph
+(the first batch of a shape runs them eagerly and captures them); mode="full" re-runs the 30-position decoder every
+step, and is the only mode for beam sizes above 32 (the incremental cross-attention has at most 32 query rows).
 The default comes from FIRA_BEAM_MODE (default "graph").  Ranking keeps the reference's candidate layout; only
 the first `beam_size` entries of its descending sort are ever used, so the sort is a device top-k.
 
@@ -31,12 +32,11 @@ hypotheses with their scores (`beam_search` stays the reference-exact default):
 A vocabulary candidate and a copy candidate that spell the same word stay two candidates (as in the reference), so an
 n-best list can hold the same message twice.
 
-The loop is decode_loop.PositionLoop (the sampler's): per position the head, then fira_pointer_mix_beam_step (per
-live slot row its top K, then per commit the merge, writing the new slots, their parents and the next tokens), the
-KV-cache reorder to the parents and the pad mask of the next tokens, all in one captured CUDA graph.  Slot state is
-double-buffered by the parity of the position (a slot's new history comes from another row).
+The loop is decode_loop.PositionLoop (described there); a position ends with fira_pointer_mix_beam_step (per live slot
+row its top K, then per commit the merge, writing the new slots, their parents and the next tokens), the KV-cache
+reorder to the parents and the pad mask of the next tokens.  Slot state is double-buffered by the parity of the
+position (a slot's new history comes from another row).
 """
-import ctypes
 import math
 import os
 import weakref
@@ -46,7 +46,7 @@ import torch
 
 from . import ops
 from ._lib import call
-from .decode_loop import PositionLoop, loop_for
+from .decode_loop import PositionLoop, _f32, check_tar_len, encode, is_int, loop_for
 from .incremental import IncrementalDecoder
 
 MAX_BEAM = 16             # the row stage keeps a per-thread top K in registers
@@ -55,12 +55,12 @@ MAX_BEAM = 16             # the row stage keeps a per-thread top K in registers
 _DECODERS = weakref.WeakKeyDictionary()          # model -> {(B, K, ...): IncrementalDecoder}
 
 
-def _incremental_decoder(model, B, K, tar_len, mem_len, graphs):
-    """IncrementalDecoder instances (static buffers, captured graphs) are kept per model and (B, K, mode)."""
+def _incremental_decoder(model, B, K, tar_len, mem_len):
+    """IncrementalDecoder instances (static buffers, captured graphs) are kept per model and shape."""
     store = _DECODERS.setdefault(model, {})
-    key = (B, K, tar_len, mem_len, bool(graphs), model.precision)
+    key = (B, K, tar_len, mem_len, model.precision)
     if key not in store:
-        store[key] = IncrementalDecoder(model.decoder, B, K, tar_len, mem_len, graphs=graphs)
+        store[key] = IncrementalDecoder(model.decoder, B, K, tar_len, mem_len, graphs=True)
     return store[key]
 
 
@@ -69,16 +69,13 @@ def beam_search(model, sou, mark, ast_change, edge, sub_token, *, beam_size=3, t
                 pad_id=0, mode=None):
     """-> (sequences [B, beam, tar_len] int64 padded with pad_id, lengths [B, beam], probs [B, beam])."""
     mode = mode or os.environ.get("FIRA_BEAM_MODE", "graph")
-    if mode not in ("full", "incremental", "graph"):
-        raise ValueError("beam search mode must be 'full', 'incremental' or 'graph'")
-    dev = model.out_fc.weight.device
-    sou, mark, ast_change, sub_token = (t.to(dev) for t in (sou, mark, ast_change, sub_token))
-    B, K = sou.shape[0], beam_size
-    V, n_code = model.vocab_size, sou.shape[1]
-    C = V + n_code + sub_token.shape[1]
-    memory = model.encoder.encode_memory(sou, mark, ast_change, edge, sub_token)        # once per batch
-    mem_mask = torch.cat((sou != pad_id, sub_token != 0), dim=1)
-    copy_src = torch.cat((sou, sub_token), dim=1)                                       # copy id -> vocabulary id
+    if mode not in ("full", "graph"):
+        raise ValueError("beam search mode must be 'full' or 'graph'")
+    memory, mem_mask, copy_src = encode(model, sou, mark, ast_change, edge, sub_token, pad_id)
+    dev = memory.device
+    B, K = memory.shape[0], beam_size
+    V = model.vocab_size
+    C = V + copy_src.shape[1]
 
     seq = torch.full((B, K, tar_len), pad_id, dtype=torch.long, device=dev)
     seq[:, :, 0] = start_id
@@ -87,8 +84,8 @@ def beam_search(model, sou, mark, ast_change, edge, sub_token, *, beam_size=3, t
     prob[:, 0] = 1.0
     ar = torch.arange(B, device=dev)
     inc = None
-    if mode != "full":
-        inc = _incremental_decoder(model, B, K, tar_len, memory.shape[1], mode == "graph").start(memory, mem_mask)
+    if mode == "graph":
+        inc = _incremental_decoder(model, B, K, tar_len, memory.shape[1]).start(memory, mem_mask)
 
     for step in range(tar_len - 1):
         last = seq.gather(2, (length - 1).unsqueeze(-1)).squeeze(-1)
@@ -155,14 +152,8 @@ class Hypotheses(NamedTuple):
     finished: torch.Tensor        # [B, K] bool: the hypothesis ends with <eos>
 
 
-def _f32(x):
-    return ctypes.c_float(x).value
-
-
 def check_nbest_args(beam_size, length_penalty, tar_len):
     """ValueError for any parameter nbest cannot honour (called before any device work)."""
-    def is_int(v):
-        return isinstance(v, int) and not isinstance(v, bool)
     if not is_int(beam_size) or not 1 <= beam_size <= MAX_BEAM:
         raise ValueError(f"beam_size must be an integer in [1, {MAX_BEAM}], got {beam_size!r}")
     if (isinstance(length_penalty, bool) or not isinstance(length_penalty, (int, float))
@@ -173,37 +164,22 @@ def check_nbest_args(beam_size, length_penalty, tar_len):
 
 
 class _NBest(PositionLoop):
-    """Double-buffered slot state ([2, B*K, ...], half t & 1 read at position t) on top of the shared position loop."""
+    """Double-buffered slot state (half t & 1 read at position t; status 2: inactive) on top of the shared position
+    loop, with each slot's score, its parent row and the row stage's workspace."""
+
+    halves = 2
 
     def __init__(self, model, B, K, T, S):
         super().__init__(model, B, K, T, S)
         R, dev = self.R, self.dev
-        i32 = dict(dtype=torch.int32, device=dev)
-        f32 = dict(dtype=torch.float32, device=dev)
-        self.seq = torch.empty((2, R, T), **i32)
-        self.raw = torch.empty((2, R, T), **i32)
-        self.tlp = torch.empty((2, R, T), **f32)
-        self.length = torch.empty((2, R), **i32)
-        self.lp = torch.empty((2, R), **f32)
-        self.score = torch.empty((2, R), **f32)
-        self.status = torch.empty((2, R), dtype=torch.uint8, device=dev)      # 0 live, 1 finished, 2 inactive
+        self.score = torch.empty((2, R), dtype=torch.float32, device=dev)
         self.parent = torch.empty(R, dtype=torch.int64, device=dev)
         self.work = torch.empty(R * K, dtype=torch.int64, device=dev)         # per-row top K rank keys (uint64)
 
     def start(self, memory, mem_mask, copy_src, start_id, pad_id):
         super().start(memory, mem_mask, copy_src, start_id, pad_id)
-        for x in (self.seq, self.raw):           # half 1 is written whole at position 0 (its columns > 1 from half 0)
-            x[0].fill_(pad_id)
-            x[0, :, 0] = start_id
-        self.tlp[0].zero_()
-        self.length[0].fill_(1)
-        self.lp[0].zero_()
         self.score[0].zero_()
-        self.status[0].view(self.B, self.N).fill_(2)
-        self.status[0].view(self.B, self.N)[:, 0] = 0          # beam 0 has probability 1, the others 0
-
-    def unfinished(self, t):
-        return self.status[t & 1].eq(0).any()
+        self.status[0].view(self.B, self.N)[:, 1:] = 2          # beam 0 has probability 1, the others 0
 
     def position(self, t, length_penalty, eos_id, pad_id):
         """Slots of position t + 1 from decoder row t (every launch on the current stream: capturable)."""
@@ -226,19 +202,11 @@ def nbest(model, sou, mark, ast_change, edge, sub_token, *, beam_size=3, length_
     check_nbest_args(beam_size, length_penalty, tar_len)
     if beam_size > model.vocab_size:
         raise ValueError(f"beam_size {beam_size} exceeds the vocabulary ({model.vocab_size})")
-    if tar_len > model.decoder.pos_encode.shape[0]:
-        raise ValueError(f"tar_len {tar_len} exceeds the decoder's {model.decoder.pos_encode.shape[0]} positions")
-    dev = model.out_fc.weight.device
-    sou, mark, ast_change, sub_token = (t.to(dev) for t in (sou, mark, ast_change, sub_token))
-    B, K, T = sou.shape[0], beam_size, tar_len
-    memory = model.encoder.encode_memory(sou, mark, ast_change, edge, sub_token)        # once per batch
-    S = memory.shape[1]
-    mem_mask = torch.cat((sou != pad_id, sub_token != 0), dim=1)
-    copy_src = torch.cat((sou, sub_token), dim=1)                                       # copy position -> vocabulary id
-    st = loop_for(_NBest, model, B, K, T, S)
+    check_tar_len(model, tar_len)
+    memory, mem_mask, copy_src = encode(model, sou, mark, ast_change, edge, sub_token, pad_id)
+    B, S = memory.shape[:2]
+    st = loop_for(_NBest, model, B, beam_size, tar_len, S)
     st.start(memory, mem_mask, copy_src, start_id, pad_id)
-    h = st.run((float(length_penalty), int(eos_id), int(pad_id))) & 1
-    shape = (B, K, T)
-    return Hypotheses(st.seq[h].view(shape).long(), st.raw[h].view(shape).long(), st.length[h].view(B, K).long(),
-                      st.lp[h].view(B, K).clone(), st.score[h].view(B, K).clone(), st.tlp[h].view(shape).clone(),
-                      st.status[h].view(B, K) == 1)
+    t = st.run((float(length_penalty), int(eos_id), int(pad_id)))
+    seq, raw, length, lp, tlp, status = st.slots(t)
+    return Hypotheses(seq, raw, length, lp, st.score[t & 1].view(B, beam_size).clone(), tlp, status == 1)

@@ -1,34 +1,59 @@
-"""The on-device decoding loop shared by seeded sampling (sample.py) and n-best beam search (beam.nbest).
+"""The on-device decoding loop shared by seeded sampling (sample.py) and n-best beam search (beam.nbest), and the batch
+front end every decoder shares (`encode`, also used by beam.beam_search).
 
 Per batch the encoder, the cross-attention K/V of the memory and LinearSource(memory) run once (`start`).  The N rows
 of a commit (samples or beam slots) are the N query rows of an incremental.IncrementalDecoder.  Per position:
 newest decoder row -> out_fc -> target projection and gate -> copy scores (`head`), then the decoder's own kernel,
-which writes the next input tokens straight into the decoder's token buffer (`position`, defined by each decoder).
-A position is captured once into a CUDA graph and replayed for every later batch of the same shape; the loop reads
-back nothing but an all-finished flag, once every POLL_EVERY positions.
+which writes the next input tokens straight into the decoder's token buffer and keeps every row's slot state
+(`position`, defined by each decoder).  A position is captured once into a CUDA graph and replayed for every later
+batch of the same shape; the loop reads back nothing but an all-finished flag, once every POLL_EVERY positions.
 """
+import ctypes
 import weakref
 
 import torch
 
 from . import ops
 from ._lib import call
-from .incremental import IncrementalDecoder
+from .incremental import IncrementalDecoder, replay_or_capture, weights_key
 
 D = ops.D
 POLL_EVERY = 8            # positions between two reads of the all-finished flag
 
 
-def _weights_key(model):
-    ps = list(model.parameters())
-    return (getattr(model.decoder, "weights_epoch", 0),) + tuple(p._version for p in ps) + tuple(p.data_ptr() for p in ps)
+def _f32(x):
+    return ctypes.c_float(x).value
+
+
+def is_int(v):
+    return isinstance(v, int) and not isinstance(v, bool)
+
+
+def check_tar_len(model, tar_len):
+    """ValueError when the decoder has fewer than tar_len positions (called before any device work)."""
+    if tar_len > model.decoder.pos_encode.shape[0]:
+        raise ValueError(f"tar_len {tar_len} exceeds the decoder's {model.decoder.pos_encode.shape[0]} positions")
+
+
+def encode(model, sou, mark, ast_change, edge, sub_token, pad_id):
+    """Encoder memory [B, S, D] on the model's device, once per batch, with the copy mask mem_mask [B, S] (bool) and
+    copy_src [B, S] (copy position -> vocabulary id)."""
+    dev = model.out_fc.weight.device
+    sou, mark, ast_change, sub_token = (t.to(dev) for t in (sou, mark, ast_change, sub_token))
+    memory = model.encoder.encode_memory(sou, mark, ast_change, edge, sub_token)
+    mem_mask = torch.cat((sou != pad_id, sub_token != 0), dim=1)
+    copy_src = torch.cat((sou, sub_token), dim=1)
+    return memory, mem_mask, copy_src
 
 
 class PositionLoop:
-    """Static buffers and captured position graphs of one (model, B, N, tar_len, S, precision).
+    """Static buffers, slot state and captured position graphs of one (model, B, N, tar_len, S, precision).
 
-    Subclasses define position(t, *cfg) (head(t), then their own launches; every launch on the current stream) and
-    unfinished(t) (a device bool: some row still decodes after t positions)."""
+    Slot state: seq, raw, tlp [halves, R, T] and length, lp, status [halves, R] (status 0 live, 1 finished); position t
+    reads half t % halves.  Subclasses set `halves` and define position(t, *cfg) (head(t), then their own launches;
+    every launch on the current stream)."""
+
+    halves = 1
 
     def __init__(self, model, B, N, T, S):
         self.model, self.B, self.N, self.T, self.S = model, B, N, T, S
@@ -46,6 +71,15 @@ class PositionLoop:
         self.tgt = torch.empty((R, D), dtype=tdt, device=dev)
         self.gl = torch.empty((R, 2), dtype=torch.float32, device=dev)
         self.sc = torch.empty((B, N, S), dtype=torch.float32, device=dev)
+        H = self.halves
+        i32 = dict(dtype=torch.int32, device=dev)
+        f32 = dict(dtype=torch.float32, device=dev)
+        self.seq = torch.empty((H, R, T), **i32)
+        self.raw = torch.empty((H, R, T), **i32)
+        self.tlp = torch.empty((H, R, T), **f32)
+        self.length = torch.empty((H, R), **i32)
+        self.lp = torch.empty((H, R), **f32)
+        self.status = torch.empty((H, R), dtype=torch.uint8, device=dev)
         self.graphs = {}
 
     def start(self, memory, mem_mask, copy_src, start_id, pad_id):
@@ -57,6 +91,24 @@ class PositionLoop:
         self.copy_src.copy_(copy_src)
         inc.tok[:self.R].fill_(start_id)
         inc.tok_mask[:, 0].fill_(int(start_id != pad_id))
+        for x in (self.seq, self.raw):        # n-best's half 1 is written whole at position 0 (columns > 1 from half 0)
+            x[0].fill_(pad_id)
+            x[0, :, 0] = start_id
+        self.tlp[0].zero_()
+        self.length[0].fill_(1)
+        self.lp[0].zero_()
+        self.status[0].zero_()
+
+    def unfinished(self, t):
+        """A device bool: some row still decodes after t positions."""
+        return self.status[t % self.halves].eq(0).any()
+
+    def slots(self, t):
+        """The slot state after t positions: seq, raw [B, N, T] int64, length [B, N] int64, lp [B, N] and
+        token log-probabilities [B, N, T] (copies), and status [B, N] (a view)."""
+        h, B, N, T = t % self.halves, self.B, self.N, self.T
+        return (self.seq[h].view(B, N, T).long(), self.raw[h].view(B, N, T).long(), self.length[h].view(B, N).long(),
+                self.lp[h].view(B, N).clone(), self.tlp[h].view(B, N, T).clone(), self.status[h].view(B, N))
 
     def head(self, t):
         """logits, copy scores and gate logits of decoder row t (every launch on the current stream: capturable)."""
@@ -76,16 +128,7 @@ class PositionLoop:
         while t < self.T - 1:
             if t and t % POLL_EVERY == 0 and not bool(self.unfinished(t)):
                 break
-            g = self.graphs.get((cfg, t))
-            if g is not None:
-                g.replay()
-            else:
-                self.position(t, *cfg)                         # this batch's result (and the warm-up of a capture) ...
-                torch.cuda.synchronize()
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):                      # ... and the same launches recorded for later batches
-                    self.position(t, *cfg)
-                self.graphs[(cfg, t)] = g
+            replay_or_capture(self.graphs, (cfg, t), lambda: self.position(t, *cfg))
             t += 1
         return t
 
@@ -97,7 +140,7 @@ def loop_for(cls, model, B, N, T, S):
     """The cached `cls` instance of this shape; rebuilt (fresh operand copies and graphs) when the weights changed."""
     store = _LOOPS.setdefault(model, {})
     key = (cls, B, N, T, S, model.precision)
-    wkey = _weights_key(model)
+    wkey = weights_key(model, model.decoder)
     if key not in store or store[key][0] != wkey:
         store[key] = (wkey, cls(model, B, N, T, S))
     return store[key][1]

@@ -27,6 +27,30 @@ from ._lib import FIRA_BF16, FIRA_F32, call
 D = ops.D
 
 
+def weights_key(module, decoder=None):
+    """A key that changes whenever a parameter of `module` may have changed.  `weights_epoch` of `decoder` (default:
+    `module`) is bumped by engine.GraphedTrainStep after every replay: parameter updates made INSIDE a captured CUDA
+    graph change neither _version nor data_ptr."""
+    ps = list(module.parameters())
+    return (getattr(module if decoder is None else decoder, "weights_epoch", 0),) + tuple(p._version for p in ps) + \
+        tuple(p.data_ptr() for p in ps)
+
+
+def replay_or_capture(graphs, key, launches):
+    """Replay graphs[key]; on a miss run `launches()` (every launch on the current stream) eagerly, which gives this
+    call's result and warms up the capture, then record the same launches into a CUDA graph kept as graphs[key]."""
+    g = graphs.get(key)
+    if g is not None:
+        g.replay()
+        return
+    launches()
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        launches()
+    graphs[key] = g
+
+
 class CudaBackend:
     """libfira_b200 kernels on the current stream; fp32 parity mode or bf16 throughput mode."""
 
@@ -103,11 +127,7 @@ class IncrementalDecoder:
     def _prepare_weights(self):
         """Concatenated / operand-form weights in STATIC tensors (captured graphs keep pointing at them);
         refreshed only when a parameter changed."""
-        ps = list(self.dec.parameters())
-        # `weights_epoch` is bumped by engine.GraphedTrainStep after every replay: parameter updates made INSIDE a
-        # captured CUDA graph change neither _version nor data_ptr
-        version = (getattr(self.dec, "weights_epoch", 0),) + tuple(p._version for p in ps) + \
-            tuple(p.data_ptr() for p in ps)
+        version = weights_key(self.dec)
         if version == self.w_version:
             return
         be = self.be
@@ -192,17 +212,10 @@ class IncrementalDecoder:
     def advance(self, t):
         """Decoder output row t for the tokens already in `tok[:B*K]` and `tok_mask[:, t]` (step() fills them from the
         host side; the sampler's kernel writes them on the device)."""
-        if not self.use_graphs:
-            self._layers(t)
-        elif t in self.graphs:
-            self.graphs[t].replay()
+        if self.use_graphs:
+            replay_or_capture(self.graphs, t, lambda: self._layers(t))
         else:
-            self._layers(t)                                   # this call's result (also the warm-up) ...
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):                         # ... and the same launches recorded for later batches
-                self._layers(t)
-            self.graphs[t] = g
+            self._layers(t)
         return self.out[:self.R]
 
     def reorder(self, src_rows):

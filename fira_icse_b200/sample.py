@@ -13,21 +13,17 @@ u comes from Philox4x32-7 keyed by `seed` with the counter (first_index + b, n, 
 on its position in the dataset, not on the batch it was decoded in or the GPU count.  The emitted log-probability is
 log(clamp(P_j, 1e-10, 1)) whatever temperature, top_k and top_p are: it is -nll of the training loss for label j.
 
-The loop is decode_loop.PositionLoop: per batch the encoder, the cross-attention K/V of the memory and
-LinearSource(memory) run once, and the N samples of a commit are the N query rows of an incremental.IncrementalDecoder.
-Per position: newest decoder row -> out_fc -> target projection and gate -> copy scores -> fira_pointer_mix_sample,
-which also writes the next input token straight into the decoder's token buffer and keeps each row's finished flag,
-length and log-probability sum.  A position is captured once into a CUDA graph and replayed for every later batch of
-the same shape; the loop reads back nothing but an all-finished flag, once every 8 positions.
+The loop is decode_loop.PositionLoop (described there); a position ends with fira_pointer_mix_sample, which also writes
+the next input token straight into the decoder's token buffer and keeps each row's finished flag, length and
+log-probability sum.
 """
-import ctypes
 from typing import NamedTuple
 
 import torch
 
 from . import ops
 from ._lib import call
-from .decode_loop import PositionLoop, loop_for
+from .decode_loop import PositionLoop, _f32, check_tar_len, encode, is_int, loop_for
 
 MAX_SAMPLES = 32          # the N samples of a commit are its query rows in fira_attn_fwd / fira_copy_scores_fwd (<= 32)
 
@@ -40,14 +36,8 @@ class Samples(NamedTuple):
     token_logprob: torch.Tensor   # [B, N, T] fp32 log(clamp(P, 1e-10, 1)) of each drawn token, 0 at 0 and after <eos>
 
 
-def _f32(x):
-    return ctypes.c_float(x).value
-
-
 def check_args(num_samples, temperature, top_k, top_p, seed, first_index, tar_len):
     """ValueError for any parameter the sampler cannot honour (called before any device work)."""
-    def is_int(v):
-        return isinstance(v, int) and not isinstance(v, bool)
     if not is_int(num_samples) or not 1 <= num_samples <= MAX_SAMPLES:
         raise ValueError(f"num_samples must be an integer in [1, {MAX_SAMPLES}], got {num_samples!r}")
     if not isinstance(temperature, (int, float)) or not 0.0 < _f32(temperature) < float("inf"):
@@ -65,37 +55,17 @@ def check_args(num_samples, temperature, top_k, top_p, seed, first_index, tar_le
 
 
 class _Sampler(PositionLoop):
-    """The sampler's state on top of the shared position loop: seed, first index and every row's draws."""
+    """The sampler's seed and first index on top of the shared position loop (status: the finished flag)."""
 
     def __init__(self, model, B, N, T, S):
         super().__init__(model, B, N, T, S)
-        R, dev = self.R, self.dev
-        i32 = dict(dtype=torch.int32, device=dev)
-        f32 = dict(dtype=torch.float32, device=dev)
-        self.seed = torch.zeros(1, dtype=torch.int64, device=dev)      # read by the kernel as uint64
-        self.first = torch.zeros(1, **i32)
-        self.seq = torch.empty((R, T), **i32)
-        self.raw = torch.empty((R, T), **i32)
-        self.tlp = torch.empty((R, T), **f32)
-        self.finished = torch.empty(R, dtype=torch.uint8, device=dev)
-        self.length = torch.empty(R, **i32)
-        self.lp = torch.empty(R, **f32)
+        self.seed = torch.zeros(1, dtype=torch.int64, device=self.dev)      # read by the kernel as uint64
+        self.first = torch.zeros(1, dtype=torch.int32, device=self.dev)
 
     def start(self, memory, mem_mask, copy_src, seed, first_index, start_id, pad_id):
         super().start(memory, mem_mask, copy_src, start_id, pad_id)
         self.seed.fill_(seed - 2 ** 64 if seed >= 2 ** 63 else seed)
         self.first.fill_(first_index)
-        self.seq.fill_(pad_id)
-        self.seq[:, 0] = start_id
-        self.raw.fill_(pad_id)
-        self.raw[:, 0] = start_id
-        self.tlp.zero_()
-        self.finished.zero_()
-        self.length.fill_(1)
-        self.lp.zero_()
-
-    def unfinished(self, t):
-        return self.finished.eq(0).any()
 
     def position(self, t, temperature, top_k, top_p, eos_id, pad_id):
         """Draw position t + 1 from decoder row t (every launch on the current stream: capturable)."""
@@ -104,7 +74,7 @@ class _Sampler(PositionLoop):
         call("fira_pointer_mix_sample", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
              p(self.copy_src), p(self.seed), p(self.first), None, float(temperature), int(top_k), float(top_p),
              int(eos_id), int(pad_id), p(self.inc.tok), p(self.seq), p(self.raw), p(self.tlp), p(self.inc.tok_mask),
-             self.T, t, p(self.finished), p(self.length), p(self.lp), self.B, self.N, self.V, self.S, self.pr.code,
+             self.T, t, p(self.status), p(self.length), p(self.lp), self.B, self.N, self.V, self.S, self.pr.code,
              ops._stream())
 
 
@@ -115,20 +85,13 @@ def sample(model, sou, mark, ast_change, edge, sub_token, *, num_samples=1, temp
 
     first_index: dataset position of the batch's first commit (the Philox counter uses first_index + b)."""
     check_args(num_samples, temperature, top_k, top_p, seed, first_index, tar_len)
-    if tar_len > model.decoder.pos_encode.shape[0]:
-        raise ValueError(f"tar_len {tar_len} exceeds the decoder's {model.decoder.pos_encode.shape[0]} positions")
+    check_tar_len(model, tar_len)
     if first_index + sou.shape[0] > 2 ** 31:
         raise ValueError("first_index + batch size must stay below 2**31")
-    dev = model.out_fc.weight.device
-    sou, mark, ast_change, sub_token = (t.to(dev) for t in (sou, mark, ast_change, sub_token))
-    B, N, T = sou.shape[0], num_samples, tar_len
-    memory = model.encoder.encode_memory(sou, mark, ast_change, edge, sub_token)        # once per batch
-    S = memory.shape[1]
-    mem_mask = torch.cat((sou != pad_id, sub_token != 0), dim=1)
-    copy_src = torch.cat((sou, sub_token), dim=1)                                       # copy position -> vocabulary id
-    st = loop_for(_Sampler, model, B, N, T, S)
+    memory, mem_mask, copy_src = encode(model, sou, mark, ast_change, edge, sub_token, pad_id)
+    B, S = memory.shape[:2]
+    st = loop_for(_Sampler, model, B, num_samples, tar_len, S)
     st.start(memory, mem_mask, copy_src, seed, first_index, start_id, pad_id)
-    st.run((float(temperature), int(top_k), float(top_p), int(eos_id), int(pad_id)))
-    shape = (B, N, T)
-    return Samples(st.seq.view(shape).long(), st.raw.view(shape).long(), st.length.view(B, N).long(),
-                   st.lp.view(B, N).clone(), st.tlp.view(shape).clone())
+    t = st.run((float(temperature), int(top_k), float(top_p), int(eos_id), int(pad_id)))
+    seq, raw, length, lp, tlp, _ = st.slots(t)
+    return Samples(seq, raw, length, lp, tlp)

@@ -102,6 +102,12 @@ def deanonymise(tokens, var_map):
     return [rev.get(t, t) for t in tokens]
 
 
+def reference_words(tar, vocab, r_vocab):
+    """The reference message of one commit (its target ids between <start> and <eos>) as words."""
+    ref = tar.tolist()
+    return [r_vocab[x] for x in ref[1:ref.index(vocab['<eos>'])]]
+
+
 def loader(ds, batch_size, shuffle, indices=None):
     sampler = None
     if indices is not None:
@@ -131,8 +137,7 @@ def dev(model, dev_loader, g, valid_index, epoch, dev):
                     elif sen[t] >= args.vocab_size:
                         sen[t] = int(whole[i][sen[t] - args.vocab_size])
                 hyp = ' '.join(r_vocab[x] for x in sen).replace('<pad>', "").replace('<unkm>', "😅").strip().split()
-                ref = tar[i].tolist()
-                ref = [r_vocab[x] for x in ref[1:ref.index(vocab['<eos>'])]]
+                ref = reference_words(tar[i], vocab, r_vocab)
                 bleu = sentence_bleu_method2([ref], hyp)
                 bleus += bleu
                 out_str += ' '.join(deanonymise(hyp, var_maps[valid_index[total + i]])) + ',' + str(bleu) + '\n'
@@ -217,94 +222,63 @@ def main_train():
         dist.destroy_process_group()
 
 
-def test(model, test_loader, g, test_index, dev_, out_path="OUTPUT/output_fira"):
-    """Beam search over the test split, one line per commit (run_model.py:187-380)."""
-    vocab, r_vocab, var_maps = g["vocab"], g["r_vocab"], g["var_maps"]
-    model.eval()
-    total, bleus = 0, 0.0
-    with open(out_path, 'w') as f:
-        for idx, batch in enumerate(test_loader):
-            b = batch_to_device(batch, dev_)
-            seq, length, prob = beam_search(model, b[0], b[3], b[4], b[5], b[7], beam_size=args.beam_size,
-                                            tar_len=args.tar_len, start_id=vocab['<start>'], eos_id=vocab['<eos>'],
-                                            pad_id=vocab['<pad>'])
-            best, blen = best_sequences(seq, length, prob)
-            best, blen, tar = best.cpu().numpy(), blen.cpu().numpy(), batch[1].numpy()
-            bleu_batch = 0.0
-            for i in range(len(best)):
-                hyp = ids_to_text(best[i][:blen[i]].tolist(), r_vocab)
-                ref = tar[i].tolist()
-                ref = [r_vocab[x] for x in ref[1:ref.index(vocab['<eos>'])]]
-                bl = sentence_bleu_method2([ref], hyp)
-                bleus += bl; bleu_batch += bl
-                f.write(' '.join(deanonymise(hyp, var_maps[test_index[total + i]])) + '\n')
-            f.flush()
-            total += len(best)
-            print("data: %d/%d bleu: %f" % (total, len(test_loader.dataset), bleu_batch / len(best)))
-    return bleus / max(1, total)
+def decoder(mode, vocab):
+    """FIRA_DECODE -> (output file, decode(model, batch, dataset position of its first commit) -> seq [B, N, T],
+    length [B, N] and the numeric columns [B, N] written before each message, how many leading hypotheses of a commit
+    count towards the BLEU)."""
+    ids = dict(tar_len=args.tar_len, start_id=vocab['<start>'], eos_id=vocab['<eos>'], pad_id=vocab['<pad>'])
+    if mode == "beam":                  # the reference's beam search: its best beam, `<message>`
+        def decode(model, b, first_index):
+            beams = beam_search(model, b[0], b[3], b[4], b[5], b[7], beam_size=args.beam_size, **ids)
+            best, blen = best_sequences(*beams)
+            return best.unsqueeze(1), blen.unsqueeze(1), ()
+        return "output_fira", decode, 1
+    if mode == "sample":                # FIRA_SAMPLES seeded samples, `<log-prob>\t<message>`
+        n = int(os.environ.get("FIRA_SAMPLES", 3))
+        opts = dict(num_samples=n, temperature=float(os.environ.get("FIRA_TEMPERATURE", 1.0)),
+                    top_k=int(os.environ.get("FIRA_TOP_K", 0)), top_p=float(os.environ.get("FIRA_TOP_P", 1.0)),
+                    seed=int(os.environ.get("FIRA_SEED", 0)))
+
+        def decode(model, b, first_index):
+            out = sample(model, b[0], b[3], b[4], b[5], b[7], first_index=first_index, **opts, **ids)
+            return out.seq, out.length, (out.logprob,)
+        return "output_fira_samples", decode, n
+    if mode == "nbest":                 # FIRA_BEAM hypotheses best first, `<score>\t<log-prob>\t<message>`
+        alpha = float(os.environ.get("FIRA_LENGTH_PENALTY", 0.0))
+
+        def decode(model, b, first_index):
+            out = nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=args.beam_size, length_penalty=alpha, **ids)
+            return out.seq, out.length, (out.score, out.logprob)
+        return "output_fira_nbest", decode, 1
+    raise SystemExit("FIRA_DECODE must be 'beam', 'sample' or 'nbest'")
 
 
-def sample_test(model, test_loader, g, test_index, dev_, first_index, out_path="OUTPUT/output_fira_samples"):
-    """Seeded sampling over the test split: FIRA_SAMPLES lines `<log-prob>\\t<message>` per commit, in test order."""
+def test(model, test_loader, g, test_index, dev_, first_index, decode, n_bleu, out_path):
+    """Decodes the test split (run_model.py:187-380): N lines per commit in test order, the numeric columns then the
+    message -> mean sentence BLEU over the first n_bleu hypotheses of every commit."""
     vocab, r_vocab, var_maps = g["vocab"], g["r_vocab"], g["var_maps"]
-    n = int(os.environ.get("FIRA_SAMPLES", 3))
-    opts = dict(num_samples=n, temperature=float(os.environ.get("FIRA_TEMPERATURE", 1.0)),
-                top_k=int(os.environ.get("FIRA_TOP_K", 0)), top_p=float(os.environ.get("FIRA_TOP_P", 1.0)),
-                seed=int(os.environ.get("FIRA_SEED", 0)))
     model.eval()
     total, bleus = 0, 0.0
     with open(out_path, 'w') as f:
         for batch in test_loader:
             b = batch_to_device(batch, dev_)
-            out = sample(model, b[0], b[3], b[4], b[5], b[7], first_index=first_index + total, tar_len=args.tar_len,
-                         start_id=vocab['<start>'], eos_id=vocab['<eos>'], pad_id=vocab['<pad>'], **opts)
-            seq, length, logprob = out.seq.cpu().numpy(), out.length.cpu().numpy(), out.logprob.cpu().numpy()
+            seq, length, cols = decode(model, b, first_index + total)
+            seq, length, cols = seq.cpu().numpy(), length.cpu().numpy(), [c.cpu().numpy() for c in cols]
             tar = batch[1].numpy()
             bleu_batch = 0.0
             for i in range(len(seq)):
-                ref = tar[i].tolist()
-                ref = [r_vocab[x] for x in ref[1:ref.index(vocab['<eos>'])]]
-                for k in range(n):
+                ref = reference_words(tar[i], vocab, r_vocab)
+                for k in range(seq.shape[1]):
                     hyp = ids_to_text(seq[i, k][:length[i, k]].tolist(), r_vocab)
-                    bl = sentence_bleu_method2([ref], hyp)
-                    bleus += bl; bleu_batch += bl
-                    f.write('%.6f\t%s\n' % (logprob[i, k], ' '.join(deanonymise(hyp, var_maps[test_index[total + i]]))))
-            f.flush()
-            total += len(seq)
-            print("data: %d/%d bleu: %f" % (total, len(test_loader.dataset), bleu_batch / (len(seq) * n)))
-    return bleus / max(1, total * n)
-
-
-def nbest_test(model, test_loader, g, test_index, dev_, out_path="OUTPUT/output_fira_nbest"):
-    """n-best beam search over the test split: FIRA_BEAM lines `<score>\t<log-prob>\t<message>` per commit, best first."""
-    vocab, r_vocab, var_maps = g["vocab"], g["r_vocab"], g["var_maps"]
-    K = args.beam_size
-    alpha = float(os.environ.get("FIRA_LENGTH_PENALTY", 0.0))
-    model.eval()
-    total, bleus = 0, 0.0
-    with open(out_path, 'w') as f:
-        for batch in test_loader:
-            b = batch_to_device(batch, dev_)
-            out = nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=K, length_penalty=alpha, tar_len=args.tar_len,
-                        start_id=vocab['<start>'], eos_id=vocab['<eos>'], pad_id=vocab['<pad>'])
-            seq, length = out.seq.cpu().numpy(), out.length.cpu().numpy()
-            score, logprob = out.score.cpu().numpy(), out.logprob.cpu().numpy()
-            tar = batch[1].numpy()
-            bleu_batch = 0.0
-            for i in range(len(seq)):
-                ref = tar[i].tolist()
-                ref = [r_vocab[x] for x in ref[1:ref.index(vocab['<eos>'])]]
-                for k in range(K):
-                    hyp = ids_to_text(seq[i, k][:length[i, k]].tolist(), r_vocab)
-                    if k == 0:
+                    if k < n_bleu:
                         bl = sentence_bleu_method2([ref], hyp)
                         bleus += bl; bleu_batch += bl
-                    f.write('%.6f\t%.6f\t%s\n' % (score[i, k], logprob[i, k],
-                                                   ' '.join(deanonymise(hyp, var_maps[test_index[total + i]]))))
+                    f.write(''.join('%.6f\t' % c[i, k] for c in cols) +
+                            ' '.join(deanonymise(hyp, var_maps[test_index[total + i]])) + '\n')
             f.flush()
             total += len(seq)
-            print("data: %d/%d bleu: %f" % (total, len(test_loader.dataset), bleu_batch / len(seq)))
-    return bleus / max(1, total)
+            print("data: %d/%d bleu: %f" % (total, len(test_loader.dataset), bleu_batch / (len(seq) * n_bleu)))
+    return bleus / max(1, total * n_bleu)
 
 
 def main_test():
@@ -318,18 +292,9 @@ def main_test():
     lo, hi = shard_range(len(test_set), RANK, WORLD)                # replicas only: index ranges, files concatenated
     idx = list(range(lo, hi)) if WORLD > 1 else None
     test_loader = loader(test_set, args.test_batch_size, False, idx)
-    decode = os.environ.get("FIRA_DECODE", "beam")
-    if decode == "beam":
-        out = "OUTPUT/output_fira" if WORLD == 1 else f"OUTPUT/output_fira.part{RANK:02d}"
-        bleu = test(model, test_loader, g, all_index['test'][lo:hi], dev_, out)
-    elif decode == "sample":
-        out = "OUTPUT/output_fira_samples" if WORLD == 1 else f"OUTPUT/output_fira_samples.part{RANK:02d}"
-        bleu = sample_test(model, test_loader, g, all_index['test'][lo:hi], dev_, lo, out)
-    elif decode == "nbest":
-        out = "OUTPUT/output_fira_nbest" if WORLD == 1 else f"OUTPUT/output_fira_nbest.part{RANK:02d}"
-        bleu = nbest_test(model, test_loader, g, all_index['test'][lo:hi], dev_, out)
-    else:
-        raise SystemExit("FIRA_DECODE must be 'beam', 'sample' or 'nbest'")
+    name, decode, n_bleu = decoder(os.environ.get("FIRA_DECODE", "beam"), g["vocab"])
+    out = f"OUTPUT/{name}" if WORLD == 1 else f"OUTPUT/{name}.part{RANK:02d}"
+    bleu = test(model, test_loader, g, all_index['test'][lo:hi], dev_, lo, decode, n_bleu, out)
     print("mean sentence bleu: %f" % bleu)
 
 

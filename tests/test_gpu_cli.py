@@ -1,5 +1,6 @@
-"""`python run_model.py train|test` end to end on a 128-commit DataSet directory, and beam-search id
-parity against the reference's own test() loop (tests/golden/beam_first16.npz)."""
+"""`python run_model.py train|test` end to end on a 128-commit DataSet directory (trained once, then decoded with
+FIRA_DECODE=beam, sample and nbest), and beam-search id parity against the reference's own test() loop
+(tests/golden/beam_first16.npz, beam5_first16.npz)."""
 import copy
 import json
 import os
@@ -24,10 +25,10 @@ def _need_cuda():
 
 
 @pytest.mark.parametrize("golden", ["beam_first16.npz", "beam5_first16.npz"])      # beam 3 (run_model.py:43), beam 5
-@pytest.mark.parametrize("mode", ["full", "incremental", "graph"])
+@pytest.mark.parametrize("mode", ["full", "graph"])
 def test_beam_search_ids_match_reference_test_loop(mode, golden):
-    """mode: full decoder re-run per step / KV-cached newest row / the same replayed as CUDA graphs
-    (first batch captures, later batches replay); goldens = outputs of the unmodified reference's test() loop
+    """mode: full decoder re-run per step / KV-cached newest row replayed as CUDA graphs (the first batch runs it
+    eagerly and captures it, later batches replay); goldens = outputs of the unmodified reference's test() loop
     (tests/golden/make_golden_beam.py) with beam 3 (the reference default) and beam 5 (BASELINE.json configs[3])"""
     from fira_icse_b200.beam import beam_search, best_sequences
     gold = np.load(os.path.join(GOLDEN, golden))
@@ -51,20 +52,55 @@ def test_beam_search_ids_match_reference_test_loop(mode, golden):
             assert np.array_equal(mine, ref), (lo + i, mine, ref)
 
 
-def test_run_model_train_then_test(tmp_path):
-    raw = load_raw_golden()
-    _write_dataset(str(tmp_path), raw)
+def _run_model(stage, cwd, env):
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "run_model.py"), stage], cwd=cwd, env=env,
+                       capture_output=True, text=True, timeout=900)
+    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
+    return r
+
+
+@pytest.fixture(scope="module")
+def trained(tmp_path_factory):
+    """`run_model.py train` once -> (its directory, the environment, the training run)."""
+    d = tmp_path_factory.mktemp("cli")
+    _write_dataset(str(d), load_raw_golden())
     env = dict(os.environ, PYTHONPATH=ROOT, FIRA_EPOCHS="1", FIRA_BATCH="16", FIRA_MAX_BATCHES="3",
                FIRA_WORKERS="0", FIRA_TEST_BATCH="4")
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "run_model.py"), "train"], cwd=tmp_path, env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
+    return d, env, _run_model("train", d, env)
+
+
+def _test_lines(trained, name, **env):
+    d, base, _ = trained
+    r = _run_model("test", d, dict(base, **env))
+    assert "mean sentence bleu" in r.stdout
+    n_test = len(json.load(open(d / "all_index"))["test"])
+    return n_test, open(d / "OUTPUT" / name).read().split("\n")
+
+
+def test_run_model_train_then_test(trained):
+    d, _, r = trained
     assert "loss:" in r.stdout
-    sd = torch.load(tmp_path / "best_model.pt", map_location="cpu")
+    sd = torch.load(d / "best_model.pt", map_location="cpu")
     assert len(sd) == 338 and not any(k.startswith("module.") for k in sd)
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "run_model.py"), "test"], cwd=tmp_path, env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
-    n_test = len(json.load(open(tmp_path / "all_index"))["test"])
-    lines = open(tmp_path / "OUTPUT" / "output_fira").read().split("\n")
+    n_test, lines = _test_lines(trained, "output_fira")
     assert len(lines) == n_test + 1 and lines[-1] == ""
+
+
+def test_run_model_test_writes_samples(trained):
+    n_test, lines = _test_lines(trained, "output_fira_samples", FIRA_DECODE="sample", FIRA_SAMPLES="3",
+                                FIRA_TOP_P="0.95", FIRA_SEED="3")
+    assert len(lines) == 3 * n_test + 1 and lines[-1] == ""
+    for ln in lines[:-1]:
+        lp, _ = ln.split("\t", 1)
+        assert float(lp) <= 0.0
+
+
+def test_run_model_test_writes_nbest(trained):
+    n_test, lines = _test_lines(trained, "output_fira_nbest", FIRA_DECODE="nbest", FIRA_BEAM="4",
+                                FIRA_LENGTH_PENALTY="0.6")
+    assert len(lines) == 4 * n_test + 1 and lines[-1] == ""
+    for c in range(n_test):
+        fields = [ln.split("\t", 2) for ln in lines[4 * c:4 * c + 4]]
+        scores = [float(f[0]) for f in fields]
+        assert all(float(f[1]) <= 0.0 for f in fields)
+        assert all(x >= y for x, y in zip(scores, scores[1:])), scores

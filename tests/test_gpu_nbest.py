@@ -1,18 +1,15 @@
 """n-best beam search on the GPU: fira_pointer_mix_beam_step against the float64 restatement (tests/beam_rule.py), and
 fira_icse_b200.beam.nbest end to end (the reference beam goldens, the existing beam search's K beams, log-probabilities
-= the training NLL, length-penalised scores, static buffers across batches, `run_model.py test` with FIRA_DECODE=nbest)."""
+= the training NLL, length-penalised scores, static buffers across batches)."""
 import copy
-import json
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 
 from beam_rule import candidates, step
-from fira_testlib import GOLDEN, ROOT, golden_batch, load_raw_golden, seeded_model
+from fira_testlib import GOLDEN, golden_batch, seeded_model
 from sample_rule import mixture
 from test_gpu_sample import _check_bookkeeping, _head_nll, _inputs, _model, _teacher_forced, _teacher_forced_nll, _vocab
 
@@ -256,27 +253,3 @@ def test_static_buffers_are_reset_between_batches():
     assert not torch.equal(first.seq, other.seq)
     assert torch.equal(first.seq, again.seq) and torch.equal(first.raw, again.raw)
     torch.testing.assert_close(first.logprob, again.logprob, rtol=0, atol=1e-4)
-
-
-def test_run_model_test_writes_nbest(tmp_path):
-    from test_data import _write_dataset
-    raw = load_raw_golden()
-    _write_dataset(str(tmp_path), raw)
-    env = dict(os.environ, PYTHONPATH=ROOT, FIRA_EPOCHS="1", FIRA_BATCH="16", FIRA_MAX_BATCHES="1",
-               FIRA_WORKERS="0", FIRA_TEST_BATCH="4")
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "run_model.py"), "train"], cwd=tmp_path, env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
-    env.update(FIRA_DECODE="nbest", FIRA_BEAM="4", FIRA_LENGTH_PENALTY="0.6")
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "run_model.py"), "test"], cwd=tmp_path, env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
-    assert "mean sentence bleu" in r.stdout
-    n_test = len(json.load(open(tmp_path / "all_index"))["test"])
-    lines = open(tmp_path / "OUTPUT" / "output_fira_nbest").read().split("\n")
-    assert len(lines) == 4 * n_test + 1 and lines[-1] == ""
-    for c in range(n_test):
-        fields = [ln.split("\t", 2) for ln in lines[4 * c:4 * c + 4]]
-        scores = [float(f[0]) for f in fields]
-        assert all(float(f[1]) <= 0.0 for f in fields)
-        assert all(x >= y for x, y in zip(scores, scores[1:])), scores

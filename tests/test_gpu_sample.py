@@ -1,17 +1,14 @@
 """Seeded sampling on the GPU: fira_pointer_mix_sample against the float64 restatement (tests/sample_rule.py), its Philox
 draws, and fira_icse_b200.sample end to end (greedy = teacher-forced argmax, log-probabilities = the training NLL,
-bookkeeping, `run_model.py test` with FIRA_DECODE=sample)."""
+bookkeeping)."""
 import copy
-import json
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 
-from fira_testlib import GOLDEN, ROOT, golden_batch, load_raw_golden, seeded_model
+from fira_testlib import GOLDEN, golden_batch, load_raw_golden, seeded_model
 from sample_rule import draw, mixture
 
 pytestmark = pytest.mark.gpu
@@ -249,25 +246,3 @@ def test_token_logprob_is_the_teacher_forced_nll(precision, kw):
         # sharpened model ~15% of positions exceed it, up to ~0.4
         d = (got[live] - ref[live]).abs()
         assert d.median().item() <= 5e-2 and d.max().item() <= 0.5
-
-
-def test_run_model_test_writes_samples(tmp_path):
-    from test_data import _write_dataset
-    raw = load_raw_golden()
-    _write_dataset(str(tmp_path), raw)
-    env = dict(os.environ, PYTHONPATH=ROOT, FIRA_EPOCHS="1", FIRA_BATCH="16", FIRA_MAX_BATCHES="1",
-               FIRA_WORKERS="0", FIRA_TEST_BATCH="4")
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "run_model.py"), "train"], cwd=tmp_path, env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
-    env.update(FIRA_DECODE="sample", FIRA_SAMPLES="3", FIRA_TOP_P="0.95", FIRA_SEED="3")
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "run_model.py"), "test"], cwd=tmp_path, env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
-    assert "mean sentence bleu" in r.stdout
-    n_test = len(json.load(open(tmp_path / "all_index"))["test"])
-    lines = open(tmp_path / "OUTPUT" / "output_fira_samples").read().split("\n")
-    assert len(lines) == 3 * n_test + 1 and lines[-1] == ""
-    for ln in lines[:-1]:
-        lp, _ = ln.split("\t", 1)
-        assert float(lp) <= 0.0

@@ -7,7 +7,7 @@ reference's own loop was timed on in BASELINE.md (72 s for 32 commits on CPU).  
 (batch, beam) configuration; timing with CUDA events around whole batches, inputs resident on the device.
 
     python tools/bench_beam.py [--batches 20,128] [--beams 3,5] [--precision fp32|bf16] [--reps 3]
-                               [--modes full,incremental,graph,sample,nbest]   (sample: N = the beam width;
+                               [--modes full,graph,sample,nbest]   (sample: N = the beam width;
                                nbest: beam.nbest, log-space n-best beam search with length_penalty 0)
 """
 import argparse
@@ -26,7 +26,7 @@ def main():
     ap.add_argument("--precision", default="fp32")
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--trim", action="store_true", help="loader-side padding trimming (data.trim_batch_host)")
-    ap.add_argument("--modes", default="full,incremental,graph")
+    ap.add_argument("--modes", default="full,graph")
     a = ap.parse_args()
     import torch
     import __graft_entry__
@@ -74,7 +74,7 @@ def main():
                 "precision": a.precision, "mode": mode, "ids_equal_full_mode": same, "trimmed": bool(a.trim), "data": "synthetic (DataSet distribution), random weights",
                 "c_abi_calls_per_batch": (_lib.LAUNCH_COUNT - n0) // a.reps,
                 "note": "encoder once per batch; full = 30-position decoder re-run per step over all live beams, "
-                        "incremental = newest row against K/V caches, graph = the same as CUDA-graph replays, "
+                        "graph = newest row against K/V caches as CUDA-graph replays, "
                         "sample = beam-width seeded samples per commit (T = 1, no top-k / top-p), one graph per position, "
                         "nbest = log-space n-best beam search (length_penalty 0), one graph per position"}),
                   flush=True)
