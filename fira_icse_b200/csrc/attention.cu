@@ -11,25 +11,18 @@
 // Forward saves (row max, row sum); backward recomputes P from them, gets delta = rowsum(P * dP) as
 // dO . O (so keys can be processed in chunks of 64 with a small shared-memory footprint, 5 CTAs/SM)
 // and writes zero gradients for the masked keys.
+//
+// bf16 activations run on the tensor cores (attn_mma_fwd/bwd_kernel below): the same key compaction, then warp-level
+// mma.sync.m16n8k16 on register fragments.
 #include <stdlib.h>
 #include "common.cuh"
 #include "fira_b200.h"
 
-// wgmma path of the bf16 mode (attention_tc.cu)
-int fira_attn_tc_fwd(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
-                     const unsigned char* key_mask, const int* ranges, long kv_rows, int causal, void* ctx, long ldo,
-                     float* stats, int B, int H, int Lq, int Lk, void* stream);
-int fira_attn_tc_bwd(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
-                     const unsigned char* key_mask, const int* ranges, long kv_rows, int causal, const void* ctx,
-                     const void* d_ctx, long ldo, const float* stats, void* dq, long lddq, void* dk, long lddk, void* dv,
-                     long lddv, int B, int H, int Lq, int Lk, void* stream);
-bool fira_attn_tc_eligible(int B, int H, int Lq, int Lk, int d_head, long ldk, long ldv, int max_chunks);
-
 namespace {
 
 // bf16 activations go to the tensor-core kernels unless FIRA_ATTN_TC=0 (A/B runs against the FFMA kernels below)
-bool use_tc(int dtype, int B, int H, int Lq, int Lk, int d_head, long ldk, long ldv, int max_chunks) {
-  if (dtype != FIRA_BF16 || !fira_attn_tc_eligible(B, H, Lq, Lk, d_head, ldk, ldv, max_chunks)) return false;
+bool use_tc(int dtype) {
+  if (dtype != FIRA_BF16) return false;
   const char* e = getenv("FIRA_ATTN_TC");      // read per call: an A/B switch, not cached process state
   return e ? atoi(e) != 0 : true;
 }
@@ -302,6 +295,466 @@ __global__ void __launch_bounds__(NTHR) attn_bwd_kernel(AttnArgs a, const T* __r
   }
 }
 
+// ------------------------------------------------------------------------------------------------ bf16 tensor cores
+// One CTA per (commit, head) on the compacted key list, warp-level mma.sync.m16n8k16 (bf16 in, fp32 accumulate).
+// A warp holds 16 query rows x 8 keys per accumulator fragment; the fragment of a score tile IS, register for
+// register, the A operand of the product that consumes it (P V, dS K), so P and dS never leave the registers there.
+// K / V / Q / dO / P / dS tiles in shared memory are [rows][32] bf16, read with ldmatrix (.trans for the operands
+// whose reduction dimension is the tile's row).
+//   forward:  warp w = query rows [16 w, 16 w + 16); 64-key blocks, double-buffered by cp.async; online softmax
+//             (ex2.approx) on the fragments; the row sum adds the bf16-rounded P that the P V product consumes.
+//   backward: warp w = key blocks w, w + 3, ... of 32 keys, all query rows; S and dP recomputed, P from the saved
+//             statistics, dS = P (dP - delta) scale; dQ += dS K into the warp's fp32 partial in shared memory (summed
+//             over the warps at the end), dK = dS^T Q and dV = P^T dO from P / dS written to the warp's shared memory.
+// Every key of a block is valid (compaction), except in causal self-attention (identity list, Lk <= 32) and in a
+// commit without valid keys (every key of the list, uniform P) -- the same rules as the FFMA kernels.
+namespace mma {
+
+constexpr int ROWB = DH * 2;     // bytes per row of a [rows][32] bf16 tile
+constexpr int FWARPS_MAX = LQ_MAX / 16;
+constexpr int FKB = 64;          // forward keys per block
+constexpr int FST = 2;           // forward K / V stages
+constexpr int BWARPS = 3;
+constexpr int BKB = 32;          // backward keys per warp block
+constexpr int BWARP_SMEM = 4 * BKB * ROWB + LQ_MAX * DH * 4;   // K, V, P, dS, fp32 dQ partial of one warp
+constexpr float kLog2e = 1.4426950408889634f;
+static_assert(LQ_MAX == 32 && BKB == 32, "tile shapes");
+
+// byte offset of 16-B chunk c (8 bf16) of row r in a [rows][32] bf16 tile: the XOR spreads the 8 rows of an ldmatrix
+// 8x8 matrix (and the 4-B fragment stores of P / dS) over all 32 banks
+__device__ __forceinline__ uint32_t swz(int r, int c) { return r * ROWB + ((c ^ ((r >> 1) & 3)) << 4); }
+__device__ __forceinline__ uint32_t su32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+// float index of (row r, column f) of a [32][32] fp32 tile, float2 pairs XOR-swizzled by the row so that the
+// accumulator fragment stores of a half warp (rows g, g + 1, .., 4 columns) hit distinct banks
+__device__ __forceinline__ int swz_f32(int r, int f) { return r * DH + 2 * ((f >> 1) ^ ((r & 3) << 2)) + (f & 1); }
+
+__device__ __forceinline__ void ldsm4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
+}
+__device__ __forceinline__ void ldsm4_t(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
+}
+// d += a b   (m16n8k16, a row-major 16x16, b column-major 16x8)
+__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ float ex2(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+__device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
+  __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&v);
+}
+__device__ __forceinline__ float round_bf16(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
+
+// A fragments (16 rows from r0 x 32 features = two k16 steps) of a [rows][32] tile
+__device__ __forceinline__ void ld_a(const unsigned char* tile, int r0, int lane, uint32_t (&a)[2][4]) {
+#pragma unroll
+  for (int kk = 0; kk < 2; ++kk)
+    ldsm4(su32(tile + swz(r0 + (lane & 7) + ((lane >> 3) & 1) * 8, 2 * kk + (lane >> 4))), a[kk]);
+}
+// s[n] += A X^T for 8-row groups n of the [rows][32] tile x (X rows = the N dimension, 32 features = K)
+template <int NT>
+__device__ __forceinline__ void mma_abt(float (&s)[NT][4], const uint32_t (&a)[2][4], const unsigned char* x, int lane) {
+#pragma unroll
+  for (int n = 0; n < NT; ++n) {
+    uint32_t b[4];
+    ldsm4(su32(x + swz(8 * n + (lane & 7), lane >> 3)), b);
+    mma16816(s[n], a[0], b[0], b[1]);
+    mma16816(s[n], a[1], b[2], b[3]);
+  }
+}
+// o[n] += A X over k16 step kk: X = rows [16 kk, 16 kk + 16) of a [rows][32] tile (rows = K, 32 features = N)
+__device__ __forceinline__ void mma_ax(float (&o)[4][4], const uint32_t (&a)[4], const unsigned char* x, int kk, int lane) {
+#pragma unroll
+  for (int np = 0; np < 2; ++np) {
+    uint32_t b[4];
+    ldsm4_t(su32(x + swz(16 * kk + (lane & 7) + ((lane >> 3) & 1) * 8, 2 * np + (lane >> 4))), b);
+    mma16816(o[2 * np], a, b[0], b[1]);
+    mma16816(o[2 * np + 1], a, b[2], b[3]);
+  }
+}
+// A fragment of a k16 step from score-layout accumulators (keys 16 kk .. 16 kk + 15)
+template <int NT>
+__device__ __forceinline__ void acc_to_a(const float (&s)[NT][4], int kk, uint32_t (&a)[4]) {
+  a[0] = pack_bf16(s[2 * kk][0], s[2 * kk][1]);
+  a[1] = pack_bf16(s[2 * kk][2], s[2 * kk][3]);
+  a[2] = pack_bf16(s[2 * kk + 1][0], s[2 * kk + 1][1]);
+  a[3] = pack_bf16(s[2 * kk + 1][2], s[2 * kk + 1][3]);
+}
+
+// K and V rows of compacted keys [c0, c0 + n) into [nk][32] tiles (rows >= n zeroed: P = 0 there must not meet NaN)
+__device__ __forceinline__ void stage_kv(unsigned char* ks, unsigned char* vs, const __nv_bfloat16* kh, long ldk,
+                                         const __nv_bfloat16* vh, long ldv, const int* kidx, int c0, int n, int nk,
+                                         int tid, int nthr) {
+  for (int i = tid; i < nk * 4; i += nthr) {
+    const int j = i >> 2, c = i & 3;
+    const uint32_t off = swz(j, c);
+    if (j < n) {
+      const long r = kidx[c0 + j];
+      cp_async16(su32(ks + off), kh + r * ldk + c * 8);
+      cp_async16(su32(vs + off), vh + r * ldv + c * 8);
+    } else {
+      *reinterpret_cast<uint4*>(ks + off) = make_uint4(0, 0, 0, 0);
+      *reinterpret_cast<uint4*>(vs + off) = make_uint4(0, 0, 0, 0);
+    }
+  }
+}
+
+// Keys valid for query row t.  Causal (identity list, Lk <= 32): key m <= t with its mask byte set; a row without one
+// is uniform over every key of the list (`fill`).  Otherwise every listed key is valid, and `fill` is the commit's.
+// mb = causal_mask_bits(): bit m = mask byte of key m.
+struct RowKeys { uint32_t causal_bits; bool fill; };
+__device__ __forceinline__ uint32_t causal_mask_bits(const AttnArgs& a, const unsigned char* km, int lane) {
+  return a.causal ? __ballot_sync(0xffffffffu, lane < a.Lk && km[lane] != 0) : 0u;
+}
+__device__ __forceinline__ RowKeys row_keys(const AttnArgs& a, uint32_t mb, int nv, bool filled, int t) {
+  RowKeys r{0u, filled};
+  if (a.causal) {
+    const uint32_t w = mb & ((2u << min(t, 31)) - 1u);
+    r.fill = w == 0;
+    r.causal_bits = r.fill ? (nv >= 32 ? 0xffffffffu : (1u << nv) - 1u) : w;
+  }
+  return r;
+}
+__device__ __forceinline__ bool key_ok(const RowKeys& r, int causal, int key, int nv) {
+  return causal ? key < 32 && ((r.causal_bits >> key) & 1u) : key < nv;
+}
+
+__global__ void __launch_bounds__(FWARPS_MAX * 32)
+attn_mma_fwd_kernel(AttnArgs a, __nv_bfloat16* __restrict__ ctx, long ldo, float* __restrict__ stats /* [B,H,Lq,2] */) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  extern __shared__ __align__(16) unsigned char mma_smem[];
+  __shared__ int nv_s, filled_s;
+  unsigned char* Ks = mma_smem;                          // [FST][FKB][32]
+  unsigned char* Vs = Ks + FST * FKB * ROWB;             // [FST][FKB][32]
+  int* kidx = reinterpret_cast<int*>(Vs + FST * FKB * ROWB);
+  const int b = blockIdx.x / a.H, h = blockIdx.x % a.H;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, q = lane & 3;
+  const unsigned char* km = a.key_mask ? a.key_mask + (long)b * a.Lk : nullptr;
+  const int* rg = a.ranges ? a.ranges + 4 * b : nullptr;
+  const long kvb = rg ? 0 : (long)b * a.Lk;
+  const __nv_bfloat16* kh = (const __nv_bfloat16*)a.k + kvb * a.ldk + h * DH;
+  const __nv_bfloat16* vh = (const __nv_bfloat16*)a.v + kvb * a.ldv + h * DH;
+  compact_keys(km, a.Lk, a.causal, kidx, &nv_s, &filled_s, rg);
+  const int nv = nv_s;
+  const int nblk = (nv + FKB - 1) / FKB;
+#pragma unroll
+  for (int s = 0; s < FST; ++s) {
+    if (s < nblk)
+      stage_kv(Ks + s * FKB * ROWB, Vs + s * FKB * ROWB, kh, a.ldk, vh, a.ldv, kidx, s * FKB, min(FKB, nv - s * FKB), FKB,
+               threadIdx.x, blockDim.x);
+    cp_async_commit();
+  }
+  // the warp's 16 query rows as A fragments, straight from global memory (rows >= Lq are zero)
+  int t[2];
+  uint32_t qa[2][4];
+  RowKeys rk[2];
+  const uint32_t mb = causal_mask_bits(a, km, lane);
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    t[r] = 16 * warp + (lane >> 2) + 8 * r;
+    const uint32_t* qr = reinterpret_cast<const uint32_t*>((const __nv_bfloat16*)a.q + ((long)b * a.Lq + t[r]) * a.ldq + h * DH);
+#pragma unroll
+    for (int kk = 0; kk < 2; ++kk) {
+      qa[kk][r] = t[r] < a.Lq ? qr[8 * kk + q] : 0u;
+      qa[kk][2 + r] = t[r] < a.Lq ? qr[8 * kk + 4 + q] : 0u;
+    }
+    rk[r] = row_keys(a, mb, nv, filled_s != 0, t[r]);
+  }
+  const float k2 = a.scale * kLog2e;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float o[4][4];
+#pragma unroll
+  for (int n = 0; n < 4; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.f;
+
+  for (int i = 0; i < nblk; ++i) {
+    cp_async_wait<FST - 1>();
+    __syncthreads();                                     // block i is in shared memory for every warp
+    const unsigned char* kt = Ks + (i % FST) * FKB * ROWB;
+    const unsigned char* vt = Vs + (i % FST) * FKB * ROWB;
+    const int c0 = i * FKB;
+    float s[8][4];
+#pragma unroll
+    for (int n = 0; n < 8; ++n) s[n][0] = s[n][1] = s[n][2] = s[n][3] = 0.f;
+    mma_abt(s, qa, kt, lane);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      // log2-domain scores of the valid keys (-inf elsewhere), online max / rescale, P = bf16(exp)
+      float mx = -INFINITY;
+#pragma unroll
+      for (int n = 0; n < 8; ++n)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& x = s[n][2 * r + e];
+          x = key_ok(rk[r], a.causal, c0 + 8 * n + 2 * q + e, nv) ? (rk[r].fill ? 0.f : x * k2) : -INFINITY;
+          mx = fmaxf(mx, x);
+        }
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float mn = fmaxf(m[r], mx);
+      const float mu = mn == -INFINITY ? 0.f : mn;       // nothing valid yet: keep everything at exactly 0
+      const float corr = ex2(m[r] - mu);
+      m[r] = mn;
+      l[r] *= corr;
+#pragma unroll
+      for (int n = 0; n < 4; ++n) { o[n][2 * r] *= corr; o[n][2 * r + 1] *= corr; }
+#pragma unroll
+      for (int n = 0; n < 8; ++n)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float p = round_bf16(ex2(s[n][2 * r + e] - mu));   // the MMA consumes bf16(p): sum the rounded value
+          s[n][2 * r + e] = p;
+          l[r] += p;
+        }
+    }
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      uint32_t pa[4];
+      acc_to_a(s, kk, pa);
+      mma_ax(o, pa, vt, kk, lane);
+    }
+    __syncthreads();                                     // stage i % FST is free
+    if (i + FST < nblk)
+      stage_kv(Ks + (i % FST) * FKB * ROWB, Vs + (i % FST) * FKB * ROWB, kh, a.ldk, vh, a.ldv, kidx, (i + FST) * FKB,
+               min(FKB, nv - (i + FST) * FKB), FKB, threadIdx.x, blockDim.x);
+    cp_async_commit();
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
+    if (t[r] >= a.Lq) continue;
+    const float inv = l[r] > 0.f ? 1.f / l[r] : 0.f;
+    __nv_bfloat16* dst = ctx + ((long)b * a.Lq + t[r]) * ldo + h * DH + 2 * q;
+#pragma unroll
+    for (int n = 0; n < 4; ++n)
+      *reinterpret_cast<__nv_bfloat162*>(dst + 8 * n) = __floats2bfloat162_rn(o[n][2 * r] * inv, o[n][2 * r + 1] * inv);
+    if (stats && q == 0) {
+      float* st = stats + (((long)b * a.H + h) * a.Lq + t[r]) * 2;
+      st[0] = rk[r].fill ? kMaskFill : m[r] / kLog2e;   // what the reference's softmax subtracts
+      st[1] = l[r];
+    }
+  }
+}
+
+// Three warps of <= 152 registers and ~42 KB shared memory: 4 CTAs per SM, so the B * H = 512 CTAs of the bench step
+// run in one wave on 132 SMs (four warps fit only 3 CTAs per SM, or spill at 128 registers).
+__global__ void __launch_bounds__(BWARPS * 32, 1)
+attn_mma_bwd_kernel(AttnArgs a, const __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __restrict__ d_ctx, long ldo,
+                    const float* __restrict__ stats, __nv_bfloat16* __restrict__ dq, long lddq,
+                    __nv_bfloat16* __restrict__ dk, long lddk, __nv_bfloat16* __restrict__ dv, long lddv) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  extern __shared__ __align__(16) unsigned char mma_smem[];
+  __shared__ int nv_s, filled_s;
+  __shared__ float delta_s[LQ_MAX], m2_s[LQ_MAX], inv_s[LQ_MAX];
+  unsigned char* Qs = mma_smem;                          // [32][32]
+  unsigned char* Os = Qs + LQ_MAX * ROWB;                // [32][32] dO
+  unsigned char* Ws = Os + LQ_MAX * ROWB;                // per warp: K, V [BKB][32]; P, dS [32 rows][BKB keys]; dQ
+  int* kidx = reinterpret_cast<int*>(Ws + BWARPS * BWARP_SMEM);
+  const int b = blockIdx.x / a.H, h = blockIdx.x % a.H;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, q = lane & 3;
+  const unsigned char* km = a.key_mask ? a.key_mask + (long)b * a.Lk : nullptr;
+  const int* rg = a.ranges ? a.ranges + 4 * b : nullptr;
+  const long kvb = rg ? 0 : (long)b * a.Lk;
+  const __nv_bfloat16* kh = (const __nv_bfloat16*)a.k + kvb * a.ldk + h * DH;
+  const __nv_bfloat16* vh = (const __nv_bfloat16*)a.v + kvb * a.ldv + h * DH;
+  unsigned char* Kw = Ws + warp * BWARP_SMEM;
+  unsigned char* Vw = Kw + BKB * ROWB;
+  unsigned char* Pw = Vw + BKB * ROWB;
+  unsigned char* Sw = Pw + LQ_MAX * ROWB;
+  float* dQw = reinterpret_cast<float*>(Sw + LQ_MAX * ROWB);   // [32][32] fp32, swz_f32
+  compact_keys(km, a.Lk, a.causal, kidx, &nv_s, &filled_s, rg);
+  const int nv = nv_s;
+  const bool filled = filled_s != 0;
+  if (warp * BKB < nv) stage_kv(Kw, Vw, kh, a.ldk, vh, a.ldv, kidx, warp * BKB, min(BKB, nv - warp * BKB), BKB, lane, 32);
+  for (int i = threadIdx.x; i < 2 * LQ_MAX * 4; i += blockDim.x) {
+    const int which = i / (LQ_MAX * 4), r = (i >> 2) & (LQ_MAX - 1), c = i & 3;
+    unsigned char* dst = (which ? Os : Qs) + swz(r, c);
+    if (r < a.Lq) cp_async16(su32(dst), which ? d_ctx + ((long)b * a.Lq + r) * ldo + h * DH + c * 8
+                                              : (const __nv_bfloat16*)a.q + ((long)b * a.Lq + r) * a.ldq + h * DH + c * 8);
+    else *reinterpret_cast<uint4*>(dst) = make_uint4(0, 0, 0, 0);
+  }
+  cp_async_commit();
+  // delta_t = dO_t . O_t over the head's 32 features; row statistics
+  if (threadIdx.x < a.Lq) {
+    const int t = threadIdx.x;
+    const __nv_bfloat16* orow = out + ((long)b * a.Lq + t) * ldo + h * DH;
+    const __nv_bfloat16* grow = d_ctx + ((long)b * a.Lq + t) * ldo + h * DH;
+    float d = 0.f;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      float ov[8], gv[8];
+      Act<__nv_bfloat16>::load8(orow + c * 8, ov);
+      Act<__nv_bfloat16>::load8(grow + c * 8, gv);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) d = fmaf(ov[e], gv[e], d);
+    }
+    const float* st = stats + (((long)b * a.H + h) * a.Lq + t) * 2;
+    delta_s[t] = d; m2_s[t] = st[0] * kLog2e; inv_s[t] = 1.f / st[1];
+  }
+  // masked keys receive exactly zero gradient (the mask bytes of 32 keys per ballot, then one row per lane group)
+  if (!filled && !a.causal && km) {
+    const int L = rg ? rg[1] + rg[3] : a.Lk;
+    for (int s0 = 32 * warp; s0 < L; s0 += 32 * BWARPS) {
+      uint32_t dead = __ballot_sync(0xffffffffu, s0 + lane < L && km[s0 + lane] == 0);
+      while (dead) {
+        const int s = s0 + __ffs(dead) - 1;
+        dead &= dead - 1;
+        const long row = rg ? (s < rg[1] ? rg[0] + s : rg[2] + (s - rg[1])) : (long)b * a.Lk + s;
+        dk[row * lddk + h * DH + lane] = __float2bfloat16_rn(0.f);
+        dv[row * lddv + h * DH + lane] = __float2bfloat16_rn(0.f);
+      }
+    }
+  }
+  cp_async_wait<0>();
+  __syncthreads();
+
+  const float k2 = a.scale * kLog2e;
+  const uint32_t mb = causal_mask_bits(a, km, lane);
+  for (int i = lane; i < LQ_MAX * DH / 4; i += 32) reinterpret_cast<float4*>(dQw)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+
+  for (int blk = warp; blk * BKB < nv; blk += BWARPS) {
+    const int c0 = blk * BKB, nc = min(BKB, nv - c0);
+    if (blk != warp) {
+      __syncwarp();                                      // the previous block's tiles are consumed
+      stage_kv(Kw, Vw, kh, a.ldk, vh, a.ldv, kidx, c0, nc, BKB, lane, 32);
+      cp_async_commit();
+      cp_async_wait<0>();
+    }
+    __syncwarp();
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt) {
+      if (16 * mt < a.Lq) {
+        // S = Q K^T -> P (kept in s) ; dP = dO V^T -> dS = P (dP - delta) scale (in s)
+        uint32_t fa[2][4];
+        float s[4][4], dp[4][4];
+#pragma unroll
+        for (int n = 0; n < 4; ++n)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) s[n][e] = dp[n][e] = 0.f;
+        ld_a(Qs, 16 * mt, lane, fa);
+        mma_abt(s, fa, Kw, lane);
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int t = 16 * mt + (lane >> 2) + 8 * r;
+          const bool live = t < a.Lq;
+          const float m2 = live ? m2_s[t] : 0.f, inv = live ? inv_s[t] : 0.f;
+          const RowKeys k = row_keys(a, mb, nv, filled, t);
+#pragma unroll
+          for (int n = 0; n < 4; ++n) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const bool ok = live && key_ok(k, a.causal, c0 + 8 * n + 2 * q + e, nv);
+              float& x = s[n][2 * r + e];
+              x = !ok ? 0.f : (k.fill ? inv : ex2(fmaf(x, k2, -m2)) * inv);
+            }
+            *reinterpret_cast<uint32_t*>(Pw + swz(t, n) + 4 * q) = pack_bf16(s[n][2 * r], s[n][2 * r + 1]);
+          }
+        }
+        ld_a(Os, 16 * mt, lane, fa);
+        mma_abt(dp, fa, Vw, lane);
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int t = 16 * mt + (lane >> 2) + 8 * r;
+          const float dl = t < a.Lq ? delta_s[t] : 0.f;
+          const bool fill = row_keys(a, mb, nv, filled, t).fill;        // masked_fill blocks the gradient
+#pragma unroll
+          for (int n = 0; n < 4; ++n) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              float& x = s[n][2 * r + e];                 // P = 0 where the key is not valid for the row
+              x = fill ? 0.f : x * (dp[n][2 * r + e] - dl) * a.scale;
+            }
+            *reinterpret_cast<uint32_t*>(Sw + swz(t, n) + 4 * q) = pack_bf16(s[n][2 * r], s[n][2 * r + 1]);
+          }
+        }
+        // dQ += dS K (each lane owns its fragment's elements of the warp's dQ partial)
+        float dqa[4][4];
+#pragma unroll
+        for (int n = 0; n < 4; ++n) dqa[n][0] = dqa[n][1] = dqa[n][2] = dqa[n][3] = 0.f;
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk) {
+          uint32_t da[4];
+          acc_to_a(s, kk, da);
+          mma_ax(dqa, da, Kw, kk, lane);
+        }
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+#pragma unroll
+          for (int n = 0; n < 4; ++n) {
+            float2& d = *reinterpret_cast<float2*>(dQw + swz_f32(16 * mt + (lane >> 2) + 8 * r, 8 * n + 2 * q));
+            d.x += dqa[n][2 * r];
+            d.y += dqa[n][2 * r + 1];
+          }
+      }
+    }
+    __syncwarp();                                        // P / dS of the block are in shared memory
+    // dK = dS^T Q, dV = P^T dO: M = the block's keys, K = query rows, N = features
+#pragma unroll 1
+    for (int which = 0; which < 2; ++which) {
+      const unsigned char* At = which ? Pw : Sw;
+      const unsigned char* Bt = which ? Os : Qs;
+      float acc[2][4][4];
+#pragma unroll
+      for (int mk = 0; mk < 2; ++mk)
+#pragma unroll
+        for (int n = 0; n < 4; ++n) acc[mk][n][0] = acc[mk][n][1] = acc[mk][n][2] = acc[mk][n][3] = 0.f;
+#pragma unroll
+      for (int kk = 0; kk < 2; ++kk) {
+        if (16 * kk >= a.Lq) break;
+#pragma unroll
+        for (int mk = 0; mk < 2; ++mk) {
+          uint32_t at[4];
+          ldsm4_t(su32(At + swz(16 * kk + (lane & 7) + (lane >> 4) * 8, 2 * mk + ((lane >> 3) & 1))), at);
+          mma_ax(acc[mk], at, Bt, kk, lane);
+        }
+      }
+      __nv_bfloat16* dst = which ? dv : dk;
+      const long ld = which ? lddv : lddk;
+#pragma unroll
+      for (int mk = 0; mk < 2; ++mk)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int j = 16 * mk + (lane >> 2) + 8 * r;
+          if (j < nc) {
+            __nv_bfloat16* row = dst + (kvb + kidx[c0 + j]) * ld + h * DH + 2 * q;
+#pragma unroll
+            for (int n = 0; n < 4; ++n)
+              *reinterpret_cast<__nv_bfloat162*>(row + 8 * n) = __floats2bfloat162_rn(acc[mk][n][2 * r], acc[mk][n][2 * r + 1]);
+          }
+        }
+    }
+  }
+  // dQ: the sum of the warps' partials
+  __syncthreads();
+  for (int i = threadIdx.x; i < a.Lq * DH; i += blockDim.x) {
+    const int t = i / DH, f = i % DH;
+    float x = 0.f;
+#pragma unroll
+    for (int w = 0; w < BWARPS; ++w)
+      x += reinterpret_cast<const float*>(Ws + w * BWARP_SMEM + 4 * BKB * ROWB)[swz_f32(t, f)];
+    dq[((long)b * a.Lq + t) * lddq + h * DH + f] = __float2bfloat16_rn(x);
+  }
+}
+
+size_t fwd_smem(int Lk) { return (size_t)2 * FST * FKB * ROWB + sizeof(int) * (size_t)Lk; }
+size_t bwd_smem(int Lk) { return (size_t)2 * LQ_MAX * ROWB + (size_t)BWARPS * BWARP_SMEM + sizeof(int) * (size_t)Lk; }
+
+}  // namespace mma
+
 size_t fwd_smem(int Lq, int Lk) {
   return sizeof(float) * ((size_t)2 * KC * KPAD + (size_t)Lq * KPAD + (size_t)NWARPS * 2 * KC) + sizeof(int) * (size_t)Lk;
 }
@@ -337,8 +790,7 @@ int check_layout(const char* name, const void* p, long ld, int dtype) {
 namespace {
 
 int attn_fwd_impl(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
-                  const unsigned char* key_mask, const int* ranges, long kv_rows, int max_chunks, int causal, void* ctx,
-                  long ldo, float* stats, int B, int H, int Lq, int Lk, int d_head, int dtype, void* stream) {
+                  const unsigned char* key_mask, const int* ranges, int causal, void* ctx, long ldo, float* stats, int B, int H, int Lq, int Lk, int d_head, int dtype, void* stream) {
   FIRA_CHECK_ARG(d_head == DH, FIRA_ERR_SHAPE, "attn_fwd: d_head %d != 32", d_head);
   FIRA_CHECK_ARG(B > 0 && H > 0 && Lq > 0 && Lk > 0 && Lq <= LQ_MAX, FIRA_ERR_SHAPE, "attn_fwd: shape (Lq <= 32)");
   FIRA_CHECK_ARG(!causal || (Lq == Lk && !ranges), FIRA_ERR_SHAPE, "attn_fwd: causal needs Lq == Lk and no ranges");
@@ -348,9 +800,15 @@ int attn_fwd_impl(const void* q, long ldq, const void* k, long ldk, const void* 
   if ((rc = check_layout("attn_fwd", q, ldq, dtype)) || (rc = check_layout("attn_fwd", k, ldk, dtype)) ||
       (rc = check_layout("attn_fwd", v, ldv, dtype)))
     return rc;
-  if (use_tc(dtype, B, H, Lq, Lk, d_head, ldk, ldv, max_chunks))
-    return fira_attn_tc_fwd(q, ldq, k, ldk, v, ldv, key_mask, ranges, kv_rows, causal, ctx, ldo, stats, B, H, Lq, Lk, stream);
   AttnArgs a{q, ldq, k, ldk, v, ldv, key_mask, ranges, causal, B, H, Lq, Lk, 1.f / sqrtf((float)d_head)};
+  if (use_tc(dtype)) {
+    const size_t smem = mma::fwd_smem(Lk);
+    if ((rc = set_smem(mma::attn_mma_fwd_kernel, smem, "attn_fwd"))) return rc;
+    launch_k(mma::attn_mma_fwd_kernel, dim3(B * H), dim3(32 * ((Lq + 15) / 16)), smem, (cudaStream_t)stream, a,
+             (__nv_bfloat16*)ctx, ldo, stats);
+    FIRA_CHECK_LAUNCH("fira_attn_fwd (mma)");
+    return FIRA_OK;
+  }
   const size_t smem = fwd_smem(Lq, Lk);
   if (dtype == FIRA_F32) {
     if ((rc = set_smem(attn_fwd_kernel<float>, smem, "attn_fwd"))) return rc;
@@ -364,8 +822,7 @@ int attn_fwd_impl(const void* q, long ldq, const void* k, long ldk, const void* 
 }
 
 int attn_bwd_impl(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
-                  const unsigned char* key_mask, const int* ranges, long kv_rows, int max_chunks, int causal,
-                  const void* ctx, const void* d_ctx, long ldo, const float* stats, void* dq, long lddq, void* dk,
+                  const unsigned char* key_mask, const int* ranges, int causal, const void* ctx, const void* d_ctx, long ldo, const float* stats, void* dq, long lddq, void* dk,
                   long lddk, void* dv, long lddv, int B, int H, int Lq, int Lk, int d_head, int dtype, void* stream) {
   FIRA_CHECK_ARG(d_head == DH, FIRA_ERR_SHAPE, "attn_bwd: d_head %d != 32", d_head);
   FIRA_CHECK_ARG(B > 0 && H > 0 && Lq > 0 && Lk > 0 && Lq <= LQ_MAX, FIRA_ERR_SHAPE, "attn_bwd: shape (Lq <= 32)");
@@ -376,11 +833,16 @@ int attn_bwd_impl(const void* q, long ldq, const void* k, long ldk, const void* 
       (rc = check_layout("attn_bwd", v, ldv, dtype)) || (rc = check_layout("attn_bwd", ctx, ldo, dtype)) ||
       (rc = check_layout("attn_bwd", d_ctx, ldo, dtype)))
     return rc;
-  if (use_tc(dtype, B, H, Lq, Lk, d_head, ldk, ldv, max_chunks) && (lddk % 8) == 0 && (lddv % 8) == 0 &&
-      (lddq % 8) == 0)
-    return fira_attn_tc_bwd(q, ldq, k, ldk, v, ldv, key_mask, ranges, kv_rows, causal, ctx, d_ctx, ldo, stats, dq, lddq,
-                            dk, lddk, dv, lddv, B, H, Lq, Lk, stream);
   AttnArgs a{q, ldq, k, ldk, v, ldv, key_mask, ranges, causal, B, H, Lq, Lk, 1.f / sqrtf((float)d_head)};
+  if (use_tc(dtype) && (lddk % 8) == 0 && (lddv % 8) == 0 && (lddq % 8) == 0) {
+    const size_t smem = mma::bwd_smem(Lk);
+    if ((rc = set_smem(mma::attn_mma_bwd_kernel, smem, "attn_bwd"))) return rc;
+    launch_k(mma::attn_mma_bwd_kernel, dim3(B * H), dim3(mma::BWARPS * 32), smem, (cudaStream_t)stream, a,
+             (const __nv_bfloat16*)ctx, (const __nv_bfloat16*)d_ctx, ldo, stats, (__nv_bfloat16*)dq, lddq,
+             (__nv_bfloat16*)dk, lddk, (__nv_bfloat16*)dv, lddv);
+    FIRA_CHECK_LAUNCH("fira_attn_bwd (mma)");
+    return FIRA_OK;
+  }
   const size_t smem = bwd_smem(Lq, Lk);
   if (dtype == FIRA_F32) {
     if ((rc = set_smem(attn_bwd_kernel<float>, smem, "attn_bwd"))) return rc;
@@ -404,7 +866,7 @@ int fira_attn_fwd(const void* q, long ldq, const void* k, long ldk, const void* 
                   const unsigned char* key_mask, int causal, void* ctx, long ldo, float* stats, int B, int H, int Lq,
                   int Lk, int d_head, int dtype, void* stream) {
   FIRA_CHECK_ARG(key_mask, FIRA_ERR_ARG, "attn_fwd: null key_mask");
-  return attn_fwd_impl(q, ldq, k, ldk, v, ldv, key_mask, nullptr, (long)B * Lk, (Lk + 127) / 128, causal, ctx, ldo, stats,
+  return attn_fwd_impl(q, ldq, k, ldk, v, ldv, key_mask, nullptr, causal, ctx, ldo, stats,
                        B, H, Lq, Lk, d_head, dtype, stream);
 }
 
@@ -413,15 +875,15 @@ int fira_attn_bwd(const void* q, long ldq, const void* k, long ldk, const void* 
                   const float* stats, void* dq, long lddq, void* dk, long lddk, void* dv, long lddv, int B, int H,
                   int Lq, int Lk, int d_head, int dtype, void* stream) {
   FIRA_CHECK_ARG(key_mask, FIRA_ERR_ARG, "attn_bwd: null key_mask");
-  return attn_bwd_impl(q, ldq, k, ldk, v, ldv, key_mask, nullptr, (long)B * Lk, (Lk + 127) / 128, causal, ctx, d_ctx, ldo,
+  return attn_bwd_impl(q, ldq, k, ldk, v, ldv, key_mask, nullptr, causal, ctx, d_ctx, ldo,
                        stats, dq, lddq, dk, lddk, dv, lddv, B, H, Lq, Lk, d_head, dtype, stream);
 }
 
 int fira_attn_packed_fwd(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv, const int* ranges,
                          long kv_rows, const unsigned char* key_mask, int mask_pitch, int max_chunks, void* ctx, long ldo,
                          float* stats, int B, int H, int Lq, int d_head, int dtype, void* stream) {
-  FIRA_CHECK_ARG(ranges && kv_rows > 0 && max_chunks > 0, FIRA_ERR_ARG, "attn_packed_fwd: ranges / kv_rows / max_chunks");
-  return attn_fwd_impl(q, ldq, k, ldk, v, ldv, key_mask, ranges, kv_rows, max_chunks, 0, ctx, ldo, stats, B, H, Lq,
+  FIRA_CHECK_ARG(ranges && kv_rows > 0, FIRA_ERR_ARG, "attn_packed_fwd: ranges / kv_rows");
+  return attn_fwd_impl(q, ldq, k, ldk, v, ldv, key_mask, ranges, 0, ctx, ldo, stats, B, H, Lq,
                        mask_pitch, d_head, dtype, stream);
 }
 
@@ -429,8 +891,8 @@ int fira_attn_packed_bwd(const void* q, long ldq, const void* k, long ldk, const
                          long kv_rows, const unsigned char* key_mask, int mask_pitch, int max_chunks, const void* ctx,
                          const void* d_ctx, long ldo, const float* stats, void* dq, long lddq, void* dk, long lddk,
                          void* dv, long lddv, int B, int H, int Lq, int d_head, int dtype, void* stream) {
-  FIRA_CHECK_ARG(ranges && kv_rows > 0 && max_chunks > 0, FIRA_ERR_ARG, "attn_packed_bwd: ranges / kv_rows / max_chunks");
-  return attn_bwd_impl(q, ldq, k, ldk, v, ldv, key_mask, ranges, kv_rows, max_chunks, 0, ctx, d_ctx, ldo, stats, dq, lddq,
+  FIRA_CHECK_ARG(ranges && kv_rows > 0, FIRA_ERR_ARG, "attn_packed_bwd: ranges / kv_rows");
+  return attn_bwd_impl(q, ldq, k, ldk, v, ldv, key_mask, ranges, 0, ctx, d_ctx, ldo, stats, dq, lddq,
                        dk, lddk, dv, lddv, B, H, Lq, mask_pitch, d_head, dtype, stream);
 }
 

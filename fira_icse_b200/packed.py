@@ -29,7 +29,7 @@ class PackedBatch:
     def __init__(self, B, Rc, Rs, Ra, S, T, nnz, chunks=4, **tensors):
         self.B, self.Rc, self.Rs, self.Ra, self.S, self.T, self.nnz = B, Rc, Rs, Ra, S, T, nnz
         # bound on the 128-key chunks cross-attention needs for any commit of the batch (3 on the whole shipped DataSet:
-        # <= 200 code tokens, <= 102 sub-tokens); part of the shape key because it selects the attention kernel
+        # <= 200 code tokens, <= 102 sub-tokens); passed to the packed attention entry points, which do not use it
         self.chunks = int(chunks)
         for k in self.FIELDS:
             setattr(self, k, tensors[k])

@@ -212,8 +212,7 @@ int fira_attn_bwd(const void* q, long ldq, const void* k, long ldk, const void* 
 /* Cross-attention of a PACKED batch (fira_icse_b200/packed.py): the keys / values of commit b are two row ranges of
  * k / v, ranges[b] = {first row, rows, first row, rows} (code rows, sub-token rows; GLOBAL row ids, kv_rows = rows of
  * k / v), key_mask [B, mask_pitch] over the commit's own key positions (NULL: all valid), mask_pitch >= rows of any
- * commit; max_chunks = an upper bound the caller guarantees on ceil(rows0 / 128) + ceil(rows1 / 128) of any commit
- * (fira_host_packed_dims reports it; <= 3 lets bf16 run on the wgmma kernels).  Rows of dk / dv outside every range
+ * commit; max_chunks is not used (any number of keys per commit is supported).  Rows of dk / dv outside every range
  * are not written (fira_zero_pad_rows clears the segment padding). */
 int fira_attn_packed_fwd(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv, const int* ranges,
                          long kv_rows, const unsigned char* key_mask, int mask_pitch, int max_chunks, void* ctx, long ldo,

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """A/B timings of single kernels with CUDA events (warm L2 like inside a training step, 20 launches after 5 warm-ups),
-at the shapes the bf16 bench step launches: attention forward/backward (FFMA vs wgmma, FIRA_ATTN_TC) and the GCN layer
+at the shapes the bf16 bench step launches: attention forward/backward (FFMA vs tensor cores, FIRA_ATTN_TC) and the GCN layer
 (scatter + GEMM + LayerNorm vs the fused kernel, forward and backward).  One JSON line per measurement.
 
     python tools/bench_kernels.py [--batch 64]
@@ -51,35 +51,60 @@ def st():
 
 
 def attention(B, out):
+    """Padded cross / causal self-attention, the packed cross-attention of the bench's first synthetic batch and one
+    incremental-decoding position (5 beams against 30 cached keys, no statistics), each on the FFMA kernels
+    (FIRA_ATTN_TC=0) and on the tensor cores."""
     from fira_icse_b200 import _lib
+    from fira_icse_b200.packed import PackedTables, pack_from_dataset
+    from fira_icse_b200.synth import SynthDataset
     H, T, dh, D = 8, 30, 32, 256
     g = torch.Generator().manual_seed(0)
-    for name, Lk, causal, valid in (("cross S=304 (127 valid)", 304, 0, 127), ("cross S=370 (all valid)", 370, 0, 370),
-                                    ("self T=30 causal", 30, 1, 30)):
-        q = torch.randn(B * T, D, generator=g).to(BF).to(DEV)
-        kv = torch.randn(B * Lk, 2 * D, generator=g).to(BF).to(DEV)
+    cases = []
+    for name, Lq, Lk, causal, valid, with_bwd in (("cross S=304 (127 valid)", T, 304, 0, 127, True),
+                                                   ("cross S=370 (all valid)", T, 370, 0, 370, True),
+                                                   ("self T=30 causal", T, 30, 1, 30, True),
+                                                   ("incremental Lq=5 Lk=30 (no stats)", 5, 30, 0, 30, False)):
         mask = torch.zeros(B, Lk, dtype=torch.uint8)
         mask[:, :valid] = 1
-        mask = mask.to(DEV)
-        ctx = torch.empty(B * T, D, device=DEV, dtype=BF)
-        stats = torch.empty(B, H, T, 2, device=DEV)
-        go = torch.randn(B * T, D, generator=g).to(BF).to(DEV)
+        cases.append((name, Lq, torch.randn(B * Lk, 2 * D, generator=g).to(BF).to(DEV), 2 * D, mask.to(DEV), None,
+                      Lk, causal, with_bwd))
+    # the bench step's cross-attention: K / V of layer 0 of the [Ms, 6 layers x 512] projection of the packed memory
+    pb = pack_from_dataset(PackedTables(SynthDataset(0, B, 24650, 71)), np.arange(B), 24650).to(DEV)
+    Ms = pb.Rc + pb.Rs
+    cases.append((f"packed cross, bench batch 0 (S={pb.S}, {int(pb.mem_mask.sum())} valid keys)", T,
+                  torch.randn(Ms, 12 * D, generator=g).to(BF).to(DEV), 12 * D, pb.mem_mask, pb, pb.S, 0, True))
+    for name, Lq, kv, ld, mask, pk, Lk, causal, with_bwd in cases:
+        q = torch.randn(B * Lq, D, generator=g).to(BF).to(DEV)
+        ctx = torch.empty(B * Lq, D, device=DEV, dtype=BF)
+        stats = torch.empty(B, H, Lq, 2, device=DEV) if with_bwd else None
+        go = torch.randn(B * Lq, D, generator=g).to(BF).to(DEV)
         dq, dkv = torch.empty_like(q), torch.zeros_like(kv)
-        ld = 2 * D
+        sp = stats.data_ptr() if stats is not None else None
 
         def fwd():
-            _lib.call("fira_attn_fwd", q.data_ptr(), D, kv.data_ptr(), ld, kv.data_ptr() + D * 2, ld, mask.data_ptr(), causal,
-                      ctx.data_ptr(), D, stats.data_ptr(), B, H, T, Lk, dh, 1, st())
+            if pk is None:
+                _lib.call("fira_attn_fwd", q.data_ptr(), D, kv.data_ptr(), ld, kv.data_ptr() + D * 2, ld, mask.data_ptr(),
+                          causal, ctx.data_ptr(), D, sp, B, H, Lq, Lk, dh, 1, st())
+            else:
+                _lib.call("fira_attn_packed_fwd", q.data_ptr(), D, kv.data_ptr(), ld, kv.data_ptr() + D * 2, ld,
+                          pk.ranges.data_ptr(), kv.shape[0], mask.data_ptr(), Lk, pk.chunks, ctx.data_ptr(), D, sp, B, H,
+                          Lq, dh, 1, st())
 
         def bwd():
-            _lib.call("fira_attn_bwd", q.data_ptr(), D, kv.data_ptr(), ld, kv.data_ptr() + D * 2, ld, mask.data_ptr(), causal,
-                      ctx.data_ptr(), go.data_ptr(), D, stats.data_ptr(), dq.data_ptr(), D, dkv.data_ptr(), ld,
-                      dkv.data_ptr() + D * 2, ld, B, H, T, Lk, dh, 1, st())
+            if pk is None:
+                _lib.call("fira_attn_bwd", q.data_ptr(), D, kv.data_ptr(), ld, kv.data_ptr() + D * 2, ld, mask.data_ptr(),
+                          causal, ctx.data_ptr(), go.data_ptr(), D, sp, dq.data_ptr(), D, dkv.data_ptr(), ld,
+                          dkv.data_ptr() + D * 2, ld, B, H, Lq, Lk, dh, 1, st())
+            else:
+                _lib.call("fira_attn_packed_bwd", q.data_ptr(), D, kv.data_ptr(), ld, kv.data_ptr() + D * 2, ld,
+                          pk.ranges.data_ptr(), kv.shape[0], mask.data_ptr(), Lk, pk.chunks, ctx.data_ptr(), go.data_ptr(),
+                          D, sp, dq.data_ptr(), D, dkv.data_ptr(), ld, dkv.data_ptr() + D * 2, ld, B, H, Lq, dh, 1, st())
         for tc in ("0", "1"):
             os.environ["FIRA_ATTN_TC"] = tc
             fwd()
-            out({"kernel": "attention fwd", "case": name, "wgmma": tc == "1", **timeit(fwd)})
-            out({"kernel": "attention bwd", "case": name, "wgmma": tc == "1", **timeit(bwd)})
+            out({"kernel": "attention fwd", "case": name, "tensor_cores": tc == "1", **timeit(fwd)})
+            if with_bwd:
+                out({"kernel": "attention bwd", "case": name, "tensor_cores": tc == "1", **timeit(bwd)})
     os.environ.pop("FIRA_ATTN_TC", None)
 
 
