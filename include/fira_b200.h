@@ -294,6 +294,20 @@ int fira_pointer_mix_beam_step(const void* logits, long ld_logits, const float* 
                                float* logprob, float* score, unsigned char* status, long* parent, int* next_tok,
                                int T_len, int pos, int B, int K, int V, int S, int dtype, void* stream);
 
+/* ---- minimum-Bayes-risk selection among each commit's N samples (fira_icse_b200/mbr.py).  seq [B, N, ld_seq] int32
+ *      (row (b, n) at (b*N + n) * ld_seq, columns 0..T_len-1), length [B, N] int32 (counts <start>; clamped to
+ *      [1, T_len]).  Rule:
+ *        words_n   = seq[b, n, 1:length[b, n]] without every id equal to start_id, eos_id or pad_id
+ *        BLEU(i,j) = bleu.sentence_bleu_method2([words_j], words_i) over the ids, in float64: clipped n-gram matches,
+ *                    n = 1..4; denominator max(1, c - n + 1) (c = len(words_i)), +1 on numerator and denominator for
+ *                    n >= 2; 0 for c = 0 or no unigram match; BP = 1 if c > r else exp(1 - r / c), r = len(words_j)
+ *        U_i       = (sum over j != i, j ascending, of BLEU(i, j)) / (N - 1)      (fixed order, no atomics)
+ *        best[b]   = the smallest i with the largest U_i
+ *      utility [B, N] float64; pair_bleu [B, N, N] float64 (pair_bleu[b, i, j] = BLEU(i, j), diagonal included) or
+ *      NULL.  2 <= N <= 32, 2 <= T_len <= 32, ld_seq >= T_len, B >= 0 (B = 0: nothing is launched). */
+int fira_mbr_select(const int* seq, const int* length, long ld_seq, int start_id, int eos_id, int pad_id,
+                    double* pair_bleu, double* utility, int* best, int B, int N, int T_len, void* stream);
+
 /* ---- HOST-side batch preparation (CPU only: every pointer below is HOST memory, there is no stream).
  *
  * fira_host_build_adjacency: the commit graph of Dataset.py:220-294 + process_edge (Dataset.py:346-357).

@@ -25,6 +25,10 @@ beam search ranking.  Differences, all below the module surface:
     OUTPUT/output_fira_nbest: FIRA_BEAM consecutive lines per commit in test order, best first,
     `<score>\t<log-probability>\t<message>`; FIRA_LENGTH_PENALTY (default 0 = rank by log-probability) sets the
     penalty alpha of score = logprob / ((5 + n) / 6) ** alpha; prints the mean sentence BLEU of the top hypothesis.
+    FIRA_DECODE=mbr: minimum-Bayes-risk decoding (fira_icse_b200.mbr) -> OUTPUT/output_fira_mbr: one line per commit in
+    test order, `<expected BLEU>\\t<log-probability>\\t<message>`, the commit's sample with the highest mean id-level
+    sentence BLEU against its other samples; FIRA_SAMPLES (default 16 here), FIRA_TEMPERATURE, FIRA_TOP_K, FIRA_TOP_P
+    and FIRA_SEED as for sampling; prints the mean sentence BLEU of the chosen messages.
 """
 import json
 import os
@@ -42,6 +46,7 @@ from fira_icse_b200.beam import beam_search, best_sequences, nbest
 from fira_icse_b200.bleu import sentence_bleu_method2
 from fira_icse_b200.data import PackedBatchLoader, TransDataset, batch_to_device, collate_packed
 from fira_icse_b200.engine import GraphedTrainStep
+from fira_icse_b200.mbr import mbr
 from fira_icse_b200.parallel import DataParallelStep, shard_range
 from fira_icse_b200.sample import sample
 
@@ -233,16 +238,22 @@ def decoder(mode, vocab):
             best, blen = best_sequences(*beams)
             return best.unsqueeze(1), blen.unsqueeze(1), ()
         return "output_fira", decode, 1
-    if mode == "sample":                # FIRA_SAMPLES seeded samples, `<log-prob>\t<message>`
-        n = int(os.environ.get("FIRA_SAMPLES", 3))
+    if mode in ("sample", "mbr"):       # FIRA_SAMPLES seeded samples per commit
+        n = int(os.environ.get("FIRA_SAMPLES", 16 if mode == "mbr" else 3))
         opts = dict(num_samples=n, temperature=float(os.environ.get("FIRA_TEMPERATURE", 1.0)),
                     top_k=int(os.environ.get("FIRA_TOP_K", 0)), top_p=float(os.environ.get("FIRA_TOP_P", 1.0)),
                     seed=int(os.environ.get("FIRA_SEED", 0)))
-
+    if mode == "sample":                # every sample, `<log-prob>\t<message>`
         def decode(model, b, first_index):
             out = sample(model, b[0], b[3], b[4], b[5], b[7], first_index=first_index, **opts, **ids)
             return out.seq, out.length, (out.logprob,)
         return "output_fira_samples", decode, n
+    if mode == "mbr":                   # the sample of highest expected BLEU, `<expected BLEU>\t<log-prob>\t<message>`
+        def decode(model, b, first_index):
+            out = mbr(model, b[0], b[3], b[4], b[5], b[7], first_index=first_index, **opts, **ids)
+            expected = out.utility.gather(1, out.index.unsqueeze(1))
+            return out.seq.unsqueeze(1), out.length.unsqueeze(1), (expected, out.logprob.unsqueeze(1))
+        return "output_fira_mbr", decode, 1
     if mode == "nbest":                 # FIRA_BEAM hypotheses best first, `<score>\t<log-prob>\t<message>`
         alpha = float(os.environ.get("FIRA_LENGTH_PENALTY", 0.0))
 
@@ -250,7 +261,7 @@ def decoder(mode, vocab):
             out = nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=args.beam_size, length_penalty=alpha, **ids)
             return out.seq, out.length, (out.score, out.logprob)
         return "output_fira_nbest", decode, 1
-    raise SystemExit("FIRA_DECODE must be 'beam', 'sample' or 'nbest'")
+    raise SystemExit("FIRA_DECODE must be 'beam', 'sample', 'nbest' or 'mbr'")
 
 
 def test(model, test_loader, g, test_index, dev_, first_index, decode, n_bleu, out_path):

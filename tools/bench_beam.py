@@ -7,16 +7,24 @@ reference's own loop was timed on in BASELINE.md (72 s for 32 commits on CPU).  
 (batch, beam) configuration; timing with CUDA events around whole batches, inputs resident on the device.
 
     python tools/bench_beam.py [--batches 20,128] [--beams 3,5] [--precision fp32|bf16] [--reps 3]
-                               [--modes full,graph,sample,nbest]   (sample: N = the beam width;
-                               nbest: beam.nbest, log-space n-best beam search with length_penalty 0)
+                               [--modes full,graph,sample,nbest,mbr]   (sample: N = the beam width;
+                               nbest: beam.nbest, log-space n-best beam search with length_penalty 0;
+                               mbr: mbr.mbr over N = the beam width samples)
+
+mbr also prints one line for fira_mbr_select alone on the batch's own samples: the median device time per launch
+(bench.time_launches: launches replayed from a CUDA graph between CUDA events), next to the host time of the same
+selection with bleu.sentence_bleu_method2 (tests/mbr_rule.py, one pass over the batch) and the largest utility difference
+between the two.
 """
 import argparse
 import json
 import os
 import sys
+import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))     # mbr_rule: the host restatement the selection is compared with
 
 
 def main():
@@ -35,6 +43,7 @@ def main():
     import fira_icse_b200 as F
     from fira_icse_b200 import _lib
     from fira_icse_b200.beam import beam_search, nbest
+    from fira_icse_b200.mbr import mbr
     from fira_icse_b200.sample import sample
     dev = torch.device("cuda", 0)
     torch.manual_seed(0)
@@ -49,6 +58,9 @@ def main():
                 if mode == "sample":                                 # N = the beam width, default T / k / p
                     return sample(model, b[0], b[3], b[4], b[5], b[7], num_samples=K, tar_len=30, start_id=1, eos_id=2,
                                   pad_id=0)
+                if mode == "mbr":
+                    return mbr(model, b[0], b[3], b[4], b[5], b[7], num_samples=K, tar_len=30, start_id=1, eos_id=2,
+                               pad_id=0)
                 if mode == "nbest":
                     return nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=K, tar_len=30, start_id=1, eos_id=2,
                                  pad_id=0)
@@ -57,27 +69,60 @@ def main():
             ref = run()                                              # warm-up (lazy CUDA state, graph capture)
             if mode == "full":
                 ref_full = ref
-            same = bool(torch.equal(ref[0], ref_full[0])) if "full" in a.modes.split(",") and mode not in ("sample", "nbest") else None
+            same = bool(torch.equal(ref[0], ref_full[0])) if "full" in a.modes.split(",") and mode not in ("sample", "nbest", "mbr") else None
             torch.cuda.synchronize()
             n0 = _lib.LAUNCH_COUNT
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             for _ in range(a.reps):
                 out = run()
-            length = out.length if mode in ("sample", "nbest") else out[1]
+            length = out.samples.length if mode == "mbr" else out.length if mode in ("sample", "nbest") else out[1]
             e1.record()
             torch.cuda.synchronize()
             ms = e0.elapsed_time(e1) / a.reps
+            metric = {"sample": "sampling", "mbr": "mbr"}.get(mode, "beam-search") + " inference throughput"
             print(json.dumps({
-                "metric": "sampling inference throughput" if mode == "sample" else "beam-search inference throughput", "unit": "commits/s", "value": B / ms * 1e3,
+                "metric": metric, "unit": "commits/s", "value": B / ms * 1e3,
                 "ms_per_batch": ms, "batch": B, "beam": K, "decoded_steps": int(length.max().item()) - 1,
                 "precision": a.precision, "mode": mode, "ids_equal_full_mode": same, "trimmed": bool(a.trim), "data": "synthetic (DataSet distribution), random weights",
                 "c_abi_calls_per_batch": (_lib.LAUNCH_COUNT - n0) // a.reps,
                 "note": "encoder once per batch; full = 30-position decoder re-run per step over all live beams, "
                         "graph = newest row against K/V caches as CUDA-graph replays, "
                         "sample = beam-width seeded samples per commit (T = 1, no top-k / top-p), one graph per position, "
-                        "nbest = log-space n-best beam search (length_penalty 0), one graph per position"}),
+                        "nbest = log-space n-best beam search (length_penalty 0), one graph per position, "
+                        "mbr = sample + one fira_mbr_select launch"}),
                   flush=True)
+            if mode == "mbr":
+                print(json.dumps(mbr_select_timing(out.samples, B, K)), flush=True)
+
+
+def mbr_select_timing(s, B, N):
+    """fira_mbr_select alone on the samples `s` of one batch, against the host restatement of the same selection."""
+    import torch
+    import bench
+    from fira_icse_b200 import ops
+    from fira_icse_b200._lib import call
+    from mbr_rule import select
+    T = s.seq.shape[2]
+    seq, length = s.seq.to(torch.int32), s.length.to(torch.int32)
+    utility = torch.empty((B, N), dtype=torch.float64, device=seq.device)
+    best = torch.empty(B, dtype=torch.int32, device=seq.device)
+
+    def launch(_):
+        call("fira_mbr_select", ops._ptr(seq), ops._ptr(length), T, 1, 2, 0, None, ops._ptr(utility), ops._ptr(best),
+             B, N, T, ops._stream())
+    _, med_ms, launches = bench.time_launches(launch, 1, reps=20)
+    host_seq, host_len = s.seq.cpu().tolist(), s.length.cpu().tolist()
+    t0 = time.perf_counter()
+    host = [select(host_seq[c], host_len[c], 1, 2, 0) for c in range(B)]
+    host_s = time.perf_counter() - t0
+    diff = max(abs(u - h) for c in range(B) for u, h in zip(utility[c].tolist(), host[c][1]))
+    return {"metric": "fira_mbr_select time", "unit": "us", "value": med_ms * 1e3, "batch": B, "samples": N,
+            "timed_launches": launches, "host_sentence_bleu_method2_us": host_s * 1e6,
+            "host_pair_evaluations": B * N * N, "max_abs_utility_diff_vs_host": diff,
+            "same_choice_as_host": all(int(best[c]) == host[c][2] for c in range(B)),
+            "note": "median device time per launch, launches replayed from one CUDA graph between CUDA events; host = "
+                    "the float64 restatement (tests/mbr_rule.py) over the same batch, one pass, one host thread"}
 
 
 if __name__ == "__main__":
