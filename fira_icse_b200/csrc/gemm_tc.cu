@@ -220,9 +220,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (p.tma_store) {
     // ---- bf16 output through TMA: each warp converts its 32 rows, 64 columns at a time, into a [32 x 64] bf16 box in
     // the SWIZZLE_128B layout (conflict-free 16-byte st.shared: lane = row, chunk slot = chunk ^ (row & 7)) and one
-    // elected lane hands the box to the TMA engine; rows / columns past M / N are clipped by the tensor map.
+    // elected lane hands the box to the TMA engine; rows past M and columns past N8 = N rounded down to 8 are clipped by
+    // the tensor map (it ends on a 16-byte boundary: a map ending inside a 16-byte chunk lets the store write the rest
+    // of that chunk, i.e. columns of C past N).  Columns [N8, N) go out as plain stores from the staging box.
     unsigned char* cst = sm + acc_region_bytes<BN, STAGES>() + (size_t)quarter * (BN / 64) * 4096;
     const int m = mrow0 + lane;
+    const int n8 = p.N & ~7;
     const float rsm = (p.rs && m < p.M) ? p.rs[m] : 0.f;
     if (warp == 0 && lane == 0) stamp(p, 6);
     const __nv_bfloat16* mrow = nullptr;            // relu-backward mask: this lane's row of the forward activations
@@ -233,6 +236,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
 #pragma unroll 1
     for (int g = colhalf; g < BN / 64; g += 2) {
+      const int gc = n0 + g * 64;                   // first column of the box
       uint4 mk[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) mk[j] = make_uint4(0x3f803f80u, 0x3f803f80u, 0x3f803f80u, 0x3f803f80u);   // 1.0: keep
@@ -277,9 +281,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           *reinterpret_cast<uint4*>(cst + g * 4096 + lane * 128 + ((chunk ^ (lane & 7)) << 4)) = o;
         }
       }
+      if (n8 < p.N && gc <= n8 && n8 < gc + 64 && m < p.M) {
+        // columns [N8, N) lie in one 16-byte chunk of this lane's staged row: copy them out of the staging box
+        const int ch = (n8 - gc) >> 3;
+        const __nv_bfloat16* src = reinterpret_cast<const __nv_bfloat16*>(cst + g * 4096 + lane * 128 + ((ch ^ (lane & 7)) << 4));
+        __nv_bfloat16* dst = (__nv_bfloat16*)p.C + (long)m * p.ldc + n8;
+        for (int e = 0; e < p.N - n8; ++e) dst[e] = src[e];
+      }
       fence_proxy_async();
       __syncwarp();
-      if (lane == 0 && n0 + g * 64 < p.N && mrow0 < p.M) tma_store_2d(&tmC, smem_addr(cst + g * 4096), n0 + g * 64, mrow0);
+      if (lane == 0 && gc < n8 && mrow0 < p.M) tma_store_2d(&tmC, smem_addr(cst + g * 4096), n0 + g * 64, mrow0);
     }
     if (lane == 0) tma_store_commit_wait_read();
     __syncwarp();
@@ -475,10 +486,10 @@ int gemm_tc_impl(const void* A, long lda, int a_kmajor, const void* B, long ldb,
   splits = (kb_total + per - 1) / per;
   // bf16 output that is neither accumulated nor split: written by TMA from a swizzled staging tile ([32 rows x 64
   // columns] boxes); everything else takes the register / shared-memory epilogue
-  const int tma_store = (c_is_bf16 && !accumulate && splits == 1 && (ldc % 8) == 0 && tma_store_on()) ? 1 : 0;
+  const int tma_store = (c_is_bf16 && !accumulate && splits == 1 && (ldc % 8) == 0 && N >= 8 && tma_store_on()) ? 1 : 0;
   CUtensorMap tc = ta;
   if (tma_store) {
-    rc_ = make_map(&tc, C, M, N, ldc, 64, 32);
+    rc_ = make_map(&tc, C, M, N & ~7, ldc, 64, 32);     // columns [N & ~7, N): plain stores in the epilogue
     if (rc_) return rc_;
   }
   FIRA_CHECK_ARG(relu_mask == nullptr || tma_store, FIRA_ERR_ARG,

@@ -60,8 +60,11 @@ int fira_gemm_f32(const float* A, long lda, int a_kcontig, const float* B, long 
 /* ---- bf16 tensor-core Linear (throughput mode): wgmma with register accumulators, TMA-staged
  *      operands.  Same contraction as fira_gemm_f32 on bf16 operands (fp32 accumulate):
  *      A(m,k) = a_kmajor ? A[m*lda+k] : A[k*lda+m];  B(k,n) = b_kmajor ? B[n*ldb+k] : B[k*ldb+n];
- *      lda/ldb multiples of 8; C fp32 or bf16 (c_is_bf16); accumulate: C += result;
- *      splits>1 = split-K with fp32 atomics (C zero-filled first unless accumulate). */
+ *      lda/ldb multiples of 8; C fp32 or bf16 (c_is_bf16), columns >= N of C never written;
+ *      accumulate: C += result, relu included
+ *      (C += relu(A B + bias + rs rc)), a bf16 C rounded once after the add;
+ *      splits>1 = split-K with fp32 atomics (C zero-filled first unless accumulate; bias and rs/rc added by the first
+ *      split only). */
 int fira_gemm_bf16_tc(const void* A, long lda, int a_kmajor, const void* B, long ldb, int b_kmajor, void* C,
                       long ldc, int c_is_bf16, int M, int N, int K, const float* bias, const float* rs,
                       const float* rc, int relu, int accumulate, int splits, void* stream);
@@ -213,7 +216,9 @@ int fira_attn_bwd(const void* q, long ldq, const void* k, long ldk, const void* 
  * k / v, ranges[b] = {first row, rows, first row, rows} (code rows, sub-token rows; GLOBAL row ids, kv_rows = rows of
  * k / v), key_mask [B, mask_pitch] over the commit's own key positions (NULL: all valid), mask_pitch >= rows of any
  * commit; max_chunks is not used (any number of keys per commit is supported).  Rows of dk / dv outside every range
- * are not written (fira_zero_pad_rows clears the segment padding). */
+ * are not written (fira_zero_pad_rows clears the segment padding).  Results equal fira_attn_fwd / _bwd bit for bit on
+ * the same keys laid out padded (mask 0 beyond the commit's rows), except for a commit without a valid key: it attends
+ * uniformly over its own rows, the padded entry points over all Lk positions. */
 int fira_attn_packed_fwd(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv, const int* ranges,
                          long kv_rows, const unsigned char* key_mask, int mask_pitch, int max_chunks, void* ctx, long ldo,
                          float* stats, int B, int H, int Lq, int d_head, int dtype, void* stream);

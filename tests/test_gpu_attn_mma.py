@@ -2,13 +2,16 @@
 gnn_transformer.py:144-156 on the same bf16-rounded inputs: the packed form (two key row ranges per commit), the
 incremental-decoding form (few query rows, no statistics), causal rows without a valid key, and key counts beyond
 any fixed chunk budget.  Tolerances as in test_gpu_ops_bf16.py: P is rounded to bf16 before P.V (2^-8 of the
-largest output), the backward consumes bf16 P / dS and the bf16 forward output (2^-6)."""
+largest output), the backward consumes bf16 P / dS and the bf16 forward output (2^-6).  The packed form also runs on
+the FFMA kernels (fp32 parity mode at the fp32 bounds of test_gpu_ops.py, bf16 with FIRA_ATTN_TC=0), and all three
+kernels must reproduce the padded entry points bit for bit on the same keys."""
 import math
 
 import pytest
 import torch
 
-from test_gpu_ops_bf16 import BF, DEV, close16, rnd16, st
+from test_gpu_ops import close
+from test_gpu_ops_bf16 import BF, DEV, close16, rnd16, rnd32, st
 
 pytestmark = pytest.mark.gpu
 
@@ -33,12 +36,15 @@ def _ref(q, k, v, mask, causal):
     return (torch.softmax(s, -1) @ V).transpose(0, 1).reshape(Lq, D)
 
 
-def test_attention_packed_ranges():
-    from fira_icse_b200 import _lib
-    Lq = 30
-    # (code rows, sub-token rows, mask rule): a long first range, an empty second range, no valid key at all,
-    # a commit whose keys are all valid, ranges that straddle a 64-key block boundary
-    spec = [(150, 27, "rand"), (100, 0, "rand"), (40, 12, "none"), (7, 3, "all"), (61, 70, "rand")]
+# (code rows, sub-token rows, mask rule): a long first range, an empty second range, no valid key at all,
+# a commit whose keys are all valid, ranges that straddle a 64-key block boundary
+PACKED_SPEC = [(150, 27, "rand"), (100, 0, "rand"), (40, 12, "none"), (7, 3, "all"), (61, 70, "rand")]
+SENTINEL = 3.0
+
+
+def _packed_layout():
+    """-> ranges [B][4], mask [B, pitch] bool, pitch, kv_rows; rows outside every range lie between and after them"""
+    spec = PACKED_SPEC
     B = len(spec)
     pitch = max(a + b for a, b, _ in spec) + 5
     gm = torch.Generator().manual_seed(7)
@@ -60,42 +66,129 @@ def test_attention_packed_ranges():
             mask[b, :L] = torch.rand(L, generator=gm) > 0.3
         elif rule == "all":
             mask[b, :L] = True
-    rg = torch.tensor(ranges, dtype=torch.int32, device=DEV)
+    return ranges, mask, pitch, kv_rows
+
+
+def _key_rows(r):
+    s0, n0, s1, n1 = r
+    return torch.cat([torch.arange(s0, s0 + n0), torch.arange(s1, s1 + n1)])
+
+
+def _packed_inputs(dtype, B, Lq, kv_rows):
+    if dtype == 1:
+        return rnd16(B * Lq, D, seed=1), rnd16(kv_rows, 2 * D, seed=2), rnd16(B * Lq, D, seed=4)
+    return rnd32(B * Lq, D, seed=1), rnd32(kv_rows, 2 * D, seed=2), rnd32(B * Lq, D, seed=4)
+
+
+def _run_attn(q, kv, go, mask, dtype, ranges=None, Lk=None):
+    """fwd + bwd through fira_attn_packed_* (ranges given; keys = rows of kv) or fira_attn_* (padded: commit b's keys at
+    rows b*Lk ..) -> ctx, stats, dq, dkv (dkv starts as SENTINEL)"""
+    from fira_icse_b200 import _lib
+    B, pitch = mask.shape
+    Lq = q.shape[0] // B
+    vo = kv.data_ptr() + D * kv.element_size()
     mask_u8 = mask.to(torch.uint8).to(DEV)
-    q = rnd16(B * Lq, D, seed=1)
-    kv = rnd16(kv_rows, 2 * D, seed=2)
-    ctx = torch.empty(B * Lq, D, device=DEV, dtype=BF)
+    ctx = torch.empty(B * Lq, D, device=DEV, dtype=q.dtype)
     stats = torch.empty(B, H, Lq, 2, device=DEV)
-    _lib.call("fira_attn_packed_fwd", q.data_ptr(), D, kv.data_ptr(), 2 * D, kv.data_ptr() + 2 * D, 2 * D, rg.data_ptr(),
-              kv_rows, mask_u8.data_ptr(), pitch, 1, ctx.data_ptr(), D, stats.data_ptr(), B, H, Lq, DH, 1, st())
-    go = rnd16(B * Lq, D, seed=4)
     dq = torch.empty_like(q)
-    sentinel = 3.0
-    dkv = torch.full_like(kv, sentinel)
-    _lib.call("fira_attn_packed_bwd", q.data_ptr(), D, kv.data_ptr(), 2 * D, kv.data_ptr() + 2 * D, 2 * D, rg.data_ptr(),
-              kv_rows, mask_u8.data_ptr(), pitch, 1, ctx.data_ptr(), go.data_ptr(), D, stats.data_ptr(), dq.data_ptr(), D,
-              dkv.data_ptr(), 2 * D, dkv.data_ptr() + 2 * D, 2 * D, B, H, Lq, DH, 1, st())
+    dkv = torch.full_like(kv, SENTINEL)
+    dvo = dkv.data_ptr() + D * dkv.element_size()
+    if ranges is not None:
+        rg = torch.tensor(ranges, dtype=torch.int32, device=DEV)
+        _lib.call("fira_attn_packed_fwd", q.data_ptr(), D, kv.data_ptr(), 2 * D, vo, 2 * D, rg.data_ptr(), kv.shape[0],
+                  mask_u8.data_ptr(), pitch, 1, ctx.data_ptr(), D, stats.data_ptr(), B, H, Lq, DH, dtype, st())
+        _lib.call("fira_attn_packed_bwd", q.data_ptr(), D, kv.data_ptr(), 2 * D, vo, 2 * D, rg.data_ptr(), kv.shape[0],
+                  mask_u8.data_ptr(), pitch, 1, ctx.data_ptr(), go.data_ptr(), D, stats.data_ptr(), dq.data_ptr(), D,
+                  dkv.data_ptr(), 2 * D, dvo, 2 * D, B, H, Lq, DH, dtype, st())
+    else:
+        _lib.call("fira_attn_fwd", q.data_ptr(), D, kv.data_ptr(), 2 * D, vo, 2 * D, mask_u8.data_ptr(), 0, ctx.data_ptr(),
+                  D, stats.data_ptr(), B, H, Lq, Lk, DH, dtype, st())
+        _lib.call("fira_attn_bwd", q.data_ptr(), D, kv.data_ptr(), 2 * D, vo, 2 * D, mask_u8.data_ptr(), 0, ctx.data_ptr(),
+                  go.data_ptr(), D, stats.data_ptr(), dq.data_ptr(), D, dkv.data_ptr(), 2 * D, dvo, 2 * D, B, H, Lq, Lk, DH,
+                  dtype, st())
     torch.cuda.synchronize()
+    return ctx, stats, dq, dkv
+
+
+def _check_packed_against_float64(dtype):
+    """the packed spec through fira_attn_packed_fwd / _bwd against _ref per commit (a commit without a valid key:
+    uniform over its own rows); rows outside every range untouched, masked keys exactly zero gradient"""
+    Lq = 30
+    ranges, mask, pitch, kv_rows = _packed_layout()
+    B = len(ranges)
+    q, kv, go = _packed_inputs(dtype, B, Lq, kv_rows)
+    ctx, stats, dq, dkv = _run_attn(q, kv, go, mask, dtype, ranges=ranges)
 
     qd = q.double().requires_grad_(True)
     kvd = kv.double().requires_grad_(True)
     outs, touched = [], torch.zeros(kv_rows, dtype=torch.bool)
     for b, (s0, n0, s1, n1) in enumerate(ranges):
-        idx = torch.cat([torch.arange(s0, s0 + n0), torch.arange(s1, s1 + n1)]).to(DEV)
+        idx = _key_rows(ranges[b]).to(DEV)
         touched[idx.cpu()] = True
         keys = kvd[idx]
         outs.append(_ref(qd[b * Lq:(b + 1) * Lq], keys[:, :D], keys[:, D:], mask[b, :n0 + n1].to(DEV), False))
     ref = torch.cat(outs)
-    close16(ctx, ref, glob=2.0 ** -8, what="packed attention fwd")
     ref.backward(go.double())
-    close16(dq, qd.grad, glob=2.0 ** -6, what="packed attention dq")
-    close16(dkv[touched], kvd.grad[touched.to(DEV)], glob=2.0 ** -6, what="packed attention dkv")
-    assert (dkv[~touched.to(DEV)] == sentinel).all(), "rows outside every range were written"
+    if dtype == 1:
+        # tensor cores: P is rounded to bf16 before P.V; FFMA: fp32 P, one rounding of the output -- the MMA bounds
+        # hold for both
+        close16(ctx, ref, glob=2.0 ** -8, what="packed attention fwd")
+        close16(dq, qd.grad, glob=2.0 ** -6, what="packed attention dq")
+        close16(dkv[touched], kvd.grad[touched.to(DEV)], glob=2.0 ** -6, what="packed attention dkv")
+    else:                                                     # the fp32 bounds of test_gpu_ops.test_attention_fwd_bwd
+        close(ctx, ref, rtol=2e-5, atol=1e-5)
+        close(dq, qd.grad, rtol=5e-5, atol=1e-5)
+        close(dkv[touched], kvd.grad[touched.to(DEV)], rtol=5e-5, atol=1e-5)
+    assert (dkv[~touched.to(DEV)] == SENTINEL).all(), "rows outside every range were written"
     for b, (s0, n0, s1, n1) in enumerate(ranges):
-        if spec[b][2] == "none":
+        if PACKED_SPEC[b][2] == "none":
             continue
-        dead = torch.cat([torch.arange(s0, s0 + n0), torch.arange(s1, s1 + n1)])[~mask[b, :n0 + n1]]
+        dead = _key_rows(ranges[b])[~mask[b, :n0 + n1]]
         assert (dkv[dead.to(DEV)] == 0).all(), "masked keys must get exactly zero gradient"
+
+
+def test_attention_packed_ranges():
+    _check_packed_against_float64(1)
+
+
+@pytest.mark.parametrize("dtype", [0, 1], ids=["fp32", "bf16"])
+def test_attention_packed_ranges_ffma(dtype, monkeypatch):
+    """the FFMA kernels on the packed spec: fp32 (parity mode), and bf16 with the tensor-core kernels switched off"""
+    monkeypatch.setenv("FIRA_ATTN_TC", "0")
+    _check_packed_against_float64(dtype)
+
+
+@pytest.mark.parametrize("kernel", ["ffma_fp32", "ffma_bf16", "mma"])
+def test_attention_packed_equals_padded(kernel, monkeypatch):
+    """Packed and padded layouts hold the same valid keys in the same order, and none of the kernels uses atomics:
+    ctx, stats, dq and dk / dv of every real key row are bit for bit those of fira_attn_fwd / _bwd on the keys scattered
+    into a [B, pitch] layout whose mask is 0 beyond the commit's rows.  A commit without a valid key is the documented
+    difference: the padded layout is uniform over all `pitch` keys, the packed one over the commit's own rows (pinned
+    against float64 in test_attention_packed_ranges*), so it is left out here."""
+    dtype = 0 if kernel == "ffma_fp32" else 1
+    monkeypatch.setenv("FIRA_ATTN_TC", "1" if kernel == "mma" else "0")
+    Lq = 30
+    ranges, mask, pitch, kv_rows = _packed_layout()
+    B = len(ranges)
+    q, kv, go = _packed_inputs(dtype, B, Lq, kv_rows)
+    ctx, stats, dq, dkv = _run_attn(q, kv, go, mask, dtype, ranges=ranges)
+    kvp = rnd16(B * pitch, 2 * D, seed=9).to(kv.dtype)        # filler beyond each commit's keys (masked)
+    for b in range(B):
+        idx = _key_rows(ranges[b]).to(DEV)
+        kvp[b * pitch:b * pitch + len(idx)] = kv[idx]
+    ctxp, statsp, dqp, dkvp = _run_attn(q, kvp, go, mask, dtype, Lk=pitch)
+    compared = 0
+    for b in range(B):
+        if not mask[b].any():
+            continue
+        idx = _key_rows(ranges[b]).to(DEV)
+        rows = slice(b * Lq, (b + 1) * Lq)
+        assert torch.equal(ctx[rows], ctxp[rows]), f"ctx of commit {b}"
+        assert torch.equal(stats[b], statsp[b]), f"stats of commit {b}"
+        assert torch.equal(dq[rows], dqp[rows]), f"dq of commit {b}"
+        assert torch.equal(dkv[idx], dkvp[b * pitch:b * pitch + len(idx)]), f"dk / dv of commit {b}"
+        compared += 1
+    assert compared == B - 1
 
 
 @pytest.mark.parametrize("Lq,Lk,causal", [(5, 30, 0), (1, 30, 0), (17, 700, 0), (30, 30, 1)])
