@@ -15,6 +15,7 @@ Buffer conventions
     (kills the per-layer torch.cat/slice of gnn_transformer.py:58,86); `Xc` holds the code rows a
     Combination reads, `Gin` holds every row a GCN layer reads.
 """
+import ctypes
 import os
 
 import torch
@@ -342,6 +343,7 @@ class Prefetch:
         self.wcache = {}
         self.items = None
         self.event = None
+        self.layer_table = None            # prefetch_decoder, bf16: fira_decoder_fwd's host pointer table
 
 
 def _prep_encoder_layer(pr, fork, mark_emb, Wq, bq, Wk, bk, Wv, bv, Wo, W1, b1, W2, fused=True):
@@ -394,6 +396,16 @@ def prefetch_decoder(bf16, lp, device):
             for w in (Wqkv, q[6], q[10], q[16], q[20], q[22]):     # Wqkv, self Wo, cross Wq, cross Wo, W1, W2
                 pr.w(w)
             layers.append((Wqkv, bqkv))
+        if bf16:
+            # fira_decoder_fwd's [L][18] table of per-layer weight / bias / LayerNorm pointers (copied into its launch
+            # parameters, so a captured graph keeps the addresses it was built with)
+            ptrs = []
+            for i in range(L):
+                q = lp[i * 26:(i + 1) * 26]
+                Wqkv, bqkv = layers[i]
+                ptrs += [pr.w(Wqkv), bqkv, pr.w(q[6]), q[7], q[8], q[9], pr.w(q[10]), q[11], pr.w(q[16]), q[17], q[18],
+                         q[19], pr.w(q[20]), q[21], pr.w(q[22]), q[23], q[24], q[25]]
+            pf.layer_table = (ctypes.c_void_p * len(ptrs))(*[t.data_ptr() for t in ptrs])
         pf.items = (Wkv, bkv, layers)
         pf.event = torch.cuda.Event()
         pf.event.record()
@@ -640,8 +652,9 @@ class DecoderFn(torch.autograd.Function):
         mem_dtype = memory.dtype
         memory = memory.contiguous().to(pr.tdt)
 
-        X = pr.empty((Mt, D), dev)
-        call("fira_embed_rows_fwd", _ptr(tar), _ptr(dec_emb), _ptr(pos_table), _ptr(X), Mt, T, D, pr.code, st)
+        if not pr.bf16:
+            X = pr.empty((Mt, D), dev)
+            call("fira_embed_rows_fwd", _ptr(tar), _ptr(dec_emb), _ptr(pos_table), _ptr(X), Mt, T, D, pr.code, st)
         pf = cfg.get("prefetch")
         if pf is None:
             pf = prefetch_decoder(pr.bf16, lp, dev)
@@ -651,6 +664,25 @@ class DecoderFn(torch.autograd.Function):
         Wkv, bkv, qkv_layers = pf.items
         ldkv = L * 2 * D
         KV = pr.linear(memory.view(Ms, D), Wkv, bkv)                                              # [Ms, L*512]
+        if pr.bf16:
+            # the whole stack in ONE launch (csrc/decoder_fwd.cu): every tensor the backward reads, leading dim = layer
+            bf = dict(dtype=torch.bfloat16, device=dev)
+            Xs = torch.empty((L + 1, Mt, D), **bf)                 # each layer's input, then the output
+            QKV, Hh = torch.empty((L, Mt, 3 * D), **bf), torch.empty((L, Mt, 4 * D), **bf)
+            ctx1, Z1, X1, Q, ctx2, Z2, X2, Z3 = torch.empty((8, L, Mt, D), **bf)
+            st1, st2 = torch.empty((2, L, B, H, T, 2), **f32)
+            ls1, ls2, ls3 = torch.empty((3, L, 2, Mt), **f32)
+            call("fira_decoder_fwd", _ptr(tar), _ptr(dec_emb), _ptr(pos_table), _ptr(tar_mask), _ptr(KV), ldkv,
+                 _ptr(mem_mask), _ptr(pk.ranges) if pk is not None else None, S, ctypes.addressof(pf.layer_table), L,
+                 _ptr(Xs), _ptr(QKV), _ptr(ctx1), _ptr(st1), _ptr(Z1), _ptr(ls1), _ptr(X1), _ptr(Q), _ptr(ctx2),
+                 _ptr(st2), _ptr(Z2), _ptr(ls2), _ptr(X2), _ptr(Hh), _ptr(Z3), _ptr(ls3), B, T, float(p), seed,
+                 _ptr(pr.seed_ctr), cfg["stream_base"] + 64, st)
+            ctx.saved = [(Xs[i], qkv_layers[i][0], QKV[i], ctx1[i], st1[i], Z1[i], ls1[i], X1[i], Q[i], ctx2[i], st2[i],
+                          Z2[i], ls2[i], X2[i], Hh[i], Z3[i], ls3[i]) for i in range(L)]
+            ctx.wcache = pr.wcache
+            ctx.misc = (cfg, tar, memory, mem_mask, tar_mask, KV, Wkv, B, T, S, p, mem_dtype, Ms)
+            ctx.save_for_backward(dec_emb, *lp)
+            return Xs[L].view(B, T, D)
         saved = []
         for i in range(L):
             (sWq, sbq, sWk, sbk, sWv, sbv, sWo, sbo, slw, slb,

@@ -227,6 +227,29 @@ int fira_attn_packed_bwd(const void* q, long ldq, const void* k, long ldk, const
                          const void* d_ctx, long ldo, const float* stats, void* dq, long lddq, void* dk, long lddk,
                          void* dv, long lddv, int B, int H, int Lq, int d_head, int dtype, void* stream);
 
+/* ---- the whole decoder forward, bf16 throughput mode (gnn_transformer.py:108-122), ONE launch of B two-CTA clusters: embedding +
+ *      PE, then L x [causal self-attention over tar_mask [B,T], cross-attention, feed-forward], each closed by
+ *      LN(dropout(z) + resid).  T <= 32, 8 heads of 32, D = 256, FFN width 1024.
+ *   kv        [Ms, ldkv] bf16: layer i's cross-attention K at column 512 i, V at 512 i + 256 (the hoisted K/V product);
+ *             keys of commit b as fira_attn_fwd (mem_mask [B,S], rows b*S + s; ranges NULL) or fira_attn_packed_fwd
+ *             (ranges [B][4], mem_mask [B,S] over the commit's key positions or NULL)
+ *   layer_ptrs HOST array [L][18] of device pointers, per layer: Wqkv (bf16 [768,256]), bqkv, Wo, bo, ln w, ln b of the
+ *             self-attention; Wq, bq, Wo, bo, ln w, ln b of the cross-attention; W1 (bf16 [1024,256]), b1, W2 (bf16
+ *             [256,1024]), b2, ln w, ln b of the feed-forward (weights bf16 [out,in], the rest fp32; copied into the
+ *             launch's parameters)
+ *   outputs   (bf16 unless noted, rows b*T + t, t >= T never written): X [L+1][B*T,256] (each layer's input, then the
+ *             output); per layer i (leading dimension L): qkv [B*T,768], ctx1, z1, x1, q, ctx2, z2, x2 [B*T,256],
+ *             hh [B*T,1024], z3 [B*T,256]; st1 / st2 fp32 [B,8,T,2] (fira_attn_fwd's statistics); ls1 / ls2 / ls3 fp32
+ *             [2][B*T] (mean, rstd).  Products are rounded to bf16 once from fp32 + bias, as fira_gemm_bf16_tc;
+ *             LayerNorm and its dropout masks are fira_ln_residual_fwd's on the stored z, site i of stream_id being
+ *             stream_id + 8 i + {0, 1, 2}. */
+int fira_decoder_fwd(const int* tar, const float* dec_emb, const float* pos_table, const unsigned char* tar_mask,
+                     const void* kv, long ldkv, const unsigned char* mem_mask, const int* ranges, int S,
+                     const void* const* layer_ptrs, int L, void* X, void* qkv, void* ctx1, float* st1, void* z1,
+                     float* ls1, void* x1, void* q, void* ctx2, float* st2, void* z2, float* ls2, void* x2, void* hh,
+                     void* z3, float* ls3, int B, int T, float p_drop, uint64_t seed, const uint64_t* seed_ctr,
+                     uint32_t stream_id, void* stream);
+
 /* ---- CopyNet scores (Model.py:17-18): sc[b,t,s] = b_res + w_res . tanh(src[b,s] + tgt[b,t]).
  *      src_mask [B,S] / row_mask [B*T] (optional, 1 = compute): positions the caller will mask anyway. */
 int fira_copy_scores_fwd(const void* src_proj, const void* tgt_proj, const float* w_res, const float* b_res,

@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """A/B timings of single kernels with CUDA events (warm L2 like inside a training step, 20 launches after 5 warm-ups),
-at the shapes the bf16 bench step launches: attention forward/backward (FFMA vs tensor cores, FIRA_ATTN_TC) and the GCN layer
-(scatter + GEMM + LayerNorm vs the fused kernel, forward and backward).  One JSON line per measurement.
+at the shapes the bf16 bench step launches: attention forward/backward (FFMA vs tensor cores, FIRA_ATTN_TC), the GCN layer
+(scatter + GEMM + LayerNorm vs the fused kernel, forward and backward) and the decoder forward (the per-layer launch
+sequence vs fira_decoder_fwd).  One JSON line per measurement.
 
-    python tools/bench_kernels.py [--batch 64]
+    python tools/bench_kernels.py [--batch 64] [--only attention|gcn|decoder]
 """
 import argparse
 import json
@@ -165,17 +166,108 @@ def gcn(B, out):
     out({"kernel": "GCN layer fwd fused: algorithmic bytes", "bytes": alg})
 
 
+DEC_NAMES = ("wqkv", "bqkv", "swo", "sbo", "slw", "slb", "cwq", "cbq", "cwo", "cbo", "clw", "clb",
+             "w1", "b1", "w2", "b2", "flw", "flb")
+
+
+def decoder(B, out):
+    """The bf16 decoder forward of a training step (six layers, T = 30, dropout 0.1): fira_decoder_fwd, one launch,
+    against the 67-launch sequence it replaced (embedding, then per layer the q|k|v product, self-attention, Wo product,
+    LayerNorm, q product, cross-attention, Wo product, LayerNorm, FFN1, FFN2, LayerNorm; products on the wgmma GEMM),
+    on the bench's first packed batch and on a padded batch (S = 304, 127 valid keys).  The hoisted K/V product that
+    precedes both is not timed."""
+    import ctypes
+    from fira_icse_b200 import _lib, ops
+    from fira_icse_b200.packed import PackedTables, pack_from_dataset
+    from fira_icse_b200.synth import SynthDataset
+    T, H, L, F, D, V = 30, 8, 6, 1024, 256, 24650
+    p, seed, sid = 0.1, 1234, 64
+    g = torch.Generator().manual_seed(0)
+
+    def r16(*s, scale=1.0):
+        return (torch.randn(*s, generator=g) * scale).to(BF).to(DEV)
+
+    def r32(*s, scale=1.0, shift=0.0):
+        return (torch.randn(*s, generator=g) * scale + shift).to(DEV)
+    shapes = {"wqkv": (3 * D, D), "swo": (D, D), "cwq": (D, D), "cwo": (D, D), "w1": (F, D), "w2": (D, F)}
+    W = [{n: (r16(*shapes[n], scale=shapes[n][1] ** -0.5) if n in shapes else
+              r32(D, scale=0.2, shift=1.0) if n.endswith("lw") else r32({"bqkv": 3 * D, "b1": F}.get(n, D), scale=0.1))
+          for n in DEC_NAMES} for _ in range(L)]
+    table = (ctypes.c_void_p * (18 * L))(*[w[n].data_ptr() for w in W for n in DEC_NAMES])
+    tar = torch.randint(0, V, (B, T), generator=g, dtype=torch.int32).to(DEV)
+    tar_mask = (torch.arange(T)[None] < torch.randint(5, T + 1, (B,), generator=g)[:, None]).to(torch.uint8).to(DEV)
+    emb, pe = r32(V, D), r32(T, D)
+    pb = pack_from_dataset(PackedTables(SynthDataset(0, B, V, 71)), np.arange(B), V).to(DEV)
+    pad_mask = torch.zeros(B, 304, dtype=torch.uint8, device=DEV)
+    pad_mask[:, :127] = 1
+    Mt = B * T
+    bf = dict(dtype=BF, device=DEV)
+    f32 = dict(dtype=torch.float32, device=DEV)
+    for name, Ms, mask, pk, S in ((f"packed, bench batch 0 (S={pb.S}, {int(pb.mem_mask.sum())} valid keys)",
+                                   pb.Rc + pb.Rs, pb.mem_mask, pb, pb.S),
+                                  ("padded S=304 (127 valid keys)", B * 304, pad_mask, None, 304)):
+        KV = r16(Ms, L * 2 * D)
+        ldkv = L * 2 * D
+        Xs = torch.empty(L + 1, Mt, D, **bf)
+        QKV, Hh = torch.empty(L, Mt, 3 * D, **bf), torch.empty(L, Mt, F, **bf)
+        ctx1, Z1, X1, Q, ctx2, Z2, X2, Z3 = torch.empty(8, L, Mt, D, **bf)
+        st1, st2 = torch.empty(2, L, B, H, T, 2, **f32)
+        ls1, ls2, ls3 = torch.empty(3, L, 2, Mt, **f32)
+
+        def fused():
+            _lib.call("fira_decoder_fwd", tar.data_ptr(), emb.data_ptr(), pe.data_ptr(), tar_mask.data_ptr(), KV.data_ptr(),
+                      ldkv, mask.data_ptr(), pk.ranges.data_ptr() if pk is not None else None, S, ctypes.addressof(table),
+                      L, *[t.data_ptr() for t in (Xs, QKV, ctx1, st1, Z1, ls1, X1, Q, ctx2, st2, Z2, ls2, X2, Hh, Z3, ls3)],
+                      B, T, p, seed, None, sid, st())
+        pr = ops.Prec(True)
+
+        def sequence():
+            _lib.call("fira_embed_rows_fwd", tar.data_ptr(), emb.data_ptr(), pe.data_ptr(), Xs[0].data_ptr(), Mt, T, D, 1, st())
+            for i, w in enumerate(W):
+                X = Xs[i]
+                ops.gemm_tc(X, D, 1, w["wqkv"], D, 1, QKV[i], 3 * D, Mt, 3 * D, D, bias=w["bqkv"])
+                q = QKV[i].data_ptr()
+                _lib.call("fira_attn_fwd", q, 3 * D, q + 2 * D, 3 * D, q + 4 * D, 3 * D, tar_mask.data_ptr(), 1,
+                          ctx1[i].data_ptr(), D, st1[i].data_ptr(), B, H, T, T, 32, 1, st())
+                ops.gemm_tc(ctx1[i], D, 1, w["swo"], D, 1, Z1[i], D, Mt, D, D, bias=w["sbo"])
+                pr.ln_fwd(Z1[i], X, w["slw"], w["slb"], X1[i], X1[i], Mt, Mt, p, seed, sid + 8 * i)
+                ops.gemm_tc(X1[i], D, 1, w["cwq"], D, 1, Q[i], D, Mt, D, D, bias=w["cbq"])
+                k = KV.data_ptr() + 2 * i * 2 * D
+                if pk is not None:
+                    _lib.call("fira_attn_packed_fwd", Q[i].data_ptr(), D, k, ldkv, k + 2 * D, ldkv, pk.ranges.data_ptr(),
+                              Ms, mask.data_ptr(), S, pk.chunks, ctx2[i].data_ptr(), D, st2[i].data_ptr(), B, H, T, 32, 1,
+                              st())
+                else:
+                    _lib.call("fira_attn_fwd", Q[i].data_ptr(), D, k, ldkv, k + 2 * D, ldkv, mask.data_ptr(), 0,
+                              ctx2[i].data_ptr(), D, st2[i].data_ptr(), B, H, T, S, 32, 1, st())
+                ops.gemm_tc(ctx2[i], D, 1, w["cwo"], D, 1, Z2[i], D, Mt, D, D, bias=w["cbo"])
+                pr.ln_fwd(Z2[i], X1[i], w["clw"], w["clb"], X2[i], X2[i], Mt, Mt, p, seed, sid + 8 * i + 1)
+                ops.gemm_tc(X2[i], D, 1, w["w1"], D, 1, Hh[i], F, Mt, F, D, bias=w["b1"], relu=True)
+                ops.gemm_tc(Hh[i], F, 1, w["w2"], F, 1, Z3[i], D, Mt, D, F, bias=w["b2"])
+                pr.ln_fwd(Z3[i], X2[i], w["flw"], w["flb"], Xs[i + 1], Xs[i + 1], Mt, Mt, p, seed, sid + 8 * i + 2)
+        sequence()
+        ref = Xs[L].float().clone()
+        fused()
+        torch.cuda.synchronize()
+        info = {"case": name, "commits": B,
+                "max_abs_diff_output_vs_sequence": (Xs[L].float() - ref).abs().max().item()}
+        out({"kernel": "decoder forward: 67-launch sequence", **info, **timeit(sequence, reps=2)})
+        out({"kernel": "decoder forward: fira_decoder_fwd (1 launch)", **info, **timeit(fused, reps=2)})
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=64)
+    ap.add_argument("--only", choices=["attention", "gcn", "decoder"], default=None)
     a = ap.parse_args()
     import __graft_entry__
     __graft_entry__.build()
 
     def out(d):
         print(json.dumps(d), flush=True)
-    attention(a.batch, out)
-    gcn(a.batch, out)
+    for name, fn in (("attention", attention), ("gcn", gcn), ("decoder", decoder)):
+        if a.only in (None, name):
+            fn(a.batch, out)
 
 
 if __name__ == "__main__":
