@@ -1,5 +1,5 @@
 // wgmma / TMA / mbarrier helpers shared by the sm_90a tensor-core kernels of libfira_b200
-// (gemm_tc.cu, gemm_ln.cu, gcn_fused.cu).  Raw PTX, no CUTLASS dependency.
+// (gemm_tc.cu, gcn_fused.cu).  Raw PTX, no CUTLASS dependency.
 //
 // A warpgroup (4 consecutive warps, 128 threads) issues wgmma.mma_async m64nNk16 on bf16 operands that sit in shared
 // memory in the SWIZZLE_128B layout TMA writes; the fp32 accumulator lives in registers.  Accumulator fragment of

@@ -235,16 +235,8 @@ class Prec:
         return gemm_tc(dy, ld_dy, 0, x, ldx, 0, dW, K, N, K, M, splits=splits, a_off=dy_off, b_off=x_off)
 
     def linear_ln(self, x, W, b, resid, gamma, beta, outA, outB, split, rows, p, seed, sid, rs=None, rc=None):
-        """z = x W^T + b (+ rs rc^T);  out = LN(dropout(z) + resid) -> (z, stats).  bf16 mode: ONE launch
-        (fira_gemm_ln_fwd, csrc/gemm_ln.cu) unless FIRA_GEMM_LN=0; fp32 mode: the GEMM, then the LayerNorm kernel."""
-        N, K = W.shape
-        if self.bf16 and N == D and FUSE_GEMM_LN:
-            z = torch.empty((rows, D), dtype=torch.bfloat16, device=x.device)
-            stats = torch.empty((2, rows), dtype=torch.float32, device=x.device)
-            call("fira_gemm_ln_fwd", _ptr(x), K, _ptr(self.w(W)), _ptr(b), _ptr(rs), _ptr(rc), _ptr(resid), _ptr(gamma),
-                 _ptr(beta), _ptr(z), _ptr(outA), _ptr(outB) if outB is not outA else None, split, _ptr(stats),
-                 _ptr(stats, rows), rows, K, float(p), seed, _ptr(self.seed_ctr), sid, _stream())
-            return z, stats
+        """z = x W^T + b (+ rs rc^T);  out = LN(dropout(z) + resid) -> (z, stats): the GEMM, then the LayerNorm kernel
+        (fira_ln_residual_fwd)"""
         z = self.linear(x, W, b, rs=rs, rc=rc, M=rows)
         return z, self.ln_fwd(z, resid, gamma, beta, outA, outB, split, rows, p, seed, sid)
 
@@ -286,13 +278,9 @@ _SIDE_STREAMS = {}
 # input-gradient chain of the main stream (timeline of GPU run F: 2.3 ms of the 4.1 ms step on that stream), so the
 # groups rotate over several streams = parallel branches of the captured graph
 N_SIDE = max(1, int(os.environ.get("FIRA_SIDE_STREAMS", "8")))
+FUSE_DX_RELU = os.environ.get("FIRA_DX_RELU", "1") != "0" and os.environ.get("FIRA_GEMM_TMA_STORE", "1") != "0"
 # the 256^3 fp32 products of the GCN weight merge (W2 W1 and its two adjoints) are 16 CTAs of the 64 x 64 tile: split-K
 # spreads them over 64 CTAs; bf16 mode only -- the fp32 parity mode keeps the deterministic single-pass sum
-# fira_gemm_ln_fwd (Linear + dropout + residual + LayerNorm in one launch) is OPT-IN: a 128-row tile owns whole rows, so a
-# decoder product runs on 15 CTAs that each pull 256 KB instead of the 60 CTAs of the product followed by the LayerNorm
-# kernel
-FUSE_GEMM_LN = os.environ.get("FIRA_GEMM_LN", "0") != "0"
-FUSE_DX_RELU = os.environ.get("FIRA_DX_RELU", "1") != "0" and os.environ.get("FIRA_GEMM_TMA_STORE", "1") != "0"
 MERGE_SPLITS = max(1, int(os.environ.get("FIRA_MERGE_SPLITS", "4")))
 _TURN = [0]            # rotation shared by every Fork, so consecutive Forks do not all start on the same stream
 

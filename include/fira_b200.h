@@ -76,18 +76,6 @@ int fira_gemm_bf16_tc(const void* A, long lda, int a_kmajor, const void* B, long
 int fira_gemm_bf16_tc_dbias(const void* A, long lda, const void* B, long ldb, int b_kmajor, void* C, long ldc,
                             int c_is_bf16, int M, int N, int K, int accumulate, int splits, float* d_bias, void* stream);
 
-/* Linear + dropout + residual + LayerNorm in one launch (bf16 throughput mode): the block that closes every sub-layer
- * (gnn_transformer.py:83 GCN, :158-161 Attention, :173-174 FeedForward, :204-205 Combination).
- *   z[m,:] = x[m,:] W^T + bias (+ rs[m] * rc[:])     W: bf16 [256, K] row-major, x: bf16 [rows, K] (leading dim ldx)
- *   out    = LN(dropout_p(z) + resid) * gamma + beta   rows < split -> outA[r], the others -> outB[r] (global row index;
- *            outB may be NULL: every row goes to outA; outB must hold all `rows` rows -- the 32-row slab that straddles
- *            `split` is stored whole, so up to 31 rows below `split` of outB are written too);  z (bf16 [rows,256]), mean / rstd (fp32 [rows]) are kept for
- *            fira_ln_residual_bwd.  Same dropout masks as fira_ln_residual_fwd with the same (seed, stream_id). */
-int fira_gemm_ln_fwd(const void* x, long ldx, const void* w, const float* bias, const float* rs, const float* rc,
-                     const void* resid, const float* gamma, const float* beta, void* z, void* outA, void* outB, long split,
-                     float* mean, float* rstd, long rows, int K, float p_drop, uint64_t seed, const uint64_t* seed_ctr,
-                     uint32_t stream_id, void* stream);
-
 /* Input gradient through a relu (gnn_transformer.py:172 under autograd): dx[m,n] = h[m,n] > 0 ? sum_k dy[m,k] W[k,n] : 0
  * with W the nn.Linear weight [K = out, N = in] as it lies in memory and h the forward activations (bf16, same shape and
  * leading dimension as dx): the relu backward folded into the epilogue of the input-gradient product (bf16 throughput mode). */

@@ -236,7 +236,7 @@ def test_csr_from_dense_and_aggregate_match_dense_bmm():
         if addend is not None:
             ref = ref + addend.double()
         close(y, ref, rtol=1e-5, atol=1e-5)
-        # bf16 activations (throughput mode kernel, half a warp per row): same sums on the bf16-rounded inputs,
+        # bf16 activations (throughput mode): same sums on the bf16-rounded inputs,
         # fp32 accumulation, one bf16 rounding of the result
         x16 = x.to(torch.bfloat16)
         a16 = addend.to(torch.bfloat16) if addend is not None else None
@@ -270,7 +270,10 @@ def test_csr_from_dense_nonsymmetric_strided_f32():
 
 
 def test_aggregate_single_segment_synthetic():
+    """one segment (identity row map) against float64: a random 3 %-dense graph in fp32, and the config-5 stress graphs
+    (N = 2048, about 64 neighbours per row) with an addend in fp32 and bf16"""
     from fira_icse_b200 import PackedEdges, _lib
+    from fira_icse_b200.synth import synth_stress_graphs
     B, N = 3, 512
     g = torch.Generator().manual_seed(1)
     a = torch.rand(B, N, N, generator=g)
@@ -281,6 +284,15 @@ def test_aggregate_single_segment_synthetic():
     _lib.call("fira_gcn_aggregate", pe.rowptr.data_ptr(), pe.col.data_ptr(), pe.val.data_ptr(), x.data_ptr(), None,
               y.data_ptr(), B, N, 0, 0, 256, 0, torch.cuda.current_stream().cuda_stream)
     close(y, torch.bmm(a.to(DEV).double(), x.double().view(B, N, 256)).view(B * N, 256), rtol=1e-5, atol=1e-5)
+    B, N = 4, 2048
+    pe = PackedEdges.from_coo_lists(synth_stress_graphs(0, B), N, DEV)
+    a = pe.to_dense(torch.float64).to(DEV)
+    for code, dt, rtol in ((0, torch.float32, 1e-5), (1, torch.bfloat16, 2 ** -7)):
+        x, add = rnd(B * N, 256, seed=4).to(dt), rnd(B * N, 256, seed=5).to(dt)
+        y = torch.empty_like(x)
+        _lib.call("fira_gcn_aggregate", pe.rowptr.data_ptr(), pe.col.data_ptr(), pe.val.data_ptr(), x.data_ptr(),
+                  add.data_ptr(), y.data_ptr(), B, N, 0, 0, 256, code, torch.cuda.current_stream().cuda_stream)
+        close(y, torch.bmm(a, x.double().view(B, N, 256)).view(B * N, 256) + add.double(), rtol=rtol, atol=0)
 
 
 # ------------------------------------------------------------------------------------ attention

@@ -1,6 +1,5 @@
 #!/usr/bin/env python
 """Micro-benchmark of the GNN scatter kernel (fira_gcn_aggregate) alone, cold L2 (rotating buffers).
-FIRA_SPMM_VARIANT=1 selects the round-1 row-at-a-time kernel, default is the staged multi-row kernel.
 Prints one JSON line per workload: DataSet-like graphs (B=64/256) and the config-5 stress graphs."""
 import json
 import os
@@ -49,8 +48,7 @@ def run(name, coo, N, segs, dtype_code=0):
     alg = 2 * R * 256 * esz + (R + 1) * 4 + pe.nnz * 8
     peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(
         os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0     # H100 SXM data-sheet HBM3 bandwidth
-    print(json.dumps({"workload": name, "variant": os.environ.get("FIRA_SPMM_VARIANT", "2"),
-                      "dtype": "f32" if dtype_code == 0 else "bf16", "rows": R, "nnz": pe.nnz,
+    print(json.dumps({"workload": name, "dtype": "f32" if dtype_code == 0 else "bf16", "rows": R, "nnz": pe.nnz,
                       "avg_us": round(avg * 1e3, 2), "min_us": round(ms[0] * 1e3, 2),
                       "alg_MB": round(alg / 1e6, 2), "GBps": round(alg / avg / 1e6, 1),
                       "frac_of_measured_peak": round(alg / avg / 1e6 / peak, 3),
