@@ -32,6 +32,16 @@ hypotheses with their scores (`beam_search` stays the reference-exact default):
 A vocabulary candidate and a copy candidate that spell the same word stay two candidates (as in the reference), so an
 n-best list can hold the same message twice.
 
+Diverse n-best (`groups` G > 1, `diversity` lambda; diverse beam search, Vijayakumar et al., 2018): the K slots form G
+groups of Kg = K / G, group g owning slots g * Kg .. (g + 1) * Kg - 1; at position 0 slot g * Kg of every group is live.
+At every position the groups choose in order, each with the rule above restricted to its own slots (the Kg best become
+its slots, parents inside the group), ranking by score - lambda * h_g(token) where h_g(w) counts the slots of groups
+0..g-1 that grew at this position with word w (a copy's word is copy_src[b, j - V], so a copy and the vocabulary entry
+spelling the same word are penalised alike; a carried finished slot counts nothing and proposes its stored score
+unpenalised).  The penalty only ranks: logprob, token_logprob and score are the quantities above.  Each commit's K
+hypotheses are returned stably sorted by score, best first.  groups = 1 is plain n-best (the same code path);
+diversity = 0 makes every group an independent nbest(beam_size=Kg).
+
 The loop is decode_loop.PositionLoop (described there); a position ends with fira_pointer_mix_beam_step (per live slot
 row its top K, then per commit the merge, writing the new slots, their parents and the next tokens), the KV-cache
 reorder to the parents and the pad mask of the next tokens.  Slot state is double-buffered by the parity of the
@@ -152,15 +162,22 @@ class Hypotheses(NamedTuple):
     finished: torch.Tensor        # [B, K] bool: the hypothesis ends with <eos>
 
 
-def check_nbest_args(beam_size, length_penalty, tar_len):
+def _finite_f32(x):
+    return not isinstance(x, bool) and isinstance(x, (int, float)) and 0.0 <= _f32(x) < math.inf
+
+
+def check_nbest_args(beam_size, length_penalty, tar_len, groups=1, diversity=0.0):
     """ValueError for any parameter nbest cannot honour (called before any device work)."""
     if not is_int(beam_size) or not 1 <= beam_size <= MAX_BEAM:
         raise ValueError(f"beam_size must be an integer in [1, {MAX_BEAM}], got {beam_size!r}")
-    if (isinstance(length_penalty, bool) or not isinstance(length_penalty, (int, float))
-            or not 0.0 <= _f32(length_penalty) < math.inf):
+    if not _finite_f32(length_penalty):
         raise ValueError(f"length_penalty must be a finite number >= 0 (in fp32), got {length_penalty!r}")
     if not is_int(tar_len) or tar_len < 2:
         raise ValueError(f"tar_len must be an integer >= 2, got {tar_len!r}")
+    if not is_int(groups) or groups < 1 or beam_size % groups:
+        raise ValueError(f"groups must be an integer >= 1 that divides beam_size {beam_size}, got {groups!r}")
+    if not _finite_f32(diversity):
+        raise ValueError(f"diversity must be a finite number >= 0 (in fp32), got {diversity!r}")
 
 
 class _NBest(PositionLoop):
@@ -195,18 +212,58 @@ class _NBest(PositionLoop):
         inc.tok_mask[:, t + 1].copy_(inc.tok[:self.R] != pad_id)
 
 
+class _DiverseNBest(_NBest):
+    """_NBest with beam groups: the token every slot grew with at the current position (`chosen`, read by the later
+    groups' penalty) and the true lp of every row winner next to its rank key."""
+
+    def __init__(self, model, B, K, T, S):
+        super().__init__(model, B, K, T, S)
+        self.chosen = torch.empty(self.R, dtype=torch.int32, device=self.dev)
+        self.work_lp = torch.empty(self.R * K, dtype=torch.float32, device=self.dev)
+
+    def start(self, memory, mem_mask, copy_src, start_id, pad_id, groups):
+        super().start(memory, mem_mask, copy_src, start_id, pad_id)
+        status = self.status[0].view(self.B, self.N)
+        status.fill_(2)
+        status[:, ::self.N // groups] = 0               # slot g * Kg of every group starts live (L = 0)
+
+    def position(self, t, length_penalty, eos_id, pad_id, groups, diversity):
+        """Slots of position t + 1 from decoder row t: one call, 2 * groups launches on the current stream."""
+        self.head(t)
+        p = ops._ptr
+        inc = self.inc
+        call("fira_pointer_mix_diverse_beam_step", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
+             p(self.copy_src), float(length_penalty), int(eos_id), int(pad_id), p(self.work), p(self.seq), p(self.raw),
+             p(self.tlp), p(self.length), p(self.lp), p(self.score), p(self.status), p(self.parent), p(inc.tok),
+             self.T, t, self.B, self.N, self.V, self.S, int(groups), float(diversity), p(self.chosen), p(self.work_lp),
+             self.pr.code, ops._stream())
+        inc.reorder(self.parent)
+        inc.tok_mask[:, t + 1].copy_(inc.tok[:self.R] != pad_id)
+
+
 @torch.no_grad()
 def nbest(model, sou, mark, ast_change, edge, sub_token, *, beam_size=3, length_penalty=0.0, tar_len=30, start_id,
-          eos_id, pad_id=0):
-    """Log-space beam search with length normalisation -> Hypotheses, each commit's K best first (module docstring)."""
-    check_nbest_args(beam_size, length_penalty, tar_len)
+          eos_id, pad_id=0, groups=1, diversity=0.0):
+    """Log-space beam search with length normalisation -> Hypotheses, each commit's K best first (module docstring).
+    groups > 1 splits the K slots into diverse beam groups penalised by `diversity` per earlier-group repeat."""
+    check_nbest_args(beam_size, length_penalty, tar_len, groups, diversity)
     if beam_size > model.vocab_size:
         raise ValueError(f"beam_size {beam_size} exceeds the vocabulary ({model.vocab_size})")
     check_tar_len(model, tar_len)
     memory, mem_mask, copy_src = encode(model, sou, mark, ast_change, edge, sub_token, pad_id)
     B, S = memory.shape[:2]
-    st = loop_for(_NBest, model, B, beam_size, tar_len, S)
-    st.start(memory, mem_mask, copy_src, start_id, pad_id)
-    t = st.run((float(length_penalty), int(eos_id), int(pad_id)))
+    if groups == 1:
+        st = loop_for(_NBest, model, B, beam_size, tar_len, S)
+        st.start(memory, mem_mask, copy_src, start_id, pad_id)
+        t = st.run((float(length_penalty), int(eos_id), int(pad_id)))
+        seq, raw, length, lp, tlp, status = st.slots(t)
+        return Hypotheses(seq, raw, length, lp, st.score[t & 1].view(B, beam_size).clone(), tlp, status == 1)
+    st = loop_for(_DiverseNBest, model, B, beam_size, tar_len, S)
+    st.start(memory, mem_mask, copy_src, start_id, pad_id, groups)
+    t = st.run((float(length_penalty), int(eos_id), int(pad_id), int(groups), _f32(diversity)))
     seq, raw, length, lp, tlp, status = st.slots(t)
-    return Hypotheses(seq, raw, length, lp, st.score[t & 1].view(B, beam_size).clone(), tlp, status == 1)
+    score = st.score[t & 1].view(B, beam_size)
+    score, order = torch.sort(score, dim=1, descending=True, stable=True)        # best first across the groups
+    o2, o3 = order, order.unsqueeze(-1).expand_as(seq)
+    return Hypotheses(seq.gather(1, o3), raw.gather(1, o3), length.gather(1, o2), lp.gather(1, o2), score,
+                      tlp.gather(1, o3), (status == 1).gather(1, o2))

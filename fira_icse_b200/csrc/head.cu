@@ -726,6 +726,182 @@ __global__ void __launch_bounds__(kBeamThreads) beam_select_kernel(
   }
 }
 
+// ------------------------------------------------------------------ one diverse n-best beam step (beam groups)
+// The K slots of a commit form G groups of Kg = K / G; group g owns slots g * Kg .. (g + 1) * Kg - 1 and the groups
+// choose in order.  A live slot i of group g proposes (i, j) with the n-best score, ranked by
+//   value = score - diversity * h,   h = how many slots of groups 0..g-1 grew at this position with j's token
+// (a copy's token is copy_src[b, j - V], so a copy and the vocabulary entry spelling the same word count alike); a
+// finished slot proposes itself with its stored score.  The Kg best by (value descending, then i * (C + 1) + j
+// ascending) become the group's slots, parents always inside the group.  The penalty only ranks: lp, L and score are
+// the n-best quantities.  Per group two launches: a row stage (one CTA per slot of the group) keeping each row's Kg
+// best by value, then a select stage (one CTA per commit) merging the group's <= Kg^2 candidates and writing `chosen`
+// (the token each new slot grew with, -1 when carried or empty) for the later groups.
+// Both stages rank by the same fp32 value from diverse_value (explicit _rn operations: no contraction can make them
+// disagree), so a select winner is always among its row's Kg best and the row prefilter is exact.
+__device__ __forceinline__ float beam_norm(int n, float alpha) { return powf((5.f + (float)n) / 6.f, alpha); }
+// -> the rank value; *score = (L_i + lp) / norm, the n-best score of the candidate
+__device__ __forceinline__ float diverse_value(float L_i, float lp, float norm, float diversity, int h, float* score) {
+  *score = __fdiv_rn(__fadd_rn(L_i, lp), norm);
+  return __fsub_rn(*score, __fmul_rn(diversity, (float)h)) + 0.f;     // + 0: -0 and +0 rank as one value
+}
+__device__ __forceinline__ int count_token(const int* s_prev, int n_prev, int tok) {
+  int h = 0;
+  for (int e = 0; e < n_prev; ++e) h += s_prev[e] == tok ? 1 : 0;
+  return h;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kBeamThreads, 1) diverse_row_kernel(
+    const T* __restrict__ logits, long ldl, const float* __restrict__ sc, const float* __restrict__ gate_logit,
+    const unsigned char* __restrict__ mem_mask, const int* __restrict__ copy_src, const unsigned char* __restrict__ status,
+    const float* __restrict__ lp_sum, const int* __restrict__ length, const int* __restrict__ chosen, float alpha,
+    float diversity, uint64_t* __restrict__ row_top, float* __restrict__ row_lp, int g, int Kg, int K, int V, int S) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  __shared__ MaxSum sh_ms[8];
+  __shared__ float bc[4];
+  __shared__ uint64_t shk[8];
+  __shared__ int s_prev[kMaxBeam];                    // tokens the earlier groups' slots grew with at this position
+  const int b = blockIdx.x / Kg;
+  const long row = (long)b * K + g * Kg + blockIdx.x % Kg;     // slot row (status / state are of the read half)
+  if (status[row] != 0) return;                       // finished or inactive: the select stage reads nothing of it
+  const int n_prev = g * Kg;
+  if (threadIdx.x < n_prev) s_prev[threadIdx.x] = chosen[(long)b * K + threadIdx.x];
+  const T* lrow = logits + row * ldl;
+  const float* srow = sc + row * S;
+  const unsigned char* mrow = mem_mask + (long)b * S;
+  const int* crow = copy_src + (long)b * S;
+  const MixRow ms = mix_row_stats(lrow, srow, mrow, gate_logit + row * 2, V, S, sh_ms, bc);   // syncs s_prev too
+  const float L_i = lp_sum[row], norm = beam_norm(length[row], alpha);
+  auto lp_of = [&](float p) { return logf(fminf(fmaxf(p, 1e-10f), 1.f)); };   // = -nll of fira_pointer_mix_nll_fwd
+
+  uint64_t top[kMaxBeam];                             // this thread's best keys, descending; 0 = empty
+#pragma unroll
+  for (int i = 0; i < kMaxBeam; ++i) top[i] = 0;
+  uint64_t thr = 0;                                   // top[Kg - 1]: the key a candidate has to beat
+  auto offer = [&](float p, int j) {
+    float score;
+    const float v0 = diverse_value(L_i, lp_of(p), norm, diversity, 0, &score);
+    if (rank_key(v0, j) <= thr) return;               // the penalty only lowers the value
+    const int h = n_prev ? count_token(s_prev, n_prev, j < V ? j : crow[j - V]) : 0;
+    const uint64_t key = h ? rank_key(diverse_value(L_i, lp_of(p), norm, diversity, h, &score), j) : rank_key(v0, j);
+    if (key > thr) thr = topk_insert(top, key, Kg);
+  };
+  const int V8 = V >> 3;
+  for (int gi = threadIdx.x; gi < V8; gi += blockDim.x) {
+    float x[8];
+    Act<T>::load8(lrow + (long)gi * 8, x);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) offer(ms.g0 * (expf(x[i] - ms.vmax) / ms.vsum), gi * 8 + i);
+  }
+  for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) offer(ms.g0 * (expf(Act<T>::ld(lrow + j) - ms.vmax) / ms.vsum), j);
+  for (int s = threadIdx.x; s < S; s += blockDim.x)
+    if (mrow[s]) offer(ms.g1 * (expf(srow[s] - ms.cmax) / ms.csum), V + s);
+
+  // block top Kg: fixed-order maxima over the list heads (keys are distinct); the winner's lp is formed again from
+  // its index with the same expression, so it is the lp its value was ranked with
+  for (int k = 0; k < Kg; ++k) {
+    const uint64_t m = block_reduce(top[0], shk, key_max);
+    if (m != 0 && top[0] == m) {
+#pragma unroll
+      for (int i = 0; i + 1 < kMaxBeam; ++i) top[i] = top[i + 1];
+      top[kMaxBeam - 1] = 0;
+    }
+    if (threadIdx.x == 0) {
+      float lp = 0.f;
+      if (m != 0) {
+        const int j = key_index(m);
+        lp = lp_of(j < V ? ms.g0 * (expf(Act<T>::ld(lrow + j) - ms.vmax) / ms.vsum)
+                         : ms.g1 * (expf(srow[j - V] - ms.cmax) / ms.csum));
+      }
+      row_top[row * Kg + k] = m;
+      row_lp[row * Kg + k] = lp;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kBeamThreads) diverse_select_kernel(
+    const uint64_t* __restrict__ row_top, const float* __restrict__ row_lp, const int* __restrict__ copy_src,
+    float alpha, float diversity, int eos_id, int pad_id, int* __restrict__ seq, int* __restrict__ raw,
+    float* __restrict__ tok_lp, int* __restrict__ length, float* __restrict__ lp_sum, float* __restrict__ score,
+    unsigned char* __restrict__ status, long* __restrict__ parent, int* __restrict__ next_tok,
+    int* __restrict__ chosen, int Tn, int pos, int B, int g, int Kg, int K, int V, int S) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  __shared__ uint64_t sh_key[kBeamThreads];
+  __shared__ int s_from[kMaxBeam], s_j[kMaxBeam], s_tok[kMaxBeam], s_prev[kMaxBeam];
+  __shared__ float s_lp[kMaxBeam], s_L[kMaxBeam], s_score[kMaxBeam];
+  const int b = blockIdx.x, C = V + S;
+  const long R = (long)B * K;
+  const long in = (pos & 1) ? R : 0, out = (pos & 1) ? 0 : R;     // row offsets of the read and the written half
+  const long base = (long)b * K;
+  const int g0 = g * Kg, n_prev = g0;                 // the group's first slot; earlier groups' slots precede it
+  if (threadIdx.x < Kg) { s_from[threadIdx.x] = g0 + threadIdx.x; s_j[threadIdx.x] = C; }   // unfilled: keeps itself
+  if (threadIdx.x < n_prev) s_prev[threadIdx.x] = chosen[base + threadIdx.x];
+  __syncthreads();
+
+  // candidate threadIdx.x = il * Kg + q: the q-th row winner of live slot i = g0 + il, or (q = 0) finished slot i
+  uint64_t mine = 0;
+  int i = 0, j = C, tok = pad_id;
+  float lp = 0.f, L = 0.f, sco = 0.f;
+  if (threadIdx.x < Kg * Kg) {
+    i = g0 + threadIdx.x / Kg;
+    const int q = threadIdx.x % Kg;
+    const long pr = in + base + i;
+    float value = 0.f;
+    if (status[pr] == 0) {
+      const uint64_t c = row_top[(base + i) * Kg + q];
+      if (c != 0) {
+        lp = row_lp[(base + i) * Kg + q];
+        j = key_index(c);
+        tok = j < V ? j : copy_src[(long)b * S + (j - V)];
+        L = __fadd_rn(lp_sum[pr], lp);
+        value = diverse_value(lp_sum[pr], lp, beam_norm(length[pr], alpha), diversity,
+                              count_token(s_prev, n_prev, tok), &sco);
+        sco += 0.f;
+        mine = 1;
+      }
+    } else if (status[pr] == 1 && q == 0) {
+      L = lp_sum[pr];
+      sco = score[pr] + 0.f;
+      value = sco;
+      mine = 1;
+    }
+    if (mine) mine = ((uint64_t)order_bits(value) << 32) | (0xFFFFFFFFu - (uint32_t)(i * (C + 1) + j));
+  }
+  sh_key[threadIdx.x] = mine;
+  __syncthreads();
+  if (mine) {
+    int rank = 0;
+    for (int u = 0; u < Kg * Kg; ++u) rank += sh_key[u] > mine ? 1 : 0;
+    if (rank < Kg) { s_from[rank] = i; s_j[rank] = j; s_lp[rank] = lp; s_L[rank] = L; s_score[rank] = sco; s_tok[rank] = tok; }
+  }
+  __syncthreads();
+  if (threadIdx.x < Kg) {
+    const int k = g0 + threadIdx.x, f = s_from[threadIdx.x];
+    const long pr = in + base + f, nr = out + base + k;
+    parent[base + k] = base + f;
+    if (s_j[threadIdx.x] == C) {                      // a finished (or inactive) slot carried unchanged
+      length[nr] = length[pr]; lp_sum[nr] = lp_sum[pr]; score[nr] = score[pr]; status[nr] = status[pr];
+      next_tok[base + k] = pad_id;
+      chosen[base + k] = -1;
+    } else {
+      const int t = s_tok[threadIdx.x];
+      length[nr] = length[pr] + 1; lp_sum[nr] = s_L[threadIdx.x]; score[nr] = s_score[threadIdx.x];
+      status[nr] = t == eos_id ? 1 : 0;
+      next_tok[base + k] = t;
+      chosen[base + k] = t;
+    }
+  }
+  // histories follow their parents; a grown slot gets its new token at column pos + 1
+  for (int e = threadIdx.x; e < Kg * Tn; e += blockDim.x) {
+    const int k = e / Tn, c = e % Tn;
+    const long src = (in + base + s_from[k]) * Tn + c, dst = (out + base + g0 + k) * Tn + c;
+    const bool grow = s_j[k] != C && c == pos + 1;
+    seq[dst] = grow ? s_tok[k] : seq[src];
+    raw[dst] = grow ? s_j[k] : raw[src];
+    tok_lp[dst] = grow ? s_lp[k] : tok_lp[src];
+  }
+}
+
 }  // namespace
 
 #define DISPATCH_T(dtype, ...)                                                            \
@@ -877,6 +1053,47 @@ int fira_pointer_mix_beam_step(const void* logits, long ld_logits, const float* 
            copy_src, length_penalty, eos_id, pad_id, seq, raw, token_logprob, length, logprob, score, status, parent,
            next_tok, T_len, pos, B, K, V, S);
   FIRA_CHECK_LAUNCH("fira_pointer_mix_beam_step (select)");
+  return FIRA_OK;
+}
+
+int fira_pointer_mix_diverse_beam_step(const void* logits, long ld_logits, const float* copy_scores,
+                                       const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
+                                       float length_penalty, int eos_id, int pad_id, uint64_t* workspace, int* seq,
+                                       int* raw, float* token_logprob, int* length, float* logprob, float* score,
+                                       unsigned char* status, long* parent, int* next_tok, int T_len, int pos, int B,
+                                       int K, int V, int S, int groups, float diversity, int* chosen,
+                                       float* lp_workspace, int dtype, void* stream) {
+  FIRA_CHECK_ARG(B >= 0 && K >= 1 && K <= kMaxBeam && V >= K && S > 0 && V + S <= 0x7FFF, FIRA_ERR_SHAPE,
+                 "pointer_mix_diverse_beam_step: shape (B %d, K %d, V %d, S %d; 1 <= K <= 16, K <= V, V + S <= 32767)",
+                 B, K, V, S);
+  FIRA_CHECK_ARG(pos >= 0 && pos + 2 <= T_len, FIRA_ERR_SHAPE, "pointer_mix_diverse_beam_step: pos %d, T_len %d",
+                 pos, T_len);
+  FIRA_CHECK_ARG(groups >= 1 && groups <= K && K % groups == 0, FIRA_ERR_ARG,
+                 "pointer_mix_diverse_beam_step: groups %d must divide K %d", groups, K);
+  FIRA_CHECK_ARG(length_penalty >= 0.f && length_penalty <= 3.4e38f, FIRA_ERR_ARG,
+                 "pointer_mix_diverse_beam_step: length_penalty %g", (double)length_penalty);
+  FIRA_CHECK_ARG(diversity >= 0.f && diversity <= 3.4e38f, FIRA_ERR_ARG,
+                 "pointer_mix_diverse_beam_step: diversity %g", (double)diversity);
+  FIRA_CHECK_ARG(workspace && lp_workspace && chosen, FIRA_ERR_ARG,
+                 "pointer_mix_diverse_beam_step: null workspace / lp_workspace / chosen");
+  FIRA_CHECK_ARG(fira_aligned16(logits) && ld_logits % 8 == 0, FIRA_ERR_ALIGN,
+                 "pointer_mix_diverse_beam_step: logits must be 16-byte aligned with a leading dimension that is a "
+                 "multiple of 8");
+  if (B == 0) return FIRA_OK;
+  const int Kg = K / groups;
+  const long in = (pos & 1) * (long)B * K;            // the read half of the slot state
+  for (int g = 0; g < groups; ++g) {
+    DISPATCH_T(dtype, launch_k(diverse_row_kernel<T>, dim3((unsigned)(B * Kg)), dim3(kBeamThreads), 0,
+        (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src,
+        (const unsigned char*)status + in, (const float*)logprob + in, (const int*)length + in, (const int*)chosen,
+        length_penalty, diversity, workspace, lp_workspace, g, Kg, K, V, S);)
+    FIRA_CHECK_LAUNCH("fira_pointer_mix_diverse_beam_step (rows)");
+    launch_k(diverse_select_kernel, dim3((unsigned)B), dim3(kBeamThreads), 0, (cudaStream_t)stream,
+             (const uint64_t*)workspace, (const float*)lp_workspace, copy_src, length_penalty, diversity, eos_id,
+             pad_id, seq, raw, token_logprob, length, logprob, score, status, parent, next_tok, chosen, T_len, pos, B,
+             g, Kg, K, V, S);
+    FIRA_CHECK_LAUNCH("fira_pointer_mix_diverse_beam_step (select)");
+  }
   return FIRA_OK;
 }
 

@@ -310,6 +310,30 @@ int fira_pointer_mix_beam_step(const void* logits, long ld_logits, const float* 
                                float* logprob, float* score, unsigned char* status, long* parent, int* next_tok,
                                int T_len, int pos, int B, int K, int V, int S, int dtype, void* stream);
 
+/* ---- one diverse n-best beam step (fira_icse_b200/beam.py nbest with groups > 1).  Arguments and slot state as
+ *      fira_pointer_mix_beam_step, plus `groups` G (G divides K, Kg = K / G), `diversity` lambda, chosen [B*K] int32
+ *      and lp_workspace [B*K, Kg] fp32 (caller-owned, like workspace [B*K, Kg]).  Group g owns slots
+ *      g*Kg .. (g+1)*Kg - 1 (the caller starts slot g*Kg of every group live, the others inactive).  Rule: the groups
+ *      choose in order g = 0 .. G-1; h_g(w) = the number of slots of groups 0..g-1 that grew at this position with
+ *      token w (the token of j is j, or copy_src[b, j - V] for a copy; <eos> counts like any word, a carried slot
+ *      counts nothing).  Only group g's slots propose, with the candidates of fira_pointer_mix_beam_step: a live slot
+ *      i proposes (i, j) with score = (logprob_i + lp_j) / powf((5 + length_i) / 6, length_penalty) and rank value
+ *      score - diversity * h_g(token of j); a finished slot proposes itself once with its stored score as rank value.
+ *      The Kg best by (rank value descending, then i * (C + 1) + j ascending, i the slot index within the commit)
+ *      become slots g*Kg + 0 .. Kg-1 in that order, their parents inside the group; chosen[b*K + g*Kg + k] = the
+ *      token the new slot grew with, -1 when carried.  The penalty is never stored: length, logprob, score,
+ *      token_logprob, parent and next_tok are written as fira_pointer_mix_beam_step writes them.  2G launches on
+ *      `stream` (per group its row stage, then its merge); both rank by the same fp32 value (correctly rounded
+ *      operations), so the row stage's prefilter to each row's Kg best is exact.  1 <= G <= K, K % G == 0,
+ *      diversity finite and >= 0, and the bounds of fira_pointer_mix_beam_step. */
+int fira_pointer_mix_diverse_beam_step(const void* logits, long ld_logits, const float* copy_scores,
+                                       const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
+                                       float length_penalty, int eos_id, int pad_id, uint64_t* workspace, int* seq,
+                                       int* raw, float* token_logprob, int* length, float* logprob, float* score,
+                                       unsigned char* status, long* parent, int* next_tok, int T_len, int pos, int B,
+                                       int K, int V, int S, int groups, float diversity, int* chosen,
+                                       float* lp_workspace, int dtype, void* stream);
+
 /* ---- minimum-Bayes-risk selection among each commit's N samples (fira_icse_b200/mbr.py).  seq [B, N, ld_seq] int32
  *      (row (b, n) at (b*N + n) * ld_seq, columns 0..T_len-1), length [B, N] int32 (counts <start>; clamped to
  *      [1, T_len]).  Rule:

@@ -25,6 +25,9 @@ beam search ranking.  Differences, all below the module surface:
     OUTPUT/output_fira_nbest: FIRA_BEAM consecutive lines per commit in test order, best first,
     `<score>\t<log-probability>\t<message>`; FIRA_LENGTH_PENALTY (default 0 = rank by log-probability) sets the
     penalty alpha of score = logprob / ((5 + n) / 6) ** alpha; prints the mean sentence BLEU of the top hypothesis.
+    FIRA_BEAM_GROUPS (default 1 = plain n-best) splits the FIRA_BEAM hypotheses into that many diverse beam groups
+    (it must divide FIRA_BEAM); a group's candidates are ranked down by FIRA_DIVERSITY (default 0.5, used only when
+    FIRA_BEAM_GROUPS > 1) per earlier-group hypothesis that chose the same word at that position.
     FIRA_DECODE=mbr: minimum-Bayes-risk decoding (fira_icse_b200.mbr) -> OUTPUT/output_fira_mbr: one line per commit in
     test order, `<expected BLEU>\\t<log-probability>\\t<message>`, the commit's sample with the highest mean id-level
     sentence BLEU against its other samples; FIRA_SAMPLES (default 16 here), FIRA_TEMPERATURE, FIRA_TOP_K, FIRA_TOP_P
@@ -256,9 +259,12 @@ def decoder(mode, vocab):
         return "output_fira_mbr", decode, 1
     if mode == "nbest":                 # FIRA_BEAM hypotheses best first, `<score>\t<log-prob>\t<message>`
         alpha = float(os.environ.get("FIRA_LENGTH_PENALTY", 0.0))
+        groups = int(os.environ.get("FIRA_BEAM_GROUPS", 1))
+        diverse = dict(groups=groups, diversity=float(os.environ.get("FIRA_DIVERSITY", 0.5))) if groups != 1 else {}
 
         def decode(model, b, first_index):
-            out = nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=args.beam_size, length_penalty=alpha, **ids)
+            out = nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=args.beam_size, length_penalty=alpha, **diverse,
+                        **ids)
             return out.seq, out.length, (out.score, out.logprob)
         return "output_fira_nbest", decode, 1
     raise SystemExit("FIRA_DECODE must be 'beam', 'sample', 'nbest' or 'mbr'")

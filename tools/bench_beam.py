@@ -7,9 +7,15 @@ reference's own loop was timed on in BASELINE.md (72 s for 32 commits on CPU).  
 (batch, beam) configuration; timing with CUDA events around whole batches, inputs resident on the device.
 
     python tools/bench_beam.py [--batches 20,128] [--beams 3,5] [--precision fp32|bf16] [--reps 3]
-                               [--modes full,graph,sample,nbest,mbr]   (sample: N = the beam width;
+                               [--modes full,graph,sample,nbest,diverse,mbr] [--diversity 0.5]
+                               (sample: N = the beam width;
                                nbest: beam.nbest, log-space n-best beam search with length_penalty 0;
+                               diverse: beam.nbest with groups = the beam width and --diversity;
                                mbr: mbr.mbr over N = the beam width samples)
+
+nbest and diverse lines also carry `self_bleu`: the mean pairwise id-level sentence BLEU among each commit's K
+hypotheses (one fira_mbr_select launch with pair_bleu, off-diagonal entries averaged over the batch); lower means a
+more diverse list.
 
 mbr also prints one line for fira_mbr_select alone on the batch's own samples: the median device time per launch
 (bench.time_launches: launches replayed from a CUDA graph between CUDA events), next to the host time of the same
@@ -35,6 +41,7 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--trim", action="store_true", help="loader-side padding trimming (data.trim_batch_host)")
     ap.add_argument("--modes", default="full,graph")
+    ap.add_argument("--diversity", type=float, default=0.5, help="diverse mode's penalty per repeated word")
     a = ap.parse_args()
     import torch
     import __graft_entry__
@@ -64,6 +71,9 @@ def main():
                 if mode == "nbest":
                     return nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=K, tar_len=30, start_id=1, eos_id=2,
                                  pad_id=0)
+                if mode == "diverse":
+                    return nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=K, tar_len=30, start_id=1, eos_id=2,
+                                 pad_id=0, groups=K, diversity=a.diversity)
                 return beam_search(model, b[0], b[3], b[4], b[5], b[7], beam_size=K, tar_len=30, start_id=1, eos_id=2,
                                    pad_id=0, mode=mode)
             ref = run()                                              # warm-up (lazy CUDA state, graph capture)
@@ -76,12 +86,18 @@ def main():
             e0.record()
             for _ in range(a.reps):
                 out = run()
-            length = out.samples.length if mode == "mbr" else out.length if mode in ("sample", "nbest") else out[1]
+            length = out.samples.length if mode == "mbr" else out.length if mode in ("sample", "nbest", "diverse") else out[1]
             e1.record()
             torch.cuda.synchronize()
             ms = e0.elapsed_time(e1) / a.reps
             metric = {"sample": "sampling", "mbr": "mbr"}.get(mode, "beam-search") + " inference throughput"
-            print(json.dumps({
+            extra = {}
+            if mode in ("nbest", "diverse"):
+                extra = {"self_bleu": self_bleu(out, B, K), "card": torch.cuda.get_device_name(dev),
+                         "power_limit_w": power_limit()}
+                if mode == "diverse":
+                    extra.update(groups=K, diversity=a.diversity)
+            print(json.dumps({**extra,
                 "metric": metric, "unit": "commits/s", "value": B / ms * 1e3,
                 "ms_per_batch": ms, "batch": B, "beam": K, "decoded_steps": int(length.max().item()) - 1,
                 "precision": a.precision, "mode": mode, "ids_equal_full_mode": same, "trimmed": bool(a.trim), "data": "synthetic (DataSet distribution), random weights",
@@ -90,10 +106,39 @@ def main():
                         "graph = newest row against K/V caches as CUDA-graph replays, "
                         "sample = beam-width seeded samples per commit (T = 1, no top-k / top-p), one graph per position, "
                         "nbest = log-space n-best beam search (length_penalty 0), one graph per position, "
+                        "diverse = nbest with groups = K and the given diversity, one graph per position, "
                         "mbr = sample + one fira_mbr_select launch"}),
                   flush=True)
             if mode == "mbr":
                 print(json.dumps(mbr_select_timing(out.samples, B, K)), flush=True)
+
+
+def self_bleu(h, B, K):
+    """mean pairwise id-level sentence BLEU among each commit's K hypotheses `h` (one fira_mbr_select launch with
+    pair_bleu; the diagonal is left out)"""
+    import torch
+    from fira_icse_b200 import ops
+    from fira_icse_b200._lib import call
+    T = h.seq.shape[2]
+    seq, length = h.seq.to(torch.int32).contiguous(), h.length.to(torch.int32).contiguous()
+    pair = torch.empty((B, K, K), dtype=torch.float64, device=seq.device)
+    utility = torch.empty((B, K), dtype=torch.float64, device=seq.device)
+    best = torch.empty(B, dtype=torch.int32, device=seq.device)
+    call("fira_mbr_select", ops._ptr(seq), ops._ptr(length), T, 1, 2, 0, ops._ptr(pair), ops._ptr(utility),
+         ops._ptr(best), B, K, T, ops._stream())
+    off = ~torch.eye(K, dtype=torch.bool, device=seq.device)
+    return pair[:, off].mean().item()
+
+
+def power_limit():
+    """the card's power limit in W as nvidia-smi reports it (None when nvidia-smi is unavailable)"""
+    import subprocess
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        return float(r.stdout.strip().splitlines()[0])
+    except (OSError, ValueError, IndexError, subprocess.SubprocessError):
+        return None
 
 
 def mbr_select_timing(s, B, N):
