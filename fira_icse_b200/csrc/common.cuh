@@ -122,7 +122,8 @@ template <> struct Act<__nv_bfloat16> {
 
 // ---- counter-based dropout RNG (Philox4x32-7): mask is a pure function of (seed, stream, index)
 //      so backward recomputes it instead of storing it.  Not bit-compatible with torch's stream
-//      order (SURVEY.md K13) -> parity tests run with dropout off.
+//      order (SURVEY.md K13); tests/philox_rule.py restates this rule in numpy, and tests/test_gpu_dropout_rule.py /
+//      tests/test_gpu_train_dropout.py check the kernels and the dropout-on training step against it.
 __device__ __forceinline__ uint4 philox4(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3,
                                          uint32_t k0, uint32_t k1) {
   const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;

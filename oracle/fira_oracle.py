@@ -53,14 +53,25 @@ def _ln(sd, prefix, x):
     return F.layer_norm(x, (x.shape[-1],), sd[prefix + ".weight"], sd[prefix + ".bias"], LN_EPS)
 
 
-def _drop(x, p, training):
-    return F.dropout(x, p, training) if (training and p > 0) else x
+def _drop(x, p, training, masks=None, sid=0, rows=None):
+    """dropout; with `masks` (a callable (stream id, row index tensor) -> bool keep mask [..., 256]) the given mask
+    instead of torch's: x * keep / (1 - p32), p32 the fp32 value of p.  rows: the row index of every row of x
+    (default: the flat row number over x's leading dims)."""
+    if not (training and p > 0):
+        return x
+    if masks is None:
+        return F.dropout(x, p, training)
+    if rows is None:
+        rows = torch.arange(x.numel() // x.shape[-1]).view(x.shape[:-1])
+    keep = torch.as_tensor(masks(sid, rows)).reshape(x.shape)
+    p32 = float(torch.tensor(p, dtype=torch.float32))
+    return x * keep.to(x.dtype) / (1.0 - p32)
 
 
-def combination(sd, prefix, x, mark_em, heads, p, training):
+def combination(sd, prefix, x, mark_em, heads, p, training, masks=None, sid=0, rows=None):
     """Per-element two-way gate between key and value (combination_layer.py:7-17)
     wrapped by three input linears, an output linear, residual and post-LN
-    (gnn_transformer.py:192-205)."""
+    (gnn_transformer.py:192-205).  masks: the gate's dropout uses stream `sid`, the LayerNorm's `sid + 1`."""
     dk = x.shape[-1] // heads
     q = _lin(sd, prefix + ".linear_layers.0", x)
     k = _lin(sd, prefix + ".linear_layers.1", x)
@@ -68,39 +79,46 @@ def combination(sd, prefix, x, mark_em, heads, p, training):
     pair_logits = torch.stack((q * k, q * v), dim=-1) / math.sqrt(dk)
     w = torch.softmax(pair_logits, dim=-1)
     mixed = w[..., 0] * k + w[..., 1] * v
-    mixed = _drop(mixed, p, training)
+    mixed = _drop(mixed, p, training, masks, sid, rows)
     y = _lin(sd, prefix + ".output_linear", mixed)
-    return _ln(sd, prefix + ".layernorm", _drop(y, p, training) + x)
+    return _ln(sd, prefix + ".layernorm", _drop(y, p, training, masks, sid + 1, rows) + x)
 
 
-def gcn(sd, prefix, nodes, adj, p, training):
+def gcn(sd, prefix, nodes, adj, p, training, masks=None, sid=2, rows=None):
     """LN(dropout(fc2(A @ fc1(H))) + H), dense batched adjacency (gnn_transformer.py:74-86)."""
     x = _lin(sd, prefix + ".fc1", nodes)
     x = torch.bmm(adj.to(x.dtype), x)
     x = _lin(sd, prefix + ".fc2", x)
-    return _ln(sd, prefix + ".layernorm", _drop(x, p, training) + nodes)
+    return _ln(sd, prefix + ".layernorm", _drop(x, p, training, masks, sid, rows) + nodes)
 
 
 def encoder(sd, sou, mark, ast_change, adj, sub_token, *, heads=8, training=False,
-            p_comb=0.1, p_gcn=0.2, collect=None):
-    """gnn_transformer.py:45-62.  Returns (code rows [B,210,D], sub-token rows [B,160,D])."""
+            p_comb=0.1, p_gcn=0.2, collect=None, masks=None, stream_base=0):
+    """gnn_transformer.py:45-62.  Returns (code rows [B,210,D], sub-token rows [B,160,D]).
+    masks: dropout masks of the CUDA kernels -- layer i draws stream stream_base + 8 i + {0, 1, 2} (gate, Combination
+    LayerNorm, GCN LayerNorm); code rows are numbered b * n_code + j, node rows segment-major (code rows of every
+    commit, then sub-token rows, then AST rows)."""
     emb = sd["encoder.embedding.weight"]
-    n_code, n_sub = sou.shape[1], sub_token.shape[1]
+    B, n_code, n_sub = sou.shape[0], sou.shape[1], sub_token.shape[1]
+    n_ast = ast_change.shape[1]
+    seg = torch.cat((torch.arange(B * n_code).view(B, n_code), B * n_code + torch.arange(B * n_sub).view(B, n_sub),
+                     B * (n_code + n_sub) + torch.arange(B * n_ast).view(B, n_ast)), dim=1)
     code = emb[sou] + position_table(n_code, emb.shape[1], emb.dtype)
     mark_em = sd["encoder.mark_embedding.weight"][mark]
     ast = sd["encoder.ast_change_embedding.weight"][ast_change]
     sub = emb[sub_token]
     for i in range(N_LAYERS):
-        code = combination(sd, f"encoder.combination_list2.{i}", code, mark_em, heads, p_comb, training)
+        sid = stream_base + 8 * i
+        code = combination(sd, f"encoder.combination_list2.{i}", code, mark_em, heads, p_comb, training, masks, sid)
         nodes = torch.cat((code, sub, ast), dim=1)
-        nodes = gcn(sd, f"encoder.gcn_list.{i}", nodes, adj, p_gcn, training)
+        nodes = gcn(sd, f"encoder.gcn_list.{i}", nodes, adj, p_gcn, training, masks, sid + 2, seg)
         code, sub, ast = nodes[:, :n_code], nodes[:, n_code:n_code + n_sub], nodes[:, n_code + n_sub:]
         if collect is not None:
             collect.append(nodes)
     return code, sub
 
 
-def attention(sd, prefix, query, memory, mask, heads, p, training):
+def attention(sd, prefix, query, memory, mask, heads, p, training, masks=None, sid=0, rows=None):
     """Post-LN multi-head attention, mask fill -1e9, no dropout on the weights
     (gnn_transformer.py:137-161).  mask broadcasts to [B, heads, Lq, Lk]."""
     B, Lq, D = query.shape
@@ -116,26 +134,28 @@ def attention(sd, prefix, query, memory, mask, heads, p, training):
     ctx = torch.matmul(torch.softmax(score, dim=-1), v)
     ctx = ctx.transpose(1, 2).reshape(B, Lq, D)
     y = _lin(sd, prefix + ".fc_o", ctx)
-    return _ln(sd, prefix + ".layernorm", _drop(y, p, training) + query)
+    return _ln(sd, prefix + ".layernorm", _drop(y, p, training, masks, sid, rows) + query)
 
 
-def feed_forward(sd, prefix, x, p, training):
+def feed_forward(sd, prefix, x, p, training, masks=None, sid=2, rows=None):
     """gnn_transformer.py:170-174."""
     y = _lin(sd, prefix + ".fc2", F.relu(_lin(sd, prefix + ".fc1", x)))
-    return _ln(sd, prefix + ".layernorm", _drop(y, p, training) + x)
+    return _ln(sd, prefix + ".layernorm", _drop(y, p, training, masks, sid, rows) + x)
 
 
-def decoder(sd, tar, memory, mem_mask, tar_pad_mask, *, heads=8, training=False, p=0.1):
-    """gnn_transformer.py:108-122.  Self-attention keys are masked by pad AND causal."""
+def decoder(sd, tar, memory, mem_mask, tar_pad_mask, *, heads=8, training=False, p=0.1, masks=None, stream_base=0):
+    """gnn_transformer.py:108-122.  Self-attention keys are masked by pad AND causal.
+    masks: layer i draws stream stream_base + 64 + 8 i + {0, 1, 2} (self-attention, cross-attention, FFN), rows b * T + t."""
     emb = sd["decoder.embedding.weight"]
     T = tar.shape[1]
     x = emb[tar] + position_table(T, emb.shape[1], emb.dtype)
     causal = torch.tril(torch.ones(T, T, dtype=torch.bool))
     self_mask = tar_pad_mask[:, None, None, :] & causal[None, None]
     for i in range(N_LAYERS):
-        x = attention(sd, f"decoder.attention_list.{i}", x, x, self_mask, heads, p, training)
-        x = attention(sd, f"decoder.cross_attention_list.{i}", x, memory, mem_mask, heads, p, training)
-        x = feed_forward(sd, f"decoder.feed_forward_list.{i}", x, p, training)
+        sid = stream_base + 64 + 8 * i
+        x = attention(sd, f"decoder.attention_list.{i}", x, x, self_mask, heads, p, training, masks, sid)
+        x = attention(sd, f"decoder.cross_attention_list.{i}", x, memory, mem_mask, heads, p, training, masks, sid + 1)
+        x = feed_forward(sd, f"decoder.feed_forward_list.{i}", x, p, training, masks, sid + 2)
     return x
 
 
@@ -165,13 +185,15 @@ def shifted_labels(tar_label):
 
 
 def forward(sd, sou, tar, attr, mark, ast_change, edge, tar_label, sub_token, stage="train",
-            training=False, detail=None):
-    """TransModel.forward (Model.py:38-86).  `attr` is accepted and ignored, as upstream."""
+            training=False, detail=None, masks=None):
+    """TransModel.forward (Model.py:38-86).  `attr` is accepted and ignored, as upstream.
+    masks: callable (stream id, row index tensor) -> keep mask [..., 256]; dropout then applies the masks the CUDA
+    kernels draw (tests/philox_rule.py) instead of torch's."""
     sou_mask = sou != 0
-    code, sub = encoder(sd, sou, mark, ast_change, edge, sub_token, training=training)
+    code, sub = encoder(sd, sou, mark, ast_change, edge, sub_token, training=training, masks=masks)
     memory = torch.cat((code, sub), dim=1)
     mem_mask = torch.cat((sou_mask, sub_token != 0), dim=1)
-    dec = decoder(sd, tar, memory, mem_mask, tar != 0, training=training)
+    dec = decoder(sd, tar, memory, mem_mask, tar != 0, training=training, masks=masks)
     logp, _ = output_distribution(sd, memory, mem_mask, dec)
     label = shifted_labels(tar_label)
     keep = label != 0
