@@ -42,6 +42,12 @@ unpenalised).  The penalty only ranks: logprob, token_logprob and score are the 
 hypotheses are returned stably sorted by score, best first.  groups = 1 is plain n-best (the same code path);
 diversity = 0 makes every group an independent nbest(beam_size=Kg).
 
+Prefix-constrained n-best (`prefix`): while a commit is inside its prefix, each live slot's row stage proposes only
+the prefix label (with its true lp); since only slot 0 (each group's first slot) is live at position 0, that slot
+grows with the prefix and the search branches at the commit's first free position.  logprob, token_logprob and
+score cover the prefix, and the length penalty's n counts it.  A prefix may not hold <eos> and leaves at least one
+free position: a commit that never branched would keep K - 1 inactive slots with score 0.
+
 The loop is decode_loop.PositionLoop (described there); a position ends with fira_pointer_mix_beam_step (per live slot
 row its top K, then per commit the merge, writing the new slots, their parents and the next tokens), the KV-cache
 reorder to the parents and the pad mask of the next tokens.  Slot state is double-buffered by the parity of the
@@ -56,7 +62,7 @@ import torch
 
 from . import ops
 from ._lib import call
-from .decode_loop import PositionLoop, _f32, check_tar_len, encode, is_int, loop_for
+from .decode_loop import PositionLoop, _f32, check_prefix, check_tar_len, encode, is_int, loop_for
 from .incremental import IncrementalDecoder
 
 MAX_BEAM = 16             # the row stage keeps a per-thread top K in registers
@@ -193,8 +199,8 @@ class _NBest(PositionLoop):
         self.parent = torch.empty(R, dtype=torch.int64, device=dev)
         self.work = torch.empty(R * K, dtype=torch.int64, device=dev)         # per-row top K rank keys (uint64)
 
-    def start(self, memory, mem_mask, copy_src, start_id, pad_id):
-        super().start(memory, mem_mask, copy_src, start_id, pad_id)
+    def start(self, memory, mem_mask, copy_src, start_id, pad_id, prefix=None):
+        super().start(memory, mem_mask, copy_src, start_id, pad_id, prefix)
         self.score[0].zero_()
         self.status[0].view(self.B, self.N)[:, 1:] = 2          # beam 0 has probability 1, the others 0
 
@@ -203,10 +209,11 @@ class _NBest(PositionLoop):
         self.head(t)
         p = ops._ptr
         inc = self.inc
-        call("fira_pointer_mix_beam_step", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
+        call("fira_pointer_mix_beam_step_prefix", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
              p(self.copy_src), float(length_penalty), int(eos_id), int(pad_id), p(self.work), p(self.seq), p(self.raw),
              p(self.tlp), p(self.length), p(self.lp), p(self.score), p(self.status), p(self.parent), p(inc.tok),
-             self.T, t, self.B, self.N, self.V, self.S, self.pr.code, ops._stream())
+             self.T, t, self.B, self.N, self.V, self.S, self.pr.code, ops._stream(), p(self.prefix), self.T,
+             p(self.prefix_len))
         # caches follow the parents BEFORE the pad mask of the new tokens is written (reorder moves tok_mask rows too)
         inc.reorder(self.parent)
         inc.tok_mask[:, t + 1].copy_(inc.tok[:self.R] != pad_id)
@@ -221,8 +228,8 @@ class _DiverseNBest(_NBest):
         self.chosen = torch.empty(self.R, dtype=torch.int32, device=self.dev)
         self.work_lp = torch.empty(self.R * K, dtype=torch.float32, device=self.dev)
 
-    def start(self, memory, mem_mask, copy_src, start_id, pad_id, groups):
-        super().start(memory, mem_mask, copy_src, start_id, pad_id)
+    def start(self, memory, mem_mask, copy_src, start_id, pad_id, groups, prefix=None):
+        super().start(memory, mem_mask, copy_src, start_id, pad_id, prefix)
         status = self.status[0].view(self.B, self.N)
         status.fill_(2)
         status[:, ::self.N // groups] = 0               # slot g * Kg of every group starts live (L = 0)
@@ -232,34 +239,38 @@ class _DiverseNBest(_NBest):
         self.head(t)
         p = ops._ptr
         inc = self.inc
-        call("fira_pointer_mix_diverse_beam_step", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
-             p(self.copy_src), float(length_penalty), int(eos_id), int(pad_id), p(self.work), p(self.seq), p(self.raw),
-             p(self.tlp), p(self.length), p(self.lp), p(self.score), p(self.status), p(self.parent), p(inc.tok),
-             self.T, t, self.B, self.N, self.V, self.S, int(groups), float(diversity), p(self.chosen), p(self.work_lp),
-             self.pr.code, ops._stream())
+        call("fira_pointer_mix_diverse_beam_step_prefix", p(self.logits), self.ldl, p(self.sc), p(self.gl),
+             p(self.mem_mask), p(self.copy_src), float(length_penalty), int(eos_id), int(pad_id), p(self.work),
+             p(self.seq), p(self.raw), p(self.tlp), p(self.length), p(self.lp), p(self.score), p(self.status),
+             p(self.parent), p(inc.tok), self.T, t, self.B, self.N, self.V, self.S, int(groups), float(diversity),
+             p(self.chosen), p(self.work_lp), self.pr.code, ops._stream(), p(self.prefix), self.T, p(self.prefix_len))
         inc.reorder(self.parent)
         inc.tok_mask[:, t + 1].copy_(inc.tok[:self.R] != pad_id)
 
 
 @torch.no_grad()
 def nbest(model, sou, mark, ast_change, edge, sub_token, *, beam_size=3, length_penalty=0.0, tar_len=30, start_id,
-          eos_id, pad_id=0, groups=1, diversity=0.0):
+          eos_id, pad_id=0, groups=1, diversity=0.0, prefix=None):
     """Log-space beam search with length normalisation -> Hypotheses, each commit's K best first (module docstring).
-    groups > 1 splits the K slots into diverse beam groups penalised by `diversity` per earlier-group repeat."""
+    groups > 1 splits the K slots into diverse beam groups penalised by `diversity` per earlier-group repeat.
+    prefix: None, or labels [B, P] every hypothesis of a commit starts with (decode_loop.check_prefix: the tar_label
+    encoding without <start>, a 0 ends a commit's prefix, no <eos>, at most tar_len - 2 labels)."""
     check_nbest_args(beam_size, length_penalty, tar_len, groups, diversity)
     if beam_size > model.vocab_size:
         raise ValueError(f"beam_size {beam_size} exceeds the vocabulary ({model.vocab_size})")
     check_tar_len(model, tar_len)
+    pre = check_prefix(prefix, sou, sub_token, V=model.vocab_size, tar_len=tar_len, eos_id=eos_id, pad_id=pad_id,
+                       eos_last=False)
     memory, mem_mask, copy_src = encode(model, sou, mark, ast_change, edge, sub_token, pad_id)
     B, S = memory.shape[:2]
     if groups == 1:
         st = loop_for(_NBest, model, B, beam_size, tar_len, S)
-        st.start(memory, mem_mask, copy_src, start_id, pad_id)
+        st.start(memory, mem_mask, copy_src, start_id, pad_id, pre)
         t = st.run((float(length_penalty), int(eos_id), int(pad_id)))
         seq, raw, length, lp, tlp, status = st.slots(t)
         return Hypotheses(seq, raw, length, lp, st.score[t & 1].view(B, beam_size).clone(), tlp, status == 1)
     st = loop_for(_DiverseNBest, model, B, beam_size, tar_len, S)
-    st.start(memory, mem_mask, copy_src, start_id, pad_id, groups)
+    st.start(memory, mem_mask, copy_src, start_id, pad_id, groups, pre)
     t = st.run((float(length_penalty), int(eos_id), int(pad_id), int(groups), _f32(diversity)))
     seq, raw, length, lp, tlp, status = st.slots(t)
     score = st.score[t & 1].view(B, beam_size)

@@ -438,6 +438,14 @@ __device__ __forceinline__ MixRow mix_row_stats(const T* __restrict__ lrow, cons
   const float g0 = e0 / (e0 + e1), g1 = e1 / (e0 + e1);
   return MixRow{vmax, vsum, cmax, csum, g0, g1};
 }
+// P_j as head_fwd_kernel forms the probability of label j (a forced label of a prefix may be any j < V + S)
+template <typename T>
+__device__ __forceinline__ float mix_prob(const MixRow& ms, const T* __restrict__ lrow, const float* __restrict__ srow,
+                                          const unsigned char* __restrict__ mrow, int V, int j) {
+  if (j < V) return ms.g0 * (expf(Act<T>::ld(lrow + j) - ms.vmax) / ms.vsum);
+  const int s = j - V;
+  return ms.g1 * (expf((mrow[s] ? srow[s] : kMaskFill) - ms.cmax) / ms.csum);
+}
 
 template <typename T>
 __global__ void __launch_bounds__(kSampleThreads) pointer_mix_sample_kernel(
@@ -446,7 +454,8 @@ __global__ void __launch_bounds__(kSampleThreads) pointer_mix_sample_kernel(
     const int* __restrict__ first_index_p, const float* __restrict__ uniforms, float temp, int top_k, float top_p,
     int eos_id, int pad_id, int* __restrict__ next_tok, int* __restrict__ seq, int* __restrict__ raw,
     float* __restrict__ tok_lp, unsigned char* __restrict__ tok_mask, long ld_out, int pos,
-    unsigned char* __restrict__ finished, int* __restrict__ length, float* __restrict__ lp_sum, int N, int V, int S) {
+    unsigned char* __restrict__ finished, int* __restrict__ length, float* __restrict__ lp_sum,
+    const int* __restrict__ prefix, int ld_prefix, const int* __restrict__ prefix_len, int N, int V, int S) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
   extern __shared__ float s_sc[];                     // [V + S] tempered scores, NaN = not a candidate
   __shared__ MaxSum sh_ms[8];
@@ -478,6 +487,19 @@ __global__ void __launch_bounds__(kSampleThreads) pointer_mix_sample_kernel(
     const int s = j - V;
     return g1 * (expf((mrow[s] ? srow[s] : kMaskFill) - cmax) / csum);
   };
+  // thread 0: label j becomes the row's token at column pos + 1, with the loop bookkeeping
+  auto emit = [&](int j) {
+    const float lp = logf(fminf(fmaxf(prob(j), 1e-10f), 1.f));        // = -nll of fira_pointer_mix_nll_fwd for label j
+    const int tok = j < V ? j : copy_src[(long)b * S + (j - V)];
+    next_tok[row] = tok; seq[o] = tok; raw[o] = j; tok_lp[o] = lp; tok_mask[o] = tok != pad_id;
+    length[row] += 1;
+    lp_sum[row] += lp;
+    if (tok == eos_id) finished[row] = 1;
+  };
+  if (prefix && pos < prefix_len[b]) {                // inside the commit's prefix: its label, no cut and no draw
+    if (threadIdx.x == 0) emit(prefix[(long)b * ld_prefix + pos]);
+    return;
+  }
 
   const int C = V + S;
   for (int j = threadIdx.x; j < C; j += blockDim.x) {
@@ -560,15 +582,7 @@ __global__ void __launch_bounds__(kSampleThreads) pointer_mix_sample_kernel(
     sh_pick = pick;
   }
   __syncthreads();
-  if (threadIdx.x == 0) {
-    const int j = sh_pick;
-    const float lp = logf(fminf(fmaxf(prob(j), 1e-10f), 1.f));        // = -nll of fira_pointer_mix_nll_fwd for label j
-    const int tok = j < V ? j : copy_src[(long)b * S + (j - V)];
-    next_tok[row] = tok; seq[o] = tok; raw[o] = j; tok_lp[o] = lp; tok_mask[o] = tok != pad_id;
-    length[row] += 1;
-    lp_sum[row] += lp;
-    if (tok == eos_id) finished[row] = 1;
-  }
+  if (threadIdx.x == 0) emit(sh_pick);
 }
 
 // ------------------------------------------------------------------ one n-best beam step from the mixture
@@ -607,7 +621,7 @@ template <typename T>
 __global__ void __launch_bounds__(kBeamThreads, 1) beam_row_kernel(
     const T* __restrict__ logits, long ldl, const float* __restrict__ sc, const float* __restrict__ gate_logit,
     const unsigned char* __restrict__ mem_mask, const unsigned char* __restrict__ status, uint64_t* __restrict__ row_top,
-    int K, int V, int S) {
+    const int* __restrict__ prefix, int ld_prefix, const int* __restrict__ prefix_len, int pos, int K, int V, int S) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
   __shared__ MaxSum sh_ms[8];
   __shared__ float bc[4];
@@ -619,6 +633,14 @@ __global__ void __launch_bounds__(kBeamThreads, 1) beam_row_kernel(
   const float* srow = sc + row * S;
   const unsigned char* mrow = mem_mask + (long)b * S;
   const MixRow ms = mix_row_stats(lrow, srow, mrow, gate_logit + row * 2, V, S, sh_ms, bc);
+  if (prefix && pos < prefix_len[b]) {                // inside the commit's prefix: its label is the row's one winner
+    if (threadIdx.x == 0) {
+      const int j = prefix[(long)b * ld_prefix + pos];
+      row_top[row * K] = rank_key(logf(fminf(fmaxf(mix_prob(ms, lrow, srow, mrow, V, j), 1e-10f), 1.f)), j);
+      for (int k = 1; k < K; ++k) row_top[row * K + k] = 0;
+    }
+    return;
+  }
 
   uint64_t top[kMaxBeam];                             // this thread's best keys, descending; 0 = empty
 #pragma unroll
@@ -755,7 +777,8 @@ __global__ void __launch_bounds__(kBeamThreads, 1) diverse_row_kernel(
     const T* __restrict__ logits, long ldl, const float* __restrict__ sc, const float* __restrict__ gate_logit,
     const unsigned char* __restrict__ mem_mask, const int* __restrict__ copy_src, const unsigned char* __restrict__ status,
     const float* __restrict__ lp_sum, const int* __restrict__ length, const int* __restrict__ chosen, float alpha,
-    float diversity, uint64_t* __restrict__ row_top, float* __restrict__ row_lp, int g, int Kg, int K, int V, int S) {
+    float diversity, uint64_t* __restrict__ row_top, float* __restrict__ row_lp, const int* __restrict__ prefix,
+    int ld_prefix, const int* __restrict__ prefix_len, int pos, int g, int Kg, int K, int V, int S) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
   __shared__ MaxSum sh_ms[8];
   __shared__ float bc[4];
@@ -773,6 +796,18 @@ __global__ void __launch_bounds__(kBeamThreads, 1) diverse_row_kernel(
   const MixRow ms = mix_row_stats(lrow, srow, mrow, gate_logit + row * 2, V, S, sh_ms, bc);   // syncs s_prev too
   const float L_i = lp_sum[row], norm = beam_norm(length[row], alpha);
   auto lp_of = [&](float p) { return logf(fminf(fmaxf(p, 1e-10f), 1.f)); };   // = -nll of fira_pointer_mix_nll_fwd
+  if (prefix && pos < prefix_len[b]) {                // inside the commit's prefix: its label is the row's one winner
+    if (threadIdx.x == 0) {
+      const int j = prefix[(long)b * ld_prefix + pos];
+      const float lp = lp_of(mix_prob(ms, lrow, srow, mrow, V, j));
+      const int h = n_prev ? count_token(s_prev, n_prev, j < V ? j : crow[j - V]) : 0;
+      float score;
+      row_top[row * Kg] = rank_key(diverse_value(L_i, lp, norm, diversity, h, &score), j);
+      row_lp[row * Kg] = lp;
+      for (int k = 1; k < Kg; ++k) { row_top[row * Kg + k] = 0; row_lp[row * Kg + k] = 0.f; }
+    }
+    return;
+  }
 
   uint64_t top[kMaxBeam];                             // this thread's best keys, descending; 0 = empty
 #pragma unroll
@@ -1001,12 +1036,14 @@ int fira_pointer_mix_nll_bwd(const void* logits, long ld_logits, const float* co
   return FIRA_OK;
 }
 
-int fira_pointer_mix_sample(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
-                            const unsigned char* mem_mask, const int* copy_src, const uint64_t* seed,
-                            const int* first_index, const float* uniforms, float temperature, int top_k, float top_p,
-                            int eos_id, int pad_id, int* next_tok, int* seq, int* raw, float* token_logprob,
-                            unsigned char* tok_mask, long ld_out, int pos, unsigned char* finished, int* length,
-                            float* logprob, int B, int N, int V, int S, int dtype, void* stream) {
+static int sample_impl(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                       const unsigned char* mem_mask, const int* copy_src, const uint64_t* seed, const int* first_index,
+                       const float* uniforms, float temperature, int top_k, float top_p, int eos_id, int pad_id,
+                       int* next_tok, int* seq, int* raw, float* token_logprob, unsigned char* tok_mask, long ld_out,
+                       int pos, unsigned char* finished, int* length, float* logprob, int B, int N, int V, int S,
+                       const int* prefix, int ld_prefix, const int* prefix_len, int dtype, void* stream) {
+  FIRA_CHECK_ARG(!prefix || (prefix_len && ld_prefix > pos), FIRA_ERR_ARG,
+                 "pointer_mix_sample_prefix: null prefix_len or ld_prefix %d <= pos %d", ld_prefix, pos);
   FIRA_CHECK_ARG(B >= 0 && N > 0 && V > 0 && S > 0 && V + S <= 0x7FFF, FIRA_ERR_SHAPE,
                  "pointer_mix_sample: shape (B %d, N %d, V %d, S %d; V + S must be <= 32767)", B, N, V, S);
   FIRA_CHECK_ARG(pos >= 0 && ld_out >= pos + 2, FIRA_ERR_SHAPE, "pointer_mix_sample: pos %d, ld_out %ld", pos, ld_out);
@@ -1026,16 +1063,43 @@ int fira_pointer_mix_sample(const void* logits, long ld_logits, const float* cop
   DISPATCH_T(dtype, launch_k(pointer_mix_sample_kernel<T>, dim3((unsigned)(B * N)), dim3(kSampleThreads), smem,
       (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, seed, first_index,
       uniforms, temperature, top_k, top_p, eos_id, pad_id, next_tok, seq, raw, token_logprob, tok_mask, ld_out, pos,
-      finished, length, logprob, N, V, S);)
+      finished, length, logprob, prefix, ld_prefix, prefix_len, N, V, S);)
   FIRA_CHECK_LAUNCH("fira_pointer_mix_sample");
   return FIRA_OK;
 }
 
-int fira_pointer_mix_beam_step(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
-                               const unsigned char* mem_mask, const int* copy_src, float length_penalty, int eos_id,
-                               int pad_id, uint64_t* workspace, int* seq, int* raw, float* token_logprob, int* length,
-                               float* logprob, float* score, unsigned char* status, long* parent, int* next_tok,
-                               int T_len, int pos, int B, int K, int V, int S, int dtype, void* stream) {
+int fira_pointer_mix_sample(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                            const unsigned char* mem_mask, const int* copy_src, const uint64_t* seed,
+                            const int* first_index, const float* uniforms, float temperature, int top_k, float top_p,
+                            int eos_id, int pad_id, int* next_tok, int* seq, int* raw, float* token_logprob,
+                            unsigned char* tok_mask, long ld_out, int pos, unsigned char* finished, int* length,
+                            float* logprob, int B, int N, int V, int S, int dtype, void* stream) {
+  return sample_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, seed, first_index, uniforms,
+                     temperature, top_k, top_p, eos_id, pad_id, next_tok, seq, raw, token_logprob, tok_mask, ld_out, pos,
+                     finished, length, logprob, B, N, V, S, nullptr, 0, nullptr, dtype, stream);
+}
+
+int fira_pointer_mix_sample_prefix(const void* logits, long ld_logits, const float* copy_scores,
+                                   const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
+                                   const uint64_t* seed, const int* first_index, const float* uniforms,
+                                   float temperature, int top_k, float top_p, int eos_id, int pad_id, int* next_tok,
+                                   int* seq, int* raw, float* token_logprob, unsigned char* tok_mask, long ld_out,
+                                   int pos, unsigned char* finished, int* length, float* logprob, int B, int N, int V,
+                                   int S, int dtype, void* stream, const int* prefix, int ld_prefix,
+                                   const int* prefix_len) {
+  return sample_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, seed, first_index, uniforms,
+                     temperature, top_k, top_p, eos_id, pad_id, next_tok, seq, raw, token_logprob, tok_mask, ld_out, pos,
+                     finished, length, logprob, B, N, V, S, prefix, ld_prefix, prefix_len, dtype, stream);
+}
+
+static int beam_step_impl(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                          const unsigned char* mem_mask, const int* copy_src, float length_penalty, int eos_id,
+                          int pad_id, uint64_t* workspace, int* seq, int* raw, float* token_logprob, int* length,
+                          float* logprob, float* score, unsigned char* status, long* parent, int* next_tok, int T_len,
+                          int pos, int B, int K, int V, int S, const int* prefix, int ld_prefix, const int* prefix_len,
+                          int dtype, void* stream) {
+  FIRA_CHECK_ARG(!prefix || (prefix_len && ld_prefix > pos), FIRA_ERR_ARG,
+                 "pointer_mix_beam_step_prefix: null prefix_len or ld_prefix %d <= pos %d", ld_prefix, pos);
   FIRA_CHECK_ARG(B >= 0 && K >= 1 && K <= kMaxBeam && V >= K && S > 0 && V + S <= 0x7FFF, FIRA_ERR_SHAPE,
                  "pointer_mix_beam_step: shape (B %d, K %d, V %d, S %d; 1 <= K <= 16, K <= V, V + S <= 32767)",
                  B, K, V, S);
@@ -1047,7 +1111,7 @@ int fira_pointer_mix_beam_step(const void* logits, long ld_logits, const float* 
   if (B == 0) return FIRA_OK;
   DISPATCH_T(dtype, launch_k(beam_row_kernel<T>, dim3((unsigned)(B * K)), dim3(kBeamThreads), 0, (cudaStream_t)stream,
       (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, (const unsigned char*)status + (pos & 1) * (long)B * K,
-      workspace, K, V, S);)
+      workspace, prefix, ld_prefix, prefix_len, pos, K, V, S);)
   FIRA_CHECK_LAUNCH("fira_pointer_mix_beam_step (rows)");
   launch_k(beam_select_kernel, dim3((unsigned)B), dim3(kBeamThreads), 0, (cudaStream_t)stream, (const uint64_t*)workspace,
            copy_src, length_penalty, eos_id, pad_id, seq, raw, token_logprob, length, logprob, score, status, parent,
@@ -1056,13 +1120,37 @@ int fira_pointer_mix_beam_step(const void* logits, long ld_logits, const float* 
   return FIRA_OK;
 }
 
-int fira_pointer_mix_diverse_beam_step(const void* logits, long ld_logits, const float* copy_scores,
-                                       const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
-                                       float length_penalty, int eos_id, int pad_id, uint64_t* workspace, int* seq,
-                                       int* raw, float* token_logprob, int* length, float* logprob, float* score,
-                                       unsigned char* status, long* parent, int* next_tok, int T_len, int pos, int B,
-                                       int K, int V, int S, int groups, float diversity, int* chosen,
-                                       float* lp_workspace, int dtype, void* stream) {
+int fira_pointer_mix_beam_step(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                               const unsigned char* mem_mask, const int* copy_src, float length_penalty, int eos_id,
+                               int pad_id, uint64_t* workspace, int* seq, int* raw, float* token_logprob, int* length,
+                               float* logprob, float* score, unsigned char* status, long* parent, int* next_tok,
+                               int T_len, int pos, int B, int K, int V, int S, int dtype, void* stream) {
+  return beam_step_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, length_penalty, eos_id, pad_id,
+                        workspace, seq, raw, token_logprob, length, logprob, score, status, parent, next_tok, T_len, pos,
+                        B, K, V, S, nullptr, 0, nullptr, dtype, stream);
+}
+
+int fira_pointer_mix_beam_step_prefix(const void* logits, long ld_logits, const float* copy_scores,
+                                      const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
+                                      float length_penalty, int eos_id, int pad_id, uint64_t* workspace, int* seq,
+                                      int* raw, float* token_logprob, int* length, float* logprob, float* score,
+                                      unsigned char* status, long* parent, int* next_tok, int T_len, int pos, int B,
+                                      int K, int V, int S, int dtype, void* stream, const int* prefix, int ld_prefix,
+                                      const int* prefix_len) {
+  return beam_step_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, length_penalty, eos_id, pad_id,
+                        workspace, seq, raw, token_logprob, length, logprob, score, status, parent, next_tok, T_len, pos,
+                        B, K, V, S, prefix, ld_prefix, prefix_len, dtype, stream);
+}
+
+static int diverse_beam_step_impl(const void* logits, long ld_logits, const float* copy_scores,
+                                  const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
+                                  float length_penalty, int eos_id, int pad_id, uint64_t* workspace, int* seq, int* raw,
+                                  float* token_logprob, int* length, float* logprob, float* score,
+                                  unsigned char* status, long* parent, int* next_tok, int T_len, int pos, int B, int K,
+                                  int V, int S, int groups, float diversity, int* chosen, float* lp_workspace,
+                                  const int* prefix, int ld_prefix, const int* prefix_len, int dtype, void* stream) {
+  FIRA_CHECK_ARG(!prefix || (prefix_len && ld_prefix > pos), FIRA_ERR_ARG,
+                 "pointer_mix_diverse_beam_step_prefix: null prefix_len or ld_prefix %d <= pos %d", ld_prefix, pos);
   FIRA_CHECK_ARG(B >= 0 && K >= 1 && K <= kMaxBeam && V >= K && S > 0 && V + S <= 0x7FFF, FIRA_ERR_SHAPE,
                  "pointer_mix_diverse_beam_step: shape (B %d, K %d, V %d, S %d; 1 <= K <= 16, K <= V, V + S <= 32767)",
                  B, K, V, S);
@@ -1086,7 +1174,7 @@ int fira_pointer_mix_diverse_beam_step(const void* logits, long ld_logits, const
     DISPATCH_T(dtype, launch_k(diverse_row_kernel<T>, dim3((unsigned)(B * Kg)), dim3(kBeamThreads), 0,
         (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src,
         (const unsigned char*)status + in, (const float*)logprob + in, (const int*)length + in, (const int*)chosen,
-        length_penalty, diversity, workspace, lp_workspace, g, Kg, K, V, S);)
+        length_penalty, diversity, workspace, lp_workspace, prefix, ld_prefix, prefix_len, pos, g, Kg, K, V, S);)
     FIRA_CHECK_LAUNCH("fira_pointer_mix_diverse_beam_step (rows)");
     launch_k(diverse_select_kernel, dim3((unsigned)B), dim3(kBeamThreads), 0, (cudaStream_t)stream,
              (const uint64_t*)workspace, (const float*)lp_workspace, copy_src, length_penalty, diversity, eos_id,
@@ -1095,6 +1183,34 @@ int fira_pointer_mix_diverse_beam_step(const void* logits, long ld_logits, const
     FIRA_CHECK_LAUNCH("fira_pointer_mix_diverse_beam_step (select)");
   }
   return FIRA_OK;
+}
+
+int fira_pointer_mix_diverse_beam_step(const void* logits, long ld_logits, const float* copy_scores,
+                                       const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
+                                       float length_penalty, int eos_id, int pad_id, uint64_t* workspace, int* seq,
+                                       int* raw, float* token_logprob, int* length, float* logprob, float* score,
+                                       unsigned char* status, long* parent, int* next_tok, int T_len, int pos, int B,
+                                       int K, int V, int S, int groups, float diversity, int* chosen,
+                                       float* lp_workspace, int dtype, void* stream) {
+  return diverse_beam_step_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, length_penalty, eos_id,
+                                pad_id, workspace, seq, raw, token_logprob, length, logprob, score, status, parent,
+                                next_tok, T_len, pos, B, K, V, S, groups, diversity, chosen, lp_workspace, nullptr, 0,
+                                nullptr, dtype, stream);
+}
+
+int fira_pointer_mix_diverse_beam_step_prefix(const void* logits, long ld_logits, const float* copy_scores,
+                                              const float* gate_logits, const unsigned char* mem_mask,
+                                              const int* copy_src, float length_penalty, int eos_id, int pad_id,
+                                              uint64_t* workspace, int* seq, int* raw, float* token_logprob,
+                                              int* length, float* logprob, float* score, unsigned char* status,
+                                              long* parent, int* next_tok, int T_len, int pos, int B, int K, int V,
+                                              int S, int groups, float diversity, int* chosen, float* lp_workspace,
+                                              int dtype, void* stream, const int* prefix, int ld_prefix,
+                                              const int* prefix_len) {
+  return diverse_beam_step_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, length_penalty, eos_id,
+                                pad_id, workspace, seq, raw, token_logprob, length, logprob, score, status, parent,
+                                next_tok, T_len, pos, B, K, V, S, groups, diversity, chosen, lp_workspace, prefix,
+                                ld_prefix, prefix_len, dtype, stream);
 }
 
 }  // extern "C"

@@ -69,28 +69,18 @@ def build_adjacency(change_code, change_ast, ast_code, ast_ast, code_sub, n_diff
     return deg, col[:nnz[0]].copy(), val[:nnz[0]].copy()
 
 
-def build_commit(raw, i, vocab, ast_vocab, upper, diff_len=210, msg_len=30, att_len=25, ast_change_len=280,
-                 sub_len=160):
-    """One commit -> padded id arrays + CSR pieces of its normalised adjacency.
-
-    Node ids: code token j -> j+1 (0 = <start>), sub-token k -> 210+k, AST node a -> 370+a,
-    edit node c -> 370+len(ast)+c.  Edges: edit-code, edit-AST, AST-code, AST-AST, code-sub-token,
-    sequential code chain; undirected, de-duplicated; self loop on all 650 nodes;
-    value 1/sqrt(deg_row)/sqrt(deg_col) in float64."""
+def _diff_words(raw, i, upper):
     var_map = raw["variable"][i]
-    diff = [_lower(var_map.get(t, t), upper) for t in raw["difftoken"][i]]
-    msg = [lemmatization.get(w, w) for w in (_lower(var_map.get(t, t), upper) for t in raw["msg"][i])]
-    atts = raw["diffatt"][i]
-    V = len(vocab)
-    n_ast = len(raw["ast"][i])
+    return [_lower(var_map.get(t, t), upper) for t in raw["difftoken"][i]]
 
-    sou = _fit([vocab["<start>"]] + _to_ids(diff, vocab, upper) + [vocab["<eos>"]], diff_len)
-    msg_ids = _to_ids(msg, vocab, upper)
-    tar = _fit([vocab["<start>"]] + msg_ids + [vocab["<eos>"]], msg_len)
-    mark = _fit([2] + list(raw["diffmark"][i]) + [2], diff_len)
-    ast_change = _fit(_to_ids(list(raw["ast"][i]) + list(raw["change"][i]), ast_vocab, upper), ast_change_len)
 
-    # sub-token nodes are shared by repeated identifiers (first occurrence defines them)
+def _msg_words(words, var_map, upper):
+    """message words as the labels see them: variable map, case, lemmatisation"""
+    return [lemmatization.get(w, w) for w in (_lower(var_map.get(t, t), upper) for t in words)]
+
+
+def _sub_tokens(diff, atts):
+    """sub-token nodes, shared by repeated identifiers (first occurrence defines them) -> (sub-tokens, code-sub pairs)"""
     sub_tokens, owner, code_sub = [], {}, []
     for j, att in enumerate(atts):
         if att:
@@ -98,9 +88,11 @@ def build_commit(raw, i, vocab, ast_vocab, upper, diff_len=210, msg_len=30, att_
                 owner[diff[j]] = range(len(sub_tokens), len(sub_tokens) + len(att))
                 sub_tokens.extend(att)
             code_sub.extend((j, k) for k in owner[diff[j]])
-    sub_token = _fit(_to_ids(sub_tokens, vocab, upper), sub_len)
+    return sub_tokens, code_sub
 
-    # dual-copy labels: position in the diff wins over position among the sub-tokens
+
+def _dual_copy_labels(msg, msg_ids, diff, sub_tokens, V, diff_len):
+    """dual-copy labels: position in the diff wins over position among the sub-tokens, then the vocabulary id"""
     first_in_diff, first_in_sub = {}, {}
     for j, t in enumerate(diff):
         first_in_diff.setdefault(t, j)
@@ -114,6 +106,45 @@ def build_commit(raw, i, vocab, ast_vocab, upper, diff_len=210, msg_len=30, att_
             label.append(first_in_sub[w] + V + diff_len)
         else:
             label.append(wid)
+    return label
+
+
+def prefix_labels(raw, i, words, vocab, upper, diff_len=210):
+    """Words a user typed as the start of commit i's message -> their labels in the tar_label encoding (without
+    <start>), for the decoders' `prefix`: build_commit's normalisation and dual-copy label rule, so the labels of a
+    message's first n words are tar_label[1:1 + n] of that message."""
+    var_map = raw["variable"][i]
+    diff = _diff_words(raw, i, upper)
+    sub_tokens, _ = _sub_tokens(diff, raw["diffatt"][i])
+    msg = _msg_words(words, var_map, upper)
+    return _dual_copy_labels(msg, _to_ids(msg, vocab, upper), diff, sub_tokens, len(vocab), diff_len)
+
+
+def build_commit(raw, i, vocab, ast_vocab, upper, diff_len=210, msg_len=30, att_len=25, ast_change_len=280,
+                 sub_len=160):
+    """One commit -> padded id arrays + CSR pieces of its normalised adjacency.
+
+    Node ids: code token j -> j+1 (0 = <start>), sub-token k -> 210+k, AST node a -> 370+a,
+    edit node c -> 370+len(ast)+c.  Edges: edit-code, edit-AST, AST-code, AST-AST, code-sub-token,
+    sequential code chain; undirected, de-duplicated; self loop on all 650 nodes;
+    value 1/sqrt(deg_row)/sqrt(deg_col) in float64."""
+    var_map = raw["variable"][i]
+    diff = _diff_words(raw, i, upper)
+    msg = _msg_words(raw["msg"][i], var_map, upper)
+    atts = raw["diffatt"][i]
+    V = len(vocab)
+    n_ast = len(raw["ast"][i])
+
+    sou = _fit([vocab["<start>"]] + _to_ids(diff, vocab, upper) + [vocab["<eos>"]], diff_len)
+    msg_ids = _to_ids(msg, vocab, upper)
+    tar = _fit([vocab["<start>"]] + msg_ids + [vocab["<eos>"]], msg_len)
+    mark = _fit([2] + list(raw["diffmark"][i]) + [2], diff_len)
+    ast_change = _fit(_to_ids(list(raw["ast"][i]) + list(raw["change"][i]), ast_vocab, upper), ast_change_len)
+
+    sub_tokens, code_sub = _sub_tokens(diff, atts)
+    sub_token = _fit(_to_ids(sub_tokens, vocab, upper), sub_len)
+
+    label = _dual_copy_labels(msg, msg_ids, diff, sub_tokens, V, diff_len)
     tar_label = _fit([vocab["<start>"]] + label + [vocab["<eos>"]], msg_len)
 
     deg_r, col, val = build_adjacency(raw["edge_change_code"][i], raw["edge_change_ast"][i], raw["edge_ast_code"][i],

@@ -7,6 +7,8 @@ newest decoder row -> out_fc -> target projection and gate -> copy scores (`head
 which writes the next input tokens straight into the decoder's token buffer and keeps every row's slot state
 (`position`, defined by each decoder).  A position is captured once into a CUDA graph and replayed for every later
 batch of the same shape; the loop reads back nothing but an all-finished flag, once every POLL_EVERY positions.
+Every position also passes the per-commit prefix buffers (`check_prefix`): a commit still inside its prefix takes the
+given label at that position instead of choosing one, inside the step kernel.
 """
 import ctypes
 import weakref
@@ -33,6 +35,57 @@ def check_tar_len(model, tar_len):
     """ValueError when the decoder has fewer than tar_len positions (called before any device work)."""
     if tar_len > model.decoder.pos_encode.shape[0]:
         raise ValueError(f"tar_len {tar_len} exceeds the decoder's {model.decoder.pos_encode.shape[0]} positions")
+
+
+def check_prefix(prefix, sou, sub_token, *, V, tar_len, eos_id, pad_id, eos_last):
+    """Validates a prefix (called before any device work) -> (prefix int32 [B, tar_len], prefix_len int32 [B]) on the
+    host, or None for prefix=None.
+
+    prefix: an integer tensor [B, P] of labels in the tar_label encoding (j < V a vocabulary id, V + s memory position
+    s of cat(sou, sub_token)) without <start>; a 0 ends a commit's prefix.  ValueError for a wrong dtype or B, a nonzero
+    entry after a 0, a label outside [0, V + S), a copy label at a masked memory position (mem_mask = cat(sou != pad_id,
+    sub_token != 0), as `encode` forms it), a pad_id label, and, with eos_last (sample / mbr), <eos> anywhere but as a
+    commit's last entry or more than tar_len - 1 entries; without it (nbest), any <eos> or more than tar_len - 2 entries,
+    so that every commit has a free position to branch at.  sou / sub_token are read once on the host."""
+    if prefix is None:
+        return None
+    B = sou.shape[0]
+    if not torch.is_tensor(prefix) or prefix.dtype == torch.bool or prefix.is_floating_point() or prefix.is_complex():
+        raise ValueError(f"prefix must be an integer tensor, got {getattr(prefix, 'dtype', type(prefix))}")
+    if prefix.dim() != 2 or prefix.shape[0] != B:
+        raise ValueError(f"prefix must have shape [B={B}, P], got {tuple(prefix.shape)}")
+    pre = prefix.detach().to("cpu", torch.int64)
+    P = pre.shape[1]
+    nz = pre != 0
+    n = nz.sum(1)                                                           # entries before the first 0, if valid
+    if (nz & (torch.arange(P).unsqueeze(0) >= n.unsqueeze(1))).any():
+        raise ValueError("prefix: a nonzero label follows a 0 (a 0 ends a commit's prefix)")
+    mem_mask = torch.cat((sou.detach().cpu() != pad_id, sub_token.detach().cpu() != 0), dim=1)
+    S = mem_mask.shape[1]
+    if ((pre < 0) | (pre >= V + S)).any():
+        raise ValueError(f"prefix: labels must be in [0, V + S = {V + S})")
+    copy = nz & (pre >= V)
+    rows = torch.arange(B).unsqueeze(1).expand(B, P)
+    if (copy & ~mem_mask[rows, (pre - V).clamp(0, S - 1)]).any():
+        raise ValueError("prefix: a copy label points at a masked memory position")
+    if pad_id != 0 and (nz & (pre == pad_id)).any():
+        raise ValueError(f"prefix: pad_id {pad_id} is not a label")
+    eos = nz & (pre == eos_id)
+    if eos_last:
+        last = torch.arange(P).unsqueeze(0) == (n - 1).unsqueeze(1)
+        if (eos & ~last).any():
+            raise ValueError("prefix: <eos> may only be a commit's last prefix label")
+        longest = tar_len - 1
+    else:
+        if eos.any():
+            raise ValueError("prefix: n-best prefixes cannot contain <eos>")
+        longest = tar_len - 2
+    if (n > longest).any():
+        raise ValueError(f"prefix: at most {longest} labels per commit with tar_len {tar_len}, got {int(n.max())}")
+    out = torch.zeros((B, tar_len), dtype=torch.int32)
+    w = min(P, tar_len)
+    out[:, :w] = pre[:, :w].to(torch.int32)
+    return out, n.to(torch.int32)
 
 
 def encode(model, sou, mark, ast_change, edge, sub_token, pad_id):
@@ -80,10 +133,21 @@ class PositionLoop:
         self.length = torch.empty((H, R), **i32)
         self.lp = torch.empty((H, R), **f32)
         self.status = torch.empty((H, R), dtype=torch.uint8, device=dev)
+        # forced labels per commit (check_prefix); every position passes them to the step kernel, so a batch without a
+        # prefix (prefix_len 0) replays the same graphs
+        self.prefix = torch.zeros((B, T), **i32)
+        self.prefix_len = torch.zeros(B, **i32)
         self.graphs = {}
 
-    def start(self, memory, mem_mask, copy_src, start_id, pad_id):
+    def start(self, memory, mem_mask, copy_src, start_id, pad_id, prefix=None):
+        """prefix: None or check_prefix's host pair (prefix [B, T], prefix_len [B])."""
         inc = self.inc
+        if prefix is None:
+            self.prefix.zero_()
+            self.prefix_len.zero_()
+        else:
+            self.prefix.copy_(prefix[0])
+            self.prefix_len.copy_(prefix[1])
         inc.start(memory, mem_mask)
         mem2 = memory.contiguous().to(inc.be.tdt).view(self.B * self.S, D)
         self.pr.linear(mem2, self.model.copy_net.LinearSource.weight, out=self.src)     # once per batch, not per row

@@ -13,9 +13,10 @@ u comes from Philox4x32-7 keyed by `seed` with the counter (first_index + b, n, 
 on its position in the dataset, not on the batch it was decoded in or the GPU count.  The emitted log-probability is
 log(clamp(P_j, 1e-10, 1)) whatever temperature, top_k and top_p are: it is -nll of the training loss for label j.
 
-The loop is decode_loop.PositionLoop (described there); a position ends with fira_pointer_mix_sample, which also writes
-the next input token straight into the decoder's token buffer and keeps each row's finished flag, length and
-log-probability sum.
+The loop is decode_loop.PositionLoop (described there); a position ends with fira_pointer_mix_sample_prefix, which also
+writes the next input token straight into the decoder's token buffer and keeps each row's finished flag, length and
+log-probability sum.  A commit still inside its `prefix` at a position takes the given label there instead of drawing
+one (same log-probability expression, same bookkeeping); `score` forces the whole message to return log p(message).
 """
 from typing import NamedTuple
 
@@ -23,7 +24,7 @@ import torch
 
 from . import ops
 from ._lib import call
-from .decode_loop import PositionLoop, _f32, check_tar_len, encode, is_int, loop_for
+from .decode_loop import PositionLoop, _f32, check_prefix, check_tar_len, encode, is_int, loop_for
 
 MAX_SAMPLES = 32          # the N samples of a commit are its query rows in fira_attn_fwd / fira_copy_scores_fwd (<= 32)
 
@@ -62,36 +63,74 @@ class _Sampler(PositionLoop):
         self.seed = torch.zeros(1, dtype=torch.int64, device=self.dev)      # read by the kernel as uint64
         self.first = torch.zeros(1, dtype=torch.int32, device=self.dev)
 
-    def start(self, memory, mem_mask, copy_src, seed, first_index, start_id, pad_id):
-        super().start(memory, mem_mask, copy_src, start_id, pad_id)
+    def start(self, memory, mem_mask, copy_src, seed, first_index, start_id, pad_id, prefix=None):
+        super().start(memory, mem_mask, copy_src, start_id, pad_id, prefix)
         self.seed.fill_(seed - 2 ** 64 if seed >= 2 ** 63 else seed)
         self.first.fill_(first_index)
 
     def position(self, t, temperature, top_k, top_p, eos_id, pad_id):
-        """Draw position t + 1 from decoder row t (every launch on the current stream: capturable)."""
+        """Draw position t + 1 from decoder row t, or take a commit's prefix label there (every launch on the current
+        stream: capturable)."""
         self.head(t)
         p = ops._ptr
-        call("fira_pointer_mix_sample", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
+        call("fira_pointer_mix_sample_prefix", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
              p(self.copy_src), p(self.seed), p(self.first), None, float(temperature), int(top_k), float(top_p),
              int(eos_id), int(pad_id), p(self.inc.tok), p(self.seq), p(self.raw), p(self.tlp), p(self.inc.tok_mask),
              self.T, t, p(self.status), p(self.length), p(self.lp), self.B, self.N, self.V, self.S, self.pr.code,
-             ops._stream())
+             ops._stream(), p(self.prefix), self.T, p(self.prefix_len))
 
 
 @torch.no_grad()
 def sample(model, sou, mark, ast_change, edge, sub_token, *, num_samples=1, temperature=1.0, top_k=0, top_p=1.0,
-           seed=0, first_index=0, tar_len=30, start_id, eos_id, pad_id=0):
+           seed=0, first_index=0, tar_len=30, start_id, eos_id, pad_id=0, prefix=None):
     """Draw `num_samples` messages per commit -> Samples(seq, raw, length, logprob, token_logprob).
 
-    first_index: dataset position of the batch's first commit (the Philox counter uses first_index + b)."""
+    first_index: dataset position of the batch's first commit (the Philox counter uses first_index + b).
+    prefix: None, or labels [B, P] every sample of a commit starts with (decode_loop.check_prefix: the tar_label
+    encoding without <start>, a 0 ends a commit's prefix, <eos> only as its last label).  The positions after a prefix
+    draw with the Philox numbers they would draw without it; logprob and token_logprob cover the prefix too."""
     check_args(num_samples, temperature, top_k, top_p, seed, first_index, tar_len)
     check_tar_len(model, tar_len)
     if first_index + sou.shape[0] > 2 ** 31:
         raise ValueError("first_index + batch size must stay below 2**31")
+    pre = check_prefix(prefix, sou, sub_token, V=model.vocab_size, tar_len=tar_len, eos_id=eos_id, pad_id=pad_id,
+                       eos_last=True)
     memory, mem_mask, copy_src = encode(model, sou, mark, ast_change, edge, sub_token, pad_id)
     B, S = memory.shape[:2]
     st = loop_for(_Sampler, model, B, num_samples, tar_len, S)
-    st.start(memory, mem_mask, copy_src, seed, first_index, start_id, pad_id)
+    st.start(memory, mem_mask, copy_src, seed, first_index, start_id, pad_id, pre)
     t = st.run((float(temperature), int(top_k), float(top_p), int(eos_id), int(pad_id)))
     seq, raw, length, lp, tlp, _ = st.slots(t)
     return Samples(seq, raw, length, lp, tlp)
+
+
+class Scores(NamedTuple):
+    token_logprob: torch.Tensor   # [B, T] fp32 log(clamp(P, 1e-10, 1)) of each label, 0 at 0 and after <eos>
+    logprob: torch.Tensor         # [B] fp32 sum of token_logprob: log p(message | commit)
+    length: torch.Tensor          # [B] int64 tokens including <start> and <eos>
+
+
+def score_prefix(tar_label, tar_len, eos_id):
+    """The labels of tar_label [B, >= tar_len] after <start> up to and including each row's first <eos> -> a prefix
+    [B, tar_len - 1] (zeros after <eos>); ValueError for a row without <eos> within tar_len (host only)."""
+    lab = tar_label.detach().to("cpu", torch.int64)[:, 1:tar_len]
+    is_eos = lab == eos_id
+    if lab.shape[1] < tar_len - 1 or not is_eos.any(1).all():
+        raise ValueError(f"every row of tar_label needs <eos> within its first tar_len = {tar_len} labels")
+    after = is_eos.to(torch.int64).cumsum(1) - is_eos.to(torch.int64) > 0       # strictly after the first <eos>
+    return lab.masked_fill(after, 0)
+
+
+@torch.no_grad()
+def score(model, sou, mark, ast_change, edge, sub_token, tar_label, *, tar_len=30, start_id, eos_id, pad_id=0):
+    """log p(message | commit) of each commit's given message -> Scores(token_logprob, logprob, length).
+
+    tar_label [B, >= tar_len]: <start>, the labels (tar_label encoding), <eos> within tar_len, anything after.  The
+    sampler with one sample per commit and the whole message forced, so token_logprob[:, t] is the -nll the training
+    loss gives label tar_label[:, t] after the labels before it."""
+    if not is_int(tar_len) or tar_len < 2:
+        raise ValueError(f"tar_len must be an integer >= 2, got {tar_len!r}")
+    prefix = score_prefix(tar_label, tar_len, eos_id)
+    s = sample(model, sou, mark, ast_change, edge, sub_token, num_samples=1, tar_len=tar_len, start_id=start_id,
+               eos_id=eos_id, pad_id=pad_id, prefix=prefix)
+    return Scores(s.token_logprob[:, 0], s.logprob[:, 0], s.length[:, 0])

@@ -334,6 +334,45 @@ int fira_pointer_mix_diverse_beam_step(const void* logits, long ld_logits, const
                                        int K, int V, int S, int groups, float diversity, int* chosen,
                                        float* lp_workspace, int dtype, void* stream);
 
+/* ---- the three steps above with forced positions (a prefix per commit; fira_icse_b200 `prefix=`, sample.score).
+ *      Arguments as the step without the suffix, plus prefix [B, ld_prefix] int32 and prefix_len [B] int32 (device;
+ *      prefix NULL = nothing forced, the step without the suffix).  Rule: a live row of commit b (not finished; for the
+ *      beam steps status 0) is forced at position pos iff pos < prefix_len[b]; its label is then
+ *      j = prefix[b * ld_prefix + pos] in the label encoding of the training loss (j < V a vocabulary id, V + s memory
+ *      position s) and its lp = log(clamp(P_j, 1e-10, 1)) is formed with the same expressions, bit for bit -nll of
+ *      fira_pointer_mix_nll_fwd for label j.  The sampler's forced row skips the candidate, top-k, top-p and draw
+ *      passes and writes what a drawn j writes (token, raw, lp, mask, length, logprob, finished on eos_id); the Philox
+ *      counter of a later free position is (first_index + b, n, pos) as without a prefix.  A forced row of a beam step
+ *      emits exactly one row winner, (lp, j) (the diverse step: with its rank value and row lp), every other entry
+ *      empty; the select stages are unchanged.  n-best starts with slot 0 (each group's first slot) alone live, so a
+ *      forced commit grows that slot with j, its parent itself, while the other slots stay inactive; the search
+ *      branches at the commit's first free position.  The caller keeps every label < V + S with its copy position
+ *      unmasked, and prefix_len[b] <= ld_prefix; pos < ld_prefix. */
+int fira_pointer_mix_sample_prefix(const void* logits, long ld_logits, const float* copy_scores,
+                                   const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
+                                   const uint64_t* seed, const int* first_index, const float* uniforms,
+                                   float temperature, int top_k, float top_p, int eos_id, int pad_id, int* next_tok,
+                                   int* seq, int* raw, float* token_logprob, unsigned char* tok_mask, long ld_out,
+                                   int pos, unsigned char* finished, int* length, float* logprob, int B, int N, int V,
+                                   int S, int dtype, void* stream, const int* prefix, int ld_prefix,
+                                   const int* prefix_len);
+int fira_pointer_mix_beam_step_prefix(const void* logits, long ld_logits, const float* copy_scores,
+                                      const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
+                                      float length_penalty, int eos_id, int pad_id, uint64_t* workspace, int* seq,
+                                      int* raw, float* token_logprob, int* length, float* logprob, float* score,
+                                      unsigned char* status, long* parent, int* next_tok, int T_len, int pos, int B,
+                                      int K, int V, int S, int dtype, void* stream, const int* prefix, int ld_prefix,
+                                      const int* prefix_len);
+int fira_pointer_mix_diverse_beam_step_prefix(const void* logits, long ld_logits, const float* copy_scores,
+                                              const float* gate_logits, const unsigned char* mem_mask,
+                                              const int* copy_src, float length_penalty, int eos_id, int pad_id,
+                                              uint64_t* workspace, int* seq, int* raw, float* token_logprob,
+                                              int* length, float* logprob, float* score, unsigned char* status,
+                                              long* parent, int* next_tok, int T_len, int pos, int B, int K, int V,
+                                              int S, int groups, float diversity, int* chosen, float* lp_workspace,
+                                              int dtype, void* stream, const int* prefix, int ld_prefix,
+                                              const int* prefix_len);
+
 /* ---- minimum-Bayes-risk selection among each commit's N samples (fira_icse_b200/mbr.py).  seq [B, N, ld_seq] int32
  *      (row (b, n) at (b*N + n) * ld_seq, columns 0..T_len-1), length [B, N] int32 (counts <start>; clamped to
  *      [1, T_len]).  Rule:

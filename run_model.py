@@ -32,6 +32,11 @@ beam search ranking.  Differences, all below the module surface:
     test order, `<expected BLEU>\\t<log-probability>\\t<message>`, the commit's sample with the highest mean id-level
     sentence BLEU against its other samples; FIRA_SAMPLES (default 16 here), FIRA_TEMPERATURE, FIRA_TOP_K, FIRA_TOP_P
     and FIRA_SEED as for sampling; prints the mean sentence BLEU of the chosen messages.
+    FIRA_PREFIX_WORDS=k (default 0 = off; FIRA_DECODE=sample, nbest or mbr): prefix-constrained completion, every test
+    commit's message starts with the first min(k, message words) words of its own reference (their labels, never
+    <eos>) and the decoder completes it -> OUTPUT/<name>_prefix<k> (output_fira_samples_prefix2, ...), so the full
+    decoding outputs stay.  Lines hold the whole message, prefix included, and the printed BLEU is of the whole
+    message against the reference.  FIRA_DECODE=beam with k > 0 exits with an error.
 """
 import json
 import os
@@ -114,6 +119,17 @@ def reference_words(tar, vocab, r_vocab):
     """The reference message of one commit (its target ids between <start> and <eos>) as words."""
     ref = tar.tolist()
     return [r_vocab[x] for x in ref[1:ref.index(vocab['<eos>'])]]
+
+
+def reference_prefix(b, k, eos_id, pad_id):
+    """The first min(k, message words) labels of each commit's tar_label (b[6]) after <start>, never <eos> -> [B, k]
+    (zeros after a message's last word), the decoders' `prefix`.  A copy label the truncated diff no longer holds (its
+    memory position is padding) ends the commit's prefix early."""
+    lab = b[6][:, 1:1 + k]
+    mem_mask = torch.cat((b[0] != pad_id, b[7] != 0), dim=1)
+    V = args.vocab_size
+    gone = (lab >= V) & ~mem_mask.gather(1, (lab - V).clamp(0, mem_mask.shape[1] - 1))
+    return lab.masked_fill(((lab == eos_id) | gone).long().cumsum(1) > 0, 0)
 
 
 def loader(ds, batch_size, shuffle, indices=None):
@@ -235,6 +251,14 @@ def decoder(mode, vocab):
     length [B, N] and the numeric columns [B, N] written before each message, how many leading hypotheses of a commit
     count towards the BLEU)."""
     ids = dict(tar_len=args.tar_len, start_id=vocab['<start>'], eos_id=vocab['<eos>'], pad_id=vocab['<pad>'])
+    k = int(os.environ.get("FIRA_PREFIX_WORDS", 0))
+    if k and mode == "beam":
+        raise SystemExit("FIRA_PREFIX_WORDS applies to FIRA_DECODE=sample, nbest and mbr; the reference beam search "
+                         "takes no prefix")
+    tag = f"_prefix{k}" if k else ""
+
+    def pre(b):                         # each commit's own first k reference labels, or no prefix
+        return reference_prefix(b, k, vocab['<eos>'], vocab['<pad>']) if k else None
     if mode == "beam":                  # the reference's beam search: its best beam, `<message>`
         def decode(model, b, first_index):
             beams = beam_search(model, b[0], b[3], b[4], b[5], b[7], beam_size=args.beam_size, **ids)
@@ -248,15 +272,15 @@ def decoder(mode, vocab):
                     seed=int(os.environ.get("FIRA_SEED", 0)))
     if mode == "sample":                # every sample, `<log-prob>\t<message>`
         def decode(model, b, first_index):
-            out = sample(model, b[0], b[3], b[4], b[5], b[7], first_index=first_index, **opts, **ids)
+            out = sample(model, b[0], b[3], b[4], b[5], b[7], first_index=first_index, prefix=pre(b), **opts, **ids)
             return out.seq, out.length, (out.logprob,)
-        return "output_fira_samples", decode, n
+        return "output_fira_samples" + tag, decode, n
     if mode == "mbr":                   # the sample of highest expected BLEU, `<expected BLEU>\t<log-prob>\t<message>`
         def decode(model, b, first_index):
-            out = mbr(model, b[0], b[3], b[4], b[5], b[7], first_index=first_index, **opts, **ids)
+            out = mbr(model, b[0], b[3], b[4], b[5], b[7], first_index=first_index, prefix=pre(b), **opts, **ids)
             expected = out.utility.gather(1, out.index.unsqueeze(1))
             return out.seq.unsqueeze(1), out.length.unsqueeze(1), (expected, out.logprob.unsqueeze(1))
-        return "output_fira_mbr", decode, 1
+        return "output_fira_mbr" + tag, decode, 1
     if mode == "nbest":                 # FIRA_BEAM hypotheses best first, `<score>\t<log-prob>\t<message>`
         alpha = float(os.environ.get("FIRA_LENGTH_PENALTY", 0.0))
         groups = int(os.environ.get("FIRA_BEAM_GROUPS", 1))
@@ -264,9 +288,9 @@ def decoder(mode, vocab):
 
         def decode(model, b, first_index):
             out = nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=args.beam_size, length_penalty=alpha, **diverse,
-                        **ids)
+                        prefix=pre(b), **ids)
             return out.seq, out.length, (out.score, out.logprob)
-        return "output_fira_nbest", decode, 1
+        return "output_fira_nbest" + tag, decode, 1
     raise SystemExit("FIRA_DECODE must be 'beam', 'sample', 'nbest' or 'mbr'")
 
 

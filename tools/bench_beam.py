@@ -12,6 +12,10 @@ reference's own loop was timed on in BASELINE.md (72 s for 32 commits on CPU).  
                                nbest: beam.nbest, log-space n-best beam search with length_penalty 0;
                                diverse: beam.nbest with groups = the beam width and --diversity;
                                mbr: mbr.mbr over N = the beam width samples)
+                               [--prefix-words k]
+                               (k > 0: sample, nbest, diverse and mbr are also timed with each commit's first k
+                               reference labels (tar_label, never <eos>) as a prefix, next to the same mode without
+                               one; those lines carry prefix_words = k)
 
 nbest and diverse lines also carry `self_bleu`: the mean pairwise id-level sentence BLEU among each commit's K
 hypotheses (one fira_mbr_select launch with pair_bleu, off-diagonal entries averaged over the batch); lower means a
@@ -42,6 +46,7 @@ def main():
     ap.add_argument("--trim", action="store_true", help="loader-side padding trimming (data.trim_batch_host)")
     ap.add_argument("--modes", default="full,graph")
     ap.add_argument("--diversity", type=float, default=0.5, help="diverse mode's penalty per repeated word")
+    ap.add_argument("--prefix-words", type=int, default=0, help="also time the decoders with k-label reference prefixes")
     a = ap.parse_args()
     import torch
     import __graft_entry__
@@ -60,20 +65,26 @@ def main():
     for B in (int(x) for x in a.batches.split(",")):
         hb = bench.host_batch(10_000, B, pin=False, trim=a.trim)
         b = bench.device_batch(hb, dev, B)
-        for K, mode in ((int(x), m) for x in a.beams.split(",") for m in a.modes.split(",")):
+        lab = b[6][:, 1:1 + a.prefix_words]                         # the reference prefixes: never <eos> (id 2)
+        ref_prefix = lab.masked_fill((lab == 2).long().cumsum(1) > 0, 0)
+        cases = [(int(x), m, pw) for x in a.beams.split(",") for m in a.modes.split(",")
+                 for pw in ((0, a.prefix_words) if a.prefix_words and m not in ("full", "graph") else (0,))]
+        for K, mode, pw in cases:
+            pre = dict(prefix=ref_prefix) if pw else {}
+
             def run():
                 if mode == "sample":                                 # N = the beam width, default T / k / p
                     return sample(model, b[0], b[3], b[4], b[5], b[7], num_samples=K, tar_len=30, start_id=1, eos_id=2,
-                                  pad_id=0)
+                                  pad_id=0, **pre)
                 if mode == "mbr":
                     return mbr(model, b[0], b[3], b[4], b[5], b[7], num_samples=K, tar_len=30, start_id=1, eos_id=2,
-                               pad_id=0)
+                               pad_id=0, **pre)
                 if mode == "nbest":
                     return nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=K, tar_len=30, start_id=1, eos_id=2,
-                                 pad_id=0)
+                                 pad_id=0, **pre)
                 if mode == "diverse":
                     return nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=K, tar_len=30, start_id=1, eos_id=2,
-                                 pad_id=0, groups=K, diversity=a.diversity)
+                                 pad_id=0, groups=K, diversity=a.diversity, **pre)
                 return beam_search(model, b[0], b[3], b[4], b[5], b[7], beam_size=K, tar_len=30, start_id=1, eos_id=2,
                                    pad_id=0, mode=mode)
             ref = run()                                              # warm-up (lazy CUDA state, graph capture)
@@ -91,10 +102,12 @@ def main():
             torch.cuda.synchronize()
             ms = e0.elapsed_time(e1) / a.reps
             metric = {"sample": "sampling", "mbr": "mbr"}.get(mode, "beam-search") + " inference throughput"
-            extra = {}
+            extra = {"prefix_words": pw} if a.prefix_words else {}
+            if a.prefix_words:
+                extra.update(card=torch.cuda.get_device_name(dev), power_limit_w=power_limit())
             if mode in ("nbest", "diverse"):
-                extra = {"self_bleu": self_bleu(out, B, K), "card": torch.cuda.get_device_name(dev),
-                         "power_limit_w": power_limit()}
+                extra.update(self_bleu=self_bleu(out, B, K), card=torch.cuda.get_device_name(dev),
+                             power_limit_w=power_limit())
                 if mode == "diverse":
                     extra.update(groups=K, diversity=a.diversity)
             print(json.dumps({**extra,
