@@ -48,6 +48,12 @@ grows with the prefix and the search branches at the commit's first free positio
 score cover the prefix, and the length penalty's n counts it.  A prefix may not hold <eos> and leaves at least one
 free position: a commit that never branched would keep K - 1 inactive slots with score 0.
 
+n-gram repeat blocking and minimum length (`no_repeat_ngram` n, `min_length` m; 0 = off; DESIGN.md §9): at position
+pos a live, non-forced slot's words are its history after <start> (a copy counts as its word, prefix words count); a
+candidate whose word would complete an n-gram already in that history, or is <eos> while the slot has fewer than m
+words, is never offered to the row stage's top K.  The select stage is unchanged, lp and score stay the model's, and a
+slot with fewer than K allowed entries proposes fewer.  A hypothesis can still end unfinished at tar_len.
+
 The loop is decode_loop.PositionLoop (described there); a position ends with fira_pointer_mix_beam_step (per live slot
 row its top K, then per commit the merge, writing the new slots, their parents and the next tokens), the KV-cache
 reorder to the parents and the pad mask of the next tokens.  Slot state is double-buffered by the parity of the
@@ -62,7 +68,7 @@ import torch
 
 from . import ops
 from ._lib import call
-from .decode_loop import PositionLoop, _f32, check_prefix, check_tar_len, encode, is_int, loop_for
+from .decode_loop import PositionLoop, _f32, check_prefix, check_rules, check_tar_len, encode, is_int, loop_for
 from .incremental import IncrementalDecoder
 
 MAX_BEAM = 16             # the row stage keeps a per-thread top K in registers
@@ -204,16 +210,16 @@ class _NBest(PositionLoop):
         self.score[0].zero_()
         self.status[0].view(self.B, self.N)[:, 1:] = 2          # beam 0 has probability 1, the others 0
 
-    def position(self, t, length_penalty, eos_id, pad_id):
+    def position(self, t, length_penalty, eos_id, pad_id, no_repeat_ngram, min_length):
         """Slots of position t + 1 from decoder row t (every launch on the current stream: capturable)."""
         self.head(t)
         p = ops._ptr
         inc = self.inc
-        call("fira_pointer_mix_beam_step_prefix", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
+        call("fira_pointer_mix_beam_step_rules", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
              p(self.copy_src), float(length_penalty), int(eos_id), int(pad_id), p(self.work), p(self.seq), p(self.raw),
              p(self.tlp), p(self.length), p(self.lp), p(self.score), p(self.status), p(self.parent), p(inc.tok),
              self.T, t, self.B, self.N, self.V, self.S, self.pr.code, ops._stream(), p(self.prefix), self.T,
-             p(self.prefix_len))
+             p(self.prefix_len), int(no_repeat_ngram), int(min_length))
         # caches follow the parents BEFORE the pad mask of the new tokens is written (reorder moves tok_mask rows too)
         inc.reorder(self.parent)
         inc.tok_mask[:, t + 1].copy_(inc.tok[:self.R] != pad_id)
@@ -234,28 +240,32 @@ class _DiverseNBest(_NBest):
         status.fill_(2)
         status[:, ::self.N // groups] = 0               # slot g * Kg of every group starts live (L = 0)
 
-    def position(self, t, length_penalty, eos_id, pad_id, groups, diversity):
+    def position(self, t, length_penalty, eos_id, pad_id, no_repeat_ngram, min_length, groups, diversity):
         """Slots of position t + 1 from decoder row t: one call, 2 * groups launches on the current stream."""
         self.head(t)
         p = ops._ptr
         inc = self.inc
-        call("fira_pointer_mix_diverse_beam_step_prefix", p(self.logits), self.ldl, p(self.sc), p(self.gl),
+        call("fira_pointer_mix_diverse_beam_step_rules", p(self.logits), self.ldl, p(self.sc), p(self.gl),
              p(self.mem_mask), p(self.copy_src), float(length_penalty), int(eos_id), int(pad_id), p(self.work),
              p(self.seq), p(self.raw), p(self.tlp), p(self.length), p(self.lp), p(self.score), p(self.status),
              p(self.parent), p(inc.tok), self.T, t, self.B, self.N, self.V, self.S, int(groups), float(diversity),
-             p(self.chosen), p(self.work_lp), self.pr.code, ops._stream(), p(self.prefix), self.T, p(self.prefix_len))
+             p(self.chosen), p(self.work_lp), self.pr.code, ops._stream(), p(self.prefix), self.T, p(self.prefix_len),
+             int(no_repeat_ngram), int(min_length))
         inc.reorder(self.parent)
         inc.tok_mask[:, t + 1].copy_(inc.tok[:self.R] != pad_id)
 
 
 @torch.no_grad()
 def nbest(model, sou, mark, ast_change, edge, sub_token, *, beam_size=3, length_penalty=0.0, tar_len=30, start_id,
-          eos_id, pad_id=0, groups=1, diversity=0.0, prefix=None):
+          eos_id, pad_id=0, groups=1, diversity=0.0, prefix=None, no_repeat_ngram=0, min_length=0):
     """Log-space beam search with length normalisation -> Hypotheses, each commit's K best first (module docstring).
     groups > 1 splits the K slots into diverse beam groups penalised by `diversity` per earlier-group repeat.
     prefix: None, or labels [B, P] every hypothesis of a commit starts with (decode_loop.check_prefix: the tar_label
-    encoding without <start>, a 0 ends a commit's prefix, no <eos>, at most tar_len - 2 labels)."""
+    encoding without <start>, a 0 ends a commit's prefix, no <eos>, at most tar_len - 2 labels).
+    no_repeat_ngram = n >= 1 / min_length = m >= 1: a slot never extends with a word that completes an n-gram already
+    in its hypothesis, nor with <eos> before m words (0 = off; module docstring)."""
     check_nbest_args(beam_size, length_penalty, tar_len, groups, diversity)
+    check_rules(no_repeat_ngram, min_length, tar_len)
     if beam_size > model.vocab_size:
         raise ValueError(f"beam_size {beam_size} exceeds the vocabulary ({model.vocab_size})")
     check_tar_len(model, tar_len)
@@ -266,12 +276,13 @@ def nbest(model, sou, mark, ast_change, edge, sub_token, *, beam_size=3, length_
     if groups == 1:
         st = loop_for(_NBest, model, B, beam_size, tar_len, S)
         st.start(memory, mem_mask, copy_src, start_id, pad_id, pre)
-        t = st.run((float(length_penalty), int(eos_id), int(pad_id)))
+        t = st.run((float(length_penalty), int(eos_id), int(pad_id), no_repeat_ngram, min_length))
         seq, raw, length, lp, tlp, status = st.slots(t)
         return Hypotheses(seq, raw, length, lp, st.score[t & 1].view(B, beam_size).clone(), tlp, status == 1)
     st = loop_for(_DiverseNBest, model, B, beam_size, tar_len, S)
     st.start(memory, mem_mask, copy_src, start_id, pad_id, groups, pre)
-    t = st.run((float(length_penalty), int(eos_id), int(pad_id), int(groups), _f32(diversity)))
+    t = st.run((float(length_penalty), int(eos_id), int(pad_id), no_repeat_ngram, min_length, int(groups),
+                _f32(diversity)))
     seq, raw, length, lp, tlp, status = st.slots(t)
     score = st.score[t & 1].view(B, beam_size)
     score, order = torch.sort(score, dim=1, descending=True, stable=True)        # best first across the groups

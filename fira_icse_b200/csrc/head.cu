@@ -447,6 +447,41 @@ __device__ __forceinline__ float mix_prob(const MixRow& ms, const T* __restrict_
   return ms.g1 * (expf((mrow[s] ? srow[s] : kMaskFill) - ms.cmax) / ms.csum);
 }
 
+// n-gram repeat blocking and minimum length (the _rules entry points).  The words of a live row at position `pos` are
+// its history hist[1..pos] (hist[0] is <start>; a copy's word is already copy_src there).  Label j with word w is banned
+// at column pos + 1 when appending w repeats an n-gram of the history (n = no_repeat >= 1) or when w is eos_id and the
+// row has fewer than min_len words (pos < min_len).  Banned words go into a list s_ban[0..nb): s_ban[0] is eos_id or
+// -1, s_ban[i] (1 <= i <= pos - n + 1) is words[i + n - 1] when words[i .. i + n - 2] == words[pos - n + 2 .. pos], else
+// -1 (no word is negative).  nb = 0 when both rules are off.
+__device__ __forceinline__ int ban_count(int pos, int no_repeat, int min_len) {
+  if (!no_repeat && !min_len) return 0;
+  return 1 + (no_repeat ? max(0, pos - no_repeat + 1) : 0);
+}
+// threads 0..pos copy the history into shared memory; a __syncthreads must follow before ban_build
+__device__ __forceinline__ void ban_load(const int* __restrict__ hist, int pos, int nb, int* s_hist) {
+  if (nb && (int)threadIdx.x <= pos) s_hist[threadIdx.x] = hist[threadIdx.x];
+}
+// threads 0..nb-1 write one entry each; a __syncthreads must follow before the list is read
+__device__ __forceinline__ void ban_build(const int* s_hist, int pos, int no_repeat, int min_len, int eos_id, int nb,
+                                          int* s_ban) {
+  const int i = threadIdx.x;
+  if (i >= nb) return;
+  int w = -1;
+  if (i == 0) {
+    if (pos < min_len) w = eos_id;
+  } else {                                            // nb > 1: no_repeat >= 1 and i + no_repeat - 1 <= pos
+    bool same = true;
+    for (int k = 0; k + 1 < no_repeat; ++k) same &= s_hist[i + k] == s_hist[pos - no_repeat + 2 + k];
+    if (same) w = s_hist[i + no_repeat - 1];
+  }
+  s_ban[i] = w;
+}
+__device__ __forceinline__ bool is_banned(const int* s_ban, int nb, int w) {
+  bool hit = false;
+  for (int e = 0; e < nb; ++e) hit |= s_ban[e] == w;
+  return hit;
+}
+
 template <typename T>
 __global__ void __launch_bounds__(kSampleThreads) pointer_mix_sample_kernel(
     const T* __restrict__ logits, long ldl, const float* __restrict__ sc, const float* __restrict__ gate_logit,
@@ -455,9 +490,11 @@ __global__ void __launch_bounds__(kSampleThreads) pointer_mix_sample_kernel(
     int eos_id, int pad_id, int* __restrict__ next_tok, int* __restrict__ seq, int* __restrict__ raw,
     float* __restrict__ tok_lp, unsigned char* __restrict__ tok_mask, long ld_out, int pos,
     unsigned char* __restrict__ finished, int* __restrict__ length, float* __restrict__ lp_sum,
-    const int* __restrict__ prefix, int ld_prefix, const int* __restrict__ prefix_len, int N, int V, int S) {
+    const int* __restrict__ prefix, int ld_prefix, const int* __restrict__ prefix_len, int no_repeat, int min_len,
+    int N, int V, int S) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
   extern __shared__ float s_sc[];                     // [V + S] tempered scores, NaN = not a candidate
+  __shared__ int s_hist[TMAX], s_ban[TMAX];           // the row's history and banned words (ban_build)
   __shared__ MaxSum sh_ms[8];
   __shared__ float bc[4];
   __shared__ float shf[8];
@@ -501,12 +538,23 @@ __global__ void __launch_bounds__(kSampleThreads) pointer_mix_sample_kernel(
     return;
   }
 
+  const int nb = ban_count(pos, no_repeat, min_len);
+  ban_load(seq + row * ld_out, pos, nb, s_hist);
   const int C = V + S;
   for (int j = threadIdx.x; j < C; j += blockDim.x) {
     const float p = prob(j);
     s_sc[j] = ((j < V || mrow[j - V]) && p > 0.f) ? logf(fminf(p, 1.f)) / temp : __int_as_float(0x7fffffff);
   }
   __syncthreads();
+  if (nb) {                                           // banned labels stop being candidates (before the cuts)
+    ban_build(s_hist, pos, no_repeat, min_len, eos_id, nb, s_ban);
+    __syncthreads();
+    if ((int)threadIdx.x < nb) { const int w = s_ban[threadIdx.x]; if (w >= 0 && w < V) s_sc[w] = __int_as_float(0x7fffffff); }
+    const int* crow = copy_src + (long)b * S;
+    for (int s = threadIdx.x; s < S; s += blockDim.x)
+      if (is_cand(s_sc[V + s]) && is_banned(s_ban, nb, crow[s])) s_sc[V + s] = __int_as_float(0x7fffffff);
+    __syncthreads();
+  }
 
   // every pass below walks a contiguous index range per thread (index order is what the draw needs)
   const int chunk = (C + kSampleThreads - 1) / kSampleThreads;
@@ -620,19 +668,23 @@ __device__ __forceinline__ uint64_t topk_insert(uint64_t (&top)[kMaxBeam], uint6
 template <typename T>
 __global__ void __launch_bounds__(kBeamThreads, 1) beam_row_kernel(
     const T* __restrict__ logits, long ldl, const float* __restrict__ sc, const float* __restrict__ gate_logit,
-    const unsigned char* __restrict__ mem_mask, const unsigned char* __restrict__ status, uint64_t* __restrict__ row_top,
-    const int* __restrict__ prefix, int ld_prefix, const int* __restrict__ prefix_len, int pos, int K, int V, int S) {
+    const unsigned char* __restrict__ mem_mask, const int* __restrict__ copy_src, const unsigned char* __restrict__ status,
+    const int* __restrict__ seq, int Tn, uint64_t* __restrict__ row_top, const int* __restrict__ prefix, int ld_prefix,
+    const int* __restrict__ prefix_len, int no_repeat, int min_len, int eos_id, int pos, int K, int V, int S) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
   __shared__ MaxSum sh_ms[8];
   __shared__ float bc[4];
   __shared__ uint64_t shk[8];
+  __shared__ int s_hist[TMAX], s_ban[TMAX];           // the row's history and banned words (ban_build)
   const long row = blockIdx.x;
   if (status[row] != 0) return;                       // finished or inactive: the select stage reads nothing of it
   const int b = (int)(row / K);
   const T* lrow = logits + row * ldl;
   const float* srow = sc + row * S;
   const unsigned char* mrow = mem_mask + (long)b * S;
-  const MixRow ms = mix_row_stats(lrow, srow, mrow, gate_logit + row * 2, V, S, sh_ms, bc);
+  const int nb = ban_count(pos, no_repeat, min_len);
+  ban_load(seq + row * Tn, pos, nb, s_hist);
+  const MixRow ms = mix_row_stats(lrow, srow, mrow, gate_logit + row * 2, V, S, sh_ms, bc);   // syncs s_hist too
   if (prefix && pos < prefix_len[b]) {                // inside the commit's prefix: its label is the row's one winner
     if (threadIdx.x == 0) {
       const int j = prefix[(long)b * ld_prefix + pos];
@@ -641,6 +693,11 @@ __global__ void __launch_bounds__(kBeamThreads, 1) beam_row_kernel(
     }
     return;
   }
+  if (nb) {
+    ban_build(s_hist, pos, no_repeat, min_len, eos_id, nb, s_ban);
+    __syncthreads();
+  }
+  const int* crow = copy_src + (long)b * S;
 
   uint64_t top[kMaxBeam];                             // this thread's best keys, descending; 0 = empty
 #pragma unroll
@@ -648,7 +705,9 @@ __global__ void __launch_bounds__(kBeamThreads, 1) beam_row_kernel(
   uint64_t thr = 0;                                   // top[K - 1]: the key a candidate has to beat
   auto offer = [&](float p, int j) {
     const uint64_t key = rank_key(logf(fminf(fmaxf(p, 1e-10f), 1.f)), j);   // lp = -nll of fira_pointer_mix_nll_fwd
-    if (key > thr) thr = topk_insert(top, key, K);
+    if (key <= thr) return;
+    if (nb && is_banned(s_ban, nb, j < V ? j : crow[j - V])) return;       // only entries that would enter the top K
+    thr = topk_insert(top, key, K);
   };
   const int V8 = V >> 3;
   for (int g = threadIdx.x; g < V8; g += blockDim.x) {
@@ -777,23 +836,27 @@ __global__ void __launch_bounds__(kBeamThreads, 1) diverse_row_kernel(
     const T* __restrict__ logits, long ldl, const float* __restrict__ sc, const float* __restrict__ gate_logit,
     const unsigned char* __restrict__ mem_mask, const int* __restrict__ copy_src, const unsigned char* __restrict__ status,
     const float* __restrict__ lp_sum, const int* __restrict__ length, const int* __restrict__ chosen, float alpha,
-    float diversity, uint64_t* __restrict__ row_top, float* __restrict__ row_lp, const int* __restrict__ prefix,
-    int ld_prefix, const int* __restrict__ prefix_len, int pos, int g, int Kg, int K, int V, int S) {
+    float diversity, uint64_t* __restrict__ row_top, float* __restrict__ row_lp, const int* __restrict__ seq, int Tn,
+    const int* __restrict__ prefix, int ld_prefix, const int* __restrict__ prefix_len, int no_repeat, int min_len,
+    int eos_id, int pos, int g, int Kg, int K, int V, int S) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
   __shared__ MaxSum sh_ms[8];
   __shared__ float bc[4];
   __shared__ uint64_t shk[8];
   __shared__ int s_prev[kMaxBeam];                    // tokens the earlier groups' slots grew with at this position
+  __shared__ int s_hist[TMAX], s_ban[TMAX];           // the row's history and banned words (ban_build)
   const int b = blockIdx.x / Kg;
   const long row = (long)b * K + g * Kg + blockIdx.x % Kg;     // slot row (status / state are of the read half)
   if (status[row] != 0) return;                       // finished or inactive: the select stage reads nothing of it
   const int n_prev = g * Kg;
   if (threadIdx.x < n_prev) s_prev[threadIdx.x] = chosen[(long)b * K + threadIdx.x];
+  const int nb = ban_count(pos, no_repeat, min_len);
+  ban_load(seq + row * Tn, pos, nb, s_hist);
   const T* lrow = logits + row * ldl;
   const float* srow = sc + row * S;
   const unsigned char* mrow = mem_mask + (long)b * S;
   const int* crow = copy_src + (long)b * S;
-  const MixRow ms = mix_row_stats(lrow, srow, mrow, gate_logit + row * 2, V, S, sh_ms, bc);   // syncs s_prev too
+  const MixRow ms = mix_row_stats(lrow, srow, mrow, gate_logit + row * 2, V, S, sh_ms, bc);   // syncs s_prev, s_hist
   const float L_i = lp_sum[row], norm = beam_norm(length[row], alpha);
   auto lp_of = [&](float p) { return logf(fminf(fmaxf(p, 1e-10f), 1.f)); };   // = -nll of fira_pointer_mix_nll_fwd
   if (prefix && pos < prefix_len[b]) {                // inside the commit's prefix: its label is the row's one winner
@@ -808,6 +871,10 @@ __global__ void __launch_bounds__(kBeamThreads, 1) diverse_row_kernel(
     }
     return;
   }
+  if (nb) {
+    ban_build(s_hist, pos, no_repeat, min_len, eos_id, nb, s_ban);
+    __syncthreads();
+  }
 
   uint64_t top[kMaxBeam];                             // this thread's best keys, descending; 0 = empty
 #pragma unroll
@@ -817,7 +884,9 @@ __global__ void __launch_bounds__(kBeamThreads, 1) diverse_row_kernel(
     float score;
     const float v0 = diverse_value(L_i, lp_of(p), norm, diversity, 0, &score);
     if (rank_key(v0, j) <= thr) return;               // the penalty only lowers the value
-    const int h = n_prev ? count_token(s_prev, n_prev, j < V ? j : crow[j - V]) : 0;
+    const int w = j < V ? j : crow[j - V];
+    if (nb && is_banned(s_ban, nb, w)) return;        // only entries that would enter the top Kg
+    const int h = n_prev ? count_token(s_prev, n_prev, w) : 0;
     const uint64_t key = h ? rank_key(diverse_value(L_i, lp_of(p), norm, diversity, h, &score), j) : rank_key(v0, j);
     if (key > thr) thr = topk_insert(top, key, Kg);
   };
@@ -1041,9 +1110,14 @@ static int sample_impl(const void* logits, long ld_logits, const float* copy_sco
                        const float* uniforms, float temperature, int top_k, float top_p, int eos_id, int pad_id,
                        int* next_tok, int* seq, int* raw, float* token_logprob, unsigned char* tok_mask, long ld_out,
                        int pos, unsigned char* finished, int* length, float* logprob, int B, int N, int V, int S,
-                       const int* prefix, int ld_prefix, const int* prefix_len, int dtype, void* stream) {
+                       const int* prefix, int ld_prefix, const int* prefix_len, int no_repeat, int min_len, int dtype,
+                       void* stream) {
   FIRA_CHECK_ARG(!prefix || (prefix_len && ld_prefix > pos), FIRA_ERR_ARG,
                  "pointer_mix_sample_prefix: null prefix_len or ld_prefix %d <= pos %d", ld_prefix, pos);
+  FIRA_CHECK_ARG(no_repeat >= 0 && min_len >= 0, FIRA_ERR_ARG,
+                 "pointer_mix_sample_rules: no_repeat_ngram %d / min_length %d < 0", no_repeat, min_len);
+  FIRA_CHECK_ARG((!no_repeat && !min_len) || ld_out <= TMAX, FIRA_ERR_SHAPE,
+                 "pointer_mix_sample_rules: ld_out %ld > %d", ld_out, TMAX);
   FIRA_CHECK_ARG(B >= 0 && N > 0 && V > 0 && S > 0 && V + S <= 0x7FFF, FIRA_ERR_SHAPE,
                  "pointer_mix_sample: shape (B %d, N %d, V %d, S %d; V + S must be <= 32767)", B, N, V, S);
   FIRA_CHECK_ARG(pos >= 0 && ld_out >= pos + 2, FIRA_ERR_SHAPE, "pointer_mix_sample: pos %d, ld_out %ld", pos, ld_out);
@@ -1063,7 +1137,7 @@ static int sample_impl(const void* logits, long ld_logits, const float* copy_sco
   DISPATCH_T(dtype, launch_k(pointer_mix_sample_kernel<T>, dim3((unsigned)(B * N)), dim3(kSampleThreads), smem,
       (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, seed, first_index,
       uniforms, temperature, top_k, top_p, eos_id, pad_id, next_tok, seq, raw, token_logprob, tok_mask, ld_out, pos,
-      finished, length, logprob, prefix, ld_prefix, prefix_len, N, V, S);)
+      finished, length, logprob, prefix, ld_prefix, prefix_len, no_repeat, min_len, N, V, S);)
   FIRA_CHECK_LAUNCH("fira_pointer_mix_sample");
   return FIRA_OK;
 }
@@ -1076,7 +1150,7 @@ int fira_pointer_mix_sample(const void* logits, long ld_logits, const float* cop
                             float* logprob, int B, int N, int V, int S, int dtype, void* stream) {
   return sample_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, seed, first_index, uniforms,
                      temperature, top_k, top_p, eos_id, pad_id, next_tok, seq, raw, token_logprob, tok_mask, ld_out, pos,
-                     finished, length, logprob, B, N, V, S, nullptr, 0, nullptr, dtype, stream);
+                     finished, length, logprob, B, N, V, S, nullptr, 0, nullptr, 0, 0, dtype, stream);
 }
 
 int fira_pointer_mix_sample_prefix(const void* logits, long ld_logits, const float* copy_scores,
@@ -1089,7 +1163,21 @@ int fira_pointer_mix_sample_prefix(const void* logits, long ld_logits, const flo
                                    const int* prefix_len) {
   return sample_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, seed, first_index, uniforms,
                      temperature, top_k, top_p, eos_id, pad_id, next_tok, seq, raw, token_logprob, tok_mask, ld_out, pos,
-                     finished, length, logprob, B, N, V, S, prefix, ld_prefix, prefix_len, dtype, stream);
+                     finished, length, logprob, B, N, V, S, prefix, ld_prefix, prefix_len, 0, 0, dtype, stream);
+}
+
+int fira_pointer_mix_sample_rules(const void* logits, long ld_logits, const float* copy_scores,
+                                  const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
+                                  const uint64_t* seed, const int* first_index, const float* uniforms,
+                                  float temperature, int top_k, float top_p, int eos_id, int pad_id, int* next_tok,
+                                  int* seq, int* raw, float* token_logprob, unsigned char* tok_mask, long ld_out,
+                                  int pos, unsigned char* finished, int* length, float* logprob, int B, int N, int V,
+                                  int S, int dtype, void* stream, const int* prefix, int ld_prefix,
+                                  const int* prefix_len, int no_repeat_ngram, int min_length) {
+  return sample_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, seed, first_index, uniforms,
+                     temperature, top_k, top_p, eos_id, pad_id, next_tok, seq, raw, token_logprob, tok_mask, ld_out, pos,
+                     finished, length, logprob, B, N, V, S, prefix, ld_prefix, prefix_len, no_repeat_ngram, min_length,
+                     dtype, stream);
 }
 
 static int beam_step_impl(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
@@ -1097,9 +1185,13 @@ static int beam_step_impl(const void* logits, long ld_logits, const float* copy_
                           int pad_id, uint64_t* workspace, int* seq, int* raw, float* token_logprob, int* length,
                           float* logprob, float* score, unsigned char* status, long* parent, int* next_tok, int T_len,
                           int pos, int B, int K, int V, int S, const int* prefix, int ld_prefix, const int* prefix_len,
-                          int dtype, void* stream) {
+                          int no_repeat, int min_len, int dtype, void* stream) {
   FIRA_CHECK_ARG(!prefix || (prefix_len && ld_prefix > pos), FIRA_ERR_ARG,
                  "pointer_mix_beam_step_prefix: null prefix_len or ld_prefix %d <= pos %d", ld_prefix, pos);
+  FIRA_CHECK_ARG(no_repeat >= 0 && min_len >= 0, FIRA_ERR_ARG,
+                 "pointer_mix_beam_step_rules: no_repeat_ngram %d / min_length %d < 0", no_repeat, min_len);
+  FIRA_CHECK_ARG((!no_repeat && !min_len) || T_len <= TMAX, FIRA_ERR_SHAPE,
+                 "pointer_mix_beam_step_rules: T_len %d > %d", T_len, TMAX);
   FIRA_CHECK_ARG(B >= 0 && K >= 1 && K <= kMaxBeam && V >= K && S > 0 && V + S <= 0x7FFF, FIRA_ERR_SHAPE,
                  "pointer_mix_beam_step: shape (B %d, K %d, V %d, S %d; 1 <= K <= 16, K <= V, V + S <= 32767)",
                  B, K, V, S);
@@ -1110,8 +1202,9 @@ static int beam_step_impl(const void* logits, long ld_logits, const float* copy_
                  "pointer_mix_beam_step: logits must be 16-byte aligned with a leading dimension that is a multiple of 8");
   if (B == 0) return FIRA_OK;
   DISPATCH_T(dtype, launch_k(beam_row_kernel<T>, dim3((unsigned)(B * K)), dim3(kBeamThreads), 0, (cudaStream_t)stream,
-      (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, (const unsigned char*)status + (pos & 1) * (long)B * K,
-      workspace, prefix, ld_prefix, prefix_len, pos, K, V, S);)
+      (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src,
+      (const unsigned char*)status + (pos & 1) * (long)B * K, (const int*)seq + (pos & 1) * (long)B * K * T_len, T_len,
+      workspace, prefix, ld_prefix, prefix_len, no_repeat, min_len, eos_id, pos, K, V, S);)
   FIRA_CHECK_LAUNCH("fira_pointer_mix_beam_step (rows)");
   launch_k(beam_select_kernel, dim3((unsigned)B), dim3(kBeamThreads), 0, (cudaStream_t)stream, (const uint64_t*)workspace,
            copy_src, length_penalty, eos_id, pad_id, seq, raw, token_logprob, length, logprob, score, status, parent,
@@ -1127,7 +1220,7 @@ int fira_pointer_mix_beam_step(const void* logits, long ld_logits, const float* 
                                int T_len, int pos, int B, int K, int V, int S, int dtype, void* stream) {
   return beam_step_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, length_penalty, eos_id, pad_id,
                         workspace, seq, raw, token_logprob, length, logprob, score, status, parent, next_tok, T_len, pos,
-                        B, K, V, S, nullptr, 0, nullptr, dtype, stream);
+                        B, K, V, S, nullptr, 0, nullptr, 0, 0, dtype, stream);
 }
 
 int fira_pointer_mix_beam_step_prefix(const void* logits, long ld_logits, const float* copy_scores,
@@ -1139,7 +1232,19 @@ int fira_pointer_mix_beam_step_prefix(const void* logits, long ld_logits, const 
                                       const int* prefix_len) {
   return beam_step_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, length_penalty, eos_id, pad_id,
                         workspace, seq, raw, token_logprob, length, logprob, score, status, parent, next_tok, T_len, pos,
-                        B, K, V, S, prefix, ld_prefix, prefix_len, dtype, stream);
+                        B, K, V, S, prefix, ld_prefix, prefix_len, 0, 0, dtype, stream);
+}
+
+int fira_pointer_mix_beam_step_rules(const void* logits, long ld_logits, const float* copy_scores,
+                                     const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
+                                     float length_penalty, int eos_id, int pad_id, uint64_t* workspace, int* seq,
+                                     int* raw, float* token_logprob, int* length, float* logprob, float* score,
+                                     unsigned char* status, long* parent, int* next_tok, int T_len, int pos, int B,
+                                     int K, int V, int S, int dtype, void* stream, const int* prefix, int ld_prefix,
+                                     const int* prefix_len, int no_repeat_ngram, int min_length) {
+  return beam_step_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, length_penalty, eos_id, pad_id,
+                        workspace, seq, raw, token_logprob, length, logprob, score, status, parent, next_tok, T_len, pos,
+                        B, K, V, S, prefix, ld_prefix, prefix_len, no_repeat_ngram, min_length, dtype, stream);
 }
 
 static int diverse_beam_step_impl(const void* logits, long ld_logits, const float* copy_scores,
@@ -1148,9 +1253,14 @@ static int diverse_beam_step_impl(const void* logits, long ld_logits, const floa
                                   float* token_logprob, int* length, float* logprob, float* score,
                                   unsigned char* status, long* parent, int* next_tok, int T_len, int pos, int B, int K,
                                   int V, int S, int groups, float diversity, int* chosen, float* lp_workspace,
-                                  const int* prefix, int ld_prefix, const int* prefix_len, int dtype, void* stream) {
+                                  const int* prefix, int ld_prefix, const int* prefix_len, int no_repeat, int min_len,
+                                  int dtype, void* stream) {
   FIRA_CHECK_ARG(!prefix || (prefix_len && ld_prefix > pos), FIRA_ERR_ARG,
                  "pointer_mix_diverse_beam_step_prefix: null prefix_len or ld_prefix %d <= pos %d", ld_prefix, pos);
+  FIRA_CHECK_ARG(no_repeat >= 0 && min_len >= 0, FIRA_ERR_ARG,
+                 "pointer_mix_diverse_beam_step_rules: no_repeat_ngram %d / min_length %d < 0", no_repeat, min_len);
+  FIRA_CHECK_ARG((!no_repeat && !min_len) || T_len <= TMAX, FIRA_ERR_SHAPE,
+                 "pointer_mix_diverse_beam_step_rules: T_len %d > %d", T_len, TMAX);
   FIRA_CHECK_ARG(B >= 0 && K >= 1 && K <= kMaxBeam && V >= K && S > 0 && V + S <= 0x7FFF, FIRA_ERR_SHAPE,
                  "pointer_mix_diverse_beam_step: shape (B %d, K %d, V %d, S %d; 1 <= K <= 16, K <= V, V + S <= 32767)",
                  B, K, V, S);
@@ -1174,7 +1284,8 @@ static int diverse_beam_step_impl(const void* logits, long ld_logits, const floa
     DISPATCH_T(dtype, launch_k(diverse_row_kernel<T>, dim3((unsigned)(B * Kg)), dim3(kBeamThreads), 0,
         (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src,
         (const unsigned char*)status + in, (const float*)logprob + in, (const int*)length + in, (const int*)chosen,
-        length_penalty, diversity, workspace, lp_workspace, prefix, ld_prefix, prefix_len, pos, g, Kg, K, V, S);)
+        length_penalty, diversity, workspace, lp_workspace, (const int*)seq + in * T_len, T_len, prefix, ld_prefix,
+        prefix_len, no_repeat, min_len, eos_id, pos, g, Kg, K, V, S);)
     FIRA_CHECK_LAUNCH("fira_pointer_mix_diverse_beam_step (rows)");
     launch_k(diverse_select_kernel, dim3((unsigned)B), dim3(kBeamThreads), 0, (cudaStream_t)stream,
              (const uint64_t*)workspace, (const float*)lp_workspace, copy_src, length_penalty, diversity, eos_id,
@@ -1195,7 +1306,7 @@ int fira_pointer_mix_diverse_beam_step(const void* logits, long ld_logits, const
   return diverse_beam_step_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, length_penalty, eos_id,
                                 pad_id, workspace, seq, raw, token_logprob, length, logprob, score, status, parent,
                                 next_tok, T_len, pos, B, K, V, S, groups, diversity, chosen, lp_workspace, nullptr, 0,
-                                nullptr, dtype, stream);
+                                nullptr, 0, 0, dtype, stream);
 }
 
 int fira_pointer_mix_diverse_beam_step_prefix(const void* logits, long ld_logits, const float* copy_scores,
@@ -1210,7 +1321,22 @@ int fira_pointer_mix_diverse_beam_step_prefix(const void* logits, long ld_logits
   return diverse_beam_step_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, length_penalty, eos_id,
                                 pad_id, workspace, seq, raw, token_logprob, length, logprob, score, status, parent,
                                 next_tok, T_len, pos, B, K, V, S, groups, diversity, chosen, lp_workspace, prefix,
-                                ld_prefix, prefix_len, dtype, stream);
+                                ld_prefix, prefix_len, 0, 0, dtype, stream);
+}
+
+int fira_pointer_mix_diverse_beam_step_rules(const void* logits, long ld_logits, const float* copy_scores,
+                                             const float* gate_logits, const unsigned char* mem_mask,
+                                             const int* copy_src, float length_penalty, int eos_id, int pad_id,
+                                             uint64_t* workspace, int* seq, int* raw, float* token_logprob,
+                                             int* length, float* logprob, float* score, unsigned char* status,
+                                             long* parent, int* next_tok, int T_len, int pos, int B, int K, int V,
+                                             int S, int groups, float diversity, int* chosen, float* lp_workspace,
+                                             int dtype, void* stream, const int* prefix, int ld_prefix,
+                                             const int* prefix_len, int no_repeat_ngram, int min_length) {
+  return diverse_beam_step_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, length_penalty, eos_id,
+                                pad_id, workspace, seq, raw, token_logprob, length, logprob, score, status, parent,
+                                next_tok, T_len, pos, B, K, V, S, groups, diversity, chosen, lp_workspace, prefix,
+                                ld_prefix, prefix_len, no_repeat_ngram, min_length, dtype, stream);
 }
 
 }  // extern "C"

@@ -8,7 +8,8 @@ which writes the next input tokens straight into the decoder's token buffer and 
 (`position`, defined by each decoder).  A position is captured once into a CUDA graph and replayed for every later
 batch of the same shape; the loop reads back nothing but an all-finished flag, once every POLL_EVERY positions.
 Every position also passes the per-commit prefix buffers (`check_prefix`): a commit still inside its prefix takes the
-given label at that position instead of choosing one, inside the step kernel.
+given label at that position instead of choosing one, inside the step kernel.  The n-gram repeat blocking and minimum
+length settings (`check_rules`) are part of a position's cfg key, so each setting replays its own graphs.
 """
 import ctypes
 import weakref
@@ -35,6 +36,25 @@ def check_tar_len(model, tar_len):
     """ValueError when the decoder has fewer than tar_len positions (called before any device work)."""
     if tar_len > model.decoder.pos_encode.shape[0]:
         raise ValueError(f"tar_len {tar_len} exceeds the decoder's {model.decoder.pos_encode.shape[0]} positions")
+
+
+MAX_RULES_TAR_LEN = 32    # the step kernels hold a row's history in a fixed shared-memory list (head.cu TMAX)
+
+
+def check_rules(no_repeat_ngram, min_length, tar_len):
+    """ValueError for n-gram blocking / minimum length settings the step kernels cannot honour (called before any device
+    work).  no_repeat_ngram = n >= 1 bans every word that would repeat an n-gram of the row's history, min_length = m
+    bans <eos> while the row has fewer than m words; 0 turns either off.  n > tar_len - 1 or m > tar_len - 2 could never
+    apply, or would leave no position for <eos>, so they are refused rather than silently ignored."""
+    for name, v in (("no_repeat_ngram", no_repeat_ngram), ("min_length", min_length)):
+        if not is_int(v) or v < 0:
+            raise ValueError(f"{name} must be an integer >= 0 (0 = off), got {v!r}")
+    if no_repeat_ngram > tar_len - 1:
+        raise ValueError(f"no_repeat_ngram must be <= tar_len - 1 = {tar_len - 1}, got {no_repeat_ngram}")
+    if min_length > tar_len - 2:
+        raise ValueError(f"min_length must be <= tar_len - 2 = {tar_len - 2}, got {min_length}")
+    if (no_repeat_ngram or min_length) and tar_len > MAX_RULES_TAR_LEN:
+        raise ValueError(f"no_repeat_ngram / min_length need tar_len <= {MAX_RULES_TAR_LEN}, got {tar_len}")
 
 
 def check_prefix(prefix, sou, sub_token, *, V, tar_len, eos_id, pad_id, eos_last):

@@ -39,9 +39,9 @@ class MBR(NamedTuple):
 
 @torch.no_grad()
 def mbr(model, sou, mark, ast_change, edge, sub_token, *, num_samples=16, temperature=1.0, top_k=0, top_p=1.0,
-        seed=0, first_index=0, tar_len=30, start_id, eos_id, pad_id=0, prefix=None):
+        seed=0, first_index=0, tar_len=30, start_id, eos_id, pad_id=0, prefix=None, no_repeat_ngram=0, min_length=0):
     """Draw `num_samples` messages per commit with sample() and keep the one of highest expected BLEU -> MBR.
-    prefix: None, or labels [B, P] every sample of a commit starts with (as for sample())."""
+    prefix, no_repeat_ngram, min_length: passed to sample(), so every candidate obeys them."""
     check_args(num_samples, temperature, top_k, top_p, seed, first_index, tar_len)
     if num_samples < 2:
         raise ValueError(f"MBR needs num_samples >= 2, got {num_samples!r}")
@@ -49,7 +49,7 @@ def mbr(model, sou, mark, ast_change, edge, sub_token, *, num_samples=16, temper
         raise ValueError(f"MBR needs tar_len <= {MAX_TAR_LEN}, got {tar_len!r}")
     s = sample(model, sou, mark, ast_change, edge, sub_token, num_samples=num_samples, temperature=temperature,
                top_k=top_k, top_p=top_p, seed=seed, first_index=first_index, tar_len=tar_len, start_id=start_id,
-               eos_id=eos_id, pad_id=pad_id, prefix=prefix)
+               eos_id=eos_id, pad_id=pad_id, prefix=prefix, no_repeat_ngram=no_repeat_ngram, min_length=min_length)
     B, N, T = s.seq.shape
     dev = s.seq.device
     seq, length = s.seq.to(torch.int32), s.length.to(torch.int32)

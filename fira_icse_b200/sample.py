@@ -13,10 +13,12 @@ u comes from Philox4x32-7 keyed by `seed` with the counter (first_index + b, n, 
 on its position in the dataset, not on the batch it was decoded in or the GPU count.  The emitted log-probability is
 log(clamp(P_j, 1e-10, 1)) whatever temperature, top_k and top_p are: it is -nll of the training loss for label j.
 
-The loop is decode_loop.PositionLoop (described there); a position ends with fira_pointer_mix_sample_prefix, which also
+The loop is decode_loop.PositionLoop (described there); a position ends with fira_pointer_mix_sample_rules, which also
 writes the next input token straight into the decoder's token buffer and keeps each row's finished flag, length and
 log-probability sum.  A commit still inside its `prefix` at a position takes the given label there instead of drawing
 one (same log-probability expression, same bookkeeping); `score` forces the whole message to return log p(message).
+`no_repeat_ngram` / `min_length` remove the labels that would repeat an n-gram of the sample or end it before m words
+from the candidates of that position, inside the same kernel (DESIGN.md §9).
 """
 from typing import NamedTuple
 
@@ -24,7 +26,7 @@ import torch
 
 from . import ops
 from ._lib import call
-from .decode_loop import PositionLoop, _f32, check_prefix, check_tar_len, encode, is_int, loop_for
+from .decode_loop import PositionLoop, _f32, check_prefix, check_rules, check_tar_len, encode, is_int, loop_for
 
 MAX_SAMPLES = 32          # the N samples of a commit are its query rows in fira_attn_fwd / fira_copy_scores_fwd (<= 32)
 
@@ -68,28 +70,34 @@ class _Sampler(PositionLoop):
         self.seed.fill_(seed - 2 ** 64 if seed >= 2 ** 63 else seed)
         self.first.fill_(first_index)
 
-    def position(self, t, temperature, top_k, top_p, eos_id, pad_id):
+    def position(self, t, temperature, top_k, top_p, eos_id, pad_id, no_repeat_ngram, min_length):
         """Draw position t + 1 from decoder row t, or take a commit's prefix label there (every launch on the current
         stream: capturable)."""
         self.head(t)
         p = ops._ptr
-        call("fira_pointer_mix_sample_prefix", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
+        call("fira_pointer_mix_sample_rules", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
              p(self.copy_src), p(self.seed), p(self.first), None, float(temperature), int(top_k), float(top_p),
              int(eos_id), int(pad_id), p(self.inc.tok), p(self.seq), p(self.raw), p(self.tlp), p(self.inc.tok_mask),
              self.T, t, p(self.status), p(self.length), p(self.lp), self.B, self.N, self.V, self.S, self.pr.code,
-             ops._stream(), p(self.prefix), self.T, p(self.prefix_len))
+             ops._stream(), p(self.prefix), self.T, p(self.prefix_len), int(no_repeat_ngram), int(min_length))
 
 
 @torch.no_grad()
 def sample(model, sou, mark, ast_change, edge, sub_token, *, num_samples=1, temperature=1.0, top_k=0, top_p=1.0,
-           seed=0, first_index=0, tar_len=30, start_id, eos_id, pad_id=0, prefix=None):
+           seed=0, first_index=0, tar_len=30, start_id, eos_id, pad_id=0, prefix=None, no_repeat_ngram=0,
+           min_length=0):
     """Draw `num_samples` messages per commit -> Samples(seq, raw, length, logprob, token_logprob).
 
     first_index: dataset position of the batch's first commit (the Philox counter uses first_index + b).
     prefix: None, or labels [B, P] every sample of a commit starts with (decode_loop.check_prefix: the tar_label
     encoding without <start>, a 0 ends a commit's prefix, <eos> only as its last label).  The positions after a prefix
-    draw with the Philox numbers they would draw without it; logprob and token_logprob cover the prefix too."""
+    draw with the Philox numbers they would draw without it; logprob and token_logprob cover the prefix too.
+    no_repeat_ngram = n >= 1: no drawn word completes an n-gram already in the sample (n = 1: no word twice; a copy
+    counts as its word).  min_length = m >= 1: no <eos> before m words.  Banned labels are dropped from the candidates
+    before the top-k / top-p cuts, nothing is renormalised and token_logprob keeps the model's log-probability; prefix
+    positions are exempt.  0 turns either off (decode_loop.check_rules)."""
     check_args(num_samples, temperature, top_k, top_p, seed, first_index, tar_len)
+    check_rules(no_repeat_ngram, min_length, tar_len)
     check_tar_len(model, tar_len)
     if first_index + sou.shape[0] > 2 ** 31:
         raise ValueError("first_index + batch size must stay below 2**31")
@@ -99,7 +107,7 @@ def sample(model, sou, mark, ast_change, edge, sub_token, *, num_samples=1, temp
     B, S = memory.shape[:2]
     st = loop_for(_Sampler, model, B, num_samples, tar_len, S)
     st.start(memory, mem_mask, copy_src, seed, first_index, start_id, pad_id, pre)
-    t = st.run((float(temperature), int(top_k), float(top_p), int(eos_id), int(pad_id)))
+    t = st.run((float(temperature), int(top_k), float(top_p), int(eos_id), int(pad_id), no_repeat_ngram, min_length))
     seq, raw, length, lp, tlp, _ = st.slots(t)
     return Samples(seq, raw, length, lp, tlp)
 

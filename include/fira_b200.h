@@ -373,6 +373,42 @@ int fira_pointer_mix_diverse_beam_step_prefix(const void* logits, long ld_logits
                                               int dtype, void* stream, const int* prefix, int ld_prefix,
                                               const int* prefix_len);
 
+/* ---- the three _prefix steps with n-gram repeat blocking and a minimum message length (fira_icse_b200
+ *      `no_repeat_ngram=`, `min_length=`).  Arguments as the _prefix step (prefix may be NULL), plus no_repeat_ngram
+ *      n >= 0 and min_length m >= 0 (0 = off; both 0 = the _prefix step, bit for bit).  Rule: the words of a live,
+ *      non-forced row at position pos are its seq ids in columns 1..pos (a copy is its word copy_src[b, j - V]; forced
+ *      prefix words count); the sampler reads its own seq row, the beam steps the read half.  Label j with word w is
+ *      banned at column pos + 1 if, with n >= 1, some i >= 1 with i + n - 1 <= pos has words[i .. i+n-2] ==
+ *      words[pos-n+2 .. pos] and words[i+n-1] == w (n = 1: no word twice), or if w == eos_id and pos < m (fewer than m
+ *      words).  A banned label is not a candidate: the sampler drops it before the top-k / top-p cuts (nothing is
+ *      renormalised, the Philox counter is unchanged), the beam row stages never offer it to their top K (a row with
+ *      fewer allowed entries proposes fewer); the select stages and every emitted lp are unchanged.  Forced rows are
+ *      exempt.  With a rule on: T_len <= 32 (the sampler: ld_out <= 32). */
+int fira_pointer_mix_sample_rules(const void* logits, long ld_logits, const float* copy_scores,
+                                  const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
+                                  const uint64_t* seed, const int* first_index, const float* uniforms,
+                                  float temperature, int top_k, float top_p, int eos_id, int pad_id, int* next_tok,
+                                  int* seq, int* raw, float* token_logprob, unsigned char* tok_mask, long ld_out,
+                                  int pos, unsigned char* finished, int* length, float* logprob, int B, int N, int V,
+                                  int S, int dtype, void* stream, const int* prefix, int ld_prefix,
+                                  const int* prefix_len, int no_repeat_ngram, int min_length);
+int fira_pointer_mix_beam_step_rules(const void* logits, long ld_logits, const float* copy_scores,
+                                     const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
+                                     float length_penalty, int eos_id, int pad_id, uint64_t* workspace, int* seq,
+                                     int* raw, float* token_logprob, int* length, float* logprob, float* score,
+                                     unsigned char* status, long* parent, int* next_tok, int T_len, int pos, int B,
+                                     int K, int V, int S, int dtype, void* stream, const int* prefix, int ld_prefix,
+                                     const int* prefix_len, int no_repeat_ngram, int min_length);
+int fira_pointer_mix_diverse_beam_step_rules(const void* logits, long ld_logits, const float* copy_scores,
+                                             const float* gate_logits, const unsigned char* mem_mask,
+                                             const int* copy_src, float length_penalty, int eos_id, int pad_id,
+                                             uint64_t* workspace, int* seq, int* raw, float* token_logprob,
+                                             int* length, float* logprob, float* score, unsigned char* status,
+                                             long* parent, int* next_tok, int T_len, int pos, int B, int K, int V,
+                                             int S, int groups, float diversity, int* chosen, float* lp_workspace,
+                                             int dtype, void* stream, const int* prefix, int ld_prefix,
+                                             const int* prefix_len, int no_repeat_ngram, int min_length);
+
 /* ---- minimum-Bayes-risk selection among each commit's N samples (fira_icse_b200/mbr.py).  seq [B, N, ld_seq] int32
  *      (row (b, n) at (b*N + n) * ld_seq, columns 0..T_len-1), length [B, N] int32 (counts <start>; clamped to
  *      [1, T_len]).  Rule:

@@ -37,6 +37,11 @@ beam search ranking.  Differences, all below the module surface:
     <eos>) and the decoder completes it -> OUTPUT/<name>_prefix<k> (output_fira_samples_prefix2, ...), so the full
     decoding outputs stay.  Lines hold the whole message, prefix included, and the printed BLEU is of the whole
     message against the reference.  FIRA_DECODE=beam with k > 0 exits with an error.
+    FIRA_NO_REPEAT_NGRAM=n and FIRA_MIN_LENGTH=m (default 0 = off; FIRA_DECODE=sample, nbest or mbr): no generated word
+    completes an n-gram already in its message (n = 1: no word twice), and no message ends before m words (DESIGN.md
+    §9).  A nonzero value appends _norepeat<n> / _minlen<m> to the output name, after any _prefix<k>
+    (output_fira_nbest_norepeat2_minlen3, ...), so the outputs without them stay.  FIRA_DECODE=beam with either set
+    exits with an error.
 """
 import json
 import os
@@ -255,7 +260,14 @@ def decoder(mode, vocab):
     if k and mode == "beam":
         raise SystemExit("FIRA_PREFIX_WORDS applies to FIRA_DECODE=sample, nbest and mbr; the reference beam search "
                          "takes no prefix")
-    tag = f"_prefix{k}" if k else ""
+    no_repeat = int(os.environ.get("FIRA_NO_REPEAT_NGRAM", 0))
+    min_len = int(os.environ.get("FIRA_MIN_LENGTH", 0))
+    if (no_repeat or min_len) and mode == "beam":
+        raise SystemExit("FIRA_NO_REPEAT_NGRAM and FIRA_MIN_LENGTH apply to FIRA_DECODE=sample, nbest and mbr; the "
+                         "reference beam search takes no rules")
+    rules = dict(no_repeat_ngram=no_repeat, min_length=min_len)
+    tag = (f"_prefix{k}" if k else "") + (f"_norepeat{no_repeat}" if no_repeat else "") + \
+        (f"_minlen{min_len}" if min_len else "")
 
     def pre(b):                         # each commit's own first k reference labels, or no prefix
         return reference_prefix(b, k, vocab['<eos>'], vocab['<pad>']) if k else None
@@ -272,12 +284,14 @@ def decoder(mode, vocab):
                     seed=int(os.environ.get("FIRA_SEED", 0)))
     if mode == "sample":                # every sample, `<log-prob>\t<message>`
         def decode(model, b, first_index):
-            out = sample(model, b[0], b[3], b[4], b[5], b[7], first_index=first_index, prefix=pre(b), **opts, **ids)
+            out = sample(model, b[0], b[3], b[4], b[5], b[7], first_index=first_index, prefix=pre(b), **rules, **opts,
+                         **ids)
             return out.seq, out.length, (out.logprob,)
         return "output_fira_samples" + tag, decode, n
     if mode == "mbr":                   # the sample of highest expected BLEU, `<expected BLEU>\t<log-prob>\t<message>`
         def decode(model, b, first_index):
-            out = mbr(model, b[0], b[3], b[4], b[5], b[7], first_index=first_index, prefix=pre(b), **opts, **ids)
+            out = mbr(model, b[0], b[3], b[4], b[5], b[7], first_index=first_index, prefix=pre(b), **rules, **opts,
+                      **ids)
             expected = out.utility.gather(1, out.index.unsqueeze(1))
             return out.seq.unsqueeze(1), out.length.unsqueeze(1), (expected, out.logprob.unsqueeze(1))
         return "output_fira_mbr" + tag, decode, 1
@@ -288,7 +302,7 @@ def decoder(mode, vocab):
 
         def decode(model, b, first_index):
             out = nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=args.beam_size, length_penalty=alpha, **diverse,
-                        prefix=pre(b), **ids)
+                        prefix=pre(b), **rules, **ids)
             return out.seq, out.length, (out.score, out.logprob)
         return "output_fira_nbest" + tag, decode, 1
     raise SystemExit("FIRA_DECODE must be 'beam', 'sample', 'nbest' or 'mbr'")

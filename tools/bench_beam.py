@@ -16,6 +16,12 @@ reference's own loop was timed on in BASELINE.md (72 s for 32 commits on CPU).  
                                (k > 0: sample, nbest, diverse and mbr are also timed with each commit's first k
                                reference labels (tar_label, never <eos>) as a prefix, next to the same mode without
                                one; those lines carry prefix_words = k)
+                               [--no-repeat-ngram n] [--min-length m]
+                               (either > 0: sample, nbest, diverse and mbr are also timed with n-gram repeat blocking
+                               and the minimum length, next to the same mode without them; every line of those modes
+                               carries repeat_share, the share of returned hypotheses (mbr: the chosen ones) in which
+                               a word repeats an n-gram, n = repeat_share_n = n or 2, and mean_length (tokens with
+                               <start> and <eos>); the lines with the rules carry no_repeat_ngram and min_length)
 
 nbest and diverse lines also carry `self_bleu`: the mean pairwise id-level sentence BLEU among each commit's K
 hypotheses (one fira_mbr_select launch with pair_bleu, off-diagonal entries averaged over the batch); lower means a
@@ -47,7 +53,10 @@ def main():
     ap.add_argument("--modes", default="full,graph")
     ap.add_argument("--diversity", type=float, default=0.5, help="diverse mode's penalty per repeated word")
     ap.add_argument("--prefix-words", type=int, default=0, help="also time the decoders with k-label reference prefixes")
+    ap.add_argument("--no-repeat-ngram", type=int, default=0, help="also time the decoders with n-gram repeat blocking")
+    ap.add_argument("--min-length", type=int, default=0, help="also time the decoders with a minimum message length")
     a = ap.parse_args()
+    rules = (a.no_repeat_ngram, a.min_length)
     import torch
     import __graft_entry__
     __graft_entry__.build()
@@ -67,10 +76,14 @@ def main():
         b = bench.device_batch(hb, dev, B)
         lab = b[6][:, 1:1 + a.prefix_words]                         # the reference prefixes: never <eos> (id 2)
         ref_prefix = lab.masked_fill((lab == 2).long().cumsum(1) > 0, 0)
-        cases = [(int(x), m, pw) for x in a.beams.split(",") for m in a.modes.split(",")
-                 for pw in ((0, a.prefix_words) if a.prefix_words and m not in ("full", "graph") else (0,))]
-        for K, mode, pw in cases:
+        decoders = ("sample", "nbest", "diverse", "mbr")
+        cases = [(int(x), m, pw, rl) for x in a.beams.split(",") for m in a.modes.split(",")
+                 for pw in ((0, a.prefix_words) if a.prefix_words and m in decoders else (0,))
+                 for rl in (((0, 0), rules) if any(rules) and m in decoders else ((0, 0),))]
+        for K, mode, pw, rl in cases:
             pre = dict(prefix=ref_prefix) if pw else {}
+            if any(rl):
+                pre.update(no_repeat_ngram=rl[0], min_length=rl[1])
 
             def run():
                 if mode == "sample":                                 # N = the beam width, default T / k / p
@@ -105,6 +118,14 @@ def main():
             extra = {"prefix_words": pw} if a.prefix_words else {}
             if a.prefix_words:
                 extra.update(card=torch.cuda.get_device_name(dev), power_limit_w=power_limit())
+            if any(rules) and mode in decoders:
+                seq, ln = (out.seq.unsqueeze(1), out.length.unsqueeze(1)) if mode == "mbr" else (out.seq, out.length)
+                count_n = a.no_repeat_ngram or 2
+                extra.update(card=torch.cuda.get_device_name(dev), power_limit_w=power_limit(),
+                             repeat_share=repeat_share(seq, ln, count_n), repeat_share_n=count_n,
+                             mean_length=ln.double().mean().item())
+                if any(rl):
+                    extra.update(no_repeat_ngram=rl[0], min_length=rl[1])
             if mode in ("nbest", "diverse"):
                 extra.update(self_bleu=self_bleu(out, B, K), card=torch.cuda.get_device_name(dev),
                              power_limit_w=power_limit())
@@ -141,6 +162,19 @@ def self_bleu(h, B, K):
          ops._ptr(best), B, K, T, ops._stream())
     off = ~torch.eye(K, dtype=torch.bool, device=seq.device)
     return pair[:, off].mean().item()
+
+
+def repeat_share(seq, length, n):
+    """the share of hypotheses seq [B, K, T] (length [B, K], <start> counted) in which some word after <start>
+    completes an n-gram that already occurred in it (counted on the host)"""
+    seq, length = seq.cpu().tolist(), length.cpu().tolist()
+    hits = total = 0
+    for rows, lens in zip(seq, length):
+        for s, ln in zip(rows, lens):
+            grams = [tuple(s[t - n + 1:t + 1]) for t in range(n, ln)]
+            hits += len(set(grams)) < len(grams)
+            total += 1
+    return hits / max(1, total)
 
 
 def power_limit():
