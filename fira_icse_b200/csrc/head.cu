@@ -195,14 +195,61 @@ __device__ __forceinline__ ArgMax am_better(ArgMax a, ArgMax b) {   // larger va
   return (b.v > a.v || (b.v == a.v && b.i < a.i)) ? b : a;
 }
 
+// Vocabulary-label rows of a training batch (label in (0, V)) in row order: vslot[row] = the row's compact slot or -1,
+// vrows[slot] = its row, -1 in the slots [count, cap).  One CTA; each thread takes a contiguous run of rows.
+constexpr int kRowsThreads = 1024;
+__global__ void __launch_bounds__(kRowsThreads) vocab_rows_kernel(const int* __restrict__ label, long rows, int V,
+                                                                  int* __restrict__ vslot, int* __restrict__ vrows,
+                                                                  int cap) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  __shared__ int warp_sum_s[kRowsThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long per = (rows + kRowsThreads - 1) / kRowsThreads;
+  const long r0 = min(rows, (long)threadIdx.x * per), r1 = min(rows, r0 + per);
+  int n = 0;
+  for (long r = r0; r < r1; ++r) n += (label[r] != 0 && label[r] < V);
+  int incl = n;                                   // inclusive scan over the warp, then over the warps
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
+  if (lane == 31) warp_sum_s[warp] = incl;
+  for (int s = threadIdx.x; s < cap; s += kRowsThreads) vrows[s] = -1;
+  __syncthreads();
+  int slot = incl - n;
+  for (int w = 0; w < warp; ++w) slot += warp_sum_s[w];
+  for (long r = r0; r < r1; ++r) {
+    // count <= cap is the caller's bound; rows past it get no slot, and head_fwd_kernel gives them a NaN loss
+    const bool v = label[r] != 0 && label[r] < V && slot < cap;
+    vslot[r] = v ? slot : -1;
+    if (v) vrows[slot++] = (int)r;
+  }
+}
+
+// dst[i] = idx[i] >= 0 ? src[idx[i]] : 0 over rows of `width` elements (width % 8 == 0); one warp per row
+template <typename T>
+__global__ void __launch_bounds__(256) gather_rows_kernel(const T* __restrict__ src, long ld_src,
+                                                          const int* __restrict__ idx, T* __restrict__ dst, long ld_dst,
+                                                          long n, int width) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  const int lane = threadIdx.x & 31;
+  for (long i = (long)blockIdx.x * 8 + (threadIdx.x >> 5); i < n; i += (long)gridDim.x * 8) {
+    const int r = idx[i];
+    for (int c = lane * 8; c < width; c += 256) {
+      float x[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+      if (r >= 0) Act<T>::load8(src + (long)r * ld_src + c, x);
+      Act<T>::store8(dst + i * ld_dst + c, x);
+    }
+  }
+}
+
 // stats row layout (8 floats): vmax, vsum, cmax, csum, g0, g1, p_label, unused
+// vslot (may be NULL): the logits of row r are row vslot[r] of `logits` (vocabulary-label rows only, training)
 template <typename T>
 __global__ void __launch_bounds__(256) head_fwd_kernel(const T* __restrict__ logits, long ldl,
                                                        const float* __restrict__ sc, const float* __restrict__ gate_logit,
                                                        const unsigned char* __restrict__ mem_mask,
-                                                       const int* __restrict__ label, float* __restrict__ stats,
-                                                       float* __restrict__ nll, int* __restrict__ argmax_out, int Tn,
-                                                       int V, int S) {
+                                                       const int* __restrict__ label, const int* __restrict__ vslot,
+                                                       float* __restrict__ stats, float* __restrict__ nll,
+                                                       int* __restrict__ argmax_out, int Tn, int V, int S) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
   __shared__ MaxSum sh_ms[8];
   __shared__ ArgMax sh_am[8];
@@ -210,7 +257,8 @@ __global__ void __launch_bounds__(256) head_fwd_kernel(const T* __restrict__ log
   const long row = blockIdx.x;
   const int b = (int)(row / Tn);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const T* lrow = logits + row * ldl;
+  const long lslot = vslot ? (long)vslot[row] : row;       // -1: the row has no logits
+  const T* lrow = logits + lslot * ldl;
   const float* srow = sc + row * S;
   const unsigned char* mrow = mem_mask + (long)b * S;
 
@@ -218,7 +266,7 @@ __global__ void __launch_bounds__(256) head_fwd_kernel(const T* __restrict__ log
   // Training (no argmax wanted): a row's loss only needs the softmax its label lives in, so rows whose label is
   // padding or a copy label skip the 24,650-wide pass (and copy-label rows are the only ones that need `sc`).
   const int lab_row = label[row];
-  const bool need_vocab = argmax_out != nullptr || (lab_row != 0 && lab_row < V);
+  const bool need_vocab = argmax_out != nullptr || (lab_row != 0 && lab_row < V && lslot >= 0);
   MaxSum v{-INFINITY, 0.f};
   if (need_vocab) {
     // 8 logits per 16-byte (bf16) / 32-byte (fp32) load; the running (max, sum) is rescaled once per group instead of
@@ -257,8 +305,10 @@ __global__ void __launch_bounds__(256) head_fwd_kernel(const T* __restrict__ log
   if (threadIdx.x == 0) {
     const int lab = label[row];
     float p = 1.f;
+    // a vocabulary-label row left without a slot (a caller's cap below the row count) reports NaN, not a plausible loss
+    const bool no_slot = lab != 0 && lab < V && lslot < 0;
     if (lab != 0) {
-      if (lab < V) p = g0 * (expf(Act<T>::ld(lrow + lab) - vmax) / vsum);
+      if (lab < V) p = no_slot ? NAN : g0 * (expf(Act<T>::ld(lrow + lab) - vmax) / vsum);
       else {
         // a copy label beyond the (possibly loader-trimmed) source is never read out of bounds: it gets p = 0 -> the
         // clamp floor, no gradient -- what the reference computes for a label on a padded (masked) source position
@@ -270,7 +320,7 @@ __global__ void __launch_bounds__(256) head_fwd_kernel(const T* __restrict__ log
     float* st = stats + row * 8;
     st[0] = vmax; st[1] = vsum; st[2] = cmax; st[3] = csum; st[4] = g0; st[5] = g1; st[6] = p; st[7] = 0.f;
     // loss = -log(clamp(p, 1e-10, 1)), zeroed where label == 0 (Model.py:69,81-82)
-    nll[row] = lab != 0 ? -logf(fminf(fmaxf(p, 1e-10f), 1.f)) : 0.f;
+    nll[row] = no_slot ? NAN : (lab != 0 ? -logf(fminf(fmaxf(p, 1e-10f), 1.f)) : 0.f);
   }
   if (argmax_out) {
     // argmax over log(clamp(p)) of the concatenation, first index wins ties (Model.py:86)
@@ -301,11 +351,15 @@ __global__ void __launch_bounds__(256) head_fwd_kernel(const T* __restrict__ log
 // d(loss_sum)/d(logits, copy scores, gate logits); `upstream` is d(loss_sum) (a device scalar).
 // Exactly one of the two softmaxes receives gradient per row (the picked element decides), rows with
 // label == 0 or p outside [1e-10, 1] (clamp) receive none.
+// vslot / vrows (may be NULL, then logits / d_logits have one row per row): logits and d_logits hold the slots of the
+// vocabulary-label rows; d_logits is written for those slots only, and CTA s < cap also zeroes slot s if it is unused.
 template <typename T>
 __global__ void __launch_bounds__(256) head_bwd_kernel(const T* __restrict__ logits, long ldl,
                                                        const float* __restrict__ sc,
                                                        const unsigned char* __restrict__ mem_mask,
-                                                       const int* __restrict__ label, const float* __restrict__ stats,
+                                                       const int* __restrict__ label, const int* __restrict__ vslot,
+                                                       const int* __restrict__ vrows, int cap,
+                                                       const float* __restrict__ stats,
                                                        const float* __restrict__ upstream, T* __restrict__ d_logits,
                                                        float* __restrict__ d_sc, float* __restrict__ d_gate_logit,
                                                        unsigned char* __restrict__ row_active, int Tn, int V, int S) {
@@ -317,11 +371,18 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(const T* __restrict__ log
   const int lab = label[row];
   const float up = *upstream;
   const bool live = lab != 0 && p >= 1e-10f && p <= 1.f;
-  const bool vocab = live && lab < V;
+  const long lslot = vslot ? (long)vslot[row] : row;      // -1: the row has no logits
+  const bool vocab = live && lab < V && lslot >= 0;
   const bool copy = live && lab >= V;
-  T* drow = d_logits + row * ldl;
-  const T* lrow = logits + row * ldl;
+  T* drow = d_logits + lslot * ldl;
+  const T* lrow = logits + lslot * ldl;
   const int V8 = V >> 3;                         // 8 logits per vector load / store, scalar tail
+  const float z[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  if (vslot && row < cap && vrows[row] < 0) {    // an unused slot: the products over the slots read it
+    T* prow = d_logits + row * ldl;
+    for (int g = threadIdx.x; g < V8; g += blockDim.x) Act<T>::store8(prow + (long)g * 8, z);
+    for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) Act<T>::st(prow + j, 0.f);
+  }
   if (vocab) {
     const float iv = 1.f / vsum;
     for (int g = threadIdx.x; g < V8; g += blockDim.x) {
@@ -335,8 +396,7 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(const T* __restrict__ log
       float pv = expf(Act<T>::ld(lrow + j) - vmax) * iv;
       Act<T>::st(drow + j, up * (pv - (j == lab ? 1.f : 0.f)));
     }
-  } else {
-    const float z[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  } else if (lslot >= 0) {
     for (int g = threadIdx.x; g < V8; g += blockDim.x) Act<T>::store8(drow + (long)g * 8, z);
     for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) Act<T>::st(drow + j, 0.f);
   }
@@ -1077,16 +1137,64 @@ int fira_copy_scores_packed_bwd(const void* src_proj, const void* tgt_proj, cons
                               d_b_res, B, T_len, S, dim, dtype, stream);
 }
 
-int fira_pointer_mix_nll_fwd(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
-                             const unsigned char* mem_mask, const int* label, float* stats, float* nll,
-                             int* argmax_out, long rows, int T_len, int V, int S, int dtype, void* stream) {
+int fira_vocab_rows(const int* label, long rows, int V, int* vslot, int* vrows, int cap, void* stream) {
+  FIRA_CHECK_ARG(label && vslot && vrows && rows >= 0 && V > 0 && cap >= 0, FIRA_ERR_ARG, "vocab_rows: arguments");
+  launch_k(vocab_rows_kernel, dim3(1), dim3(kRowsThreads), 0, (cudaStream_t)stream, label, rows, V, vslot, vrows, cap);
+  FIRA_CHECK_LAUNCH("fira_vocab_rows");
+  return FIRA_OK;
+}
+
+int fira_gather_rows(const void* src, long ld_src, const int* idx, void* dst, long ld_dst, long n, int width, int dtype,
+                     void* stream) {
+  FIRA_CHECK_ARG(idx && n >= 0 && width > 0 && width % 8 == 0 && ld_src >= width && ld_dst >= width, FIRA_ERR_ARG,
+                 "gather_rows: arguments");
+  FIRA_CHECK_ARG(fira_aligned16(src) && fira_aligned16(dst) && ld_src % 8 == 0 && ld_dst % 8 == 0, FIRA_ERR_ALIGN,
+                 "gather_rows: 16-B alignment");
+  if (n == 0) return FIRA_OK;
+  const long g = (n + 7) / 8, gmax = (long)fira_num_sms() * 16;
+  DISPATCH_T(dtype, launch_k(gather_rows_kernel<T>, dim3((unsigned)(g < gmax ? g : gmax)), dim3(256), 0,
+      (cudaStream_t)stream, (const T*)src, ld_src, idx, (T*)dst, ld_dst, n, width);)
+  FIRA_CHECK_LAUNCH("fira_gather_rows");
+  return FIRA_OK;
+}
+
+int fira_pointer_mix_nll_fwd_rows(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                                  const unsigned char* mem_mask, const int* label, const int* vslot, float* stats,
+                                  float* nll, int* argmax_out, long rows, int T_len, int V, int S, int dtype,
+                                  void* stream) {
   FIRA_CHECK_ARG(rows >= 0 && T_len > 0 && V > 0 && S > 0, FIRA_ERR_SHAPE, "pointer_mix_nll_fwd: shape");
   FIRA_CHECK_ARG(fira_aligned16(logits) && ld_logits % 8 == 0, FIRA_ERR_ALIGN,
                  "pointer_mix_nll_fwd: logits must be 16-byte aligned with a leading dimension that is a multiple of 8");
+  FIRA_CHECK_ARG(!(vslot && argmax_out), FIRA_ERR_ARG, "pointer_mix_nll_fwd: the argmax needs the logits of every row");
   if (rows == 0) return FIRA_OK;
-  DISPATCH_T(dtype, launch_k(head_fwd_kernel<T>, dim3((unsigned)rows), dim3(256), 0, (cudaStream_t)stream, 
-      (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, label, stats, nll, argmax_out, T_len, V, S);)
+  DISPATCH_T(dtype, launch_k(head_fwd_kernel<T>, dim3((unsigned)rows), dim3(256), 0, (cudaStream_t)stream,
+      (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, label, vslot, stats, nll, argmax_out, T_len, V,
+      S);)
   FIRA_CHECK_LAUNCH("fira_pointer_mix_nll_fwd");
+  return FIRA_OK;
+}
+
+int fira_pointer_mix_nll_fwd(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                             const unsigned char* mem_mask, const int* label, float* stats, float* nll,
+                             int* argmax_out, long rows, int T_len, int V, int S, int dtype, void* stream) {
+  return fira_pointer_mix_nll_fwd_rows(logits, ld_logits, copy_scores, gate_logits, mem_mask, label, nullptr, stats, nll,
+                                       argmax_out, rows, T_len, V, S, dtype, stream);
+}
+
+int fira_pointer_mix_nll_bwd_rows(const void* logits, long ld_logits, const float* copy_scores,
+                                  const unsigned char* mem_mask, const int* label, const int* vslot, const int* vrows,
+                                  int cap, const float* stats, const float* upstream, void* d_logits,
+                                  float* d_copy_scores, float* d_gate_logits, unsigned char* row_active, long rows,
+                                  int T_len, int V, int S, int dtype, void* stream) {
+  FIRA_CHECK_ARG(rows >= 0 && T_len > 0 && V > 0 && S > 0, FIRA_ERR_SHAPE, "pointer_mix_nll_bwd: shape");
+  FIRA_CHECK_ARG(fira_aligned16(logits) && fira_aligned16(d_logits) && ld_logits % 8 == 0, FIRA_ERR_ALIGN,
+                 "pointer_mix_nll_bwd: logits / d_logits must be 16-byte aligned with a leading dimension that is a multiple of 8");
+  FIRA_CHECK_ARG(!vslot || (vrows && cap >= 0 && cap <= rows), FIRA_ERR_ARG, "pointer_mix_nll_bwd: vrows / cap");
+  if (rows == 0) return FIRA_OK;
+  DISPATCH_T(dtype, launch_k(head_bwd_kernel<T>, dim3((unsigned)rows), dim3(256), 0, (cudaStream_t)stream,
+      (const T*)logits, ld_logits, copy_scores, mem_mask, label, vslot, vrows, cap, stats, upstream, (T*)d_logits,
+      d_copy_scores, d_gate_logits, row_active, T_len, V, S);)
+  FIRA_CHECK_LAUNCH("fira_pointer_mix_nll_bwd");
   return FIRA_OK;
 }
 
@@ -1094,15 +1202,9 @@ int fira_pointer_mix_nll_bwd(const void* logits, long ld_logits, const float* co
                              const unsigned char* mem_mask, const int* label, const float* stats,
                              const float* upstream, void* d_logits, float* d_copy_scores, float* d_gate_logits,
                              unsigned char* row_active, long rows, int T_len, int V, int S, int dtype, void* stream) {
-  FIRA_CHECK_ARG(rows >= 0 && T_len > 0 && V > 0 && S > 0, FIRA_ERR_SHAPE, "pointer_mix_nll_bwd: shape");
-  FIRA_CHECK_ARG(fira_aligned16(logits) && fira_aligned16(d_logits) && ld_logits % 8 == 0, FIRA_ERR_ALIGN,
-                 "pointer_mix_nll_bwd: logits / d_logits must be 16-byte aligned with a leading dimension that is a multiple of 8");
-  if (rows == 0) return FIRA_OK;
-  DISPATCH_T(dtype, launch_k(head_bwd_kernel<T>, dim3((unsigned)rows), dim3(256), 0, (cudaStream_t)stream, 
-      (const T*)logits, ld_logits, copy_scores, mem_mask, label, stats, upstream, (T*)d_logits, d_copy_scores,
-      d_gate_logits, row_active, T_len, V, S);)
-  FIRA_CHECK_LAUNCH("fira_pointer_mix_nll_bwd");
-  return FIRA_OK;
+  return fira_pointer_mix_nll_bwd_rows(logits, ld_logits, copy_scores, mem_mask, label, nullptr, nullptr, 0, stats,
+                                       upstream, d_logits, d_copy_scores, d_gate_logits, row_active, rows, T_len, V, S,
+                                       dtype, stream);
 }
 
 static int sample_impl(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,

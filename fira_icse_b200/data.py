@@ -379,7 +379,8 @@ class PackedBatchLoader:
         self.pin = torch.cuda.is_available() if pin is None else pin
         self.n_slots = max(2, int(prefetch) + 1)
         # packed=True: per-commit packed batches (packed.PackedBatch, SURVEY.md 8f rank 4) instead of batch-trimmed padded
-        # ones; row_buckets = rounding of (code rows, sub-token rows, AST rows, memory rows of one commit)
+        # ones; row_buckets = rounding of (code rows, sub-token rows, AST rows, memory rows of one commit); the
+        # vocabulary-label target rows round to packed.VOCAB_ROW_BUCKET, and max_shapes bounds the shapes with them
         self.packed = bool(packed)
         if self.packed:
             from . import packed as P
@@ -415,8 +416,7 @@ class PackedBatchLoader:
         index = np.ascontiguousarray(index, dtype=np.int64)
         if self.packed:
             from . import packed as P
-            need = self.tables.dims(index)
-            want = tuple(P._round_up(need[i], self.row_buckets[i]) for i in range(4))
+            want = P.packed_needs(self.tables, index, self.V, self.row_buckets)
             return P.gather_packed(self.tables, index, self.V, slot, pad_dims=self._choose_dims(want))
         b = len(index)
         n0, n1, n2 = self.lens

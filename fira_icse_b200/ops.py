@@ -846,8 +846,20 @@ class HeadFn(torch.autograd.Function):
         dec2 = dec.contiguous().to(pr.tdt).view(Mt, D)
         dec32 = dec2 if not pr.bf16 else dec2.float()            # the 2-wide gate stays on the fp32 path
         ldl = _ld_logits(V)
-        logits = pr.empty((Mt, ldl), dev)
-        pr.linear(dec2, Wout, bout, out=logits, ld_out=ldl)
+        if want_argmax:
+            cap, vslot, vrows, dec_v = Mt, None, None, dec2
+        else:
+            # training: out_fc runs on the vocabulary-label rows alone, compacted into `cap` slots (a packed batch
+            # bounds them by pk.Rv); no other row reads the vocabulary softmax.  A padded batch has no such bound:
+            # cap = B*T, and it pays the row list and the two row copies for no gain, to keep one code path
+            cap = Mt if pk is None else pk.Rv
+            vslot = torch.empty((Mt,), dtype=torch.int32, device=dev)
+            vrows = torch.empty((cap,), dtype=torch.int32, device=dev)
+            call("fira_vocab_rows", _ptr(label), Mt, V, _ptr(vslot), _ptr(vrows), cap, st)
+            dec_v = pr.empty((cap, D), dev)
+            call("fira_gather_rows", _ptr(dec2), D, _ptr(vrows), _ptr(dec_v), D, cap, D, pr.code, st)
+        logits = pr.empty((cap, ldl), dev)
+        pr.linear(dec_v, Wout, bout, out=logits, ld_out=ldl)
         # training only needs pointer scores of real source positions at target rows whose label is a COPY
         # label (vocabulary-label rows take their loss from the vocabulary softmax alone, Model.py:64-81)
         row_mask = None if want_argmax else (label >= V).to(torch.uint8)
@@ -857,10 +869,10 @@ class HeadFn(torch.autograd.Function):
         stats = torch.empty((Mt, 8), **f32)
         nll = torch.empty((Mt,), **f32)
         amax = torch.empty((Mt,), dtype=torch.int32, device=dev) if want_argmax else None
-        call("fira_pointer_mix_nll_fwd", _ptr(logits), ldl, _ptr(sc), _ptr(gl), _ptr(mem_mask), _ptr(label),
-             _ptr(stats), _ptr(nll), _ptr(amax), Mt, T, V, S, pr.code, st)
+        call("fira_pointer_mix_nll_fwd_rows", _ptr(logits), ldl, _ptr(sc), _ptr(gl), _ptr(mem_mask), _ptr(label),
+             _ptr(vslot), _ptr(stats), _ptr(nll), _ptr(amax), Mt, T, V, S, pr.code, st)
         ctx.misc = (pr, memory2, dec2, dec32, mem_mask, label, logits, ldl, src, tgt, sc, stats, B, T, S, V,
-                    memory.dtype, dec.dtype, pk, memory.shape)
+                    memory.dtype, dec.dtype, pk, memory.shape, cap, vslot, vrows, dec_v)
         ctx.save_for_backward(Wout, Ws, Wt, Wres, Wp, bout, bres, bp)
         loss_sum = colsum(nll, 1, Mt, 1).view(())
         ids = amax.view(B, T) if want_argmax else None
@@ -871,19 +883,20 @@ class HeadFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_loss, g_nll, g_ids):
         (pr, memory2, dec2, dec32, mem_mask, label, logits, ldl, src, tgt, sc, stats, B, T, S, V,
-         mem_dt, dec_dt, pk, mem_shape) = ctx.misc
+         mem_dt, dec_dt, pk, mem_shape, cap, vslot, vrows, dec_v) = ctx.misc
         Wout, Ws, Wt, Wres, Wp, bout, bres, bp = ctx.saved_tensors
         Mt, Ms = B * T, memory2.shape[0]
         dev = dec2.device
         f32 = dict(dtype=torch.float32, device=dev)
         st = _stream()
         up = g_loss.contiguous().float()
-        dlogits = pr.empty((Mt, ldl), dev)
+        dlogits = pr.empty((cap, ldl), dev)
         dsc = torch.empty((B, T, S), **f32)
         dgl = torch.empty((Mt, 2), **f32)
         active = torch.empty((Mt,), dtype=torch.uint8, device=dev)
-        call("fira_pointer_mix_nll_bwd", _ptr(logits), ldl, _ptr(sc), _ptr(mem_mask), _ptr(label), _ptr(stats),
-             _ptr(up), _ptr(dlogits), _ptr(dsc), _ptr(dgl), _ptr(active), Mt, T, V, S, pr.code, st)
+        call("fira_pointer_mix_nll_bwd_rows", _ptr(logits), ldl, _ptr(sc), _ptr(mem_mask), _ptr(label), _ptr(vslot),
+             _ptr(vrows), cap, _ptr(stats), _ptr(up), _ptr(dlogits), _ptr(dsc), _ptr(dgl), _ptr(active), Mt, T, V, S,
+             pr.code, st)
         # pointer scores
         d_src = pr.empty((Ms, D), dev)
         d_tgt = torch.zeros((Mt, D), **f32)
@@ -899,9 +912,9 @@ class HeadFn(torch.autograd.Function):
         fork = Fork(dev)
         with fork(d_src, memory2):                           # three independent groups, three side streams
             d_Ws = pr.linear_dw(d_src, D, memory2, D, Ms, D, D, out=_gdest(Ws, (D, D)))
-        with fork(dlogits, dec2):
+        with fork(dlogits, dec_v):
             d_bout = _gdest(bout, (V,), zero=True)
-            d_Wout = pr.linear_dw(dlogits, ldl, dec2, D, Mt, V, D, out=_gdest(Wout, (V, D)), dbias=d_bout)
+            d_Wout = pr.linear_dw(dlogits, ldl, dec_v, D, cap, V, D, out=_gdest(Wout, (V, D)), dbias=d_bout)
         with fork(dgl, dec32, d_tgt):
             d_bp = colsum(dgl, 2, Mt, 2, out=_gdest(bp, (2,), zero=True))
             d_Wp = linear_dw(dgl, 2, dec32, D, Mt, 2, D, out=_gdest(Wp, (2, D)))
@@ -909,11 +922,14 @@ class HeadFn(torch.autograd.Function):
         d_mem = pr.linear_dx(d_src, D, Ws, Ms)
         # vocabulary projection (the big one), gate and target projection; d_dec accumulates in fp32
         if pr.bf16:
-            d_dec = torch.empty((Mt, D), **f32)
-            gemm_tc(dlogits, ldl, 1, pr.w(Wout), D, 0, d_dec, D, Mt, D, V,
-                    splits=_tc_splits(_ceil(Mt, 128), _ceil(V, 64)))
+            d_dec = torch.empty((cap, D), **f32)
+            gemm_tc(dlogits, ldl, 1, pr.w(Wout), D, 0, d_dec, D, cap, D, V,
+                    splits=_tc_splits(_ceil(cap, 128), _ceil(V, 64)))
         else:
-            d_dec = linear_dx(dlogits, ldl, Wout, Mt)
+            d_dec = linear_dx(dlogits, ldl, Wout, cap)
+        if vslot is not None:                      # slots -> rows; rows without a slot get zeros
+            d_dec_v, d_dec = d_dec, torch.empty((Mt, D), **f32)
+            call("fira_gather_rows", _ptr(d_dec_v), D, _ptr(vslot), _ptr(d_dec), D, Mt, D, FIRA_F32, st)
         linear_dx(dgl, 2, Wp, Mt, out=d_dec, accumulate=True)
         linear_dx(d_tgt, D, Wt, Mt, out=d_dec, accumulate=True)
         fork.join()

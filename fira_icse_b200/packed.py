@@ -18,6 +18,7 @@ import torch
 from ._lib import host_call
 
 SEGMENT_BUCKETS = (1024, 512, 512, 64)          # rounding of (code rows, sub rows, AST rows, memory rows per commit)
+VOCAB_ROW_BUCKET = 128                          # rounding of the vocabulary-label target rows: one GEMM row tile
 
 
 class PackedBatch:
@@ -26,17 +27,20 @@ class PackedBatch:
     FIELDS = ("code", "mark", "pos", "sub", "ast", "off", "ranges", "mem_mask", "tar", "label", "tar_mask",
               "rowptr", "col", "val")
 
-    def __init__(self, B, Rc, Rs, Ra, S, T, nnz, chunks=4, **tensors):
+    def __init__(self, B, Rc, Rs, Ra, S, T, nnz, chunks=4, Rv=None, **tensors):
         self.B, self.Rc, self.Rs, self.Ra, self.S, self.T, self.nnz = B, Rc, Rs, Ra, S, T, nnz
         # bound on the 128-key chunks cross-attention needs for any commit of the batch (3 on the whole shipped DataSet:
         # <= 200 code tokens, <= 102 sub-tokens); passed to the packed attention entry points, which do not use it
         self.chunks = int(chunks)
+        # bound on the target rows whose label is a vocabulary word: the rows of the training step's vocabulary
+        # projection (ops.HeadFn); None = every row
+        self.Rv = B * T if Rv is None else int(Rv)
         for k in self.FIELDS:
             setattr(self, k, tensors[k])
 
     @property
     def shape_key(self):
-        return (self.B, self.Rc, self.Rs, self.Ra, self.S, self.chunks)
+        return (self.B, self.Rc, self.Rs, self.Ra, self.S, self.chunks, self.Rv)
 
     @property
     def rows(self):
@@ -48,7 +52,7 @@ class PackedBatch:
 
     def to(self, device, non_blocking=True):
         t = {k: getattr(self, k).to(device, non_blocking=non_blocking) for k in self.FIELDS}
-        return PackedBatch(self.B, self.Rc, self.Rs, self.Ra, self.S, self.T, self.nnz, self.chunks, **t)
+        return PackedBatch(self.B, self.Rc, self.Rs, self.Ra, self.S, self.T, self.nnz, self.chunks, self.Rv, **t)
 
     def h2d_bytes(self):
         return sum(getattr(self, k).numel() * getattr(self, k).element_size() for k in self.FIELDS)
@@ -84,6 +88,12 @@ class PackedTables:
                   self.deg.ctypes.data, index.ctypes.data, len(index), *self.lens, out.ctypes.data)
         return tuple(int(x) for x in out)
 
+    def vocab_rows(self, index, vocab_size):
+        """-> target rows of `index` whose shifted label is a vocabulary word (0 < label < V; fira_host_gather_packed
+        renumbers copy labels only, so the count is the same before and after the gather)"""
+        lab = self.tab["tar_label"][np.asarray(index, dtype=np.int64), 1:]
+        return int(np.count_nonzero((lab > 0) & (lab < vocab_size)))
+
 
 class PackedSlot:
     """Staging buffers (pinned when CUDA is present) sized for the largest packed batch of `B` commits."""
@@ -112,15 +122,20 @@ class PackedSlot:
 
 def gather_packed(tables, index, vocab_size, slot, pad_dims=None, buckets=SEGMENT_BUCKETS):
     """One packed batch of commits `index` written into `slot` (views of the slot are returned as a PackedBatch).
-    pad_dims: (Rc, Rs, Ra, S) to use (>= the batch's needs); default = the needs rounded up to `buckets`."""
+    pad_dims: (Rc, Rs, Ra, S[, Rv]) to use (>= the batch's needs, packed_needs); default = the needs rounded up to
+    `buckets`.  Rv is capped at the batch's target rows."""
     index = np.ascontiguousarray(index, dtype=np.int64)
     b = len(index)
     need = tables.dims(index)
     if pad_dims is None:
-        pad_dims = tuple(_round_up(need[i], buckets[i]) for i in range(4))
-    Rc, Rs, Ra, S = (int(x) for x in pad_dims)
+        pad_dims = packed_needs(tables, index, vocab_size, buckets)
+    elif len(pad_dims) == 4:
+        pad_dims = tuple(pad_dims) + packed_needs(tables, index, vocab_size, buckets)[4:]
+    Rc, Rs, Ra, S, Rv = (int(x) for x in pad_dims)
     if Rc > slot.cap[0] or Rs > slot.cap[1] or Ra > slot.cap[2] or S > slot.cap[3]:
         raise ValueError(f"packed batch {pad_dims} exceeds the staging capacity {slot.cap}")
+    if Rv < tables.vocab_rows(index, vocab_size):
+        raise ValueError(f"packed batch: Rv = {Rv} is below its vocabulary-label rows")
     t = tables.tab
     pd = np.asarray((Rc, Rs, Ra, S), np.int32)
     nnz = np.zeros(1, np.int32)
@@ -134,13 +149,21 @@ def gather_packed(tables, index, vocab_size, slot, pad_dims=None, buckets=SEGMEN
               slot.val.data_ptr(), slot.edge_cap, nnz.ctypes.data)
     e, T = int(nnz[0]), tables.msg_len
     slot.batch = PackedBatch(
-        b, Rc, Rs, Ra, S, T, e, max(3, need[5]),
+        b, Rc, Rs, Ra, S, T, e, max(3, need[5]), min(Rv, b * T),
         code=slot.code[:Rc], mark=slot.mark[:Rc], pos=slot.pos[:Rc], sub=slot.sub[:Rs], ast=slot.ast[:Ra],
         off=slot.off[:3 * (b + 1)].view(3, b + 1), ranges=slot.ranges[:4 * b].view(b, 4),
         mem_mask=slot.mem_mask[:b * S].view(b, S), tar=slot.tar[:b * T].view(b, T), label=slot.label[:b * T].view(b, T),
         tar_mask=slot.tar_mask[:b * T].view(b, T), rowptr=slot.rowptr[:Rc + Rs + Ra + 1], col=slot.col[:e],
         val=slot.val[:e])
     return slot.batch
+
+
+def packed_needs(tables, index, vocab_size, buckets=SEGMENT_BUCKETS):
+    """-> (Rc, Rs, Ra, S, Rv) of commits `index`: the rows each segment needs rounded up to `buckets`, and the
+    vocabulary-label target rows rounded up to VOCAB_ROW_BUCKET"""
+    need = tables.dims(index)
+    return tuple(_round_up(need[i], buckets[i]) for i in range(4)) + \
+        (_round_up(tables.vocab_rows(index, vocab_size), VOCAB_ROW_BUCKET),)
 
 
 def pack_from_dataset(dataset, index, vocab_size, pin=False, pad_dims=None, buckets=SEGMENT_BUCKETS):

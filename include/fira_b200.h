@@ -268,6 +268,31 @@ int fira_pointer_mix_nll_bwd(const void* logits, long ld_logits, const float* co
                              const float* upstream, void* d_logits, float* d_copy_scores, float* d_gate_logits,
                              unsigned char* row_active, long rows, int T_len, int V, int S, int dtype, void* stream);
 
+/* ---- training on the vocabulary-label rows only (a row whose label is 0 or a copy label takes nothing from the
+ *      vocabulary softmax, Model.py:64-81, so its logits are never needed):
+ *   fira_vocab_rows: label [rows] -> vslot [rows] = compact slot of each row with 0 < label < V in row order, else -1;
+ *                    vrows [cap] = the row of each slot, -1 in the slots past the count (count <= cap: the caller's
+ *                    bound; rows beyond it get no slot, and the _rows loss gives such a row a NaN loss).
+ *   fira_gather_rows: dst[i] = idx[i] >= 0 ? src[idx[i]] : 0 for i < n (rows of `width` elements, width, ld_src, ld_dst
+ *                    multiples of 8, 16-byte aligned): gathers dec rows by vrows, and scatters the slots' input gradient
+ *                    back to the rows by vslot.
+ *   _rows twins of the loss kernels: logits / d_logits hold one row per slot (vslot NULL: one per row, as the entry points
+ *                    above, which call these).  The forward cannot take argmax_out with vslot.  The backward writes the
+ *                    slots of vocabulary-label rows and zero-fills the unused slots s < cap (cap <= rows); rows without
+ *                    a slot write no logits gradient. */
+int fira_vocab_rows(const int* label, long rows, int V, int* vslot, int* vrows, int cap, void* stream);
+int fira_gather_rows(const void* src, long ld_src, const int* idx, void* dst, long ld_dst, long n, int width, int dtype,
+                     void* stream);
+int fira_pointer_mix_nll_fwd_rows(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                                  const unsigned char* mem_mask, const int* label, const int* vslot, float* stats,
+                                  float* nll, int* argmax_out, long rows, int T_len, int V, int S, int dtype,
+                                  void* stream);
+int fira_pointer_mix_nll_bwd_rows(const void* logits, long ld_logits, const float* copy_scores,
+                                  const unsigned char* mem_mask, const int* label, const int* vslot, const int* vrows,
+                                  int cap, const float* stats, const float* upstream, void* d_logits,
+                                  float* d_copy_scores, float* d_gate_logits, unsigned char* row_active, long rows,
+                                  int T_len, int V, int S, int dtype, void* stream);
+
 /* ---- one seeded sampling step from the same mixture (fira_icse_b200/sample.py).  Rows are (commit b, sample n),
  *      B*N of them: logits [B*N, ld_logits], copy_scores [B, N, S], gate_logits [B*N, 2], mem_mask / copy_src [B, S]
  *      (copy_src: the vocabulary id behind each memory position).  Candidates: vocabulary entries and unmasked copy
