@@ -187,13 +187,9 @@ def _head_nll(m, batch):
                             m.out_fc.weight, m.out_fc.bias, *m.copy_net.flat_params())
 
 
-def _cos(a, b):
-    a, b = a.double().flatten(), b.double().flatten()
-    return float((a @ b) / (a.norm() * b.norm() + 1e-30))
-
-
 def test_bf16_mode_tracks_fp32_mode(model, gold):
-    """bf16 activations + tensor-core GEMMs: loss within 2e-2 of the reference, gradients aligned."""
+    """bf16 activations + tensor-core GEMMs: loss within 2e-2 of the reference, argmax ids and per-position NLL within a
+    near-tie of the fp32 mode (the gradients are checked element by element in tests/test_gpu_bf16_step.py)."""
     import copy
     m = copy.deepcopy(model).set_precision("bf16")
     n = int(gold["grad_commits"])
@@ -204,23 +200,6 @@ def test_bf16_mode_tracks_fp32_mode(model, gold):
     loss.backward()
     ref = float(gold["grad_loss"])
     assert abs(loss.item() - ref) <= 2e-2 * ref, (loss.item(), ref)
-    model.zero_grad(set_to_none=True)
-    l32, t32 = model(*batch, "train")
-    (l32 / t32).backward()
-    p32, p16 = dict(model.named_parameters()), dict(m.named_parameters())
-    worst = 1.0
-    for k, p in p32.items():
-        if p.grad is None:
-            assert p16[k].grad is None
-            continue
-        if p.grad.norm().item() < 1e-6:
-            continue
-        c = _cos(p.grad, p16[k].grad)
-        worst = min(worst, c)
-        assert c > 0.98, (k, c)
-        r = p16[k].grad.norm().item() / p.grad.norm().item()
-        assert 0.9 < r < 1.1, (k, r)
-    print("worst bf16-vs-fp32 gradient cosine", worst)
     with torch.no_grad():
         ids16 = m(*batch, "dev")
         ids32 = model(*batch, "dev")
