@@ -351,6 +351,8 @@ __global__ void __launch_bounds__(256) head_fwd_kernel(const T* __restrict__ log
 // d(loss_sum)/d(logits, copy scores, gate logits); `upstream` is d(loss_sum) (a device scalar).
 // Exactly one of the two softmaxes receives gradient per row (the picked element decides), rows with
 // label == 0 or p outside [1e-10, 1] (clamp) receive none.
+// seq_weight (may be NULL = all 1): loss_sum = sum_row seq_weight[row / Tn] * nll[row], so row `row` takes upstream
+// *upstream * seq_weight[row / Tn]; a row of weight exactly 0 receives nothing, like a label-0 row.
 // vslot / vrows (may be NULL, then logits / d_logits have one row per row): logits and d_logits hold the slots of the
 // vocabulary-label rows; d_logits is written for those slots only, and CTA s < cap also zeroes slot s if it is unused.
 template <typename T>
@@ -362,15 +364,17 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(const T* __restrict__ log
                                                        const float* __restrict__ stats,
                                                        const float* __restrict__ upstream, T* __restrict__ d_logits,
                                                        float* __restrict__ d_sc, float* __restrict__ d_gate_logit,
-                                                       unsigned char* __restrict__ row_active, int Tn, int V, int S) {
+                                                       unsigned char* __restrict__ row_active, int Tn, int V, int S,
+                                                       const float* __restrict__ seq_weight) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
   const long row = blockIdx.x;
   const int b = (int)(row / Tn);
   const float* st = stats + row * 8;
   const float vmax = st[0], vsum = st[1], cmax = st[2], csum = st[3], g0 = st[4], g1 = st[5], p = st[6];
   const int lab = label[row];
-  const float up = *upstream;
-  const bool live = lab != 0 && p >= 1e-10f && p <= 1.f;
+  const float w = seq_weight ? seq_weight[b] : 1.f;
+  const float up = seq_weight ? *upstream * w : *upstream;
+  const bool live = lab != 0 && w != 0.f && p >= 1e-10f && p <= 1.f;
   const long lslot = vslot ? (long)vslot[row] : row;      // -1: the row has no logits
   const bool vocab = live && lab < V && lslot >= 0;
   const bool copy = live && lab >= V;
@@ -1181,11 +1185,11 @@ int fira_pointer_mix_nll_fwd(const void* logits, long ld_logits, const float* co
                                        argmax_out, rows, T_len, V, S, dtype, stream);
 }
 
-int fira_pointer_mix_nll_bwd_rows(const void* logits, long ld_logits, const float* copy_scores,
-                                  const unsigned char* mem_mask, const int* label, const int* vslot, const int* vrows,
-                                  int cap, const float* stats, const float* upstream, void* d_logits,
-                                  float* d_copy_scores, float* d_gate_logits, unsigned char* row_active, long rows,
-                                  int T_len, int V, int S, int dtype, void* stream) {
+static int nll_bwd_impl(const void* logits, long ld_logits, const float* copy_scores, const unsigned char* mem_mask,
+                        const int* label, const int* vslot, const int* vrows, int cap, const float* stats,
+                        const float* upstream, const float* seq_weight, void* d_logits, float* d_copy_scores,
+                        float* d_gate_logits, unsigned char* row_active, long rows, int T_len, int V, int S, int dtype,
+                        void* stream) {
   FIRA_CHECK_ARG(rows >= 0 && T_len > 0 && V > 0 && S > 0, FIRA_ERR_SHAPE, "pointer_mix_nll_bwd: shape");
   FIRA_CHECK_ARG(fira_aligned16(logits) && fira_aligned16(d_logits) && ld_logits % 8 == 0, FIRA_ERR_ALIGN,
                  "pointer_mix_nll_bwd: logits / d_logits must be 16-byte aligned with a leading dimension that is a multiple of 8");
@@ -1193,9 +1197,29 @@ int fira_pointer_mix_nll_bwd_rows(const void* logits, long ld_logits, const floa
   if (rows == 0) return FIRA_OK;
   DISPATCH_T(dtype, launch_k(head_bwd_kernel<T>, dim3((unsigned)rows), dim3(256), 0, (cudaStream_t)stream,
       (const T*)logits, ld_logits, copy_scores, mem_mask, label, vslot, vrows, cap, stats, upstream, (T*)d_logits,
-      d_copy_scores, d_gate_logits, row_active, T_len, V, S);)
+      d_copy_scores, d_gate_logits, row_active, T_len, V, S, seq_weight);)
   FIRA_CHECK_LAUNCH("fira_pointer_mix_nll_bwd");
   return FIRA_OK;
+}
+
+int fira_pointer_mix_nll_bwd_rows(const void* logits, long ld_logits, const float* copy_scores,
+                                  const unsigned char* mem_mask, const int* label, const int* vslot, const int* vrows,
+                                  int cap, const float* stats, const float* upstream, void* d_logits,
+                                  float* d_copy_scores, float* d_gate_logits, unsigned char* row_active, long rows,
+                                  int T_len, int V, int S, int dtype, void* stream) {
+  return nll_bwd_impl(logits, ld_logits, copy_scores, mem_mask, label, vslot, vrows, cap, stats, upstream, nullptr,
+                      d_logits, d_copy_scores, d_gate_logits, row_active, rows, T_len, V, S, dtype, stream);
+}
+
+int fira_pointer_mix_nll_bwd_rows_weighted(const void* logits, long ld_logits, const float* copy_scores,
+                                           const unsigned char* mem_mask, const int* label, const int* vslot,
+                                           const int* vrows, int cap, const float* stats, const float* upstream,
+                                           void* d_logits, float* d_copy_scores, float* d_gate_logits,
+                                           unsigned char* row_active, long rows, int T_len, int V, int S, int dtype,
+                                           void* stream, const float* seq_weight) {
+  FIRA_CHECK_ARG(seq_weight, FIRA_ERR_ARG, "pointer_mix_nll_bwd_rows_weighted: null seq_weight");
+  return nll_bwd_impl(logits, ld_logits, copy_scores, mem_mask, label, vslot, vrows, cap, stats, upstream, seq_weight,
+                      d_logits, d_copy_scores, d_gate_logits, row_active, rows, T_len, V, S, dtype, stream);
 }
 
 int fira_pointer_mix_nll_bwd(const void* logits, long ld_logits, const float* copy_scores,

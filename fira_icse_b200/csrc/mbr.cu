@@ -132,7 +132,88 @@ __global__ void __launch_bounds__(kMbrThreads) mbr_select_kernel(
   }
 }
 
+// Self-critical rewards (fira_icse_b200/scst.py, fira_bleu_reward): per commit, the sentence BLEU of each sample against
+// the commit's reference and its leave-one-out advantage.  One CTA per commit, one warp per sample:
+//   reference  warp 0 cleans ref columns 1..T_len-1 before the first eos_id (start / pad ids dropped) into shared memory
+//   sample     warp n cleans sample n as fira_mbr_select does, then lane p keeps c_p = the count of the sample's n-gram at
+//              p where it occurs first (match_masks of the sample against itself) and the warp sums min(c_p, occurrences
+//              in the reference) per order: the clipped matches of sentence_bleu_method2([ref], sample)
+//   baseline   thread n: A_n = (sum over m != n, m ascending, of (r_n - r_m)) / (N - 1): exactly 0 when the rewards tie
+__global__ void __launch_bounds__(kMaxCand * kWarp) bleu_reward_kernel(
+    const int* __restrict__ seq, const int* __restrict__ length, long ld_seq, const int* __restrict__ ref, long ld_ref,
+    int start_id, int eos_id, int pad_id, double* __restrict__ reward, double* __restrict__ advantage, int N, int T_len) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  __shared__ int s_ref[kWarp];
+  __shared__ int s_ref_len;
+  __shared__ int s_words[kMaxCand][kWarp];
+  __shared__ double s_r[kMaxCand];
+  const int b = blockIdx.x, n = threadIdx.x / kWarp, lane = threadIdx.x % kWarp;
+  const int col = 1 + lane;
+
+  if (n == 0) {
+    const int id = col < T_len ? ref[(long)b * ld_ref + col] : eos_id;
+    const unsigned eos = __ballot_sync(0xffffffffu, id == eos_id);    // lane 31 (col = T_len at most) always votes
+    const bool keep = lane < __ffs(eos) - 1 && id != start_id && id != pad_id;
+    const unsigned ballot = __ballot_sync(0xffffffffu, keep);
+    if (keep) s_ref[__popc(ballot & ((1u << lane) - 1u))] = id;
+    if (lane == 0) s_ref_len = __popc(ballot);
+  }
+  const long row = (long)b * N + n;
+  const int L = min(max(length[row], 1), T_len);
+  int id = 0;
+  bool keep = false;
+  if (col < L) {
+    id = seq[row * ld_seq + col];
+    keep = id != start_id && id != eos_id && id != pad_id;
+  }
+  const unsigned ballot = __ballot_sync(0xffffffffu, keep);
+  if (keep) s_words[n][__popc(ballot & ((1u << lane) - 1u))] = id;
+  const int c = __popc(ballot);
+  __syncthreads();
+
+  unsigned M[4];
+  match_masks(s_words[n], c, s_words[n], c, lane, M);
+  const unsigned below = (1u << lane) - 1u;
+  unsigned cnt[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) cnt[k] = (lane + k < c && (M[k] & below) == 0) ? __popc(M[k]) : 0u;
+  match_masks(s_words[n], c, s_ref, s_ref_len, lane, M);
+  int num[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) num[k] = (int)__reduce_add_sync(0xffffffffu, min(cnt[k], (unsigned)__popc(M[k])));
+  if (lane == 0) {
+    s_r[n] = method2_bleu(num, c, s_ref_len);
+    reward[row] = s_r[n];
+  }
+  __syncthreads();
+
+  if (threadIdx.x < N) {
+    const int i = threadIdx.x;
+    double sum = 0.0;
+    for (int m = 0; m < N; ++m)
+      if (m != i) sum = __dadd_rn(sum, __dsub_rn(s_r[i], s_r[m]));
+    advantage[(long)b * N + i] = sum / (double)(N - 1);
+  }
+}
+
 }  // namespace
+
+extern "C" int fira_bleu_reward(const int* seq, const int* length, long ld_seq, const int* ref, long ld_ref,
+                                int start_id, int eos_id, int pad_id, double* reward, double* advantage, int B, int N,
+                                int T_len, void* stream) {
+  FIRA_CHECK_ARG(B >= 0 && N >= 2 && N <= kMaxCand, FIRA_ERR_SHAPE, "bleu_reward: B %d, N %d (2 <= N <= %d)", B, N,
+                 kMaxCand);
+  FIRA_CHECK_ARG(T_len >= 2 && T_len <= kMaxT && ld_seq >= T_len && ld_ref >= T_len, FIRA_ERR_SHAPE,
+                 "bleu_reward: T_len %d, ld_seq %ld, ld_ref %ld (2 <= T_len <= %d, ld_seq, ld_ref >= T_len)", T_len,
+                 ld_seq, ld_ref, kMaxT);
+  if (B == 0) return FIRA_OK;
+  FIRA_CHECK_ARG(seq && length && ref && reward && advantage, FIRA_ERR_ARG,
+                 "bleu_reward: null seq / length / ref / reward / advantage");
+  launch_k(bleu_reward_kernel, dim3((unsigned)B), dim3((unsigned)(N * kWarp)), 0, (cudaStream_t)stream, seq, length,
+           ld_seq, ref, ld_ref, start_id, eos_id, pad_id, reward, advantage, N, T_len);
+  FIRA_CHECK_LAUNCH("fira_bleu_reward");
+  return FIRA_OK;
+}
 
 extern "C" int fira_mbr_select(const int* seq, const int* length, long ld_seq, int start_id, int eos_id, int pad_id,
                                double* pair_bleu, double* utility, int* best, int B, int N, int T_len, void* stream) {

@@ -17,6 +17,7 @@ import weakref
 import torch
 
 from . import ops
+from . import optim as _optim
 from ._lib import call
 from .incremental import IncrementalDecoder, replay_or_capture, weights_key
 
@@ -183,6 +184,16 @@ class PositionLoop:
         self.lp[0].zero_()
         self.status[0].zero_()
 
+    def refresh_weights(self):
+        """The parameters changed in place (an optimizer step): refresh the operand copies the captured graphs read, so
+        they replay with the new weights.  The decoder's concatenated weights follow in start() (IncrementalDecoder
+        compares weights_key); here the bf16 mirror and the bf16 copies of the head's weights.  fp32 mode reads the
+        parameters themselves."""
+        if self.pr.bf16:
+            _optim.ensure_fresh(self.model)
+            for W, W16 in self.pr.wcache.values():
+                W16.copy_(W.detach())
+
     def unfinished(self, t):
         """A device bool: some row still decodes after t positions."""
         return self.status[t % self.halves].eq(0).any()
@@ -217,14 +228,22 @@ class PositionLoop:
         return t
 
 
-_LOOPS = weakref.WeakKeyDictionary()          # model -> {(class, B, N, T, S, precision): (weights key, loop)}
+_LOOPS = weakref.WeakKeyDictionary()   # model -> {(class, B, N, T, S, precision): (weights key, addresses, loop)}
 
 
 def loop_for(cls, model, B, N, T, S):
-    """The cached `cls` instance of this shape; rebuilt (fresh operand copies and graphs) when the weights changed."""
+    """The cached `cls` instance of this shape.  Weights updated in place (a new weights_key, every parameter at the
+    address the graphs captured) are refreshed inside the loop, whose position graphs keep replaying: a training loop
+    that samples after every optimizer step (scst.py) does not recapture them.  A parameter that moved rebuilds the
+    loop (fresh operand copies and graphs)."""
     store = _LOOPS.setdefault(model, {})
     key = (cls, B, N, T, S, model.precision)
     wkey = weights_key(model, model.decoder)
-    if key not in store or store[key][0] != wkey:
-        store[key] = (wkey, cls(model, B, N, T, S))
-    return store[key][1]
+    addr = tuple(p.data_ptr() for p in model.parameters())
+    cur = store.get(key)
+    if cur is None or cur[1] != addr:
+        store[key] = (wkey, addr, cls(model, B, N, T, S))
+    elif cur[0] != wkey:
+        cur[2].refresh_weights()
+        store[key] = (wkey, addr, cur[2])
+    return store[key][2]

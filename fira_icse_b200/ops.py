@@ -824,15 +824,22 @@ def copy_scores_fwd(pr, memory2, dec2, Ws, Wt, wres, bres, B, T, S, src_mask=Non
 class HeadFn(torch.autograd.Function):
     """Model.py:54-86 fused: out_fc, CopyNet, both softmaxes, gate mixing, log(clamp), shifted-label
     NLL -- returns (loss_sum, per-position nll, argmax ids or None).  The B x 30 x 25,020 distribution
-    is never built."""
+    is never built.  seq_weight (fp32 [B] on the device, padded batches only): loss_sum = sum_b seq_weight[b] *
+    sum_t nll[b, t] (self-critical training, scst.py); a target sequence of weight 0 takes no gradient."""
 
     @staticmethod
     def forward(ctx, want_argmax, bf16, pf, memory, dec, mem_mask, label, Wout, bout, Ws, Wt, Wres, bres, Wp, bp,
-                pk=None):
+                pk=None, seq_weight=None):
         _require_cuda(memory, dec, Wout)
         B, T = dec.shape[0], dec.shape[1]
         S = pk.S if pk is not None else memory.shape[1]      # packed batch: memory is [1, Rc + Rs, D]
         V = Wout.shape[0]
+        if seq_weight is not None:
+            if pk is not None or want_argmax:
+                raise ValueError("HeadFn: seq_weight applies to the padded training path only")
+            if seq_weight.dtype != torch.float32 or tuple(seq_weight.shape) != (B,) or not seq_weight.is_cuda:
+                raise ValueError(f"HeadFn: seq_weight must be a CUDA fp32 tensor of shape ({B},)")
+            seq_weight = seq_weight.contiguous()
         Mt, Ms = B * T, memory.shape[0] * memory.shape[1]
         pr = Prec(bf16)
         if pf is not None and pf.event is not None:
@@ -872,9 +879,12 @@ class HeadFn(torch.autograd.Function):
         call("fira_pointer_mix_nll_fwd_rows", _ptr(logits), ldl, _ptr(sc), _ptr(gl), _ptr(mem_mask), _ptr(label),
              _ptr(vslot), _ptr(stats), _ptr(nll), _ptr(amax), Mt, T, V, S, pr.code, st)
         ctx.misc = (pr, memory2, dec2, dec32, mem_mask, label, logits, ldl, src, tgt, sc, stats, B, T, S, V,
-                    memory.dtype, dec.dtype, pk, memory.shape, cap, vslot, vrows, dec_v)
+                    memory.dtype, dec.dtype, pk, memory.shape, cap, vslot, vrows, dec_v, seq_weight)
         ctx.save_for_backward(Wout, Ws, Wt, Wres, Wp, bout, bres, bp)
-        loss_sum = colsum(nll, 1, Mt, 1).view(())
+        if seq_weight is None:
+            loss_sum = colsum(nll, 1, Mt, 1).view(())
+        else:                                      # per position t: sum_b w[b] nll[b, t], then over t
+            loss_sum = colsum(colsum(nll, T, B, T, weight=seq_weight), 1, T, 1).view(())
         ids = amax.view(B, T) if want_argmax else None
         nll2 = nll.view(B, T)
         ctx.mark_non_differentiable(*([nll2, ids] if ids is not None else [nll2]))
@@ -883,7 +893,7 @@ class HeadFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_loss, g_nll, g_ids):
         (pr, memory2, dec2, dec32, mem_mask, label, logits, ldl, src, tgt, sc, stats, B, T, S, V,
-         mem_dt, dec_dt, pk, mem_shape, cap, vslot, vrows, dec_v) = ctx.misc
+         mem_dt, dec_dt, pk, mem_shape, cap, vslot, vrows, dec_v, seq_weight) = ctx.misc
         Wout, Ws, Wt, Wres, Wp, bout, bres, bp = ctx.saved_tensors
         Mt, Ms = B * T, memory2.shape[0]
         dev = dec2.device
@@ -894,9 +904,12 @@ class HeadFn(torch.autograd.Function):
         dsc = torch.empty((B, T, S), **f32)
         dgl = torch.empty((Mt, 2), **f32)
         active = torch.empty((Mt,), dtype=torch.uint8, device=dev)
-        call("fira_pointer_mix_nll_bwd_rows", _ptr(logits), ldl, _ptr(sc), _ptr(mem_mask), _ptr(label), _ptr(vslot),
-             _ptr(vrows), cap, _ptr(stats), _ptr(up), _ptr(dlogits), _ptr(dsc), _ptr(dgl), _ptr(active), Mt, T, V, S,
-             pr.code, st)
+        args = (_ptr(logits), ldl, _ptr(sc), _ptr(mem_mask), _ptr(label), _ptr(vslot), _ptr(vrows), cap, _ptr(stats),
+                _ptr(up), _ptr(dlogits), _ptr(dsc), _ptr(dgl), _ptr(active), Mt, T, V, S, pr.code, st)
+        if seq_weight is None:
+            call("fira_pointer_mix_nll_bwd_rows", *args)
+        else:
+            call("fira_pointer_mix_nll_bwd_rows_weighted", *args, _ptr(seq_weight))
         # pointer scores
         d_src = pr.empty((Ms, D), dev)
         d_tgt = torch.zeros((Mt, D), **f32)
@@ -934,7 +947,7 @@ class HeadFn(torch.autograd.Function):
         linear_dx(d_tgt, D, Wt, Mt, out=d_dec, accumulate=True)
         fork.join()
         return (None, None, None, d_mem.view(mem_shape).to(mem_dt), d_dec.view(B, T, D).to(dec_dt), None, None, d_Wout,
-                d_bout, d_Ws, d_Wt, d_wres, d_bres, d_Wp, d_bp, None)
+                d_bout, d_Ws, d_Wt, d_wres, d_bres, d_Wp, d_bp, None, None)
 
 
 # ============================================================================= module-surface pieces

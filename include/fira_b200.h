@@ -292,6 +292,17 @@ int fira_pointer_mix_nll_bwd_rows(const void* logits, long ld_logits, const floa
                                   int cap, const float* stats, const float* upstream, void* d_logits,
                                   float* d_copy_scores, float* d_gate_logits, unsigned char* row_active, long rows,
                                   int T_len, int V, int S, int dtype, void* stream);
+/* Sequence-weighted backward (self-critical training, fira_icse_b200/scst.py): fira_pointer_mix_nll_bwd_rows for
+ *      loss_sum = sum_row seq_weight[row / T_len] * nll[row], seq_weight [rows / T_len] fp32 (device, not NULL): row
+ *      `row` takes upstream *upstream * seq_weight[row / T_len].  A row whose weight is exactly 0 is treated as a
+ *      label-0 row: no gradient, row_active 0 (the copy-score backward skips it).  Weights of 1.0 give bit for bit the
+ *      results of fira_pointer_mix_nll_bwd_rows. */
+int fira_pointer_mix_nll_bwd_rows_weighted(const void* logits, long ld_logits, const float* copy_scores,
+                                           const unsigned char* mem_mask, const int* label, const int* vslot,
+                                           const int* vrows, int cap, const float* stats, const float* upstream,
+                                           void* d_logits, float* d_copy_scores, float* d_gate_logits,
+                                           unsigned char* row_active, long rows, int T_len, int V, int S, int dtype,
+                                           void* stream, const float* seq_weight);
 
 /* ---- one seeded sampling step from the same mixture (fira_icse_b200/sample.py).  Rows are (commit b, sample n),
  *      B*N of them: logits [B*N, ld_logits], copy_scores [B, N, S], gate_logits [B*N, 2], mem_mask / copy_src [B, S]
@@ -447,6 +458,19 @@ int fira_pointer_mix_diverse_beam_step_rules(const void* logits, long ld_logits,
  *      NULL.  2 <= N <= 32, 2 <= T_len <= 32, ld_seq >= T_len, B >= 0 (B = 0: nothing is launched). */
 int fira_mbr_select(const int* seq, const int* length, long ld_seq, int start_id, int eos_id, int pad_id,
                     double* pair_bleu, double* utility, int* best, int B, int N, int T_len, void* stream);
+
+/* ---- self-critical rewards (fira_icse_b200/scst.py): each of a commit's N samples scored against its reference.
+ *      seq / length as fira_mbr_select; ref [B, ld_ref] int32, the commit's target ids (<start> first).  Rule:
+ *        words_n   = as fira_mbr_select
+ *        ref_b     = ref[b, 1:e] without start_id / pad_id ids, e = the first column >= 1 holding eos_id (T_len if none)
+ *        reward    = bleu.sentence_bleu_method2([ref_b], words_n) over the ids, in float64 (the BLEU of fira_mbr_select
+ *                    with r = len(ref_b))
+ *        advantage = (sum over m != n, m ascending, of (reward[b, n] - reward[b, m])) / (N - 1)
+ *                    (reward minus the mean of the other samples' rewards, written so that tied rewards give exactly 0)
+ *      reward, advantage [B, N] float64.  One CTA per commit, one warp per sample.  2 <= N <= 32, 2 <= T_len <= 32,
+ *      ld_seq >= T_len, ld_ref >= T_len, B >= 0 (B = 0: nothing is launched). */
+int fira_bleu_reward(const int* seq, const int* length, long ld_seq, const int* ref, long ld_ref, int start_id,
+                     int eos_id, int pad_id, double* reward, double* advantage, int B, int N, int T_len, void* stream);
 
 /* ---- HOST-side batch preparation (CPU only: every pointer below is HOST memory, there is no stream).
  *

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""`python run_model.py train|test` -- the reference's CLI (run_model.py:417-425) on the CUDA path.
+"""`python run_model.py train|test|finetune` -- the reference's CLI (run_model.py:417-425) on the CUDA path.
 
 Same CWD-relative files (DataSet/*.json, all_index, VOCAB_UPPER_CASE, best_model.pt,
 OUTPUT/{output_fira,train_process,dev_output}), same hyper-parameters (run_model.py:27-46), same
@@ -42,6 +42,15 @@ beam search ranking.  Differences, all below the module surface:
     §9).  A nonzero value appends _norepeat<n> / _minlen<m> to the output name, after any _prefix<k>
     (output_fira_nbest_norepeat2_minlen3, ...), so the outputs without them stay.  FIRA_DECODE=beam with either set
     exits with an error.
+    FIRA_CHECKPOINT (default best_model.pt): the state_dict `test` decodes with (best_model_scst.pt after finetune).
+  * `finetune`: self-critical fine-tuning on sentence BLEU (fira_icse_b200.scst, DESIGN.md §9), one GPU.  Loads
+    best_model.pt and runs FIRA_SCST_EPOCHS (default 1) epochs of scst_step with optim.FlatAdam at FIRA_SCST_LR
+    (default 1e-5) over padded batches of FIRA_BATCH commits (FIRA_MAX_BATCHES bounds an epoch): FIRA_SAMPLES (default
+    5, 2..32) seeded samples per commit with FIRA_TEMPERATURE, FIRA_TOP_K, FIRA_TOP_P, FIRA_SEED (epoch e draws with
+    seed FIRA_SEED + e), FIRA_NO_REPEAT_NGRAM and FIRA_MIN_LENGTH, each rewarded with its id-level sentence BLEU
+    against the reference and weighted by its leave-one-out advantage.  Prints the mean reward every 10 batches, runs
+    dev() after every epoch and saves the state_dict of the best dev BLEU to best_model_scst.pt; best_model.pt is never
+    overwritten.  WORLD_SIZE > 1 exits with an error.
 """
 import json
 import os
@@ -62,6 +71,7 @@ from fira_icse_b200.engine import GraphedTrainStep
 from fira_icse_b200.mbr import mbr
 from fira_icse_b200.parallel import DataParallelStep, shard_range
 from fira_icse_b200.sample import sample
+from fira_icse_b200.scst import check_step, scst_step
 
 
 class DotDict(dict):
@@ -342,7 +352,7 @@ def main_test():
     test_set = TransDataset(args, 'test')
     all_index = json.load(open('all_index'))
     model = TransModel(args)
-    model.load_state_dict(torch.load("best_model.pt", map_location="cpu"))
+    model.load_state_dict(torch.load(os.environ.get("FIRA_CHECKPOINT", "best_model.pt"), map_location="cpu"))
     model = model.to(dev_)
     lo, hi = shard_range(len(test_set), RANK, WORLD)                # replicas only: index ranges, files concatenated
     idx = list(range(lo, hi)) if WORLD > 1 else None
@@ -353,6 +363,74 @@ def main_test():
     print("mean sentence bleu: %f" % bleu)
 
 
+def finetune_settings():
+    """The finetune stage's settings from the environment, checked before any device work (SystemExit on an error)."""
+    if WORLD > 1:
+        raise SystemExit("run_model.py finetune runs on one GPU: launch it without torchrun (WORLD_SIZE=1)")
+    try:
+        s = dict(epochs=int(os.environ.get("FIRA_SCST_EPOCHS", 1)), lr=float(os.environ.get("FIRA_SCST_LR", 1e-5)),
+                 num_samples=int(os.environ.get("FIRA_SAMPLES", 5)),
+                 temperature=float(os.environ.get("FIRA_TEMPERATURE", 1.0)), top_k=int(os.environ.get("FIRA_TOP_K", 0)),
+                 top_p=float(os.environ.get("FIRA_TOP_P", 1.0)), seed=int(os.environ.get("FIRA_SEED", 0)),
+                 no_repeat_ngram=int(os.environ.get("FIRA_NO_REPEAT_NGRAM", 0)),
+                 min_length=int(os.environ.get("FIRA_MIN_LENGTH", 0)))
+    except ValueError as e:
+        raise SystemExit(f"run_model.py finetune: {e}")
+    if s["epochs"] < 1:
+        raise SystemExit(f"FIRA_SCST_EPOCHS must be >= 1, got {s['epochs']}")
+    if not 0.0 < s["lr"] < float("inf"):
+        raise SystemExit(f"FIRA_SCST_LR must be a positive finite number, got {s['lr']}")
+    sampling = {k: s[k] for k in ("num_samples", "temperature", "top_k", "top_p", "seed", "no_repeat_ngram",
+                                  "min_length")}
+    try:                # the batches' references are checked per step
+        check_step(None, **sampling, first_index=0, tar_len=args.tar_len, eos_id=None)
+    except ValueError as e:
+        raise SystemExit(f"run_model.py finetune: {e}")
+    return s, sampling
+
+
+def main_finetune():
+    s, sampling = finetune_settings()
+    dev_ = device()
+    g = load_globals()
+    vocab = g["vocab"]
+    ids = dict(tar_len=args.tar_len, start_id=vocab['<start>'], eos_id=vocab['<eos>'], pad_id=vocab['<pad>'])
+    train_set = TransDataset(args, 'train')
+    dev_set = TransDataset(args, 'valid')
+    all_index = json.load(open('all_index'))
+    model = TransModel(args)
+    model.load_state_dict(torch.load("best_model.pt", map_location="cpu"))
+    model = model.to(dev_)
+    from fira_icse_b200 import optim
+    opt = optim.FlatAdam(model.live_parameters(), lr=s["lr"], groups=model.flat_groups())
+    optim.attach(model, [opt])
+    train_loader = loader(train_set, args.batch_size, True)
+    dev_loader = loader(dev_set, args.batch_size, False)
+    max_batches = int(os.environ.get("FIRA_MAX_BATCHES", 0))
+    best_bleu = -1.0
+    for epoch in range(s["epochs"]):
+        total, rewards = 0, []
+        for idx, batch in enumerate(train_loader):
+            if max_batches and idx >= max_batches:
+                break
+            b = batch_to_device(batch, dev_)
+            step = scst_step(model, opt, b, **dict(sampling, seed=sampling["seed"] + epoch), first_index=total, **ids)
+            rewards.append(step.reward)
+            total += len(b[0])
+            if idx % 10 == 0:
+                print("scst epoch: %d batch: %d/%d reward: %.4f |advantage|: %.4f loss: %.6f" % (
+                    epoch, idx, len(train_loader), sum(rewards) / len(rewards), step.advantage, step.loss))
+                rewards = []
+        cur_bleu, output_str = dev(model, dev_loader, g, all_index['valid'], epoch, dev_)
+        open('OUTPUT/train_process', 'a').write(
+            'scst epoch: {} dev bleu: {} is better: {}\n'.format(epoch, cur_bleu, cur_bleu > best_bleu))
+        if cur_bleu > best_bleu:
+            best_bleu = cur_bleu
+            torch.save(model.state_dict(), "best_model_scst.pt")
+            open('OUTPUT/dev_output_scst', 'w').write(output_str)
+    print("best dev bleu: %f" % best_bleu)
+
+
 if __name__ == '__main__':
     stage = str(sys.argv[1])
     seed_everything()
@@ -361,5 +439,7 @@ if __name__ == '__main__':
         main_train()
     elif stage == 'test':
         main_test()
+    elif stage == 'finetune':
+        main_finetune()
     else:
-        raise SystemExit("usage: python run_model.py train|test")
+        raise SystemExit("usage: python run_model.py train|test|finetune")
