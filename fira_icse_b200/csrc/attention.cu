@@ -360,6 +360,26 @@ attn_mma_bwd_kernel(AttnArgs a, const __nv_bfloat16* __restrict__ out, const __n
                     const float* __restrict__ stats, __nv_bfloat16* __restrict__ dq, long lddq,
                     __nv_bfloat16* __restrict__ dk, long lddk, __nv_bfloat16* __restrict__ dv, long lddv) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  // with qoff, a.Lq / a.Lk become the commit's query rows (and causal keys) from here on; sp / kp keep the pitches
+  const int sp = a.Lq, kp = a.Lk;
+  const long qb = a.qoff ? (long)a.qoff[blockIdx.x / a.H] : (long)(blockIdx.x / a.H) * sp;
+  if (a.qoff) {
+    a.Lq = a.qoff[blockIdx.x / a.H + 1] - (int)qb;
+    if (a.causal) a.Lk = a.Lq;
+    if (blockIdx.x / a.H == a.B - 1) {           // the last commit's CTAs zero the head's columns of the pad rows
+      const int h = blockIdx.x % a.H;
+      const long p0 = a.qoff[a.B];
+      for (long i = threadIdx.x; i < (a.qrows - p0) * 4; i += blockDim.x) {
+        const long r = p0 + (i >> 2);
+        const int c = (int)(i & 3) * 8 + h * DH;
+        *reinterpret_cast<uint4*>(dq + r * lddq + c) = make_uint4(0, 0, 0, 0);
+        if (a.causal) {
+          *reinterpret_cast<uint4*>(dk + r * lddk + c) = make_uint4(0, 0, 0, 0);
+          *reinterpret_cast<uint4*>(dv + r * lddv + c) = make_uint4(0, 0, 0, 0);
+        }
+      }
+    }
+  }
   extern __shared__ __align__(16) unsigned char mma_smem[];
   __shared__ int nv_s, filled_s;
   __shared__ float delta_s[LQ_MAX], m2_s[LQ_MAX], inv_s[LQ_MAX];
@@ -369,9 +389,9 @@ attn_mma_bwd_kernel(AttnArgs a, const __nv_bfloat16* __restrict__ out, const __n
   int* kidx = reinterpret_cast<int*>(Ws + BWARPS * BWARP_SMEM);
   const int b = blockIdx.x / a.H, h = blockIdx.x % a.H;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, q = lane & 3;
-  const unsigned char* km = a.key_mask ? a.key_mask + (long)b * a.Lk : nullptr;
+  const unsigned char* km = a.key_mask ? a.key_mask + (long)b * kp : nullptr;
   const int* rg = a.ranges ? a.ranges + 4 * b : nullptr;
-  const long kvb = rg ? 0 : (long)b * a.Lk;
+  const long kvb = rg ? 0 : a.qoff && a.causal ? qb : (long)b * kp;
   const __nv_bfloat16* kh = (const __nv_bfloat16*)a.k + kvb * a.ldk + h * DH;
   const __nv_bfloat16* vh = (const __nv_bfloat16*)a.v + kvb * a.ldv + h * DH;
   unsigned char* Kw = Ws + warp * BWARP_SMEM;
@@ -386,16 +406,16 @@ attn_mma_bwd_kernel(AttnArgs a, const __nv_bfloat16* __restrict__ out, const __n
   for (int i = threadIdx.x; i < 2 * LQ_MAX * 4; i += blockDim.x) {
     const int which = i / (LQ_MAX * 4), r = (i >> 2) & (LQ_MAX - 1), c = i & 3;
     unsigned char* dst = (which ? Os : Qs) + swz(r, c);
-    if (r < a.Lq) cp_async16(su32(dst), which ? d_ctx + ((long)b * a.Lq + r) * ldo + h * DH + c * 8
-                                              : (const __nv_bfloat16*)a.q + ((long)b * a.Lq + r) * a.ldq + h * DH + c * 8);
+    if (r < a.Lq) cp_async16(su32(dst), which ? d_ctx + (qb + r) * ldo + h * DH + c * 8
+                                              : (const __nv_bfloat16*)a.q + (qb + r) * a.ldq + h * DH + c * 8);
     else *reinterpret_cast<uint4*>(dst) = make_uint4(0, 0, 0, 0);
   }
   cp_async_commit();
   // delta_t = dO_t . O_t over the head's 32 features; row statistics
   if (threadIdx.x < a.Lq) {
     const int t = threadIdx.x;
-    const __nv_bfloat16* orow = out + ((long)b * a.Lq + t) * ldo + h * DH;
-    const __nv_bfloat16* grow = d_ctx + ((long)b * a.Lq + t) * ldo + h * DH;
+    const __nv_bfloat16* orow = out + (qb + t) * ldo + h * DH;
+    const __nv_bfloat16* grow = d_ctx + (qb + t) * ldo + h * DH;
     float d = 0.f;
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
@@ -405,7 +425,7 @@ attn_mma_bwd_kernel(AttnArgs a, const __nv_bfloat16* __restrict__ out, const __n
 #pragma unroll
       for (int e = 0; e < 8; ++e) d = fmaf(ov[e], gv[e], d);
     }
-    const float* st = stats + (((long)b * a.H + h) * a.Lq + t) * 2;
+    const float* st = stats + (((long)b * a.H + h) * sp + t) * 2;
     delta_s[t] = d; m2_s[t] = st[0] * kLog2e; inv_s[t] = 1.f / st[1];
   }
   // masked keys receive exactly zero gradient (the mask bytes of 32 keys per ballot, then one row per lane group)
@@ -549,7 +569,7 @@ attn_mma_bwd_kernel(AttnArgs a, const __nv_bfloat16* __restrict__ out, const __n
 #pragma unroll
     for (int w = 0; w < BWARPS; ++w)
       x += reinterpret_cast<const float*>(Ws + w * BWARP_SMEM + 4 * BKB * ROWB)[swz_f32(t, f)];
-    dq[((long)b * a.Lq + t) * lddq + h * DH + f] = __float2bfloat16_rn(x);
+    dq[(qb + t) * lddq + h * DH + f] = __float2bfloat16_rn(x);
   }
 }
 
@@ -626,7 +646,8 @@ int attn_fwd_impl(const void* q, long ldq, const void* k, long ldk, const void* 
 
 int attn_bwd_impl(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv,
                   const unsigned char* key_mask, const int* ranges, int causal, const void* ctx, const void* d_ctx, long ldo, const float* stats, void* dq, long lddq, void* dk,
-                  long lddk, void* dv, long lddv, int B, int H, int Lq, int Lk, int d_head, int dtype, void* stream) {
+                  long lddk, void* dv, long lddv, int B, int H, int Lq, int Lk, int d_head, int dtype, void* stream,
+                  const int* qoff = nullptr, long qrows = 0) {
   FIRA_CHECK_ARG(d_head == DH, FIRA_ERR_SHAPE, "attn_bwd: d_head %d != 32", d_head);
   FIRA_CHECK_ARG(B > 0 && H > 0 && Lq > 0 && Lk > 0 && Lq <= LQ_MAX, FIRA_ERR_SHAPE, "attn_bwd: shape (Lq <= 32)");
   FIRA_CHECK_ARG(key_mask || ranges, FIRA_ERR_ARG, "attn_bwd: key_mask may only be NULL with ranges");
@@ -636,8 +657,11 @@ int attn_bwd_impl(const void* q, long ldq, const void* k, long ldk, const void* 
       (rc = check_layout("attn_bwd", v, ldv, dtype)) || (rc = check_layout("attn_bwd", ctx, ldo, dtype)) ||
       (rc = check_layout("attn_bwd", d_ctx, ldo, dtype)))
     return rc;
-  AttnArgs a{q, ldq, k, ldk, v, ldv, key_mask, ranges, causal, B, H, Lq, Lk, 1.f / sqrtf((float)d_head)};
-  if (use_tc(dtype) && (lddk % 8) == 0 && (lddv % 8) == 0 && (lddq % 8) == 0) {
+  AttnArgs a{q, ldq, k, ldk, v, ldv, key_mask, ranges, causal, B, H, Lq, Lk, 1.f / sqrtf((float)d_head), qoff, qrows};
+  FIRA_CHECK_ARG(!qoff || (dtype == FIRA_BF16 && (lddk % 8) == 0 && (lddv % 8) == 0 && (lddq % 8) == 0 &&
+                           (!causal || (Lq == Lk && !ranges))),
+                 FIRA_ERR_ARG, "attn_bwd_rows: bf16, 16-B gradient pitches, causal with Lq == Lk and no ranges");
+  if (qoff || (use_tc(dtype) && (lddk % 8) == 0 && (lddv % 8) == 0 && (lddq % 8) == 0)) {
     const size_t smem = mma::bwd_smem(Lk);
     if ((rc = set_smem(mma::attn_mma_bwd_kernel, smem, "attn_bwd"))) return rc;
     launch_k(mma::attn_mma_bwd_kernel, dim3(B * H), dim3(mma::BWARPS * 32), smem, (cudaStream_t)stream, a,
@@ -697,6 +721,15 @@ int fira_attn_packed_bwd(const void* q, long ldq, const void* k, long ldk, const
   FIRA_CHECK_ARG(ranges && kv_rows > 0, FIRA_ERR_ARG, "attn_packed_bwd: ranges / kv_rows");
   return attn_bwd_impl(q, ldq, k, ldk, v, ldv, key_mask, ranges, 0, ctx, d_ctx, ldo, stats, dq, lddq,
                        dk, lddk, dv, lddv, B, H, Lq, mask_pitch, d_head, dtype, stream);
+}
+
+int fira_attn_bwd_rows(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv, const int* ranges,
+                       const unsigned char* key_mask, int mask_pitch, int causal, const int* qoff, long rows,
+                       const void* ctx, const void* d_ctx, long ldo, const float* stats, void* dq, long lddq, void* dk,
+                       long lddk, void* dv, long lddv, int B, int H, int Lq, int d_head, int dtype, void* stream) {
+  FIRA_CHECK_ARG(qoff && rows > 0, FIRA_ERR_ARG, "attn_bwd_rows: null qoff or no rows");
+  return attn_bwd_impl(q, ldq, k, ldk, v, ldv, key_mask, ranges, causal, ctx, d_ctx, ldo, stats, dq, lddq, dk, lddk,
+                       dv, lddv, B, H, Lq, mask_pitch, d_head, dtype, stream, qoff, rows);
 }
 
 }  // extern "C"

@@ -19,6 +19,10 @@ struct AttnArgs {
   int causal;
   int B, H, Lq, Lk;
   float scale;
+  // NULL, or [B+1] (attn_mma_bwd_kernel): the query rows of commit b are rows qoff[b] .. qoff[b+1] - 1 (at most Lq; Lq
+  // stays the pitch of stats); causal: so are its keys, and key_mask keeps the pitch Lk
+  const int* qoff = nullptr;
+  long qrows = 0;                // with qoff: rows of q / dq (causal: of k / v too); rows qoff[B] .. qrows - 1 are pad
 };
 
 // valid-key compaction by warp 0: kidx[0..nv) = original indices of keys with mask == 1 (ascending).

@@ -25,7 +25,10 @@
 //   LayerNorm  Z (bf16) staged in shared memory, then ln_fwd_kernel's arithmetic row by row (warp per row, lane per
 //              8 features, same Philox dropout key), so the statistics come from the bf16-rounded Z; both CTAs normalise
 //              every row, each stores the rows of its parity.
-// Every tensor the backward reads is written in the layouts of the per-layer launch sequence (rows t >= T never).
+// Every tensor the backward reads is written in the layouts of the per-layer launch sequence, one row per slot: with a
+// live-row map (fira_target_rows) only the rows t < tlen[b] of commit b, to slots toff[b] + t, the pad slots zeroed;
+// without one the slot is the row b T + t.  The rows are computed as without a map, so a live row's values do not depend
+// on it.  The output (the head's input) keeps the rows b T + t, zero past tlen[b].
 #include <string.h>
 #include <cooperative_groups.h>
 #include "attn_mma.cuh"
@@ -61,10 +64,13 @@ struct DecParams {
   const int* tar; const float* emb; const float* pe; const unsigned char* tar_mask;
   const bf16* kv; long ldkv;                    // [Ms, L*512]: layer i's K at column 512 i, V at 512 i + 256
   const unsigned char* mem_mask; const int* ranges; int S;
-  bf16* X;                                      // [L+1][B*T][256]: every layer's input, then the output
+  bf16* X;                                      // [L][R][256]: every layer's input
+  bf16* out;                                    // [B*T][256]: the last layer's output
   bf16* qkv; bf16* ctx1; float* st1; bf16* z1; float* ls1; bf16* x1;
   bf16* q; bf16* ctx2; float* st2; bf16* z2; float* ls2; bf16* x2;
   bf16* hh; bf16* z3; float* ls3;
+  const int* tlen; const int* toff;             // the live-row map, or NULL: slot = row
+  long R;                                       // slots of the saved tensors
   int B, T, L;
   float scale, p_drop;
   uint64_t seed; const uint64_t* seed_ctr; uint32_t stream_id;
@@ -173,12 +179,15 @@ __device__ __forceinline__ void copy_out(bf16* __restrict__ dst, int N, int T, i
 }
 
 // out = LN(dropout(Z) + resid) * gamma + beta over the commit's rows, two per warp: ln_fwd_kernel's arithmetic and
-// dropout key (global row r, 8 features per lane).  Both CTAs of the pair compute every row (the same values); Z, out and
-// the statistics of the rows of parity `rank` go to global memory.  Rows >= T of out are zeroed.
+// dropout key (global row r0 + t, 8 features per lane).  Both CTAs of the pair compute every row (the same values); Z,
+// out and the statistics of the rows of parity `rank` go to global memory, row t < n to slot s0 + t.  Rows >= T of the
+// shared-memory out are zeroed.  out_rows: og takes rows r0 + t < r0 + T instead -- zero from tl on, NaN for a live row
+// without a slot (t >= n), so that a live-row count above the slots shows as a NaN loss.
 __device__ __forceinline__ void ln_rows(const unsigned char* sm, int off_z, int off_res, int off_out, const float* gamma,
                                         const float* beta, bf16* __restrict__ zg, bf16* __restrict__ og,
-                                        float* __restrict__ stats, long rows, long r0, int T, float p_drop, uint64_t seed,
-                                        const uint64_t* seed_ctr, uint32_t sid, int rank, int warp, int lane) {
+                                        float* __restrict__ stats, long rows, long r0, long s0, int T, int n, int tl,
+                                        bool out_rows, float p_drop, uint64_t seed, const uint64_t* seed_ctr,
+                                        uint32_t sid, int rank, int warp, int lane) {
   if (seed_ctr) seed += *seed_ctr;
   float g[8], bt[8];
   Act<float>::load8(gamma + lane * 8, g);
@@ -188,10 +197,10 @@ __device__ __forceinline__ void ln_rows(const unsigned char* sm, int off_z, int 
     const int o = (t * LDA + lane * 8) * 2;
     bf16* os = (bf16*)(sm + off_out + o);
     if (t >= T) { *reinterpret_cast<uint4*>(os) = make_uint4(0, 0, 0, 0); continue; }
-    const long r = r0 + t;
+    const long r = r0 + t, sl = s0 + t;
     const bool mine = (t & 1) == rank;
     const uint4 zraw = *reinterpret_cast<const uint4*>(sm + off_z + o);
-    if (mine) *reinterpret_cast<uint4*>(zg + r * D + lane * 8) = zraw;
+    if (mine && t < n) *reinterpret_cast<uint4*>(zg + sl * D + lane * 8) = zraw;
     float y[8], x[8];
     Act<bf16>::load8((const bf16*)&zraw, y);
     Act<bf16>::load8((const bf16*)(sm + off_res + o), x);
@@ -212,8 +221,14 @@ __device__ __forceinline__ void ln_rows(const unsigned char* sm, int off_z, int 
     for (int i = 0; i < 8; ++i) y[i] = (y[i] - mean) * rstd * g[i] + bt[i];
     Act<bf16>::store8(os, y);
     if (mine) {
-      *reinterpret_cast<uint4*>(og + r * D + lane * 8) = *reinterpret_cast<const uint4*>(os);
-      if (lane == 0) { stats[r] = mean; stats[rows + r] = rstd; }
+      if (out_rows) {
+        const uint32_t fill = t < tl ? 0x7fc07fc0u : 0u;      // bf16 NaN pairs / zeros
+        *reinterpret_cast<uint4*>(og + r * D + lane * 8) =
+            t < n ? *reinterpret_cast<const uint4*>(os) : make_uint4(fill, fill, fill, fill);
+      } else if (t < n) {
+        *reinterpret_cast<uint4*>(og + sl * D + lane * 8) = *reinterpret_cast<const uint4*>(os);
+      }
+      if (lane == 0 && t < n) { stats[sl] = mean; stats[rows + sl] = rstd; }
     }
   }
 }
@@ -266,14 +281,14 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHR, 1)
 decoder_fwd_kernel(const __grid_constant__ DecParams p) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
   extern __shared__ __align__(16) unsigned char sm[];
-  __shared__ int nv_s, filled_s;
+  __shared__ int nv_s, filled_s, s0_s, n_s, tl_s;
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = (int)cluster.block_rank();
   unsigned char* peer = cluster.map_shared_rank(sm, rank ^ 1);
   // (few values stay live across the layer loop: the products need the registers)
   const int b = blockIdx.x >> 1, T = p.T;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, hl = (warp >> 1) & 3, r0q = 16 * (warp & 1);
-  const long Mt = (long)p.B * T, grow0 = (long)b * T;
+  const long grow0 = (long)b * T, R = p.R;
   int* kidx = reinterpret_cast<int*>(sm + SMEM_FIXED);
   bf16* Xs = (bf16*)(sm + OFF_X);
   bf16* Ys = (bf16*)(sm + OFF_Y);
@@ -283,6 +298,35 @@ decoder_fwd_kernel(const __grid_constant__ DecParams p) {
     *reinterpret_cast<uint32_t*>(peer + off) = v;
   };
 
+  if (threadIdx.x == 0) {
+    s0_s = p.toff ? p.toff[b] : (int)grow0;
+    n_s = p.toff ? p.toff[b + 1] - s0_s : T;
+    tl_s = p.tlen ? p.tlen[b] : T;
+  }
+  // pad slots [toff[B], R) of every saved bf16 tensor are zeroed (the backward's products read all R slots); a slot's
+  // 4,096 columns of one layer are one uint4 per thread
+  if (p.toff) {
+    const int c = 8 * threadIdx.x;
+    for (long sl = p.toff[p.B] + blockIdx.x; sl < R; sl += gridDim.x)
+      for (int i = 0; i < p.L; ++i) {
+        const long ro = i * R + sl;
+        bf16* dst;
+        switch (c >> 8) {
+          case 0: dst = p.X + ro * D + c; break;
+          case 1: dst = p.ctx1 + ro * D + c - 256; break;
+          case 2: dst = p.z1 + ro * D + c - 512; break;
+          case 3: dst = p.x1 + ro * D + c - 768; break;
+          case 4: dst = p.q + ro * D + c - 1024; break;
+          case 5: dst = p.ctx2 + ro * D + c - 1280; break;
+          case 6: dst = p.z2 + ro * D + c - 1536; break;
+          case 7: dst = p.x2 + ro * D + c - 1792; break;
+          case 8: dst = p.z3 + ro * D + c - 2048; break;
+          case 9: case 10: case 11: dst = p.qkv + ro * 3 * D + c - 2304; break;
+          default: dst = p.hh + ro * F + c - 3072; break;
+        }
+        *reinterpret_cast<uint4*>(dst) = make_uint4(0, 0, 0, 0);
+      }
+  }
   // cross-attention keys of the commit (the same for every layer)
   compact_keys(p.mem_mask ? p.mem_mask + (long)b * p.S : nullptr, p.S, 0, kidx, &nv_s, &filled_s,
                p.ranges ? p.ranges + 4 * b : nullptr);
@@ -296,7 +340,7 @@ decoder_fwd_kernel(const __grid_constant__ DecParams p) {
       Act<float>::load8(p.pe + (long)t * D + lane * 8, pe);
 #pragma unroll
       for (int i = 0; i < 8; ++i) v[i] += pe[i];
-      if ((t & 1) == rank) Act<bf16>::store8(p.X + (grow0 + t) * D + lane * 8, v);
+      if ((t & 1) == rank && t < n_s) Act<bf16>::store8(p.X + ((long)s0_s + t) * D + lane * 8, v);
     } else {
 #pragma unroll
       for (int i = 0; i < 8; ++i) v[i] = 0.f;
@@ -307,13 +351,14 @@ decoder_fwd_kernel(const __grid_constant__ DecParams p) {
 
   for (int i = 0; i < p.L; ++i) {
     const LayerW& w = p.w[i];
-    const long o256 = i * Mt * D;
+    const long o256 = i * R * D, s0 = s0_s;
+    const int n = n_s;
 
     // ---- masked self-attention (gnn_transformer.py:117-119): q | k | v of this CTA's heads stay local
     product<D, 1, 8, false>(Xs, w.wqkv, w.bqkv, 3 * D, rank, warp, lane,
                             [&](int t, int n, int, uint32_t v) { *reinterpret_cast<uint32_t*>(big + head_off(t, n)) = v; });
     __syncthreads();
-    copy_out(p.qkv + (i * Mt + grow0) * 3 * D, 3 * D, T, rank, warp, lane, [&](int t, int n) { return big + head_off(t, n); });
+    copy_out(p.qkv + (i * R + s0) * 3 * D, 3 * D, n, rank, warp, lane, [&](int t, int n) { return big + head_off(t, n); });
     if (warp < 8) {
       // causal over tar_mask, identity key list of the T target rows
       AttnArgs sa{};
@@ -329,19 +374,19 @@ decoder_fwd_kernel(const __grid_constant__ DecParams p) {
       ar.finish(sm + OFF_Y, peer + OFF_Y, h, T, p.st1 + (((long)i * p.B + b) * NH + h) * T * 2, lane);
     }
     cluster.sync();
-    copy_out(p.ctx1 + o256 + grow0 * D, D, T, rank, warp, lane, [&](int t, int n) { return Ys + t * LDA + gcol(n, rank); });
+    copy_out(p.ctx1 + o256 + s0 * D, D, n, rank, warp, lane, [&](int t, int n) { return Ys + t * LDA + gcol(n, rank); });
     product<D, 1, 8, false>(Ys, w.swo, w.sbo, D, rank, warp, lane,
                             [&](int t, int, int c, uint32_t v) { to_both(OFF_Z + (t * LDA + c) * 2, v); });
     cluster.sync();
-    ln_rows(sm, OFF_Z, OFF_X, OFF_X1, w.slw, w.slb, p.z1 + o256, p.x1 + o256, p.ls1 + 2 * i * Mt, Mt, grow0, T,
-            p.p_drop, p.seed, p.seed_ctr, p.stream_id + 8 * i + 0, rank, warp, lane);
+    ln_rows(sm, OFF_Z, OFF_X, OFF_X1, w.slw, w.slb, p.z1 + o256, p.x1 + o256, p.ls1 + 2 * i * R, R, grow0, s0, T, n,
+            T, false, p.p_drop, p.seed, p.seed_ctr, p.stream_id + 8 * i + 0, rank, warp, lane);
     __syncthreads();
 
     // ---- cross-attention over the encoder memory (gnn_transformer.py:120): q of this CTA's heads stays local
     product<D, 1, 8, false>((const bf16*)(sm + OFF_X1), w.cwq, w.cbq, D, rank, warp, lane,
                             [&](int t, int n, int, uint32_t v) { *reinterpret_cast<uint32_t*>(big + head_off(t, n)) = v; });
     __syncthreads();
-    copy_out(p.q + o256 + grow0 * D, D, T, rank, warp, lane, [&](int t, int n) { return big + head_off(t, n); });
+    copy_out(p.q + o256 + s0 * D, D, n, rank, warp, lane, [&](int t, int n) { return big + head_off(t, n); });
     if (warp < 8) {
       const int h = 4 * rank + hl;
       const int nv = nv_s, nblk = (nv + CKB - 1) / CKB;
@@ -374,12 +419,12 @@ decoder_fwd_kernel(const __grid_constant__ DecParams p) {
       ar.finish(sm + OFF_Y, peer + OFF_Y, h, T, p.st2 + (((long)i * p.B + b) * NH + h) * T * 2, lane);
     }
     cluster.sync();
-    copy_out(p.ctx2 + o256 + grow0 * D, D, T, rank, warp, lane, [&](int t, int n) { return Ys + t * LDA + gcol(n, rank); });
+    copy_out(p.ctx2 + o256 + s0 * D, D, n, rank, warp, lane, [&](int t, int n) { return Ys + t * LDA + gcol(n, rank); });
     product<D, 1, 8, false>(Ys, w.cwo, w.cbo, D, rank, warp, lane,
                             [&](int t, int, int c, uint32_t v) { to_both(OFF_Z + (t * LDA + c) * 2, v); });
     cluster.sync();
-    ln_rows(sm, OFF_Z, OFF_X1, OFF_X2, w.clw, w.clb, p.z2 + o256, p.x2 + o256, p.ls2 + 2 * i * Mt, Mt, grow0, T,
-            p.p_drop, p.seed, p.seed_ctr, p.stream_id + 8 * i + 1, rank, warp, lane);
+    ln_rows(sm, OFF_Z, OFF_X1, OFF_X2, w.clw, w.clb, p.z2 + o256, p.x2 + o256, p.ls2 + 2 * i * R, R, grow0, s0, T, n,
+            T, false, p.p_drop, p.seed, p.seed_ctr, p.stream_id + 8 * i + 1, rank, warp, lane);
     __syncthreads();
 
     // ---- feed-forward (gnn_transformer.py:170-174)
@@ -387,38 +432,42 @@ decoder_fwd_kernel(const __grid_constant__ DecParams p) {
     product<D, 2, 4, true>((const bf16*)(sm + OFF_X2), w.w1, w.b1, F, rank, warp, lane,
                            [&](int t, int, int c, uint32_t v) { to_both(OFF_BIG + (t * LDF + c) * 2, v); });
     cluster.sync();
-    copy_out(p.hh + (i * Mt + grow0) * F, F, T, rank, warp, lane, [&](int t, int n) { return Hs + t * LDF + gcol(n, rank); });
+    copy_out(p.hh + (i * R + s0) * F, F, n, rank, warp, lane, [&](int t, int n) { return Hs + t * LDF + gcol(n, rank); });
     product<F, 1, 8, false>(Hs, w.w2, w.b2, D, rank, warp, lane,
                             [&](int t, int, int c, uint32_t v) { to_both(OFF_Z + (t * LDA + c) * 2, v); });
     cluster.sync();
-    ln_rows(sm, OFF_Z, OFF_X2, OFF_X, w.flw, w.flb, p.z3 + o256, p.X + o256 + Mt * D, p.ls3 + 2 * i * Mt, Mt, grow0, T,
-            p.p_drop, p.seed, p.seed_ctr, p.stream_id + 8 * i + 2, rank, warp, lane);
+    const bool last = i == p.L - 1;
+    ln_rows(sm, OFF_Z, OFF_X2, OFF_X, w.flw, w.flb, p.z3 + o256, last ? p.out : p.X + o256 + R * D, p.ls3 + 2 * i * R, R,
+            grow0, s0, T, n, tl_s, last, p.p_drop, p.seed, p.seed_ctr, p.stream_id + 8 * i + 2, rank, warp, lane);
     __syncthreads();
   }
 }
 
 }  // namespace
 
-extern "C" int fira_decoder_fwd(const int* tar, const float* dec_emb, const float* pos_table,
-                                const unsigned char* tar_mask, const void* kv, long ldkv, const unsigned char* mem_mask,
-                                const int* ranges, int S, const void* const* layer_ptrs, int L, void* X, void* qkv,
-                                void* ctx1, float* st1, void* z1, float* ls1, void* x1, void* q, void* ctx2, float* st2,
-                                void* z2, float* ls2, void* x2, void* hh, void* z3, float* ls3, int B, int T,
-                                float p_drop, uint64_t seed, const uint64_t* seed_ctr, uint32_t stream_id,
-                                void* stream) {
+extern "C" int fira_decoder_fwd_rows(const int* tar, const float* dec_emb, const float* pos_table,
+                                     const unsigned char* tar_mask, const void* kv, long ldkv,
+                                     const unsigned char* mem_mask, const int* ranges, int S,
+                                     const void* const* layer_ptrs, int L, void* X, void* out, void* qkv, void* ctx1,
+                                     float* st1, void* z1, float* ls1, void* x1, void* q, void* ctx2, float* st2,
+                                     void* z2, float* ls2, void* x2, void* hh, void* z3, float* ls3, const int* tlen,
+                                     const int* toff, long R, int B, int T, float p_drop, uint64_t seed,
+                                     const uint64_t* seed_ctr, uint32_t stream_id, void* stream) {
   FIRA_CHECK_ARG(B > 0 && T > 0 && T <= TP, FIRA_ERR_SHAPE, "decoder_fwd: B %d, T %d (T <= 32)", B, T);
   FIRA_CHECK_ARG(L > 0 && L <= MAX_LAYERS, FIRA_ERR_SHAPE, "decoder_fwd: %d layers (1..%d)", L, MAX_LAYERS);
   FIRA_CHECK_ARG(S > 0, FIRA_ERR_SHAPE, "decoder_fwd: S %d", S);
+  FIRA_CHECK_ARG(!tlen == !toff && (toff ? R > 0 && R <= (long)B * T : R == (long)B * T), FIRA_ERR_ARG,
+                 "decoder_fwd: tlen and toff both or neither, 0 < R <= B*T (R = B*T without them)");
   FIRA_CHECK_ARG(mem_mask || ranges, FIRA_ERR_ARG, "decoder_fwd: mem_mask may only be NULL with ranges");
   FIRA_CHECK_ARG(layer_ptrs && tar && dec_emb && pos_table && tar_mask && kv, FIRA_ERR_ARG, "decoder_fwd: null input");
   FIRA_CHECK_ARG(fira_aligned16(kv) && ldkv % 8 == 0 && ldkv >= (long)L * 2 * D, FIRA_ERR_ALIGN,
                  "decoder_fwd: kv must be 16-B aligned with ldkv a multiple of 8 and >= L*512");
-  void* outs[] = {X, qkv, ctx1, z1, x1, q, ctx2, z2, x2, hh, z3};
+  void* outs[] = {X, out, qkv, ctx1, z1, x1, q, ctx2, z2, x2, hh, z3};
   for (void* o : outs) FIRA_CHECK_ARG(o && fira_aligned16(o), FIRA_ERR_ALIGN, "decoder_fwd: outputs must be 16-B aligned");
   FIRA_CHECK_ARG(st1 && ls1 && st2 && ls2 && ls3, FIRA_ERR_ARG, "decoder_fwd: null statistics");
   DecParams p{tar, dec_emb, pos_table, tar_mask, (const bf16*)kv, ldkv, mem_mask, ranges, S,
-              (bf16*)X, (bf16*)qkv, (bf16*)ctx1, st1, (bf16*)z1, ls1, (bf16*)x1,
-              (bf16*)q, (bf16*)ctx2, st2, (bf16*)z2, ls2, (bf16*)x2, (bf16*)hh, (bf16*)z3, ls3,
+              (bf16*)X, (bf16*)out, (bf16*)qkv, (bf16*)ctx1, st1, (bf16*)z1, ls1, (bf16*)x1,
+              (bf16*)q, (bf16*)ctx2, st2, (bf16*)z2, ls2, (bf16*)x2, (bf16*)hh, (bf16*)z3, ls3, tlen, toff, R,
               B, T, L, 1.f / sqrtf((float)DH), p_drop, seed, seed_ctr, stream_id, {}};
   for (int i = 0; i < L; ++i) {
     const void* const* t = layer_ptrs + 18 * i;
@@ -433,4 +482,18 @@ extern "C" int fira_decoder_fwd(const int* tar, const float* dec_emb, const floa
   launch_k(decoder_fwd_kernel, dim3(2 * B), dim3(NTHR), smem, (cudaStream_t)stream, p);
   FIRA_CHECK_LAUNCH("fira_decoder_fwd");
   return FIRA_OK;
+}
+
+extern "C" int fira_decoder_fwd(const int* tar, const float* dec_emb, const float* pos_table,
+                                const unsigned char* tar_mask, const void* kv, long ldkv, const unsigned char* mem_mask,
+                                const int* ranges, int S, const void* const* layer_ptrs, int L, void* X, void* qkv,
+                                void* ctx1, float* st1, void* z1, float* ls1, void* x1, void* q, void* ctx2, float* st2,
+                                void* z2, float* ls2, void* x2, void* hh, void* z3, float* ls3, int B, int T,
+                                float p_drop, uint64_t seed, const uint64_t* seed_ctr, uint32_t stream_id,
+                                void* stream) {
+  FIRA_CHECK_ARG(X && L > 0 && B > 0 && T > 0, FIRA_ERR_ARG, "decoder_fwd: arguments");
+  void* out = (bf16*)X + (long)L * B * T * D;
+  return fira_decoder_fwd_rows(tar, dec_emb, pos_table, tar_mask, kv, ldkv, mem_mask, ranges, S, layer_ptrs, L, X, out,
+                               qkv, ctx1, st1, z1, ls1, x1, q, ctx2, st2, z2, ls2, x2, hh, z3, ls3, nullptr, nullptr,
+                               (long)B * T, B, T, p_drop, seed, seed_ctr, stream_id, stream);
 }

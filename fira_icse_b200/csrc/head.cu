@@ -224,6 +224,37 @@ __global__ void __launch_bounds__(kRowsThreads) vocab_rows_kernel(const int* __r
   }
 }
 
+// Live target rows of a training batch, the rows before each commit's last non-zero shifted label: tlen[b] = 1 + that
+// t (0 without one); toff[b] = the commit's first slot, slots in row order; trows[slot] = b T + t, -1 in the slots past
+// the count.  A commit past cap gets the slots left (toff clamps to cap), so toff[b + 1] - toff[b] < tlen[b] flags it.
+// One CTA, one thread per commit.
+__global__ void __launch_bounds__(kRowsThreads) target_rows_kernel(const int* __restrict__ label, int B, int T,
+                                                                   int* __restrict__ tlen, int* __restrict__ toff,
+                                                                   int* __restrict__ trows, int cap) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  __shared__ int warp_sum_s[kRowsThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, b = threadIdx.x;
+  int n = 0;
+  if (b < B)
+    for (int t = T - 1; t >= 0; --t)
+      if (label[(long)b * T + t] != 0) { n = t + 1; break; }
+  int incl = n;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
+  if (lane == 31) warp_sum_s[warp] = incl;
+  for (int s = threadIdx.x; s < cap; s += kRowsThreads) trows[s] = -1;
+  __syncthreads();
+  int off = incl - n;
+  for (int w = 0; w < warp; ++w) off += warp_sum_s[w];
+  if (b < B) {
+    const int s0 = min(off, cap), s1 = min(off + n, cap);
+    tlen[b] = n;
+    toff[b] = s0;
+    if (b == B - 1) toff[B] = s1;
+    for (int s = s0; s < s1; ++s) trows[s] = b * T + (s - off);
+  }
+}
+
 // dst[i] = idx[i] >= 0 ? src[idx[i]] : 0 over rows of `width` elements (width % 8 == 0); one warp per row
 template <typename T>
 __global__ void __launch_bounds__(256) gather_rows_kernel(const T* __restrict__ src, long ld_src,
@@ -1145,6 +1176,14 @@ int fira_vocab_rows(const int* label, long rows, int V, int* vslot, int* vrows, 
   FIRA_CHECK_ARG(label && vslot && vrows && rows >= 0 && V > 0 && cap >= 0, FIRA_ERR_ARG, "vocab_rows: arguments");
   launch_k(vocab_rows_kernel, dim3(1), dim3(kRowsThreads), 0, (cudaStream_t)stream, label, rows, V, vslot, vrows, cap);
   FIRA_CHECK_LAUNCH("fira_vocab_rows");
+  return FIRA_OK;
+}
+
+int fira_target_rows(const int* label, int B, int T, int* tlen, int* toff, int* trows, int cap, void* stream) {
+  FIRA_CHECK_ARG(label && tlen && toff && trows && B > 0 && B <= kRowsThreads && T > 0 && cap >= 0, FIRA_ERR_ARG,
+                 "target_rows: arguments (B <= %d)", kRowsThreads);
+  launch_k(target_rows_kernel, dim3(1), dim3(kRowsThreads), 0, (cudaStream_t)stream, label, B, T, tlen, toff, trows, cap);
+  FIRA_CHECK_LAUNCH("fira_target_rows");
   return FIRA_OK;
 }
 

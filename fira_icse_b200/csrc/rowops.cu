@@ -95,12 +95,15 @@ __global__ void embed_rows_kernel(const int* __restrict__ ids, const float* __re
     Act<T>::store8(out + r * D + lane * 8, v);
   }
 }
+// rmap (may be NULL): row r of g is row rmap[r] of ids, -1 = no row
 template <typename T>
-__global__ void embed_rows_bwd_kernel(const int* __restrict__ ids, const T* __restrict__ g, float* __restrict__ d_emb,
-                                      long rows) {
+__global__ void embed_rows_bwd_kernel(const int* __restrict__ ids, const int* __restrict__ rmap, const T* __restrict__ g,
+                                      float* __restrict__ d_emb, long rows) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
   const int lane = threadIdx.x & 31;
   for (long r = (long)blockIdx.x * ROWS_PER_CTA + (threadIdx.x >> 5); r < rows; r += (long)gridDim.x * ROWS_PER_CTA) {
+    const long src = rmap ? rmap[r] : r;
+    if (src < 0) continue;
     float v[8];
     Act<T>::load8(g + r * D + lane * 8, v);
     // rows whose gradient is exactly zero (padded target positions: no loss, masked as keys) add nothing; skipping
@@ -109,7 +112,7 @@ __global__ void embed_rows_bwd_kernel(const int* __restrict__ ids, const T* __re
 #pragma unroll
     for (int i = 0; i < 8; ++i) nz |= v[i] != 0.f;
     if (!__any_sync(0xffffffffu, nz)) continue;
-    float* o = d_emb + (long)ids[r] * D + lane * 8;
+    float* o = d_emb + (long)ids[src] * D + lane * 8;
     // two 16-byte vector reductions per lane (red.global.add.v4.f32, sm_90+) instead of eight scalar ones
     atomicAdd(reinterpret_cast<float4*>(o), make_float4(v[0], v[1], v[2], v[3]));
     atomicAdd(reinterpret_cast<float4*>(o + 4), make_float4(v[4], v[5], v[6], v[7]));
@@ -165,7 +168,7 @@ __global__ void ln_bwd_kernel(const T* __restrict__ doutA, const T* __restrict__
                               const float* __restrict__ rstd_in, const float* __restrict__ gamma, T* __restrict__ d_z,
                               T* __restrict__ d_resid, int d_resid_accum, float* __restrict__ d_gamma,
                               float* __restrict__ d_beta, long rows, float p_drop, uint64_t seed,
-                              const uint64_t* __restrict__ seed_ctr, uint32_t stream_id) {
+                              const uint64_t* __restrict__ seed_ctr, uint32_t stream_id, const int* __restrict__ rmap) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
   if (seed_ctr) seed += *seed_ctr;
   __shared__ __align__(16) float red[2][ROWS_PER_CTA][D];
@@ -176,13 +179,21 @@ __global__ void ln_bwd_kernel(const T* __restrict__ doutA, const T* __restrict__
   for (int i = 0; i < 8; ++i) { dg[i] = 0.f; db[i] = 0.f; }
   const float keep_scale = p_drop > 0.f ? 1.f / (1.f - p_drop) : 1.f;
   for (long r = (long)blockIdx.x * ROWS_PER_CTA + warp; r < rows; r += (long)gridDim.x * ROWS_PER_CTA) {
+    const long pr = rmap ? rmap[r] : r;            // the row the forward's dropout mask was drawn for
     float y[8], x[8], go[8];
+    if (pr < 0) {                                  // pad slot: zero gradients, nothing to d_gamma / d_beta
+#pragma unroll
+      for (int i = 0; i < 8; ++i) y[i] = 0.f;
+      Act<T>::store8(d_z + r * D + lane * 8, y);
+      if (d_resid && !d_resid_accum) Act<T>::store8(d_resid + r * D + lane * 8, y);
+      continue;
+    }
     Act<T>::load8(z + r * D + lane * 8, y);
     Act<T>::load8(resid + r * D + lane * 8, x);
     Act<T>::load8((r < split ? doutA : doutB) + r * D + lane * 8, go);
     uint32_t m = 0xffu;
     if (p_drop > 0.f) {
-      m = dropout_keep8(seed, stream_id, (uint64_t)r * 32 + lane, p_drop);
+      m = dropout_keep8(seed, stream_id, (uint64_t)pr * 32 + lane, p_drop);
 #pragma unroll
       for (int i = 0; i < 8; ++i) y[i] = ((m >> i) & 1) ? y[i] * keep_scale : 0.f;
     }
@@ -571,9 +582,15 @@ int fira_embed_rows_fwd(const int* ids, const float* emb, const float* pos_table
 }
 
 int fira_embed_rows_bwd(const int* ids, const void* d_out, float* d_emb, long rows, int dim, int dtype, void* stream) {
+  return fira_embed_rows_bwd_rows(ids, nullptr, d_out, d_emb, rows, dim, dtype, stream);
+}
+
+int fira_embed_rows_bwd_rows(const int* ids, const int* rows_map, const void* d_out, float* d_emb, long rows, int dim,
+                             int dtype, void* stream) {
   FIRA_CHECK_ARG(dim == D, FIRA_ERR_SHAPE, "embed_rows_bwd: dim %d != 256", dim);
-  DISPATCH_T(dtype, launch_k(embed_rows_bwd_kernel<T>, dim3(row_grid(rows)), dim3(CTA), 0, (cudaStream_t)stream, ids, (const T*)d_out,
-                                                                                             d_emb, rows);)
+  if (rows == 0) return FIRA_OK;
+  DISPATCH_T(dtype, launch_k(embed_rows_bwd_kernel<T>, dim3(row_grid(rows)), dim3(CTA), 0, (cudaStream_t)stream, ids,
+                             rows_map, (const T*)d_out, d_emb, rows);)
   FIRA_CHECK_LAUNCH("fira_embed_rows_bwd");
   return FIRA_OK;
 }
@@ -596,13 +613,22 @@ int fira_ln_residual_bwd(const void* d_outA, const void* d_outB, long split, con
                          const float* mean, const float* rstd, const float* gamma, void* d_z, void* d_resid,
                          int d_resid_accum, float* d_gamma, float* d_beta, long rows, int dim, float p_drop,
                          uint64_t seed, const uint64_t* seed_ctr, uint32_t stream_id, int dtype, void* stream) {
+  return fira_ln_residual_bwd_rows(d_outA, d_outB, split, z, resid, mean, rstd, gamma, d_z, d_resid, d_resid_accum,
+                                   d_gamma, d_beta, nullptr, rows, dim, p_drop, seed, seed_ctr, stream_id, dtype, stream);
+}
+
+int fira_ln_residual_bwd_rows(const void* d_outA, const void* d_outB, long split, const void* z, const void* resid,
+                              const float* mean, const float* rstd, const float* gamma, void* d_z, void* d_resid,
+                              int d_resid_accum, float* d_gamma, float* d_beta, const int* rows_map, long rows, int dim,
+                              float p_drop, uint64_t seed, const uint64_t* seed_ctr, uint32_t stream_id, int dtype,
+                              void* stream) {
   FIRA_CHECK_ARG(dim == D, FIRA_ERR_SHAPE, "ln_residual_bwd: dim %d != 256", dim);
   if (rows == 0) return FIRA_OK;
   long g = (rows + ROWS_PER_CTA - 1) / ROWS_PER_CTA;
   int grid = (int)(g < (long)fira_num_sms() * 4 ? g : (long)fira_num_sms() * 4);   // few CTAs -> few d_gamma/d_beta atomics
   DISPATCH_T(dtype, launch_k(ln_bwd_kernel<T>, dim3(grid), dim3(CTA), 0, (cudaStream_t)stream, 
       (const T*)d_outA, (const T*)d_outB, split, (const T*)z, (const T*)resid, mean, rstd, gamma, (T*)d_z,
-      (T*)d_resid, d_resid_accum, d_gamma, d_beta, rows, p_drop, seed, seed_ctr, stream_id);)
+      (T*)d_resid, d_resid_accum, d_gamma, d_beta, rows, p_drop, seed, seed_ctr, stream_id, rows_map);)
   FIRA_CHECK_LAUNCH("fira_ln_residual_bwd");
   return FIRA_OK;
 }

@@ -364,7 +364,7 @@ class PackedBatchLoader:
                              "bounds-check")
         self.multiples = (0, 0, 0) if multiples is None else tuple(int(m) for m in multiples)
         self.max_shapes = max_shapes
-        self.shapes = {}
+        self.dims_used = {}            # every batch shape emitted (packed: Rc, Rs, Ra, S, Rv, Rt) -> batches
         self.lens = (dataset.diff_len, dataset.sub_token_len, dataset.ast_change_len)
         self.msg_len = dataset.msg_len
         d = dataset.d
@@ -380,7 +380,7 @@ class PackedBatchLoader:
         self.n_slots = max(2, int(prefetch) + 1)
         # packed=True: per-commit packed batches (packed.PackedBatch, SURVEY.md 8f rank 4) instead of batch-trimmed padded
         # ones; row_buckets = rounding of (code rows, sub-token rows, AST rows, memory rows of one commit); the
-        # vocabulary-label target rows round to packed.VOCAB_ROW_BUCKET, and max_shapes bounds the shapes with them
+        # vocabulary-label and live target rows round to packed.VOCAB_ROW_BUCKET, and max_shapes bounds the shapes with them
         self.packed = bool(packed)
         if self.packed:
             from . import packed as P
@@ -396,17 +396,26 @@ class PackedBatchLoader:
         return n // self.B if self.drop_last else -(-n // self.B)
 
     # ------------------------------------------------------------------ shape policy
+    @property
+    def shapes(self):
+        """batches per emitted (code, sub-token, AST) lengths, or packed (Rc, Rs, Ra, S, Rv) rows"""
+        out = {}
+        for k, n in self.dims_used.items():
+            out[k[:5]] = out.get(k[:5], 0) + n
+        return out
+
     def _choose_dims(self, need):
         need = tuple(int(x) for x in need)
-        if need in self.shapes or self.max_shapes is None or len(self.shapes) < self.max_shapes:
-            self.shapes[need] = self.shapes.get(need, 0) + 1
+        used = self.dims_used
+        if need in used or self.max_shapes is None or len(used) < self.max_shapes:
+            used[need] = used.get(need, 0) + 1
             return need
-        fits = [s for s in self.shapes if all(a >= b for a, b in zip(s, need))]
+        fits = [s for s in used if all(a >= b for a, b in zip(s, need))]
         if self.packed and not fits:                     # nothing emitted so far holds it: a new shape after all
-            self.shapes[need] = 1
+            used[need] = 1
             return need
         best = min(fits, key=sum) if fits else self.lens
-        self.shapes[best] = self.shapes.get(best, 0) + 1
+        used[best] = used.get(best, 0) + 1
         return best
 
     # ------------------------------------------------------------------ one batch

@@ -56,7 +56,7 @@ class _CapturedPacked:
             return torch.zeros(t.shape if n is None else (n,), dtype=t.dtype, device=dev)
         t = {k: z(getattr(pb, k)) for k in PackedBatch.FIELDS if k not in ("col", "val")}
         t["col"], t["val"] = z(pb.col, cap), z(pb.val, cap)
-        self.pb = PackedBatch(pb.B, pb.Rc, pb.Rs, pb.Ra, pb.S, pb.T, cap, pb.chunks, pb.Rv, **t)
+        self.pb = PackedBatch(pb.B, pb.Rc, pb.Rs, pb.Ra, pb.S, pb.T, cap, pb.chunks, pb.Rv, pb.Rt, **t)
         self.B, self.cap = pb.B, cap
         self.graph = None
         self.grads = None

@@ -119,8 +119,8 @@ class TransModel(nn.Module):
         memory = self.encoder.encode_memory_packed(pb)                       # [1, Rc + Rs, D]
         if self._memory_hook is not None:
             memory = self._memory_hook(memory)
-        dec = self.decoder(pb.tar, memory, pb.mem_mask, pb.tar_mask, packed=pb)
         want_ids = stage != "train"
+        dec = self.decoder(pb.tar, memory, pb.mem_mask, pb.tar_mask, packed=pb, label=None if want_ids else pb.label)
         loss_sum, _, ids = ops.HeadFn.apply(want_ids, bf16, pf_head, memory, dec, pb.mem_mask, pb.label.view(-1),
                                             self.out_fc.weight, self.out_fc.bias, *self.copy_net.flat_params(), pb)
         if stage == "train":

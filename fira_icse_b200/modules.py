@@ -251,14 +251,17 @@ class Decoder(nn.Module):
         if dev.type == "cuda":
             self._prefetched = ops.prefetch_decoder(bool(getattr(self, "bf16", False)), self._flat(), dev)
 
-    def forward(self, output_token, input_em, sou_mask, tar_mask_pad, packed=None):
+    def forward(self, output_token, input_em, sou_mask, tar_mask_pad, packed=None, label=None):
         """packed: a packed.PackedBatch -- `input_em` is then the [1, Rc + Rs, D] memory-row matrix of
-        Encoder.encode_memory_packed and `sou_mask` the [B, S] mask over each commit's own memory rows"""
+        Encoder.encode_memory_packed and `sou_mask` the [B, S] mask over each commit's own memory rows.
+        label (packed training batches): the shifted labels [B, T]; the bf16 mode then computes the gradient on the rows
+        before each commit's last label only, and the output rows after it are zero (ops.DecoderFn)"""
         dev = self.embedding.weight.device
         if self.pos_encode.device != dev:
             self.pos_encode = self.pos_encode.to(dev)
         cfg = _run_cfg(self)
-        cfg.update(p_dec=self.attention_list[0].dropout.p, prefetch=getattr(self, "_prefetched", None), packed=packed)
+        cfg.update(p_dec=self.attention_list[0].dropout.p, prefetch=getattr(self, "_prefetched", None), packed=packed,
+                   label=None if label is None else _i32(label))
         self._prefetched = None
         lp = self._flat()
         return ops.DecoderFn.apply(cfg, _i32(output_token), input_em, _u8(sou_mask), _u8(tar_mask_pad),

@@ -246,17 +246,19 @@ class Prec:
              _ptr(stats), _ptr(stats, rows), rows, D, float(p), seed, _ptr(self.seed_ctr), sid, self.code, _stream())
         return stats
 
-    def ln_bwd(self, dA, dB, split, z, resid, stats, gamma, rows, p, seed, sid, d_resid=None, accum=False, beta=None):
+    def ln_bwd(self, dA, dB, split, z, resid, stats, gamma, rows, p, seed, sid, d_resid=None, accum=False, beta=None,
+               rows_map=None):
         """beta: the LayerNorm bias parameter; with (gamma, beta) re-homed back to back by optim.FlatAdam their
-        gradients are accumulated straight into its flat gradient buffer"""
+        gradients are accumulated straight into its flat gradient buffer.  rows_map: the rows are slots of
+        fira_target_rows (dropout mask of row rows_map[r], zeros for a pad slot)"""
         dz = torch.empty_like(z)
         if d_resid is None:
             d_resid = torch.empty_like(z)
         dgb = _gdest((gamma, beta), (2, D), zero=True) if beta is not None else \
             torch.zeros((2, D), dtype=torch.float32, device=z.device)
-        call("fira_ln_residual_bwd", _ptr(dA), _ptr(dB), split, _ptr(z), _ptr(resid), _ptr(stats), _ptr(stats, rows),
-             _ptr(gamma), _ptr(dz), _ptr(d_resid), int(accum), _ptr(dgb), _ptr(dgb, D), rows, D, float(p), seed,
-             _ptr(self.seed_ctr), sid, self.code, _stream())
+        call("fira_ln_residual_bwd_rows", _ptr(dA), _ptr(dB), split, _ptr(z), _ptr(resid), _ptr(stats),
+             _ptr(stats, rows), _ptr(gamma), _ptr(dz), _ptr(d_resid), int(accum), _ptr(dgb), _ptr(dgb, D), _ptr(rows_map),
+             rows, D, float(p), seed, _ptr(self.seed_ctr), sid, self.code, _stream())
         return dz, d_resid, dgb[0], dgb[1]
 
 
@@ -620,7 +622,12 @@ DEC_LAYER_PARAMS = 26   # self: Wq bq Wk bk Wv bv Wo bo lnw lnb ; cross: same 10
 
 class DecoderFn(torch.autograd.Function):
     """gnn_transformer.py:108-122: embedding + PE, 6 x [self-attn, cross-attn, FFN], all post-LN.
-    The 12 cross-attention K/V projections of the (layer-invariant) memory run as ONE GEMM."""
+    The 12 cross-attention K/V projections of the (layer-invariant) memory run as ONE GEMM.
+
+    cfg["label"] (the shifted labels [B, T] of a packed bf16 training batch, else absent): the backward runs on the live
+    target rows alone, the rows before each commit's last label (fira_target_rows, at most pk.Rt).  No later row carries
+    a loss, and causal self-attention never lets a live row read one, so they change neither the loss nor a gradient;
+    their output rows are zero."""
 
     @staticmethod
     def forward(ctx, cfg, tar, memory, mem_mask, tar_mask, pos_table, dec_emb, *lp):
@@ -653,24 +660,33 @@ class DecoderFn(torch.autograd.Function):
         ldkv = L * 2 * D
         KV = pr.linear(memory.view(Ms, D), Wkv, bkv)                                              # [Ms, L*512]
         if pr.bf16:
-            # the whole stack in ONE launch (csrc/decoder_fwd.cu): every tensor the backward reads, leading dim = layer
+            # the whole stack in ONE launch (csrc/decoder_fwd.cu): every tensor the backward reads, leading dim = layer,
+            # R rows each: the live-row slots of a packed training batch (fira_target_rows), else every row
+            label = cfg.get("label")
+            rmap = None
+            R = Mt
+            if label is not None and pk is not None:
+                R = pk.Rt
+                rmap = torch.empty((2 * B + 1 + R,), dtype=torch.int32, device=dev)      # tlen | toff | trows
+                call("fira_target_rows", _ptr(label), B, T, _ptr(rmap), _ptr(rmap, B), _ptr(rmap, 2 * B + 1), R, st)
             bf = dict(dtype=torch.bfloat16, device=dev)
-            Xs = torch.empty((L + 1, Mt, D), **bf)                 # each layer's input, then the output
-            QKV, Hh = torch.empty((L, Mt, 3 * D), **bf), torch.empty((L, Mt, 4 * D), **bf)
-            ctx1, Z1, X1, Q, ctx2, Z2, X2, Z3 = torch.empty((8, L, Mt, D), **bf)
+            Xs = torch.empty((L, R, D), **bf)                      # each layer's input
+            out = torch.empty((Mt, D), **bf)
+            QKV, Hh = torch.empty((L, R, 3 * D), **bf), torch.empty((L, R, 4 * D), **bf)
+            ctx1, Z1, X1, Q, ctx2, Z2, X2, Z3 = torch.empty((8, L, R, D), **bf)
             st1, st2 = torch.empty((2, L, B, H, T, 2), **f32)
-            ls1, ls2, ls3 = torch.empty((3, L, 2, Mt), **f32)
-            call("fira_decoder_fwd", _ptr(tar), _ptr(dec_emb), _ptr(pos_table), _ptr(tar_mask), _ptr(KV), ldkv,
+            ls1, ls2, ls3 = torch.empty((3, L, 2, R), **f32)
+            call("fira_decoder_fwd_rows", _ptr(tar), _ptr(dec_emb), _ptr(pos_table), _ptr(tar_mask), _ptr(KV), ldkv,
                  _ptr(mem_mask), _ptr(pk.ranges) if pk is not None else None, S, ctypes.addressof(pf.layer_table), L,
-                 _ptr(Xs), _ptr(QKV), _ptr(ctx1), _ptr(st1), _ptr(Z1), _ptr(ls1), _ptr(X1), _ptr(Q), _ptr(ctx2),
-                 _ptr(st2), _ptr(Z2), _ptr(ls2), _ptr(X2), _ptr(Hh), _ptr(Z3), _ptr(ls3), B, T, float(p), seed,
-                 _ptr(pr.seed_ctr), cfg["stream_base"] + 64, st)
+                 _ptr(Xs), _ptr(out), _ptr(QKV), _ptr(ctx1), _ptr(st1), _ptr(Z1), _ptr(ls1), _ptr(X1), _ptr(Q),
+                 _ptr(ctx2), _ptr(st2), _ptr(Z2), _ptr(ls2), _ptr(X2), _ptr(Hh), _ptr(Z3), _ptr(ls3), _ptr(rmap),
+                 _ptr(rmap, B), R, B, T, float(p), seed, _ptr(pr.seed_ctr), cfg["stream_base"] + 64, st)
             ctx.saved = [(Xs[i], qkv_layers[i][0], QKV[i], ctx1[i], st1[i], Z1[i], ls1[i], X1[i], Q[i], ctx2[i], st2[i],
                           Z2[i], ls2[i], X2[i], Hh[i], Z3[i], ls3[i]) for i in range(L)]
             ctx.wcache = pr.wcache
-            ctx.misc = (cfg, tar, memory, mem_mask, tar_mask, KV, Wkv, B, T, S, p, mem_dtype, Ms)
+            ctx.misc = (cfg, tar, memory, mem_mask, tar_mask, KV, Wkv, B, T, S, p, mem_dtype, Ms, R, rmap)
             ctx.save_for_backward(dec_emb, *lp)
-            return Xs[L].view(B, T, D)
+            return out.view(B, T, D)
         saved = []
         for i in range(L):
             (sWq, sbq, sWk, sbk, sWv, sbv, sWo, sbo, slw, slb,
@@ -706,13 +722,14 @@ class DecoderFn(torch.autograd.Function):
             X = X3
         ctx.saved = saved
         ctx.wcache = pr.wcache
-        ctx.misc = (cfg, tar, memory, mem_mask, tar_mask, KV, Wkv, B, T, S, p, mem_dtype, Ms)
+        ctx.misc = (cfg, tar, memory, mem_mask, tar_mask, KV, Wkv, B, T, S, p, mem_dtype, Ms, Mt, None)
         ctx.save_for_backward(dec_emb, *lp)
         return X.view(B, T, D)
 
     @staticmethod
     def backward(ctx, d_out):
-        cfg, tar, memory, mem_mask, tar_mask, KV, Wkv, B, T, S, p, mem_dtype, Ms = ctx.misc
+        # R rows per saved tensor; rmap = tlen [B] | toff [B+1] | trows [R] of the live-row slots, or None (R = B*T)
+        cfg, tar, memory, mem_mask, tar_mask, KV, Wkv, B, T, S, p, mem_dtype, Ms, R, rmap = ctx.misc
         dec_emb, *lp = ctx.saved_tensors
         Mt = B * T
         pk = cfg.get("packed")
@@ -723,6 +740,12 @@ class DecoderFn(torch.autograd.Function):
         st = _stream()
         ldkv = L * 2 * D
         dX = d_out.contiguous().to(pr.tdt).view(Mt, D)
+        toff = trows = None
+        if rmap is not None:
+            toff, trows = rmap[B:2 * B + 1], rmap[2 * B + 1:]
+            dXs = pr.empty((R, D), dev)
+            call("fira_gather_rows", _ptr(dX), D, _ptr(trows), _ptr(dXs), D, R, D, pr.code, st)
+            dX = dXs
         dKV = pr.empty((Ms, ldkv), dev)
         if pk is not None:          # the attention kernels write the rows of every commit; the segment padding stays
             call("fira_zero_pad_rows", _ptr(dKV), ldkv, ldkv, _ptr(pk.off), B, pk.Rc, pk.Rs, pr.code, st)
@@ -736,23 +759,27 @@ class DecoderFn(torch.autograd.Function):
             X, Wqkv, QKV, ctx1, st1, Z1, ls1, X1, Q, ctx2, st2, Z2, ls2, X2, Hh, Z3, ls3 = ctx.saved[i]
             sid = cfg["stream_base"] + 64 + i * 8
             # ---- FFN
-            dZ3, dX2, d_flw, d_flb = pr.ln_bwd(dX, dX, Mt, Z3, X2, ls3, flw, Mt, p, seed, sid + 2, beta=flb)
+            dZ3, dX2, d_flw, d_flb = pr.ln_bwd(dX, dX, R, Z3, X2, ls3, flw, R, p, seed, sid + 2, beta=flb, rows_map=trows)
             with fork(dZ3, Hh):
                 d_fb2 = _gdest(fb2, (D,), zero=True)
-                d_fW2 = pr.linear_dw(dZ3, D, Hh, F, Mt, D, F, out=_gdest(fW2, (D, F)), dbias=d_fb2)
-            dHh = pr.linear_dx_relu(dZ3, D, fW2, Mt, Hh)                  # [Mt, 1024], relu backward in the epilogue
+                d_fW2 = pr.linear_dw(dZ3, D, Hh, F, R, D, F, out=_gdest(fW2, (D, F)), dbias=d_fb2)
+            dHh = pr.linear_dx_relu(dZ3, D, fW2, R, Hh)                  # [R, 1024], relu backward in the epilogue
             with fork(dHh, X2):
                 d_fb1 = _gdest(fb1, (F,), zero=True)
-                d_fW1 = pr.linear_dw(dHh, F, X2, D, Mt, F, D, out=_gdest(fW1, (F, D)), dbias=d_fb1)
-            pr.linear_dx(dHh, F, fW1, Mt, out=dX2, accumulate=True)
+                d_fW1 = pr.linear_dw(dHh, F, X2, D, R, F, D, out=_gdest(fW1, (F, D)), dbias=d_fb1)
+            pr.linear_dx(dHh, F, fW1, R, out=dX2, accumulate=True)
             # ---- cross-attention
-            dZ2, dX1, d_clw, d_clb = pr.ln_bwd(dX2, dX2, Mt, Z2, X1, ls2, clw, Mt, p, seed, sid + 1, beta=clb)
+            dZ2, dX1, d_clw, d_clb = pr.ln_bwd(dX2, dX2, R, Z2, X1, ls2, clw, R, p, seed, sid + 1, beta=clb, rows_map=trows)
             with fork(dZ2, ctx2):
                 d_cbo = _gdest(cbo, (D,), zero=True)
-                d_cWo = pr.linear_dw(dZ2, D, ctx2, D, Mt, D, D, out=_gdest(cWo, (D, D)), dbias=d_cbo)
-            dctx2 = pr.linear_dx(dZ2, D, cWo, Mt)
-            dQ = pr.empty((Mt, D), dev)
-            if pk is not None:
+                d_cWo = pr.linear_dw(dZ2, D, ctx2, D, R, D, D, out=_gdest(cWo, (D, D)), dbias=d_cbo)
+            dctx2 = pr.linear_dx(dZ2, D, cWo, R)
+            dQ = pr.empty((R, D), dev)
+            if toff is not None:        # query rows = the commit's slots, keys = its memory ranges
+                call("fira_attn_bwd_rows", _ptr(Q), D, _ptr(KV, i * 2 * D), ldkv, _ptr(KV, i * 2 * D + D), ldkv,
+                     _ptr(pk.ranges), _ptr(mem_mask), S, 0, _ptr(toff), R, _ptr(ctx2), _ptr(dctx2), D, _ptr(st2), _ptr(dQ), D,
+                     _ptr(dKV, i * 2 * D), ldkv, _ptr(dKV, i * 2 * D + D), ldkv, B, H, T, D // H, pr.code, st)
+            elif pk is not None:
                 call("fira_attn_packed_bwd", _ptr(Q), D, _ptr(KV, i * 2 * D), ldkv, _ptr(KV, i * 2 * D + D), ldkv,
                      _ptr(pk.ranges), Ms, _ptr(mem_mask), S, pk.chunks, _ptr(ctx2), _ptr(dctx2), D, _ptr(st2), _ptr(dQ), D,
                      _ptr(dKV, i * 2 * D), ldkv, _ptr(dKV, i * 2 * D + D), ldkv, B, H, T, D // H, pr.code, st)
@@ -762,22 +789,27 @@ class DecoderFn(torch.autograd.Function):
                      _ptr(dKV, i * 2 * D + D), ldkv, B, H, T, S, D // H, pr.code, st)
             with fork(dQ, X1):
                 d_cbq = _gdest(cbq, (D,), zero=True)
-                d_cWq = pr.linear_dw(dQ, D, X1, D, Mt, D, D, out=_gdest(cWq, (D, D)), dbias=d_cbq)
-            pr.linear_dx(dQ, D, cWq, Mt, out=dX1, accumulate=True)
+                d_cWq = pr.linear_dw(dQ, D, X1, D, R, D, D, out=_gdest(cWq, (D, D)), dbias=d_cbq)
+            pr.linear_dx(dQ, D, cWq, R, out=dX1, accumulate=True)
             # ---- self-attention
-            dZ1, dX0, d_slw, d_slb = pr.ln_bwd(dX1, dX1, Mt, Z1, X, ls1, slw, Mt, p, seed, sid + 0, beta=slb)
+            dZ1, dX0, d_slw, d_slb = pr.ln_bwd(dX1, dX1, R, Z1, X, ls1, slw, R, p, seed, sid + 0, beta=slb, rows_map=trows)
             with fork(dZ1, ctx1):
                 d_sbo = _gdest(sbo, (D,), zero=True)
-                d_sWo = pr.linear_dw(dZ1, D, ctx1, D, Mt, D, D, out=_gdest(sWo, (D, D)), dbias=d_sbo)
-            dctx1 = pr.linear_dx(dZ1, D, sWo, Mt)
-            dQKV = pr.empty((Mt, 3 * D), dev)
-            call("fira_attn_bwd", _ptr(QKV), 3 * D, _ptr(QKV, D), 3 * D, _ptr(QKV, 2 * D), 3 * D, _ptr(tar_mask), 1,
-                 _ptr(ctx1), _ptr(dctx1), D, _ptr(st1), _ptr(dQKV), 3 * D, _ptr(dQKV, D), 3 * D, _ptr(dQKV, 2 * D), 3 * D,
-                 B, H, T, T, D // H, pr.code, st)
+                d_sWo = pr.linear_dw(dZ1, D, ctx1, D, R, D, D, out=_gdest(sWo, (D, D)), dbias=d_sbo)
+            dctx1 = pr.linear_dx(dZ1, D, sWo, R)
+            dQKV = pr.empty((R, 3 * D), dev)
+            if toff is not None:        # queries and keys = the commit's slots
+                call("fira_attn_bwd_rows", _ptr(QKV), 3 * D, _ptr(QKV, D), 3 * D, _ptr(QKV, 2 * D), 3 * D, None,
+                     _ptr(tar_mask), T, 1, _ptr(toff), R, _ptr(ctx1), _ptr(dctx1), D, _ptr(st1), _ptr(dQKV), 3 * D,
+                     _ptr(dQKV, D), 3 * D, _ptr(dQKV, 2 * D), 3 * D, B, H, T, D // H, pr.code, st)
+            else:
+                call("fira_attn_bwd", _ptr(QKV), 3 * D, _ptr(QKV, D), 3 * D, _ptr(QKV, 2 * D), 3 * D, _ptr(tar_mask), 1,
+                     _ptr(ctx1), _ptr(dctx1), D, _ptr(st1), _ptr(dQKV), 3 * D, _ptr(dQKV, D), 3 * D, _ptr(dQKV, 2 * D),
+                     3 * D, B, H, T, T, D // H, pr.code, st)
             with fork(dQKV, X):
                 d_bqkv = _gdest((sbq, sbk, sbv), (3 * D,), zero=True)
-                d_Wqkv = pr.linear_dw(dQKV, 3 * D, X, D, Mt, 3 * D, D, out=_gdest((sWq, sWk, sWv), (3 * D, D)), dbias=d_bqkv)
-            pr.linear_dx(dQKV, 3 * D, Wqkv, Mt, out=dX0, accumulate=True)
+                d_Wqkv = pr.linear_dw(dQKV, 3 * D, X, D, R, 3 * D, D, out=_gdest((sWq, sWk, sWv), (3 * D, D)), dbias=d_bqkv)
+            pr.linear_dx(dQKV, 3 * D, Wqkv, R, out=dX0, accumulate=True)
             grads[i * 26:(i + 1) * 26] = [
                 d_Wqkv[:D], d_bqkv[:D], d_Wqkv[D:2 * D], d_bqkv[D:2 * D], d_Wqkv[2 * D:], d_bqkv[2 * D:],
                 d_sWo, d_sbo, d_slw, d_slb,
@@ -798,7 +830,7 @@ class DecoderFn(torch.autograd.Function):
             grads[i * 26 + 12], grads[i * 26 + 13] = d_Wkv[o:o + D], d_bkv[o:o + D]
             grads[i * 26 + 14], grads[i * 26 + 15] = d_Wkv[o + D:o + 2 * D], d_bkv[o + D:o + 2 * D]
         d_emb = _gdest(dec_emb, tuple(dec_emb.shape), zero=True)
-        call("fira_embed_rows_bwd", _ptr(tar), _ptr(dX), _ptr(d_emb), Mt, D, pr.code, st)
+        call("fira_embed_rows_bwd_rows", _ptr(tar), _ptr(trows), _ptr(dX), _ptr(d_emb), R, D, pr.code, st)
         fork.join()
         return (None, None, d_mem, None, None, None, d_emb, *grads)
 

@@ -18,7 +18,7 @@ import torch
 from ._lib import host_call
 
 SEGMENT_BUCKETS = (1024, 512, 512, 64)          # rounding of (code rows, sub rows, AST rows, memory rows per commit)
-VOCAB_ROW_BUCKET = 128                          # rounding of the vocabulary-label target rows: one GEMM row tile
+VOCAB_ROW_BUCKET = 128                          # rounding of the vocabulary-label and live target rows: one GEMM row tile
 
 
 class PackedBatch:
@@ -27,7 +27,7 @@ class PackedBatch:
     FIELDS = ("code", "mark", "pos", "sub", "ast", "off", "ranges", "mem_mask", "tar", "label", "tar_mask",
               "rowptr", "col", "val")
 
-    def __init__(self, B, Rc, Rs, Ra, S, T, nnz, chunks=4, Rv=None, **tensors):
+    def __init__(self, B, Rc, Rs, Ra, S, T, nnz, chunks=4, Rv=None, Rt=None, **tensors):
         self.B, self.Rc, self.Rs, self.Ra, self.S, self.T, self.nnz = B, Rc, Rs, Ra, S, T, nnz
         # bound on the 128-key chunks cross-attention needs for any commit of the batch (3 on the whole shipped DataSet:
         # <= 200 code tokens, <= 102 sub-tokens); passed to the packed attention entry points, which do not use it
@@ -35,12 +35,15 @@ class PackedBatch:
         # bound on the target rows whose label is a vocabulary word: the rows of the training step's vocabulary
         # projection (ops.HeadFn); None = every row
         self.Rv = B * T if Rv is None else int(Rv)
+        # bound on the live target rows, the rows before each commit's last label (>= Rv): the rows of the training
+        # step's decoder backward (ops.DecoderFn); None = every row
+        self.Rt = B * T if Rt is None else int(Rt)
         for k in self.FIELDS:
             setattr(self, k, tensors[k])
 
     @property
     def shape_key(self):
-        return (self.B, self.Rc, self.Rs, self.Ra, self.S, self.chunks, self.Rv)
+        return (self.B, self.Rc, self.Rs, self.Ra, self.S, self.chunks, self.Rt, self.Rv)
 
     @property
     def rows(self):
@@ -52,7 +55,7 @@ class PackedBatch:
 
     def to(self, device, non_blocking=True):
         t = {k: getattr(self, k).to(device, non_blocking=non_blocking) for k in self.FIELDS}
-        return PackedBatch(self.B, self.Rc, self.Rs, self.Ra, self.S, self.T, self.nnz, self.chunks, self.Rv, **t)
+        return PackedBatch(self.B, self.Rc, self.Rs, self.Ra, self.S, self.T, self.nnz, self.chunks, self.Rv, self.Rt, **t)
 
     def h2d_bytes(self):
         return sum(getattr(self, k).numel() * getattr(self, k).element_size() for k in self.FIELDS)
@@ -94,6 +97,12 @@ class PackedTables:
         lab = self.tab["tar_label"][np.asarray(index, dtype=np.int64), 1:]
         return int(np.count_nonzero((lab > 0) & (lab < vocab_size)))
 
+    def live_rows(self, index):
+        """-> target rows of `index` before each commit's last non-zero shifted label (the count of fira_target_rows)"""
+        lab = self.tab["tar_label"][np.asarray(index, dtype=np.int64), 1:] != 0
+        last = lab.shape[1] - np.argmax(lab[:, ::-1], axis=1)
+        return int(np.where(lab.any(axis=1), last, 0).sum())
+
 
 class PackedSlot:
     """Staging buffers (pinned when CUDA is present) sized for the largest packed batch of `B` commits."""
@@ -122,20 +131,24 @@ class PackedSlot:
 
 def gather_packed(tables, index, vocab_size, slot, pad_dims=None, buckets=SEGMENT_BUCKETS):
     """One packed batch of commits `index` written into `slot` (views of the slot are returned as a PackedBatch).
-    pad_dims: (Rc, Rs, Ra, S[, Rv]) to use (>= the batch's needs, packed_needs); default = the needs rounded up to
-    `buckets`.  Rv is capped at the batch's target rows."""
+    pad_dims: (Rc, Rs, Ra, S[, Rv[, Rt]]) to use (>= the batch's needs, packed_needs); default = the needs rounded up
+    to `buckets`.  Rv and Rt are capped at the batch's target rows; an Rt not given is the need, at least Rv."""
     index = np.ascontiguousarray(index, dtype=np.int64)
     b = len(index)
     need = tables.dims(index)
     if pad_dims is None:
         pad_dims = packed_needs(tables, index, vocab_size, buckets)
-    elif len(pad_dims) == 4:
-        pad_dims = tuple(pad_dims) + packed_needs(tables, index, vocab_size, buckets)[4:]
-    Rc, Rs, Ra, S, Rv = (int(x) for x in pad_dims)
+    elif len(pad_dims) < 6:
+        need_all = packed_needs(tables, index, vocab_size, buckets)
+        pad_dims = tuple(pad_dims) + need_all[len(pad_dims):]
+        pad_dims = pad_dims[:5] + (max(pad_dims[4], pad_dims[5]),)
+    Rc, Rs, Ra, S, Rv, Rt = (int(x) for x in pad_dims)
     if Rc > slot.cap[0] or Rs > slot.cap[1] or Ra > slot.cap[2] or S > slot.cap[3]:
         raise ValueError(f"packed batch {pad_dims} exceeds the staging capacity {slot.cap}")
     if Rv < tables.vocab_rows(index, vocab_size):
         raise ValueError(f"packed batch: Rv = {Rv} is below its vocabulary-label rows")
+    if Rt < max(Rv, tables.live_rows(index)):
+        raise ValueError(f"packed batch: Rt = {Rt} is below its live target rows or Rv = {Rv}")
     t = tables.tab
     pd = np.asarray((Rc, Rs, Ra, S), np.int32)
     nnz = np.zeros(1, np.int32)
@@ -149,7 +162,7 @@ def gather_packed(tables, index, vocab_size, slot, pad_dims=None, buckets=SEGMEN
               slot.val.data_ptr(), slot.edge_cap, nnz.ctypes.data)
     e, T = int(nnz[0]), tables.msg_len
     slot.batch = PackedBatch(
-        b, Rc, Rs, Ra, S, T, e, max(3, need[5]), min(Rv, b * T),
+        b, Rc, Rs, Ra, S, T, e, max(3, need[5]), min(Rv, b * T), min(Rt, b * T),
         code=slot.code[:Rc], mark=slot.mark[:Rc], pos=slot.pos[:Rc], sub=slot.sub[:Rs], ast=slot.ast[:Ra],
         off=slot.off[:3 * (b + 1)].view(3, b + 1), ranges=slot.ranges[:4 * b].view(b, 4),
         mem_mask=slot.mem_mask[:b * S].view(b, S), tar=slot.tar[:b * T].view(b, T), label=slot.label[:b * T].view(b, T),
@@ -159,11 +172,14 @@ def gather_packed(tables, index, vocab_size, slot, pad_dims=None, buckets=SEGMEN
 
 
 def packed_needs(tables, index, vocab_size, buckets=SEGMENT_BUCKETS):
-    """-> (Rc, Rs, Ra, S, Rv) of commits `index`: the rows each segment needs rounded up to `buckets`, and the
-    vocabulary-label target rows rounded up to VOCAB_ROW_BUCKET"""
+    """-> (Rc, Rs, Ra, S, Rv, Rt) of commits `index`: the rows each segment needs rounded up to `buckets`, the
+    vocabulary-label target rows and the live target rows rounded up to VOCAB_ROW_BUCKET (Rt >= Rv), capped at the
+    batch's target rows"""
     need = tables.dims(index)
-    return tuple(_round_up(need[i], buckets[i]) for i in range(4)) + \
-        (_round_up(tables.vocab_rows(index, vocab_size), VOCAB_ROW_BUCKET),)
+    cap = len(index) * tables.msg_len
+    Rv = min(_round_up(tables.vocab_rows(index, vocab_size), VOCAB_ROW_BUCKET), cap)
+    Rt = min(max(_round_up(tables.live_rows(index), VOCAB_ROW_BUCKET), Rv), cap)
+    return tuple(_round_up(need[i], buckets[i]) for i in range(4)) + (Rv, Rt)
 
 
 def pack_from_dataset(dataset, index, vocab_size, pin=False, pad_dims=None, buckets=SEGMENT_BUCKETS):

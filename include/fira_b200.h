@@ -108,6 +108,9 @@ int fira_embed_nodes_bwd(const int* sou, const int* sub_token, const int* ast_ch
 int fira_embed_rows_fwd(const int* ids, const float* emb, const float* pos_table, void* out, long rows, int period,
                         int dim, int dtype, void* stream);
 int fira_embed_rows_bwd(const int* ids, const void* d_out, float* d_emb, long rows, int dim, int dtype, void* stream);
+/* The same with d_out in slots (fira_target_rows): slot r is row rows_map[r] of ids, -1 = none (rows = slots). */
+int fira_embed_rows_bwd_rows(const int* ids, const int* rows_map, const void* d_out, float* d_emb, long rows, int dim,
+                             int dtype, void* stream);
 
 /* ---- LN(dropout(z) + resid)  (gnn_transformer.py:83,161,174,205) -------------------------------
  * rows < split are written to outA[row], the others to outB[row] (lets a GCN layer hand its code
@@ -119,6 +122,14 @@ int fira_ln_residual_bwd(const void* d_outA, const void* d_outB, long split, con
                          const float* mean, const float* rstd, const float* gamma, void* d_z, void* d_resid,
                          int d_resid_accum, float* d_gamma, float* d_beta, long rows, int dim, float p_drop,
                          uint64_t seed, const uint64_t* seed_ctr, uint32_t stream_id, int dtype, void* stream);
+/* The same over slots (fira_target_rows): the dropout mask of slot r is the one drawn for row rows_map[r]; a slot with
+ * rows_map[r] < 0 writes zeros to d_z (and d_resid unless d_resid_accum) and adds nothing to d_gamma / d_beta.
+ * rows_map NULL: fira_ln_residual_bwd. */
+int fira_ln_residual_bwd_rows(const void* d_outA, const void* d_outB, long split, const void* z, const void* resid,
+                              const float* mean, const float* rstd, const float* gamma, void* d_z, void* d_resid,
+                              int d_resid_accum, float* d_gamma, float* d_beta, const int* rows_map, long rows, int dim,
+                              float p_drop, uint64_t seed, const uint64_t* seed_ctr, uint32_t stream_id, int dtype,
+                              void* stream);
 
 /* ---- Combination gate (combination_layer.py:7-17): c = v + sigmoid(q*(k-v)/sqrt(d_head))*(k-v),
  *      dropout; qk = [q | k] per row, v = vtab[mark[row]] (4 x dim table = Linear(mark_embedding)). */
@@ -214,6 +225,16 @@ int fira_attn_packed_bwd(const void* q, long ldq, const void* k, long ldk, const
                          long kv_rows, const unsigned char* key_mask, int mask_pitch, int max_chunks, const void* ctx,
                          const void* d_ctx, long ldo, const float* stats, void* dq, long lddq, void* dk, long lddk,
                          void* dv, long lddv, int B, int H, int Lq, int d_head, int dtype, void* stream);
+/* Backward over per-commit query-row ranges (bf16 only): the query rows of commit b (q, ctx, d_ctx, dq) are rows
+ * qoff[b] .. qoff[b+1] - 1 (at most Lq; stats keep the [B,H,Lq,2] layout, rows past the count unread); dq has `rows`
+ * rows, and its pad rows qoff[B] .. rows - 1 are zeroed (causal: those of dk / dv too).  Keys as
+ * fira_attn_packed_bwd (ranges != NULL) or fira_attn_bwd (key_mask [B, mask_pitch], rows b*mask_pitch + s); causal
+ * (self-attention, ranges NULL, mask_pitch = Lq): the keys are the commit's query rows, masked by its first key_mask
+ * bytes.  A commit without query rows writes zero gradients to its keys (causal: it has none). */
+int fira_attn_bwd_rows(const void* q, long ldq, const void* k, long ldk, const void* v, long ldv, const int* ranges,
+                       const unsigned char* key_mask, int mask_pitch, int causal, const int* qoff, long rows,
+                       const void* ctx, const void* d_ctx, long ldo, const float* stats, void* dq, long lddq, void* dk,
+                       long lddk, void* dv, long lddv, int B, int H, int Lq, int d_head, int dtype, void* stream);
 
 /* ---- the whole decoder forward, bf16 throughput mode (gnn_transformer.py:108-122), ONE launch of B two-CTA clusters: embedding +
  *      PE, then L x [causal self-attention over tar_mask [B,T], cross-attention, feed-forward], each closed by
@@ -237,6 +258,19 @@ int fira_decoder_fwd(const int* tar, const float* dec_emb, const float* pos_tabl
                      float* ls1, void* x1, void* q, void* ctx2, float* st2, void* z2, float* ls2, void* x2, void* hh,
                      void* z3, float* ls3, int B, int T, float p_drop, uint64_t seed, const uint64_t* seed_ctr,
                      uint32_t stream_id, void* stream);
+/* The same with a live-row map (fira_target_rows; tlen and toff both NULL: slot = row b*T + t, R = B*T, which is
+ * fira_decoder_fwd with out = X + L*B*T*256).  X [L][R,256] holds each layer's input and every per-layer output
+ * above has R slot rows: row t < toff[b+1] - toff[b] of commit b in slot toff[b] + t, the slots from toff[B] on zero;
+ * st1 / st2 and the dropout masks keep the rows b*T + t.  out [B*T,256] is the last layer's output: rows t >= tlen[b]
+ * zero, a live row without a slot NaN.  Every row is computed as without the map, so the live rows' values are the
+ * same. */
+int fira_decoder_fwd_rows(const int* tar, const float* dec_emb, const float* pos_table, const unsigned char* tar_mask,
+                          const void* kv, long ldkv, const unsigned char* mem_mask, const int* ranges, int S,
+                          const void* const* layer_ptrs, int L, void* X, void* out, void* qkv, void* ctx1, float* st1,
+                          void* z1, float* ls1, void* x1, void* q, void* ctx2, float* st2, void* z2, float* ls2,
+                          void* x2, void* hh, void* z3, float* ls3, const int* tlen, const int* toff, long R, int B,
+                          int T, float p_drop, uint64_t seed, const uint64_t* seed_ctr, uint32_t stream_id,
+                          void* stream);
 
 /* ---- CopyNet scores (Model.py:17-18): sc[b,t,s] = b_res + w_res . tanh(src[b,s] + tgt[b,t]).
  *      src_mask [B,S] / row_mask [B*T] (optional, 1 = compute): positions the caller will mask anyway. */
@@ -281,6 +315,12 @@ int fira_pointer_mix_nll_bwd(const void* logits, long ld_logits, const float* co
  *                    slots of vocabulary-label rows and zero-fills the unused slots s < cap (cap <= rows); rows without
  *                    a slot write no logits gradient. */
 int fira_vocab_rows(const int* label, long rows, int V, int* vslot, int* vrows, int cap, void* stream);
+/* ---- the live target rows of a training batch: the rows before each commit's last non-zero shifted label (no later row
+ *      carries a loss, and causal self-attention never lets an earlier row read one).  label [B,T] ->
+ *      tlen [B] = 1 + the last t with label != 0 (0 without one); toff [B+1] = each commit's first slot, slots in row
+ *      order; trows [cap] = b*T + t of each slot, -1 past the count.  B <= 1024.  A count above cap (the caller's bound)
+ *      leaves the commits past it short of slots (toff clamps to cap): fira_decoder_fwd_rows gives those rows NaN. */
+int fira_target_rows(const int* label, int B, int T, int* tlen, int* toff, int* trows, int cap, void* stream);
 int fira_gather_rows(const void* src, long ld_src, const int* idx, void* dst, long ld_dst, long n, int width, int dtype,
                      void* stream);
 int fira_pointer_mix_nll_fwd_rows(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
