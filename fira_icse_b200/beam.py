@@ -68,7 +68,9 @@ import torch
 
 from . import ops
 from ._lib import call
-from .decode_loop import PositionLoop, _f32, check_prefix, check_rules, check_tar_len, encode, is_int, loop_for
+from .decode_loop import (PositionLoop, _f32, check_prefix, check_rules, check_tar_len, encode, encode_members, is_int,
+                          loop_for)
+from .ensemble import refuse
 from .incremental import IncrementalDecoder
 
 MAX_BEAM = 16             # the row stage keeps a per-thread top K in registers
@@ -90,6 +92,7 @@ def _incremental_decoder(model, B, K, tar_len, mem_len):
 def beam_search(model, sou, mark, ast_change, edge, sub_token, *, beam_size=3, tar_len=30, start_id, eos_id,
                 pad_id=0, mode=None):
     """-> (sequences [B, beam, tar_len] int64 padded with pad_id, lengths [B, beam], probs [B, beam])."""
+    refuse(model, "beam_search")
     mode = mode or os.environ.get("FIRA_BEAM_MODE", "graph")
     if mode not in ("full", "graph"):
         raise ValueError("beam search mode must be 'full' or 'graph'")
@@ -218,10 +221,10 @@ class _NBest(PositionLoop):
         call("fira_pointer_mix_beam_step_rules", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
              p(self.copy_src), float(length_penalty), int(eos_id), int(pad_id), p(self.work), p(self.seq), p(self.raw),
              p(self.tlp), p(self.length), p(self.lp), p(self.score), p(self.status), p(self.parent), p(inc.tok),
-             self.T, t, self.B, self.N, self.V, self.S, self.pr.code, ops._stream(), p(self.prefix), self.T,
+             self.T, t, self.B, self.N, self.V, self.S, self.code, ops._stream(), p(self.prefix), self.T,
              p(self.prefix_len), int(no_repeat_ngram), int(min_length))
         # caches follow the parents BEFORE the pad mask of the new tokens is written (reorder moves tok_mask rows too)
-        inc.reorder(self.parent)
+        self.reorder(self.parent)
         inc.tok_mask[:, t + 1].copy_(inc.tok[:self.R] != pad_id)
 
 
@@ -249,9 +252,9 @@ class _DiverseNBest(_NBest):
              p(self.mem_mask), p(self.copy_src), float(length_penalty), int(eos_id), int(pad_id), p(self.work),
              p(self.seq), p(self.raw), p(self.tlp), p(self.length), p(self.lp), p(self.score), p(self.status),
              p(self.parent), p(inc.tok), self.T, t, self.B, self.N, self.V, self.S, int(groups), float(diversity),
-             p(self.chosen), p(self.work_lp), self.pr.code, ops._stream(), p(self.prefix), self.T, p(self.prefix_len),
+             p(self.chosen), p(self.work_lp), self.code, ops._stream(), p(self.prefix), self.T, p(self.prefix_len),
              int(no_repeat_ngram), int(min_length))
-        inc.reorder(self.parent)
+        self.reorder(self.parent)
         inc.tok_mask[:, t + 1].copy_(inc.tok[:self.R] != pad_id)
 
 
@@ -259,6 +262,7 @@ class _DiverseNBest(_NBest):
 def nbest(model, sou, mark, ast_change, edge, sub_token, *, beam_size=3, length_penalty=0.0, tar_len=30, start_id,
           eos_id, pad_id=0, groups=1, diversity=0.0, prefix=None, no_repeat_ngram=0, min_length=0):
     """Log-space beam search with length normalisation -> Hypotheses, each commit's K best first (module docstring).
+    model: a TransModel, or an ensemble.Ensemble (ranked by its averaged distribution).
     groups > 1 splits the K slots into diverse beam groups penalised by `diversity` per earlier-group repeat.
     prefix: None, or labels [B, P] every hypothesis of a commit starts with (decode_loop.check_prefix: the tar_label
     encoding without <start>, a 0 ends a commit's prefix, no <eos>, at most tar_len - 2 labels).
@@ -271,8 +275,8 @@ def nbest(model, sou, mark, ast_change, edge, sub_token, *, beam_size=3, length_
     check_tar_len(model, tar_len)
     pre = check_prefix(prefix, sou, sub_token, V=model.vocab_size, tar_len=tar_len, eos_id=eos_id, pad_id=pad_id,
                        eos_last=False)
-    memory, mem_mask, copy_src = encode(model, sou, mark, ast_change, edge, sub_token, pad_id)
-    B, S = memory.shape[:2]
+    memory, mem_mask, copy_src = encode_members(model, sou, mark, ast_change, edge, sub_token, pad_id)
+    B, S = memory[0].shape[:2]
     if groups == 1:
         st = loop_for(_NBest, model, B, beam_size, tar_len, S)
         st.start(memory, mem_mask, copy_src, start_id, pad_id, pre)

@@ -1101,6 +1101,119 @@ __global__ void __launch_bounds__(kBeamThreads) diverse_select_kernel(
   }
 }
 
+// ------------------------------------------------------------------ ensemble combine
+// M members' (logits, copy scores, gate logits) -> one fp32 triple whose mixture (Model.py:54-86, as the step kernels
+// form it) is the weighted average sum_m w_m P^m.  With member m's row statistics from mix_row_stats (bit for bit those
+// its own step kernel would form) and G0 = sum_m w_m g0^m, G1 = sum_m w_m g1^m:
+//   x'_j = LSE over m with w_m g0^m > 0 of [log(w_m g0^m / G0) + x^m_j - vmax^m - log vsum^m]
+//   c'_s = LSE over m with w_m g1^m > 0 of [log(w_m g1^m / G1) + c^m_s - cmax^m - log csum^m]   (masked s: kMaskFill)
+//   gl'  = (log G0, log G1)
+// softmax(x') sums to 1, so g0' softmax(x')_j = G0 * sum_m (w_m g0^m / G0) softmax(x^m)_j.  G0 == 0 (every member's gate
+// saturated to the copy side) uses log w_m as the offsets: x' stays finite and gl'_0 = -inf makes g0' exactly 0; the
+// same for G1.  The log domain keeps x' and c' finite where every member's probability underflows in fp32.
+constexpr int kMaxMembers = 8;
+constexpr int kEnsThreads = 256;                      // = the step kernels' block: mix_row_stats' reduction order
+struct Members {                                      // by value: a captured launch bakes the pointers in
+  const void* logits[kMaxMembers];
+  const float* sc[kMaxMembers];
+  const float* gl[kMaxMembers];
+};
+
+// running log-sum-exp (mx, s): one expf per term
+__device__ __forceinline__ void lse_add(float& mx, float& s, float y) {
+  if (y > mx) { s = s * expf(mx - y) + 1.f; mx = y; }
+  else s += expf(y - mx);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kEnsThreads) pointer_mix_ensemble_kernel(
+    Members mem, int M, long ldl, const float* __restrict__ log_w, const unsigned char* __restrict__ mem_mask,
+    float* __restrict__ logits_out, long ld_out, float* __restrict__ sc_out, float* __restrict__ gl_out, int N, int V,
+    int S) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  __shared__ MaxSum sh_ms[8];
+  __shared__ float bc[4];
+  __shared__ const T* s_l[kMaxMembers];
+  __shared__ const float* s_c[kMaxMembers];
+  __shared__ const float* s_gl[kMaxMembers];
+  __shared__ float s_g0[kMaxMembers], s_g1[kMaxMembers], s_ov[kMaxMembers], s_oc[kMaxMembers];
+  __shared__ float s_gate[2];
+  const long row = blockIdx.x;
+  const int b = (int)(row / N);
+  const unsigned char* mrow = mem_mask + (long)b * S;
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int m = 0; m < kMaxMembers; ++m) {           // static indices: the parameter struct stays in constant space
+      s_l[m] = (const T*)mem.logits[m] + row * ldl;
+      s_c[m] = mem.sc[m] + row * S;
+      s_gl[m] = mem.gl[m] + row * 2;
+    }
+  }
+  __syncthreads();
+  // pass 1 per member: its row statistics (vocab max / sum, copy max / sum, gates)
+  for (int m = 0; m < M; ++m) {
+    const MixRow ms = mix_row_stats(s_l[m], s_c[m], mrow, s_gl[m], V, S, sh_ms, bc);
+    if (threadIdx.x == 0) {
+      s_g0[m] = ms.g0; s_g1[m] = ms.g1;
+      s_ov[m] = -ms.vmax - logf(ms.vsum);
+      s_oc[m] = -ms.cmax - logf(ms.csum);
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float G0 = 0.f, G1 = 0.f;
+    for (int m = 0; m < M; ++m) { const float w = expf(log_w[m]); G0 += w * s_g0[m]; G1 += w * s_g1[m]; }
+    const float lG0 = logf(G0), lG1 = logf(G1);
+    for (int m = 0; m < M; ++m) {
+      const float w = expf(log_w[m]);
+      const float a0 = w * s_g0[m], a1 = w * s_g1[m];
+      // -inf drops a member whose weighted gate is 0; with G == 0 every member keeps log w_m
+      s_ov[m] += G0 > 0.f ? (a0 > 0.f ? logf(a0) - lG0 : -INFINITY) : log_w[m];
+      s_oc[m] += G1 > 0.f ? (a1 > 0.f ? logf(a1) - lG1 : -INFINITY) : log_w[m];
+    }
+    s_gate[0] = lG0; s_gate[1] = lG1;
+  }
+  __syncthreads();
+  // pass 2: vocabulary entries, 8 per vector load / store (the step kernels' load8), scalar tail
+  float* orow = logits_out + row * ld_out;
+  const int V8 = V >> 3;
+  for (int g = threadIdx.x; g < V8; g += blockDim.x) {
+    float mx[8], s[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { mx[i] = -INFINITY; s[i] = 0.f; }
+    for (int m = 0; m < M; ++m) {
+      const float o = s_ov[m];
+      if (o == -INFINITY) continue;
+      float x[8];
+      Act<T>::load8(s_l[m] + (long)g * 8, x);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) lse_add(mx[i], s[i], o + x[i]);
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) mx[i] += logf(s[i]);
+    Act<float>::store8(orow + (long)g * 8, mx);
+  }
+  for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) {
+    float mx = -INFINITY, s = 0.f;
+    for (int m = 0; m < M; ++m)
+      if (s_ov[m] != -INFINITY) lse_add(mx, s, s_ov[m] + Act<T>::ld(s_l[m] + j));
+    orow[j] = mx + logf(s);
+  }
+  // copy positions
+  float* crow = sc_out + row * S;
+  for (int j = threadIdx.x; j < S; j += blockDim.x) {
+    float r = kMaskFill;
+    if (mrow[j]) {
+      float mx = -INFINITY, s = 0.f;
+      for (int m = 0; m < M; ++m)
+        if (s_oc[m] != -INFINITY) lse_add(mx, s, s_oc[m] + s_c[m][j]);
+      r = mx + logf(s);
+    }
+    crow[j] = r;
+  }
+  if (threadIdx.x == 0) { gl_out[row * 2] = s_gate[0]; gl_out[row * 2 + 1] = s_gate[1]; }
+}
+
 }  // namespace
 
 #define DISPATCH_T(dtype, ...)                                                            \
@@ -1502,6 +1615,34 @@ int fira_pointer_mix_diverse_beam_step_rules(const void* logits, long ld_logits,
                                 pad_id, workspace, seq, raw, token_logprob, length, logprob, score, status, parent,
                                 next_tok, T_len, pos, B, K, V, S, groups, diversity, chosen, lp_workspace, prefix,
                                 ld_prefix, prefix_len, no_repeat_ngram, min_length, dtype, stream);
+}
+
+int fira_pointer_mix_ensemble(const void* const* logits, long ld_logits, const float* const* copy_scores,
+                              const float* const* gate_logits, int M, const float* log_weights,
+                              const unsigned char* mem_mask, float* logits_out, long ld_out, float* copy_out,
+                              float* gate_out, int B, int N, int V, int S, int dtype, void* stream) {
+  FIRA_CHECK_ARG(M >= 1 && M <= kMaxMembers, FIRA_ERR_ARG, "pointer_mix_ensemble: M %d not in [1, %d]", M, kMaxMembers);
+  FIRA_CHECK_ARG(logits && copy_scores && gate_logits && log_weights && mem_mask && logits_out && copy_out && gate_out,
+                 FIRA_ERR_ARG, "pointer_mix_ensemble: null pointer");
+  Members mem = {};
+  for (int m = 0; m < M; ++m) {
+    FIRA_CHECK_ARG(logits[m] && copy_scores[m] && gate_logits[m], FIRA_ERR_ARG,
+                   "pointer_mix_ensemble: null pointer of member %d", m);
+    FIRA_CHECK_ARG(fira_aligned16(logits[m]), FIRA_ERR_ALIGN,
+                   "pointer_mix_ensemble: logits of member %d must be 16-byte aligned", m);
+    mem.logits[m] = logits[m]; mem.sc[m] = copy_scores[m]; mem.gl[m] = gate_logits[m];
+  }
+  FIRA_CHECK_ARG(fira_aligned16(logits_out) && ld_logits % 8 == 0 && ld_out % 8 == 0, FIRA_ERR_ALIGN,
+                 "pointer_mix_ensemble: logits_out must be 16-byte aligned, ld_logits %ld and ld_out %ld multiples of 8",
+                 ld_logits, ld_out);
+  FIRA_CHECK_ARG(B >= 0 && N > 0 && V > 0 && S > 0 && V + S <= 0x7FFF && ld_logits >= V && ld_out >= V, FIRA_ERR_SHAPE,
+                 "pointer_mix_ensemble: shape (B %d, N %d, V %d, S %d, ld_logits %ld, ld_out %ld; V + S must be <= 32767)",
+                 B, N, V, S, ld_logits, ld_out);
+  if (B == 0) return FIRA_OK;
+  DISPATCH_T(dtype, launch_k(pointer_mix_ensemble_kernel<T>, dim3((unsigned)(B * N)), dim3(kEnsThreads), 0,
+      (cudaStream_t)stream, mem, M, ld_logits, log_weights, mem_mask, logits_out, ld_out, copy_out, gate_out, N, V, S);)
+  FIRA_CHECK_LAUNCH("fira_pointer_mix_ensemble");
+  return FIRA_OK;
 }
 
 }  // extern "C"

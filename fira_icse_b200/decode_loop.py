@@ -18,7 +18,8 @@ import torch
 
 from . import ops
 from . import optim as _optim
-from ._lib import call
+from ._lib import FIRA_F32, call
+from .ensemble import Ensemble, members
 from .incremental import IncrementalDecoder, replay_or_capture, weights_key
 
 D = ops.D
@@ -34,9 +35,11 @@ def is_int(v):
 
 
 def check_tar_len(model, tar_len):
-    """ValueError when the decoder has fewer than tar_len positions (called before any device work)."""
-    if tar_len > model.decoder.pos_encode.shape[0]:
-        raise ValueError(f"tar_len {tar_len} exceeds the decoder's {model.decoder.pos_encode.shape[0]} positions")
+    """ValueError when the decoder (of any member of an ensemble) has fewer than tar_len positions (called before any
+    device work)."""
+    for m in members(model):
+        if tar_len > m.decoder.pos_encode.shape[0]:
+            raise ValueError(f"tar_len {tar_len} exceeds the decoder's {m.decoder.pos_encode.shape[0]} positions")
 
 
 MAX_RULES_TAR_LEN = 32    # the step kernels hold a row's history in a fixed shared-memory list (head.cu TMAX)
@@ -120,31 +123,94 @@ def encode(model, sou, mark, ast_change, edge, sub_token, pad_id):
     return memory, mem_mask, copy_src
 
 
+def encode_members(model, sou, mark, ast_change, edge, sub_token, pad_id):
+    """encode() with every member of an ensemble (one model: itself) -> ([memory per member], mem_mask, copy_src)."""
+    out = [encode(m, sou, mark, ast_change, edge, sub_token, pad_id) for m in members(model)]
+    return [o[0] for o in out], out[0][1], out[0][2]
+
+
+class _Head:
+    """One model's part of a position: its IncrementalDecoder and the buffers its output head writes (src = the
+    memory's LinearSource projection, logits, tgt, gate logits gl, copy scores sc)."""
+
+    def __init__(self, model, B, N, T, S, share=None):
+        self.model = model
+        self.inc = IncrementalDecoder(model.decoder, B, N, T, S, graphs=False, share=share)   # launches go into our graphs
+        self.pr = ops.Prec(self.inc.be.bf16)
+        dev = model.out_fc.weight.device
+        R, tdt = B * N, self.inc.be.tdt
+        self.src = torch.empty((B * S, D), dtype=tdt, device=dev)
+        self.logits = torch.empty((R, ops._ld_logits(model.vocab_size)), dtype=tdt, device=dev)
+        self.tgt = torch.empty((R, D), dtype=tdt, device=dev)
+        self.gl = torch.empty((R, 2), dtype=torch.float32, device=dev)
+        self.sc = torch.empty((B, N, S), dtype=torch.float32, device=dev)
+
+    def start(self, memory, mem_mask):
+        self.inc.start(memory, mem_mask)
+        mem2 = memory.contiguous().to(self.inc.be.tdt).view(self.src.shape[0], D)
+        self.pr.linear(mem2, self.model.copy_net.LinearSource.weight, out=self.src)     # once per batch, not per row
+
+    def run(self, t, mem_mask, B, N, S):
+        """logits, copy scores and gate logits of decoder row t (every launch on the current stream: capturable)."""
+        m, pr = self.model, self.pr
+        cn = m.copy_net
+        x = self.inc.advance(t)                                                  # [R, D]
+        pr.linear(x, m.out_fc.weight, m.out_fc.bias, out=self.logits, ld_out=self.logits.shape[1])
+        pr.linear(x, cn.LinearTarget.weight, out=self.tgt)
+        ops.linear(x.float() if pr.bf16 else x, cn.LinearProb.weight, cn.LinearProb.bias, out=self.gl)   # fp32 gate
+        p = ops._ptr
+        call("fira_copy_scores_fwd", p(self.src), p(self.tgt), p(cn.LinearRes.weight), p(cn.LinearRes.bias),
+             p(mem_mask), None, p(self.sc), B, N, S, D, pr.code, ops._stream())
+
+    def refresh_weights(self):
+        if self.pr.bf16:
+            _optim.ensure_fresh(self.model)
+            for W, W16 in self.pr.wcache.values():
+                W16.copy_(W.detach())
+
+
 class PositionLoop:
     """Static buffers, slot state and captured position graphs of one (model, B, N, tar_len, S, precision).
 
     Slot state: seq, raw, tlp [halves, R, T] and length, lp, status [halves, R] (status 0 live, 1 finished); position t
     reads half t % halves.  Subclasses set `halves` and define position(t, *cfg) (head(t), then their own launches;
-    every launch on the current stream)."""
+    every launch on the current stream), passing logits / sc / gl with dtype code `code` to their step kernel.
+
+    An ensemble.Ensemble gets one _Head per member.  The members decode the same tokens, so their decoders share the
+    first one's token buffer and pad mask (`inc`, which the step kernels write); reorder() moves every member's KV
+    cache and the shared mask once.  head(t) runs the members one after another, then fira_pointer_mix_ensemble writes
+    the averaged triple into the loop's own fp32 logits / sc / gl.  One model is one _Head whose buffers are the
+    loop's, with no combine."""
 
     halves = 1
 
     def __init__(self, model, B, N, T, S):
         self.model, self.B, self.N, self.T, self.S = model, B, N, T, S
-        self.inc = IncrementalDecoder(model.decoder, B, N, T, S, graphs=False)   # its launches go into our graphs
-        self.pr = ops.Prec(self.inc.be.bf16)
-        self.dev = dev = model.out_fc.weight.device
+        ms = members(model)
+        self.heads = [_Head(ms[0], B, N, T, S)]
+        self.heads += [_Head(m, B, N, T, S, share=self.heads[0].inc) for m in ms[1:]]
+        h0 = self.heads[0]
+        self.inc, self.pr = h0.inc, h0.pr
+        self.dev = dev = ms[0].out_fc.weight.device
         R = self.R = B * N
-        tdt = self.inc.be.tdt
         self.V = model.vocab_size
         self.ldl = ops._ld_logits(self.V)
         self.mem_mask = torch.zeros((B, S), dtype=torch.uint8, device=dev)
         self.copy_src = torch.zeros((B, S), dtype=torch.int32, device=dev)
-        self.src = torch.empty((B * S, D), dtype=tdt, device=dev)
-        self.logits = torch.empty((R, self.ldl), dtype=tdt, device=dev)
-        self.tgt = torch.empty((R, D), dtype=tdt, device=dev)
-        self.gl = torch.empty((R, 2), dtype=torch.float32, device=dev)
-        self.sc = torch.empty((B, N, S), dtype=torch.float32, device=dev)
+        self.ensemble = isinstance(model, Ensemble)
+        if self.ensemble:
+            f32 = dict(dtype=torch.float32, device=dev)
+            self.logits = torch.empty((R, self.ldl), **f32)
+            self.gl = torch.empty((R, 2), **f32)
+            self.sc = torch.empty((B, N, S), **f32)
+            self.code = FIRA_F32
+            self.log_w = torch.zeros(len(ms), **f32)
+            self.log_weights = model.log_weights           # loop_for sets the calling ensemble's; start() writes them
+            M = len(ms)
+            self._members = tuple((ctypes.c_void_p * M)(*[ops._ptr(getattr(h, k)) for h in self.heads])
+                                  for k in ("logits", "sc", "gl"))
+        else:
+            self.logits, self.gl, self.sc, self.code = h0.logits, h0.gl, h0.sc, self.pr.code
         H = self.halves
         i32 = dict(dtype=torch.int32, device=dev)
         f32 = dict(dtype=torch.float32, device=dev)
@@ -161,7 +227,8 @@ class PositionLoop:
         self.graphs = {}
 
     def start(self, memory, mem_mask, copy_src, start_id, pad_id, prefix=None):
-        """prefix: None or check_prefix's host pair (prefix [B, T], prefix_len [B])."""
+        """memory: encode_members' list (one encoder memory per member); prefix: None or check_prefix's host pair
+        (prefix [B, T], prefix_len [B])."""
         inc = self.inc
         if prefix is None:
             self.prefix.zero_()
@@ -169,9 +236,10 @@ class PositionLoop:
         else:
             self.prefix.copy_(prefix[0])
             self.prefix_len.copy_(prefix[1])
-        inc.start(memory, mem_mask)
-        mem2 = memory.contiguous().to(inc.be.tdt).view(self.B * self.S, D)
-        self.pr.linear(mem2, self.model.copy_net.LinearSource.weight, out=self.src)     # once per batch, not per row
+        for h, mem in zip(self.heads, memory):
+            h.start(mem, mem_mask)
+        if self.ensemble:
+            self.log_w.copy_(torch.tensor(self.log_weights, dtype=torch.float32))
         self.mem_mask.copy_(mem_mask)
         self.copy_src.copy_(copy_src)
         inc.tok[:self.R].fill_(start_id)
@@ -189,10 +257,8 @@ class PositionLoop:
         they replay with the new weights.  The decoder's concatenated weights follow in start() (IncrementalDecoder
         compares weights_key); here the bf16 mirror and the bf16 copies of the head's weights.  fp32 mode reads the
         parameters themselves."""
-        if self.pr.bf16:
-            _optim.ensure_fresh(self.model)
-            for W, W16 in self.pr.wcache.values():
-                W16.copy_(W.detach())
+        for h in self.heads:
+            h.refresh_weights()
 
     def unfinished(self, t):
         """A device bool: some row still decodes after t positions."""
@@ -207,15 +273,21 @@ class PositionLoop:
 
     def head(self, t):
         """logits, copy scores and gate logits of decoder row t (every launch on the current stream: capturable)."""
-        m, pr, B, N, S = self.model, self.pr, self.B, self.N, self.S
-        cn = m.copy_net
-        x = self.inc.advance(t)                                                  # [R, D]
-        pr.linear(x, m.out_fc.weight, m.out_fc.bias, out=self.logits, ld_out=self.ldl)
-        pr.linear(x, cn.LinearTarget.weight, out=self.tgt)
-        ops.linear(x.float() if pr.bf16 else x, cn.LinearProb.weight, cn.LinearProb.bias, out=self.gl)   # fp32 gate
-        p = ops._ptr
-        call("fira_copy_scores_fwd", p(self.src), p(self.tgt), p(cn.LinearRes.weight), p(cn.LinearRes.bias),
-             p(self.mem_mask), None, p(self.sc), B, N, S, D, pr.code, ops._stream())
+        B, N, S = self.B, self.N, self.S
+        for h in self.heads:
+            h.run(t, self.mem_mask, B, N, S)
+        if self.ensemble:
+            lg, sc, gl = self._members
+            p = ops._ptr
+            call("fira_pointer_mix_ensemble", ctypes.addressof(lg), self.heads[0].logits.shape[1], ctypes.addressof(sc),
+                 ctypes.addressof(gl), len(self.heads), p(self.log_w), p(self.mem_mask), p(self.logits), self.ldl,
+                 p(self.sc), p(self.gl), B, N, self.V, S, self.pr.code, ops._stream())
+
+    def reorder(self, parent):
+        """Row r of every member's KV cache and of the shared pad mask continues row parent[r] (n-best)."""
+        self.inc.reorder(parent)
+        for h in self.heads[1:]:
+            h.inc.reorder(parent, tok_mask=False)       # the mask is the first decoder's, already moved
 
     def run(self, cfg):
         """Positions 0..T-2 (fewer once every row has finished) -> the number of positions run."""
@@ -228,22 +300,29 @@ class PositionLoop:
         return t
 
 
-_LOOPS = weakref.WeakKeyDictionary()   # model -> {(class, B, N, T, S, precision): (weights key, addresses, loop)}
+_LOOPS = weakref.WeakKeyDictionary()   # model (an ensemble's first member) -> {key: (weights keys, addresses, loop)}
 
 
 def loop_for(cls, model, B, N, T, S):
     """The cached `cls` instance of this shape.  Weights updated in place (a new weights_key, every parameter at the
     address the graphs captured) are refreshed inside the loop, whose position graphs keep replaying: a training loop
     that samples after every optimizer step (scst.py) does not recapture them.  A parameter that moved rebuilds the
-    loop (fresh operand copies and graphs)."""
-    store = _LOOPS.setdefault(model, {})
-    key = (cls, B, N, T, S, model.precision)
-    wkey = weights_key(model, model.decoder)
-    addr = tuple(p.data_ptr() for p in model.parameters())
+    loop (fresh operand copies and graphs).  An ensemble is keyed by its members, not by the Ensemble object: a new
+    Ensemble of the same models replays the same graphs, with its own weights written at start()."""
+    ms = members(model)
+    store = _LOOPS.setdefault(ms[0], {})
+    key = (cls, B, N, T, S, ms[0].precision)
+    if isinstance(model, Ensemble):        # the loop holds its members, so their ids stay theirs while it is cached
+        key += (tuple(id(m) for m in ms),)
+    wkey = tuple(weights_key(m, m.decoder) for m in ms)
+    addr = tuple(p.data_ptr() for m in ms for p in m.parameters())
     cur = store.get(key)
     if cur is None or cur[1] != addr:
         store[key] = (wkey, addr, cls(model, B, N, T, S))
     elif cur[0] != wkey:
         cur[2].refresh_weights()
         store[key] = (wkey, addr, cur[2])
-    return store[key][2]
+    loop = store[key][2]
+    if isinstance(model, Ensemble):
+        loop.log_weights = model.log_weights
+    return loop

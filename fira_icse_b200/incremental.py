@@ -97,11 +97,13 @@ class CudaBackend:
 
 
 class IncrementalDecoder:
-    """decoder = fira_icse_b200.modules.Decoder; B commits x K beams; rows are ordered (commit, beam)."""
+    """decoder = fira_icse_b200.modules.Decoder; B commits x K beams; rows are ordered (commit, beam).
+    share: another IncrementalDecoder of the same B, K and tar_len whose token buffer and pad mask this one reads (the
+    members of an ensemble decode the same tokens)."""
 
     MIN_ROWS = 128          # row count the projections run on (tensor-core tiles are 128 rows; pad rows are zeros)
 
-    def __init__(self, decoder, B, K, tar_len, mem_len, graphs=False, backend=None):
+    def __init__(self, decoder, B, K, tar_len, mem_len, graphs=False, backend=None, share=None):
         self.dec, self.B, self.K, self.T, self.S = decoder, B, K, tar_len, mem_len
         self.H = decoder.num_head
         self.L = len(decoder.attention_list)
@@ -112,8 +114,12 @@ class IncrementalDecoder:
         tdt = self.be.tdt
         self.R = B * K
         self.Rp = max(self.R, self.MIN_ROWS)
-        self.tok = torch.zeros(self.Rp, dtype=torch.int32, device=dev)
-        self.tok_mask = torch.zeros((self.R, tar_len), dtype=torch.uint8, device=dev)
+        if share is None:
+            self.tok = torch.zeros(self.Rp, dtype=torch.int32, device=dev)
+            self.tok_mask = torch.zeros((self.R, tar_len), dtype=torch.uint8, device=dev)
+        else:
+            assert (share.R, share.T) == (self.R, tar_len)
+            self.tok, self.tok_mask = share.tok, share.tok_mask
         self.kv_self = torch.zeros((self.L, self.R, tar_len, 2 * D), dtype=tdt, device=dev)
         self.kv_mem = torch.zeros((B * mem_len, self.L * 2 * D), dtype=tdt, device=dev)
         self.mem_mask = torch.zeros((B, mem_len), dtype=torch.uint8, device=dev)
@@ -218,7 +224,9 @@ class IncrementalDecoder:
             self._layers(t)
         return self.out[:self.R]
 
-    def reorder(self, src_rows):
-        """src_rows int64 [B*K]: new row r continues old row src_rows[r] (beam re-ranking)."""
+    def reorder(self, src_rows, tok_mask=True):
+        """src_rows int64 [B*K]: new row r continues old row src_rows[r] (beam re-ranking).  tok_mask=False leaves the
+        pad mask alone (a shared mask moved by its owner)."""
         self.kv_self.copy_(self.kv_self.index_select(1, src_rows))
-        self.tok_mask.copy_(self.tok_mask.index_select(0, src_rows))
+        if tok_mask:
+            self.tok_mask.copy_(self.tok_mask.index_select(0, src_rows))

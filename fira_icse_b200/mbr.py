@@ -41,7 +41,8 @@ class MBR(NamedTuple):
 def mbr(model, sou, mark, ast_change, edge, sub_token, *, num_samples=16, temperature=1.0, top_k=0, top_p=1.0,
         seed=0, first_index=0, tar_len=30, start_id, eos_id, pad_id=0, prefix=None, no_repeat_ngram=0, min_length=0):
     """Draw `num_samples` messages per commit with sample() and keep the one of highest expected BLEU -> MBR.
-    prefix, no_repeat_ngram, min_length: passed to sample(), so every candidate obeys them."""
+    prefix, no_repeat_ngram, min_length: passed to sample(), so every candidate obeys them.  model: a TransModel or an
+    ensemble.Ensemble (the candidates are drawn from its averaged distribution)."""
     check_args(num_samples, temperature, top_k, top_p, seed, first_index, tar_len)
     if num_samples < 2:
         raise ValueError(f"MBR needs num_samples >= 2, got {num_samples!r}")

@@ -26,7 +26,8 @@ import torch
 
 from . import ops
 from ._lib import call
-from .decode_loop import PositionLoop, _f32, check_prefix, check_rules, check_tar_len, encode, is_int, loop_for
+from .decode_loop import (PositionLoop, _f32, check_prefix, check_rules, check_tar_len, encode_members, is_int,
+                          loop_for)
 
 MAX_SAMPLES = 32          # the N samples of a commit are its query rows in fira_attn_fwd / fira_copy_scores_fwd (<= 32)
 
@@ -78,7 +79,7 @@ class _Sampler(PositionLoop):
         call("fira_pointer_mix_sample_rules", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
              p(self.copy_src), p(self.seed), p(self.first), None, float(temperature), int(top_k), float(top_p),
              int(eos_id), int(pad_id), p(self.inc.tok), p(self.seq), p(self.raw), p(self.tlp), p(self.inc.tok_mask),
-             self.T, t, p(self.status), p(self.length), p(self.lp), self.B, self.N, self.V, self.S, self.pr.code,
+             self.T, t, p(self.status), p(self.length), p(self.lp), self.B, self.N, self.V, self.S, self.code,
              ops._stream(), p(self.prefix), self.T, p(self.prefix_len), int(no_repeat_ngram), int(min_length))
 
 
@@ -88,6 +89,7 @@ def sample(model, sou, mark, ast_change, edge, sub_token, *, num_samples=1, temp
            min_length=0):
     """Draw `num_samples` messages per commit -> Samples(seq, raw, length, logprob, token_logprob).
 
+    model: a TransModel, or an ensemble.Ensemble (its averaged distribution; token_logprob is the ensemble's).
     first_index: dataset position of the batch's first commit (the Philox counter uses first_index + b).
     prefix: None, or labels [B, P] every sample of a commit starts with (decode_loop.check_prefix: the tar_label
     encoding without <start>, a 0 ends a commit's prefix, <eos> only as its last label).  The positions after a prefix
@@ -103,8 +105,8 @@ def sample(model, sou, mark, ast_change, edge, sub_token, *, num_samples=1, temp
         raise ValueError("first_index + batch size must stay below 2**31")
     pre = check_prefix(prefix, sou, sub_token, V=model.vocab_size, tar_len=tar_len, eos_id=eos_id, pad_id=pad_id,
                        eos_last=True)
-    memory, mem_mask, copy_src = encode(model, sou, mark, ast_change, edge, sub_token, pad_id)
-    B, S = memory.shape[:2]
+    memory, mem_mask, copy_src = encode_members(model, sou, mark, ast_change, edge, sub_token, pad_id)
+    B, S = memory[0].shape[:2]
     st = loop_for(_Sampler, model, B, num_samples, tar_len, S)
     st.start(memory, mem_mask, copy_src, seed, first_index, start_id, pad_id, pre)
     t = st.run((float(temperature), int(top_k), float(top_p), int(eos_id), int(pad_id), no_repeat_ngram, min_length))
@@ -132,6 +134,7 @@ def score_prefix(tar_label, tar_len, eos_id):
 @torch.no_grad()
 def score(model, sou, mark, ast_change, edge, sub_token, tar_label, *, tar_len=30, start_id, eos_id, pad_id=0):
     """log p(message | commit) of each commit's given message -> Scores(token_logprob, logprob, length).
+    model: a TransModel or an ensemble.Ensemble (then log of the averaged probability).
 
     tar_label [B, >= tar_len]: <start>, the labels (tar_label encoding), <eos> within tar_len, anything after.  The
     sampler with one sample per commit and the whole message forced, so token_logprob[:, t] is the -nll the training

@@ -36,6 +36,7 @@ from . import ops
 from . import optim as _optim
 from ._lib import call
 from .decode_loop import check_rules, check_tar_len, is_int
+from .ensemble import refuse
 from .modules import _i32, _u8
 from .sample import MAX_SAMPLES, check_args, sample
 
@@ -119,6 +120,7 @@ def scst_step(model, optimizer, batch, *, num_samples, temperature=1.0, top_k=0,
               no_repeat_ngram=0, min_length=0, tar_len=30, start_id, eos_id, pad_id=0):
     """One self-critical step on the padded batch (the 8-tuple of run_model.py on the model's device) -> Step(mean
     reward, mean |advantage|, loss).  Sampling settings as sample(); leaves the model in training mode."""
+    refuse(model, "scst_step")
     check_step(batch[1], num_samples=num_samples, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed,
                first_index=first_index, no_repeat_ngram=no_repeat_ngram, min_length=min_length, tar_len=tar_len,
                eos_id=eos_id, model=model)

@@ -485,6 +485,25 @@ int fira_pointer_mix_diverse_beam_step_rules(const void* logits, long ld_logits,
                                              int dtype, void* stream, const int* prefix, int ld_prefix,
                                              const int* prefix_len, int no_repeat_ngram, int min_length);
 
+/* ---- ensemble decoding (fira_icse_b200/ensemble.py): M <= 8 models' mixtures (Model.py:54-86) averaged into one fp32
+ *      triple the three step kernels above read with dtype FIRA_F32.  Member m: logits[m] (`dtype`, [B*N, ld_logits],
+ *      16-byte aligned), copy_scores[m] [B, N, S] fp32, gate_logits[m] [B*N, 2] fp32 (host arrays of M device
+ *      pointers, copied into the launch); log_weights [M] fp32 device (log w_m, sum w_m = 1; read at run time, so a
+ *      captured launch follows new weights); mem_mask [B, S].  With P^m_j = g0^m softmax(x^m)_j (j < V) and
+ *      g1^m softmax(masked c^m)_s (j = V + s), and member m's row statistics vmax, vsum, cmax, csum, g0, g1 formed as
+ *      its own step kernel forms them, G0 = sum_m w_m g0^m, G1 = sum_m w_m g1^m:
+ *        x'_j = LSE over m with w_m g0^m > 0 of [log(w_m g0^m / G0) + x^m_j - vmax^m - log vsum^m]
+ *        c'_s = LSE over m with w_m g1^m > 0 of [log(w_m g1^m / G1) + c^m_s - cmax^m - log csum^m]  (masked s: -1e9)
+ *        gl'  = (log G0, log G1)
+ *      so the step kernels' mixture of (x', c', gl') is P = sum_m w_m P^m up to fp32 rounding.  G0 == 0 (G1 == 0) uses
+ *      log w_m as the offsets of x' (c'), and gl'_0 = -inf (gl'_1) makes that gate exactly 0.  Output: logits_out
+ *      [B*N, ld_out] fp32 (16-byte aligned, columns >= V untouched), copy_out [B, N, S], gate_out [B*N, 2].  One CTA of
+ *      256 threads per row.  1 <= M <= 8, ld_logits and ld_out multiples of 8 and >= V, V + S <= 32767. */
+int fira_pointer_mix_ensemble(const void* const* logits, long ld_logits, const float* const* copy_scores,
+                              const float* const* gate_logits, int M, const float* log_weights,
+                              const unsigned char* mem_mask, float* logits_out, long ld_out, float* copy_out,
+                              float* gate_out, int B, int N, int V, int S, int dtype, void* stream);
+
 /* ---- minimum-Bayes-risk selection among each commit's N samples (fira_icse_b200/mbr.py).  seq [B, N, ld_seq] int32
  *      (row (b, n) at (b*N + n) * ld_seq, columns 0..T_len-1), length [B, N] int32 (counts <start>; clamped to
  *      [1, T_len]).  Rule:

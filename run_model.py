@@ -43,6 +43,11 @@ beam search ranking.  Differences, all below the module surface:
     (output_fira_nbest_norepeat2_minlen3, ...), so the outputs without them stay.  FIRA_DECODE=beam with either set
     exits with an error.
     FIRA_CHECKPOINT (default best_model.pt): the state_dict `test` decodes with (best_model_scst.pt after finetune).
+    FIRA_ENSEMBLE=a.pt,b.pt[,...] (FIRA_DECODE=sample, nbest or mbr; up to 8 state_dicts, not with FIRA_CHECKPOINT):
+    decode with the ensemble of those checkpoints (fira_icse_b200.ensemble: the weighted average of their
+    distributions at every position), weighted by FIRA_ENSEMBLE_WEIGHTS=w1,w2,... (positive, one per checkpoint;
+    default uniform).  Appends _ens<M> to the output name after the other tags (output_fira_nbest_norepeat2_ens2, ...),
+    so single-model outputs stay.  FIRA_DECODE=beam with an ensemble exits with an error.
   * `finetune`: self-critical fine-tuning on sentence BLEU (fira_icse_b200.scst, DESIGN.md §9), one GPU.  Loads
     best_model.pt and runs FIRA_SCST_EPOCHS (default 1) epochs of scst_step with optim.FlatAdam at FIRA_SCST_LR
     (default 1e-5) over padded batches of FIRA_BATCH commits (FIRA_MAX_BATCHES bounds an epoch): FIRA_SAMPLES (default
@@ -68,6 +73,7 @@ from fira_icse_b200.beam import beam_search, best_sequences, nbest
 from fira_icse_b200.bleu import sentence_bleu_method2
 from fira_icse_b200.data import PackedBatchLoader, TransDataset, batch_to_device, collate_packed
 from fira_icse_b200.engine import GraphedTrainStep
+from fira_icse_b200.ensemble import MAX_MEMBERS, Ensemble
 from fira_icse_b200.mbr import mbr
 from fira_icse_b200.parallel import DataParallelStep, shard_range
 from fira_icse_b200.sample import sample
@@ -276,8 +282,9 @@ def decoder(mode, vocab):
         raise SystemExit("FIRA_NO_REPEAT_NGRAM and FIRA_MIN_LENGTH apply to FIRA_DECODE=sample, nbest and mbr; the "
                          "reference beam search takes no rules")
     rules = dict(no_repeat_ngram=no_repeat, min_length=min_len)
+    ens = ensemble_settings(mode)
     tag = (f"_prefix{k}" if k else "") + (f"_norepeat{no_repeat}" if no_repeat else "") + \
-        (f"_minlen{min_len}" if min_len else "")
+        (f"_minlen{min_len}" if min_len else "") + (f"_ens{len(ens[0])}" if ens else "")
 
     def pre(b):                         # each commit's own first k reference labels, or no prefix
         return reference_prefix(b, k, vocab['<eos>'], vocab['<pad>']) if k else None
@@ -346,18 +353,59 @@ def test(model, test_loader, g, test_index, dev_, first_index, decode, n_bleu, o
     return bleus / max(1, total * n_bleu)
 
 
+def ensemble_settings(mode):
+    """FIRA_ENSEMBLE / FIRA_ENSEMBLE_WEIGHTS -> (checkpoint paths, weights or None for uniform), or None without an
+    ensemble; checked before any device work (SystemExit on an error)."""
+    spec, wspec = os.environ.get("FIRA_ENSEMBLE", ""), os.environ.get("FIRA_ENSEMBLE_WEIGHTS", "")
+    if not spec:
+        if wspec:
+            raise SystemExit("FIRA_ENSEMBLE_WEIGHTS needs FIRA_ENSEMBLE")
+        return None
+    if mode == "beam":
+        raise SystemExit("FIRA_ENSEMBLE applies to FIRA_DECODE=sample, nbest and mbr; the reference beam search decodes "
+                         "one model")
+    if "FIRA_CHECKPOINT" in os.environ:
+        raise SystemExit("FIRA_ENSEMBLE names the checkpoints itself: unset FIRA_CHECKPOINT")
+    paths = [p.strip() for p in spec.split(",")]
+    if not all(paths) or not 1 <= len(paths) <= MAX_MEMBERS:
+        raise SystemExit(f"FIRA_ENSEMBLE must list 1 to {MAX_MEMBERS} checkpoints separated by commas, got {spec!r}")
+    weights = None
+    if wspec:
+        try:
+            weights = [float(w) for w in wspec.split(",")]
+        except ValueError:
+            raise SystemExit(f"FIRA_ENSEMBLE_WEIGHTS must be numbers separated by commas, got {wspec!r}")
+        if len(weights) != len(paths):
+            raise SystemExit(f"FIRA_ENSEMBLE_WEIGHTS has {len(weights)} weights for {len(paths)} checkpoints")
+        if not all(0.0 < w < float("inf") for w in weights):
+            raise SystemExit(f"FIRA_ENSEMBLE_WEIGHTS must be positive finite numbers, got {wspec!r}")
+    for p in paths:
+        if not os.path.isfile(p):
+            raise SystemExit(f"FIRA_ENSEMBLE: checkpoint {p} not found")
+    return paths, weights
+
+
+def load_model(path, dev_):
+    model = TransModel(args)
+    model.load_state_dict(torch.load(path, map_location="cpu"))
+    return model.to(dev_)
+
+
 def main_test():
+    mode = os.environ.get("FIRA_DECODE", "beam")
+    ens = ensemble_settings(mode)
     dev_ = device()
     g = load_globals()
     test_set = TransDataset(args, 'test')
     all_index = json.load(open('all_index'))
-    model = TransModel(args)
-    model.load_state_dict(torch.load(os.environ.get("FIRA_CHECKPOINT", "best_model.pt"), map_location="cpu"))
-    model = model.to(dev_)
+    if ens:
+        model = Ensemble([load_model(p, dev_) for p in ens[0]], ens[1])
+    else:
+        model = load_model(os.environ.get("FIRA_CHECKPOINT", "best_model.pt"), dev_)
     lo, hi = shard_range(len(test_set), RANK, WORLD)                # replicas only: index ranges, files concatenated
     idx = list(range(lo, hi)) if WORLD > 1 else None
     test_loader = loader(test_set, args.test_batch_size, False, idx)
-    name, decode, n_bleu = decoder(os.environ.get("FIRA_DECODE", "beam"), g["vocab"])
+    name, decode, n_bleu = decoder(mode, g["vocab"])
     out = f"OUTPUT/{name}" if WORLD == 1 else f"OUTPUT/{name}.part{RANK:02d}"
     bleu = test(model, test_loader, g, all_index['test'][lo:hi], dev_, lo, decode, n_bleu, out)
     print("mean sentence bleu: %f" % bleu)

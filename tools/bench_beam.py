@@ -23,6 +23,14 @@ reference's own loop was timed on in BASELINE.md (72 s for 32 commits on CPU).  
                                a word repeats an n-gram, n = repeat_share_n = n or 2, and mean_length (tokens with
                                <start> and <eos>); the lines with the rules carry no_repeat_ngram and min_length)
 
+    python tools/bench_beam.py --ensemble 1,2,4 [--batches ...] [--beams ...] [--precision ...] [--reps ...]
+                               (ensemble decoding instead of the modes above: for each member count M, an
+                               ensemble.Ensemble of the bench model and M - 1 copies whose out_fc / copy_net weights
+                               carry their own seeded perturbation; sample, nbest and mbr per batch at the first beam
+                               width, then fira_pointer_mix_ensemble alone with its algorithmic bytes per row
+                               M * 2 * (V * s + S * 4) + (V + S) * 4 (s = 2 bytes in bf16, 4 in fp32: each member row is
+                               read twice, the fp32 triple written once) and the share of HBM peak that implies)
+
 nbest and diverse lines also carry `self_bleu`: the mean pairwise id-level sentence BLEU among each commit's K
 hypotheses (one fira_mbr_select launch with pair_bleu, off-diagonal entries averaged over the batch); lower means a
 more diverse list.
@@ -33,7 +41,9 @@ selection with bleu.sentence_bleu_method2 (tests/mbr_rule.py, one pass over the 
 between the two.
 """
 import argparse
+import ctypes
 import json
+import math
 import os
 import sys
 import time
@@ -55,6 +65,7 @@ def main():
     ap.add_argument("--prefix-words", type=int, default=0, help="also time the decoders with k-label reference prefixes")
     ap.add_argument("--no-repeat-ngram", type=int, default=0, help="also time the decoders with n-gram repeat blocking")
     ap.add_argument("--min-length", type=int, default=0, help="also time the decoders with a minimum message length")
+    ap.add_argument("--ensemble", default="", help="member counts M to time ensemble decoding at (e.g. 1,2,4)")
     a = ap.parse_args()
     rules = (a.no_repeat_ngram, a.min_length)
     import torch
@@ -71,6 +82,8 @@ def main():
     model = F.TransModel(bench.model_args()).to(dev)
     model.set_precision(a.precision)
     model.eval()
+    if a.ensemble:
+        return bench_ensemble(a, model, dev)
     for B in (int(x) for x in a.batches.split(",")):
         hb = bench.host_batch(10_000, B, pin=False, trim=a.trim)
         b = bench.device_batch(hb, dev, B)
@@ -145,6 +158,97 @@ def main():
                   flush=True)
             if mode == "mbr":
                 print(json.dumps(mbr_select_timing(out.samples, B, K)), flush=True)
+
+
+HBM_PEAK_GBS = 3350.0     # H100 SXM5 80 GB HBM3 peak
+
+
+def bench_ensemble(a, model, dev):
+    """--ensemble: decoders and the combine kernel at each member count (module docstring)."""
+    import copy
+    import torch
+    import bench
+    from fira_icse_b200 import ops
+    from fira_icse_b200._lib import FIRA_BF16, FIRA_F32, call
+    from fira_icse_b200.beam import nbest
+    from fira_icse_b200.ensemble import Ensemble
+    from fira_icse_b200.mbr import mbr
+    from fira_icse_b200.sample import sample
+    counts = [int(x) for x in a.ensemble.split(",")]
+    K = int(a.beams.split(",")[0])
+    pool = [model]
+    for i in range(1, max(counts)):
+        m = copy.deepcopy(model)
+        g = torch.Generator(device=dev).manual_seed(i)
+        with torch.no_grad():
+            for p in (m.out_fc.weight, m.copy_net.LinearRes.weight, m.copy_net.LinearProb.weight):
+                p.add_(torch.randn(p.shape, generator=g, device=dev) * p.std() * 0.1)
+        pool.append(m.set_precision(a.precision).eval())
+    card, watts = torch.cuda.get_device_name(dev), power_limit()
+    ids = dict(tar_len=30, start_id=1, eos_id=2, pad_id=0)
+    for B in (int(x) for x in a.batches.split(",")):
+        b = bench.device_batch(bench.host_batch(10_000, B, pin=False, trim=a.trim), dev, B)
+        S = b[0].shape[1] + b[7].shape[1]
+        for M in counts:
+            ens = Ensemble(pool[:M])
+            runs = {"sample": lambda: sample(ens, b[0], b[3], b[4], b[5], b[7], num_samples=K, **ids),
+                    "nbest": lambda: nbest(ens, b[0], b[3], b[4], b[5], b[7], beam_size=K, **ids),
+                    "mbr": lambda: mbr(ens, b[0], b[3], b[4], b[5], b[7], num_samples=K, **ids)}
+            for mode, run in runs.items():
+                out = run()                                              # warm-up (graph capture)
+                torch.cuda.synchronize()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                for _ in range(a.reps):
+                    out = run()
+                e1.record()
+                torch.cuda.synchronize()
+                ms = e0.elapsed_time(e1) / a.reps
+                length = out.samples.length if mode == "mbr" else out.length
+                print(json.dumps({"metric": "ensemble decoding throughput", "unit": "commits/s", "value": B / ms * 1e3,
+                                  "ms_per_batch": ms, "batch": B, "beam": K, "members": M, "mode": mode,
+                                  "decoded_steps": int(length.max().item()) - 1, "precision": a.precision,
+                                  "card": card, "power_limit_w": watts,
+                                  "data": "synthetic (DataSet distribution), random weights, perturbed copies"}),
+                      flush=True)
+            # the combine alone: rotating member buffers (more than L2 in all), launches replayed from a CUDA graph
+            V, R = model.vocab_size, B * K
+            ldl = ops._ld_logits(V)
+            tdt = torch.bfloat16 if a.precision == "bf16" else torch.float32
+            es = 2 if a.precision == "bf16" else 4
+            set_bytes = M * R * (ldl * es + S * 4 + 8)
+            n_rot = max(2, -(-200 * 2 ** 20 // set_bytes))
+            gen = torch.Generator(device=dev).manual_seed(M)
+            sets = []
+            for _ in range(n_rot):
+                mem = [(torch.randn((R, ldl), generator=gen, device=dev).to(tdt),
+                        torch.randn((B, K, S), generator=gen, device=dev), torch.randn((R, 2), generator=gen, device=dev))
+                       for _ in range(M)]
+                arr = [(ctypes.c_void_p * M)(*[ops._ptr(t[k]) for t in mem]) for k in range(3)]
+                sets.append((mem, arr))
+            mask = torch.ones((B, S), dtype=torch.uint8, device=dev)
+            lw = torch.full((M,), -math.log(M), dtype=torch.float32, device=dev)
+            x = torch.empty((R, ldl), dtype=torch.float32, device=dev)
+            c = torch.empty((B, K, S), dtype=torch.float32, device=dev)
+            gl = torch.empty((R, 2), dtype=torch.float32, device=dev)
+
+            def launch(i):
+                arr = sets[i % n_rot][1]
+                call("fira_pointer_mix_ensemble", ctypes.addressof(arr[0]), ldl, ctypes.addressof(arr[1]),
+                     ctypes.addressof(arr[2]), M, ops._ptr(lw), ops._ptr(mask), ops._ptr(x), ldl, ops._ptr(c),
+                     ops._ptr(gl), B, K, V, S, FIRA_BF16 if a.precision == "bf16" else FIRA_F32, ops._stream())
+            _, med_ms, launches = bench.time_launches(launch, n_rot)
+            row_bytes = M * 2 * (V * es + S * 4) + (V + S) * 4
+            gbs = row_bytes * R / (med_ms * 1e-3) / 1e9
+            print(json.dumps({"metric": "fira_pointer_mix_ensemble time", "unit": "us", "value": med_ms * 1e3,
+                              "batch": B, "rows": R, "members": M, "V": V, "S": S, "precision": a.precision,
+                              "algorithmic_bytes_per_row": row_bytes, "algorithmic_GB_per_s": gbs,
+                              "share_of_hbm_peak": gbs / HBM_PEAK_GBS, "hbm_peak_GB_per_s": HBM_PEAK_GBS,
+                              "timed_launches": launches, "rotating_sets": n_rot, "card": card, "power_limit_w": watts,
+                              "note": "median device time per launch, launches replayed from one CUDA graph between "
+                                      "CUDA events; bytes count each member row twice (the second read is meant to "
+                                      "come from L2)"}), flush=True)
+            del sets
 
 
 def self_bleu(h, B, K):
