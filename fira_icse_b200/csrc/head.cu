@@ -1214,6 +1214,252 @@ __global__ void __launch_bounds__(kEnsThreads) pointer_mix_ensemble_kernel(
   if (threadIdx.x == 0) { gl_out[row * 2] = s_gate[0]; gl_out[row * 2 + 1] = s_gate[1]; }
 }
 
+// ------------------------------------------------------------------ knowledge distillation loss
+// Row r with shifted label y != 0: the student's mixture P (head_fwd_kernel's expressions) against the teacher's t (the
+// same expressions on the teacher's fp32 triple, fira_pointer_mix_ensemble's output):
+//   nll = -log clamp(P_y, 1e-10, 1),  kd = -sum_j t_j log clamp(P_j, 1e-10, 1),  loss = (1 - alpha) nll + alpha kd
+//   a_j = [(1 - alpha) [j == y] + alpha t_j] live_j  (live_j: 1e-10 <= P_j <= 1),  A_V = sum_{j<V} a_j,  A_C = the rest
+// The clamp needs the final row statistics before any term, so the forward walks both rows twice: statistics, then kd,
+// A_V and A_C.  The backward reads A_V / A_C from the stats row and walks both rows once.
+// stats row (16 floats): student vmax vsum cmax csum g0 g1, p_label, 0, teacher vmax vsum cmax csum g0 g1, A_V, A_C
+constexpr int kKdThreads = 256;                       // = head_fwd_kernel's block: the same student statistics
+constexpr int kKdStats = 16;
+
+struct KdRow {
+  float vmax, iv, g0, lv;            // student vocabulary side: P_j = g0 (e^(x_j - vmax) iv), log P_j = x_j + lv
+  float cmax, ic, g1, lc;            // student copy side
+  float tvmax, tiv, tg0, tcmax, tic, tg1;
+  float p_lab, lp_lab, hard, alpha;  // P_y as head_fwd_kernel forms it, log clamp(P_y), 1 - alpha, alpha
+  int y;
+};
+__device__ __forceinline__ KdRow kd_row(const float* st, float alpha, int y) {
+  KdRow k;
+  k.vmax = st[0]; k.iv = 1.f / st[1]; k.g0 = st[4]; k.lv = logf(st[4]) - st[0] - logf(st[1]);
+  k.cmax = st[2]; k.ic = 1.f / st[3]; k.g1 = st[5]; k.lc = logf(st[5]) - st[2] - logf(st[3]);
+  k.tvmax = st[8]; k.tiv = 1.f / st[9]; k.tcmax = st[10]; k.tic = 1.f / st[11]; k.tg0 = st[12]; k.tg1 = st[13];
+  k.p_lab = st[6]; k.lp_lab = logf(fminf(fmaxf(st[6], 1e-10f), 1.f));
+  k.hard = 1.f - alpha; k.alpha = alpha; k.y = y;
+  return k;
+}
+// a_j of entry j from the student's P_j and the teacher's t_j (forward and backward form it the same way)
+__device__ __forceinline__ float kd_weight(const KdRow& k, int j, float p, float t) {
+  return (p >= 1e-10f && p <= 1.f) ? fmaf(k.alpha, t, j == k.y ? k.hard : 0.f) : 0.f;
+}
+// forward term of entry j: a_j into `acc`, -t_j log clamp(P_j) into `kd` (t_j == 0 adds nothing; lp: log P_j if live)
+__device__ __forceinline__ void kd_term(const KdRow& k, int j, float p, float t, float lp, float& kd, float& acc) {
+  acc += kd_weight(k, j, p, t);
+  if (t > 0.f) {
+    const float l = j == k.y ? k.lp_lab : (p >= 1e-10f && p <= 1.f) ? lp : (p < 1e-10f ? logf(1e-10f) : 0.f);
+    kd = fmaf(-t, l, kd);
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kKdThreads) pointer_mix_kd_fwd_kernel(
+    const T* __restrict__ logits, long ldl, const float* __restrict__ sc, const float* __restrict__ gate_logit,
+    const unsigned char* __restrict__ mem_mask, const int* __restrict__ label, const float* __restrict__ t_logits,
+    long ldt, const float* __restrict__ t_sc, const float* __restrict__ t_gate_logit, float alpha,
+    float* __restrict__ stats, float* __restrict__ nll, float* __restrict__ kd, float* __restrict__ loss, int Tn, int V,
+    int S) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  __shared__ MaxSum sh_ms[2][8];
+  __shared__ float bc[8];
+  __shared__ float shf[8];
+  __shared__ float s_st[kKdStats];
+  const long row = blockIdx.x;
+  const int y = label[row];
+  float* st = stats + row * kKdStats;
+  if (y == 0) {                                       // no loss: neither row is read
+    if (threadIdx.x < kKdStats) st[threadIdx.x] = 0.f;
+    if (threadIdx.x == 0) { nll[row] = 0.f; kd[row] = 0.f; loss[row] = 0.f; }
+    return;
+  }
+  const int b = (int)(row / Tn);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const T* lrow = logits + row * ldl;
+  const float* srow = sc + row * S;
+  const float* trow = t_logits + row * ldt;
+  const float* tsrow = t_sc + row * S;
+  const unsigned char* mrow = mem_mask + (long)b * S;
+
+  // pass 1: both rows' statistics, student and teacher in the same loops.  The student's arithmetic and reduction order
+  // are mix_row_stats' (= head_fwd_kernel's), so its P_y and nll are fira_pointer_mix_nll_fwd's bit for bit.
+  MaxSum v{-INFINITY, 0.f}, u{-INFINITY, 0.f};
+  const int V8 = V >> 3;
+  for (int g = threadIdx.x; g < V8; g += blockDim.x) {
+    float x[8], z[8];
+    Act<T>::load8(lrow + (long)g * 8, x);
+    Act<float>::load8(trow + (long)g * 8, z);
+    float m8 = x[0], n8 = z[0];
+#pragma unroll
+    for (int i = 1; i < 8; ++i) { m8 = fmaxf(m8, x[i]); n8 = fmaxf(n8, z[i]); }
+    if (m8 > v.m) { v.s *= expf(v.m - m8); v.m = m8; }
+    if (n8 > u.m) { u.s *= expf(u.m - n8); u.m = n8; }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { v.s += expf(x[i] - v.m); u.s += expf(z[i] - u.m); }
+  }
+  for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) {
+    v = ms_merge(v, MaxSum{Act<T>::ld(lrow + j), 1.f});
+    u = ms_merge(u, MaxSum{trow[j], 1.f});
+  }
+  v = ms_warp(v); u = ms_warp(u);
+  if (lane == 0) { sh_ms[0][warp] = v; sh_ms[1][warp] = u; }
+  __syncthreads();
+  if (warp < 2) {
+    MaxSum w = lane < 8 ? sh_ms[warp][lane] : MaxSum{-INFINITY, 0.f};
+    w = ms_warp(w);
+    if (lane == 0) { bc[4 * warp] = w.m; bc[4 * warp + 1] = w.s; }
+  }
+  __syncthreads();
+  MaxSum c{-INFINITY, 0.f}, d{-INFINITY, 0.f};
+  for (int j = threadIdx.x; j < S; j += blockDim.x) {
+    const bool m = mrow[j];
+    c = ms_merge(c, MaxSum{m ? srow[j] : kMaskFill, 1.f});
+    d = ms_merge(d, MaxSum{m ? tsrow[j] : kMaskFill, 1.f});
+  }
+  c = ms_warp(c); d = ms_warp(d);
+  if (lane == 0) { sh_ms[0][warp] = c; sh_ms[1][warp] = d; }
+  __syncthreads();
+  if (warp < 2) {
+    MaxSum w = lane < 8 ? sh_ms[warp][lane] : MaxSum{-INFINITY, 0.f};
+    w = ms_warp(w);
+    if (lane == 0) { bc[4 * warp + 2] = w.m; bc[4 * warp + 3] = w.s; }
+  }
+  __syncthreads();
+  if (threadIdx.x < 2) {                              // thread 0: the student's gates, thread 1: the teacher's
+    const float* gl = (threadIdx.x ? t_gate_logit : gate_logit) + row * 2;
+    const float gl0 = gl[0], gl1 = gl[1];
+    const float gm = fmaxf(gl0, gl1);
+    const float e0 = expf(gl0 - gm), e1 = expf(gl1 - gm);
+    float* o = s_st + 8 * threadIdx.x;
+    o[0] = bc[4 * threadIdx.x]; o[1] = bc[4 * threadIdx.x + 1]; o[2] = bc[4 * threadIdx.x + 2];
+    o[3] = bc[4 * threadIdx.x + 3]; o[4] = e0 / (e0 + e1); o[5] = e1 / (e0 + e1);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {                             // P_y exactly as head_fwd_kernel forms it
+    const float vmax = s_st[0], vsum = s_st[1], cmax = s_st[2], csum = s_st[3], g0 = s_st[4], g1 = s_st[5];
+    float p;
+    if (y < V) p = g0 * (expf(Act<T>::ld(lrow + y) - vmax) / vsum);
+    else {
+      const int s = y - V;                            // a copy label beyond S: p = 0, the clamp floor, no gradient
+      p = s < S ? g1 * (expf((mrow[s] ? srow[s] : kMaskFill) - cmax) / csum) : 0.f;
+    }
+    s_st[6] = p; s_st[7] = 0.f;
+  }
+  __syncthreads();
+
+  // pass 2: kd, A_V and A_C in fixed order (per-thread sums, then block_reduce)
+  const KdRow k = kd_row(s_st, alpha, y);
+  float kdp = 0.f, av = 0.f, ac = 0.f;
+  for (int g = threadIdx.x; g < V8; g += blockDim.x) {
+    float x[8], z[8];
+    Act<T>::load8(lrow + (long)g * 8, x);
+    Act<float>::load8(trow + (long)g * 8, z);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int j = g * 8 + i;
+      const float p = j == y ? k.p_lab : k.g0 * (expf(x[i] - k.vmax) * k.iv);
+      kd_term(k, j, p, k.tg0 * (expf(z[i] - k.tvmax) * k.tiv), x[i] + k.lv, kdp, av);
+    }
+  }
+  for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) {
+    const float x = Act<T>::ld(lrow + j);
+    const float p = j == y ? k.p_lab : k.g0 * (expf(x - k.vmax) * k.iv);
+    kd_term(k, j, p, k.tg0 * (expf(trow[j] - k.tvmax) * k.tiv), x + k.lv, kdp, av);
+  }
+  for (int s = threadIdx.x; s < S; s += blockDim.x) {
+    const bool m = mrow[s];
+    const float x = m ? srow[s] : kMaskFill;
+    const float p = V + s == y ? k.p_lab : k.g1 * (expf(x - k.cmax) * k.ic);
+    kd_term(k, V + s, p, m ? k.tg1 * (expf(tsrow[s] - k.tcmax) * k.tic) : 0.f, x + k.lc, kdp, ac);
+  }
+  auto add = [](float a, float x) { return a + x; };
+  kdp = block_reduce(kdp, shf, add);
+  av = block_reduce(av, shf, add);
+  ac = block_reduce(ac, shf, add);
+  if (threadIdx.x < kKdStats) st[threadIdx.x] = threadIdx.x == 14 ? av : threadIdx.x == 15 ? ac : s_st[threadIdx.x];
+  if (threadIdx.x == 0) {
+    const float h = -k.lp_lab;                        // = fira_pointer_mix_nll_fwd's nll
+    nll[row] = h;
+    kd[row] = kdp;
+    loss[row] = fmaf(alpha, kdp, k.hard * h);
+  }
+}
+
+// d(sum_r upstream * loss_r) / d(logits, copy scores, gate logits) from the forward's stats rows:
+//   dx_k = u (p_k A_V - a_k),  dc_s = u (q_s A_C - a_{V+s}) (0 at a masked s),  dgl = u (g (A_V + A_C) - (A_V, A_C))
+// with p, q the two softmaxes.  A side whose A is 0 is written as zeros without reading the rows.
+template <typename T>
+__global__ void __launch_bounds__(kKdThreads) pointer_mix_kd_bwd_kernel(
+    const T* __restrict__ logits, long ldl, const float* __restrict__ sc, const unsigned char* __restrict__ mem_mask,
+    const int* __restrict__ label, const float* __restrict__ t_logits, long ldt, const float* __restrict__ t_sc,
+    float alpha, const float* __restrict__ stats, const float* __restrict__ upstream, T* __restrict__ d_logits,
+    float* __restrict__ d_sc, float* __restrict__ d_gate_logit, unsigned char* __restrict__ row_active, int Tn, int V,
+    int S) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  const long row = blockIdx.x;
+  const int b = (int)(row / Tn);
+  const int y = label[row];
+  const float* st = stats + row * kKdStats;
+  const float A_V = y ? st[14] : 0.f, A_C = y ? st[15] : 0.f;
+  const float up = *upstream;
+  const KdRow k = kd_row(st, alpha, y);
+  const T* lrow = logits + row * ldl;
+  const float* trow = t_logits + row * ldt;
+  T* drow = d_logits + row * ldl;
+  const int V8 = V >> 3;                              // 8 logits per vector load / store, scalar tail
+  if (A_V != 0.f) {
+    const float sv = k.iv * A_V;
+    for (int g = threadIdx.x; g < V8; g += blockDim.x) {
+      float x[8], z[8];
+      Act<T>::load8(lrow + (long)g * 8, x);
+      Act<float>::load8(trow + (long)g * 8, z);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int j = g * 8 + i;
+        const float e = expf(x[i] - k.vmax);
+        const float a = kd_weight(k, j, j == y ? k.p_lab : k.g0 * (e * k.iv), k.tg0 * (expf(z[i] - k.tvmax) * k.tiv));
+        x[i] = up * (e * sv - a);
+      }
+      Act<T>::store8(drow + (long)g * 8, x);
+    }
+    for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) {
+      const float e = expf(Act<T>::ld(lrow + j) - k.vmax);
+      const float a = kd_weight(k, j, j == y ? k.p_lab : k.g0 * (e * k.iv), k.tg0 * (expf(trow[j] - k.tvmax) * k.tiv));
+      Act<T>::st(drow + j, up * (e * sv - a));
+    }
+  } else {
+    const float z[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int g = threadIdx.x; g < V8; g += blockDim.x) Act<T>::store8(drow + (long)g * 8, z);
+    for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) Act<T>::st(drow + j, 0.f);
+  }
+  const float* srow = sc + row * S;
+  const float* tsrow = t_sc + row * S;
+  const unsigned char* mrow = mem_mask + (long)b * S;
+  float* dsrow = d_sc + row * S;
+  if (A_C != 0.f) {
+    const float scc = k.ic * A_C;
+    for (int s = threadIdx.x; s < S; s += blockDim.x) {
+      float r = 0.f;                                  // a masked position takes no gradient (masked_fill)
+      if (mrow[s]) {
+        const int j = V + s;
+        const float e = expf(srow[s] - k.cmax);
+        const float a = kd_weight(k, j, j == y ? k.p_lab : k.g1 * (e * k.ic), k.tg1 * (expf(tsrow[s] - k.tcmax) * k.tic));
+        r = up * (e * scc - a);
+      }
+      dsrow[s] = r;
+    }
+  } else {
+    for (int s = threadIdx.x; s < S; s += blockDim.x) dsrow[s] = 0.f;
+  }
+  if (threadIdx.x == 0) {
+    const float A = A_V + A_C;
+    d_gate_logit[row * 2] = y ? up * (k.g0 * A - A_V) : 0.f;
+    d_gate_logit[row * 2 + 1] = y ? up * (k.g1 * A - A_C) : 0.f;
+    row_active[row] = A_C != 0.f ? 1 : 0;
+  }
+}
+
 }  // namespace
 
 #define DISPATCH_T(dtype, ...)                                                            \
@@ -1642,6 +1888,53 @@ int fira_pointer_mix_ensemble(const void* const* logits, long ld_logits, const f
   DISPATCH_T(dtype, launch_k(pointer_mix_ensemble_kernel<T>, dim3((unsigned)(B * N)), dim3(kEnsThreads), 0,
       (cudaStream_t)stream, mem, M, ld_logits, log_weights, mem_mask, logits_out, ld_out, copy_out, gate_out, N, V, S);)
   FIRA_CHECK_LAUNCH("fira_pointer_mix_ensemble");
+  return FIRA_OK;
+}
+
+static int kd_check(const char* who, const void* logits, long ld_logits, const float* t_logits, long ld_t, float alpha,
+                    long rows, int T_len, int V, int S) {
+  FIRA_CHECK_ARG(alpha >= 0.f && alpha <= 1.f, FIRA_ERR_ARG, "%s: alpha %g not in [0, 1]", who, (double)alpha);
+  FIRA_CHECK_ARG(rows >= 0 && T_len > 0 && V > 0 && S > 0 && V + S <= 0x7FFF && ld_logits >= V && ld_t >= V,
+                 FIRA_ERR_SHAPE, "%s: shape (rows %ld, T_len %d, V %d, S %d, ld_logits %ld, ld_t %ld; V + S must be <= 32767)",
+                 who, rows, T_len, V, S, ld_logits, ld_t);
+  FIRA_CHECK_ARG(fira_aligned16(logits) && fira_aligned16(t_logits) && ld_logits % 8 == 0 && ld_t % 8 == 0,
+                 FIRA_ERR_ALIGN, "%s: logits / teacher logits must be 16-byte aligned with leading dimensions that are "
+                 "multiples of 8", who);
+  return FIRA_OK;
+}
+
+int fira_pointer_mix_kd_fwd(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                            const unsigned char* mem_mask, const int* label, const float* t_logits, long ld_t,
+                            const float* t_copy_scores, const float* t_gate_logits, float alpha, float* stats,
+                            float* nll, float* kd, float* loss, long rows, int T_len, int V, int S, int dtype,
+                            void* stream) {
+  FIRA_CHECK_ARG(logits && copy_scores && gate_logits && mem_mask && label && t_logits && t_copy_scores && t_gate_logits
+                 && stats && nll && kd && loss, FIRA_ERR_ARG, "pointer_mix_kd_fwd: null pointer");
+  const int rc = kd_check("pointer_mix_kd_fwd", logits, ld_logits, t_logits, ld_t, alpha, rows, T_len, V, S);
+  if (rc != FIRA_OK) return rc;
+  if (rows == 0) return FIRA_OK;
+  DISPATCH_T(dtype, launch_k(pointer_mix_kd_fwd_kernel<T>, dim3((unsigned)rows), dim3(kKdThreads), 0,
+      (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, label, t_logits, ld_t,
+      t_copy_scores, t_gate_logits, alpha, stats, nll, kd, loss, T_len, V, S);)
+  FIRA_CHECK_LAUNCH("fira_pointer_mix_kd_fwd");
+  return FIRA_OK;
+}
+
+int fira_pointer_mix_kd_bwd(const void* logits, long ld_logits, const float* copy_scores,
+                            const unsigned char* mem_mask, const int* label, const float* t_logits, long ld_t,
+                            const float* t_copy_scores, float alpha, const float* stats, const float* upstream,
+                            void* d_logits, float* d_copy_scores, float* d_gate_logits, unsigned char* row_active,
+                            long rows, int T_len, int V, int S, int dtype, void* stream) {
+  FIRA_CHECK_ARG(logits && copy_scores && mem_mask && label && t_logits && t_copy_scores && stats && upstream && d_logits
+                 && d_copy_scores && d_gate_logits && row_active, FIRA_ERR_ARG, "pointer_mix_kd_bwd: null pointer");
+  const int rc = kd_check("pointer_mix_kd_bwd", logits, ld_logits, t_logits, ld_t, alpha, rows, T_len, V, S);
+  if (rc != FIRA_OK) return rc;
+  FIRA_CHECK_ARG(fira_aligned16(d_logits), FIRA_ERR_ALIGN, "pointer_mix_kd_bwd: d_logits must be 16-byte aligned");
+  if (rows == 0) return FIRA_OK;
+  DISPATCH_T(dtype, launch_k(pointer_mix_kd_bwd_kernel<T>, dim3((unsigned)rows), dim3(kKdThreads), 0,
+      (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, mem_mask, label, t_logits, ld_t, t_copy_scores,
+      alpha, stats, upstream, (T*)d_logits, d_copy_scores, d_gate_logits, row_active, T_len, V, S);)
+  FIRA_CHECK_LAUNCH("fira_pointer_mix_kd_bwd");
   return FIRA_OK;
 }
 

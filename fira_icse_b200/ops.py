@@ -853,15 +853,32 @@ def copy_scores_fwd(pr, memory2, dec2, Ws, Wt, wres, bres, B, T, S, src_mask=Non
     return src, tgt, sc
 
 
+def head_products(pr, memory2, dec2, dec32, dec_v, cap, Wout, bout, Ws, Wt, Wres, bres, Wp, bp, B, T, S, mem_mask,
+                  row_mask, ranges=None):
+    """The output head's three products (Model.py:54-60): out_fc logits of the `cap` rows dec_v ([cap, _ld_logits(V)],
+    pr's dtype), the pointer scores [B, T, S] with the two projections their backward reads, and the fp32 gate logits
+    [B*T, 2] of dec32 -> (logits, src, tgt, sc, gl)."""
+    logits = pr.empty((cap, _ld_logits(Wout.shape[0])), dec2.device)
+    pr.linear(dec_v, Wout, bout, out=logits, ld_out=logits.shape[1])
+    src, tgt, sc = copy_scores_fwd(pr, memory2, dec2, Ws, Wt, Wres, bres, B, T, S, src_mask=mem_mask, row_mask=row_mask,
+                                   ranges=ranges)
+    gl = linear(dec32, Wp, bp)                # fp32 [Mt, 2]
+    return logits, src, tgt, sc, gl
+
+
 class HeadFn(torch.autograd.Function):
     """Model.py:54-86 fused: out_fc, CopyNet, both softmaxes, gate mixing, log(clamp), shifted-label
     NLL -- returns (loss_sum, per-position nll, argmax ids or None).  The B x 30 x 25,020 distribution
     is never built.  seq_weight (fp32 [B] on the device, padded batches only): loss_sum = sum_b seq_weight[b] *
-    sum_t nll[b, t] (self-critical training, scst.py); a target sequence of weight 0 takes no gradient."""
+    sum_t nll[b, t] (self-critical training, scst.py); a target sequence of weight 0 takes no gradient.
+    teacher (padded training batches only, not with seq_weight): (t_logits fp32 [B*T, >= V], t_copy_scores fp32
+    [B, T, S], t_gate_logits fp32 [B*T, 2], alpha, kd fp32 [B*T]), a teacher's triple (distill.teacher_targets):
+    loss_sum = sum_r (1 - alpha) nll_r + alpha kd_r with kd_r = -sum_j t_j log clamp(P_j, 1e-10, 1), written to `kd`
+    (fira_pointer_mix_kd_fwd / _bwd; distill.py)."""
 
     @staticmethod
     def forward(ctx, want_argmax, bf16, pf, memory, dec, mem_mask, label, Wout, bout, Ws, Wt, Wres, bres, Wp, bp,
-                pk=None, seq_weight=None):
+                pk=None, seq_weight=None, teacher=None):
         _require_cuda(memory, dec, Wout)
         B, T = dec.shape[0], dec.shape[1]
         S = pk.S if pk is not None else memory.shape[1]      # packed batch: memory is [1, Rc + Rs, D]
@@ -873,6 +890,17 @@ class HeadFn(torch.autograd.Function):
                 raise ValueError(f"HeadFn: seq_weight must be a CUDA fp32 tensor of shape ({B},)")
             seq_weight = seq_weight.contiguous()
         Mt, Ms = B * T, memory.shape[0] * memory.shape[1]
+        if teacher is not None:
+            if pk is not None or want_argmax or seq_weight is not None:
+                raise ValueError("HeadFn: a teacher applies to the padded training path without seq_weight")
+            t_logits, t_sc, t_gl, alpha, kd = teacher
+            ok = all(t is not None and t.is_cuda and t.dtype == torch.float32 for t in (t_logits, t_sc, t_gl, kd))
+            if not ok or t_logits.dim() != 2 or t_logits.shape[0] != Mt or t_logits.shape[1] < V or \
+                    t_logits.stride(1) != 1 or tuple(t_sc.shape) != (B, T, S) or not t_sc.is_contiguous() or \
+                    tuple(t_gl.shape) != (Mt, 2) or not t_gl.is_contiguous() or kd.numel() != Mt or \
+                    not kd.is_contiguous():
+                raise ValueError(f"HeadFn: the teacher needs CUDA fp32 logits [{Mt}, >= {V}], copy scores "
+                                 f"[{B}, {T}, {S}], gate logits [{Mt}, 2] and a kd buffer of {Mt}")
         pr = Prec(bf16)
         if pf is not None and pf.event is not None:
             torch.cuda.current_stream().wait_event(pf.event)
@@ -885,7 +913,7 @@ class HeadFn(torch.autograd.Function):
         dec2 = dec.contiguous().to(pr.tdt).view(Mt, D)
         dec32 = dec2 if not pr.bf16 else dec2.float()            # the 2-wide gate stays on the fp32 path
         ldl = _ld_logits(V)
-        if want_argmax:
+        if want_argmax or teacher is not None:        # every loss row of a teacher's batch reads its logits
             cap, vslot, vrows, dec_v = Mt, None, None, dec2
         else:
             # training: out_fc runs on the vocabulary-label rows alone, compacted into `cap` slots (a packed batch
@@ -897,23 +925,30 @@ class HeadFn(torch.autograd.Function):
             call("fira_vocab_rows", _ptr(label), Mt, V, _ptr(vslot), _ptr(vrows), cap, st)
             dec_v = pr.empty((cap, D), dev)
             call("fira_gather_rows", _ptr(dec2), D, _ptr(vrows), _ptr(dec_v), D, cap, D, pr.code, st)
-        logits = pr.empty((cap, ldl), dev)
-        pr.linear(dec_v, Wout, bout, out=logits, ld_out=ldl)
         # training only needs pointer scores of real source positions at target rows whose label is a COPY
-        # label (vocabulary-label rows take their loss from the vocabulary softmax alone, Model.py:64-81)
-        row_mask = None if want_argmax else (label >= V).to(torch.uint8)
-        src, tgt, sc = copy_scores_fwd(pr, memory2, dec2, Ws, Wt, Wres, bres, B, T, S, src_mask=mem_mask,
-                                       row_mask=row_mask, ranges=pk.ranges if pk is not None else None)
-        gl = linear(dec32, Wp, bp)                # fp32 [Mt, 2]
-        stats = torch.empty((Mt, 8), **f32)
+        # label (vocabulary-label rows take their loss from the vocabulary softmax alone, Model.py:64-81); with a
+        # teacher every loss row spreads over the copy positions too
+        row_mask = None if want_argmax else ((label != 0) if teacher is not None else (label >= V)).to(torch.uint8)
+        logits, src, tgt, sc, gl = head_products(pr, memory2, dec2, dec32, dec_v, cap, Wout, bout, Ws, Wt, Wres, bres,
+                                                 Wp, bp, B, T, S, mem_mask, row_mask,
+                                                 ranges=pk.ranges if pk is not None else None)
+        stats = torch.empty((Mt, 8 if teacher is None else 16), **f32)
         nll = torch.empty((Mt,), **f32)
         amax = torch.empty((Mt,), dtype=torch.int32, device=dev) if want_argmax else None
-        call("fira_pointer_mix_nll_fwd_rows", _ptr(logits), ldl, _ptr(sc), _ptr(gl), _ptr(mem_mask), _ptr(label),
-             _ptr(vslot), _ptr(stats), _ptr(nll), _ptr(amax), Mt, T, V, S, pr.code, st)
+        if teacher is None:
+            call("fira_pointer_mix_nll_fwd_rows", _ptr(logits), ldl, _ptr(sc), _ptr(gl), _ptr(mem_mask), _ptr(label),
+                 _ptr(vslot), _ptr(stats), _ptr(nll), _ptr(amax), Mt, T, V, S, pr.code, st)
+        else:
+            loss_rows = torch.empty((Mt,), **f32)
+            call("fira_pointer_mix_kd_fwd", _ptr(logits), ldl, _ptr(sc), _ptr(gl), _ptr(mem_mask), _ptr(label),
+                 _ptr(t_logits), t_logits.stride(0), _ptr(t_sc), _ptr(t_gl), float(alpha), _ptr(stats), _ptr(nll),
+                 _ptr(kd), _ptr(loss_rows), Mt, T, V, S, pr.code, st)
         ctx.misc = (pr, memory2, dec2, dec32, mem_mask, label, logits, ldl, src, tgt, sc, stats, B, T, S, V,
-                    memory.dtype, dec.dtype, pk, memory.shape, cap, vslot, vrows, dec_v, seq_weight)
+                    memory.dtype, dec.dtype, pk, memory.shape, cap, vslot, vrows, dec_v, seq_weight, teacher)
         ctx.save_for_backward(Wout, Ws, Wt, Wres, Wp, bout, bres, bp)
-        if seq_weight is None:
+        if teacher is not None:
+            loss_sum = colsum(loss_rows, 1, Mt, 1).view(())
+        elif seq_weight is None:
             loss_sum = colsum(nll, 1, Mt, 1).view(())
         else:                                      # per position t: sum_b w[b] nll[b, t], then over t
             loss_sum = colsum(colsum(nll, T, B, T, weight=seq_weight), 1, T, 1).view(())
@@ -925,7 +960,7 @@ class HeadFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_loss, g_nll, g_ids):
         (pr, memory2, dec2, dec32, mem_mask, label, logits, ldl, src, tgt, sc, stats, B, T, S, V,
-         mem_dt, dec_dt, pk, mem_shape, cap, vslot, vrows, dec_v, seq_weight) = ctx.misc
+         mem_dt, dec_dt, pk, mem_shape, cap, vslot, vrows, dec_v, seq_weight, teacher) = ctx.misc
         Wout, Ws, Wt, Wres, Wp, bout, bres, bp = ctx.saved_tensors
         Mt, Ms = B * T, memory2.shape[0]
         dev = dec2.device
@@ -938,7 +973,12 @@ class HeadFn(torch.autograd.Function):
         active = torch.empty((Mt,), dtype=torch.uint8, device=dev)
         args = (_ptr(logits), ldl, _ptr(sc), _ptr(mem_mask), _ptr(label), _ptr(vslot), _ptr(vrows), cap, _ptr(stats),
                 _ptr(up), _ptr(dlogits), _ptr(dsc), _ptr(dgl), _ptr(active), Mt, T, V, S, pr.code, st)
-        if seq_weight is None:
+        if teacher is not None:
+            t_logits, t_sc, _, alpha, _ = teacher
+            call("fira_pointer_mix_kd_bwd", _ptr(logits), ldl, _ptr(sc), _ptr(mem_mask), _ptr(label), _ptr(t_logits),
+                 t_logits.stride(0), _ptr(t_sc), float(alpha), _ptr(stats), _ptr(up), _ptr(dlogits), _ptr(dsc),
+                 _ptr(dgl), _ptr(active), Mt, T, V, S, pr.code, st)
+        elif seq_weight is None:
             call("fira_pointer_mix_nll_bwd_rows", *args)
         else:
             call("fira_pointer_mix_nll_bwd_rows_weighted", *args, _ptr(seq_weight))
@@ -979,7 +1019,7 @@ class HeadFn(torch.autograd.Function):
         linear_dx(d_tgt, D, Wt, Mt, out=d_dec, accumulate=True)
         fork.join()
         return (None, None, None, d_mem.view(mem_shape).to(mem_dt), d_dec.view(B, T, D).to(dec_dt), None, None, d_Wout,
-                d_bout, d_Ws, d_Wt, d_wres, d_bres, d_Wp, d_bp, None, None)
+                d_bout, d_Ws, d_Wt, d_wres, d_bres, d_Wp, d_bp, None, None, None)
 
 
 # ============================================================================= module-surface pieces

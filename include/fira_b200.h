@@ -504,6 +504,34 @@ int fira_pointer_mix_ensemble(const void* const* logits, long ld_logits, const f
                               const unsigned char* mem_mask, float* logits_out, long ld_out, float* copy_out,
                               float* gate_out, int B, int N, int V, int S, int dtype, void* stream);
 
+/* ---- knowledge distillation (fira_icse_b200/distill.py): the student's mixture P against a teacher's fp32 triple
+ *      (t_logits [rows, ld_t], t_copy_scores [B, T_len, S], t_gate_logits [rows, 2]; fira_pointer_mix_ensemble's output
+ *      with N = T_len), whose mixture t is formed by the same expressions.  Student operands as
+ *      fira_pointer_mix_nll_fwd.  Row r with shifted label y = label[r] != 0 (a y = 0 row carries no loss and no kernel
+ *      reads its logits, copy scores or teacher row):
+ *        nll_r  = -log clamp(P_y, 1e-10, 1)                 (fira_pointer_mix_nll_fwd's value; a copy label beyond S: 0)
+ *        kd_r   = -sum_{j < V+S} t_j log clamp(P_j, 1e-10, 1)   (a masked copy position has t_j = 0 and adds 0)
+ *        loss_r = (1 - alpha) nll_r + alpha kd_r,  0 <= alpha <= 1
+ *      Backward with u = *upstream (d(sum_r loss_r)), live_j = (1e-10 <= P_j <= 1), the clamp's pass-through:
+ *        a_j = [(1 - alpha) [j == y] + alpha t_j] live_j,  A_V = sum_{j < V} a_j,  A_C = sum_s a_{V+s}
+ *        d_logits_k = u (softmax(x)_k A_V - a_k),  d_copy_scores_s = u (softmax(masked c)_s A_C - a_{V+s}) (0 if masked)
+ *        d_gate_logits = u ((g0, g1) (A_V + A_C) - (A_V, A_C)),  row_active = (A_C != 0)
+ *      With alpha = 0 every output equals fira_pointer_mix_nll_fwd / _bwd's bit for bit.  stats: 16 floats per row
+ *      (the student's vmax, vsum, cmax, csum, g0, g1, p_label, 0, the teacher's six, A_V, A_C) from the forward, read by
+ *      the backward.  nll / kd / loss [rows]; d_logits dense [rows, ld_logits] (zeros on y = 0 rows).  One CTA of 256
+ *      threads per row.  logits, d_logits, t_logits 16-byte aligned, ld_logits and ld_t multiples of 8 and >= V,
+ *      V + S <= 32767, alpha in [0, 1]. */
+int fira_pointer_mix_kd_fwd(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                            const unsigned char* mem_mask, const int* label, const float* t_logits, long ld_t,
+                            const float* t_copy_scores, const float* t_gate_logits, float alpha, float* stats,
+                            float* nll, float* kd, float* loss, long rows, int T_len, int V, int S, int dtype,
+                            void* stream);
+int fira_pointer_mix_kd_bwd(const void* logits, long ld_logits, const float* copy_scores,
+                            const unsigned char* mem_mask, const int* label, const float* t_logits, long ld_t,
+                            const float* t_copy_scores, float alpha, const float* stats, const float* upstream,
+                            void* d_logits, float* d_copy_scores, float* d_gate_logits, unsigned char* row_active,
+                            long rows, int T_len, int V, int S, int dtype, void* stream);
+
 /* ---- minimum-Bayes-risk selection among each commit's N samples (fira_icse_b200/mbr.py).  seq [B, N, ld_seq] int32
  *      (row (b, n) at (b*N + n) * ld_seq, columns 0..T_len-1), length [B, N] int32 (counts <start>; clamped to
  *      [1, T_len]).  Rule:

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""`python run_model.py train|test|finetune` -- the reference's CLI (run_model.py:417-425) on the CUDA path.
+"""`python run_model.py train|test|finetune|distill` -- the reference's CLI (run_model.py:417-425) on the CUDA path.
 
 Same CWD-relative files (DataSet/*.json, all_index, VOCAB_UPPER_CASE, best_model.pt,
 OUTPUT/{output_fira,train_process,dev_output}), same hyper-parameters (run_model.py:27-46), same
@@ -56,6 +56,15 @@ beam search ranking.  Differences, all below the module surface:
     against the reference and weighted by its leave-one-out advantage.  Prints the mean reward every 10 batches, runs
     dev() after every epoch and saves the state_dict of the best dev BLEU to best_model_scst.pt; best_model.pt is never
     overwritten.  WORLD_SIZE > 1 exits with an error.
+  * `distill`: word-level knowledge distillation from an ensemble (fira_icse_b200.distill, DESIGN.md §9), one GPU.  The
+    student is FIRA_CHECKPOINT (default best_model.pt), the teacher the Ensemble of FIRA_ENSEMBLE=a.pt[,b.pt,...]
+    weighted by FIRA_ENSEMBLE_WEIGHTS (as for `test`; both are needed here).  Runs FIRA_KD_EPOCHS (default 1) epochs of
+    distill_step with optim.FlatAdam at FIRA_KD_LR (default 1e-4, the reference's rate) over padded batches of
+    FIRA_BATCH commits (FIRA_MAX_BATCHES bounds an epoch), on the loss (1 - FIRA_KD_ALPHA) NLL + FIRA_KD_ALPHA
+    cross-entropy against the teacher's distribution (FIRA_KD_ALPHA in [0, 1], default 0.5).  Prints loss / nll / kd
+    every 10 batches, runs dev() after every epoch and saves the state_dict of the best dev BLEU to best_model_kd.pt
+    (dev output: OUTPUT/dev_output_kd); best_model.pt and the teacher checkpoints are never overwritten.  WORLD_SIZE > 1
+    exits with an error.
 """
 import json
 import os
@@ -71,6 +80,7 @@ from torch.utils.data import DataLoader
 from fira_icse_b200 import TransModel
 from fira_icse_b200.beam import beam_search, best_sequences, nbest
 from fira_icse_b200.bleu import sentence_bleu_method2
+from fira_icse_b200.distill import distill_step
 from fira_icse_b200.data import PackedBatchLoader, TransDataset, batch_to_device, collate_packed
 from fira_icse_b200.engine import GraphedTrainStep
 from fira_icse_b200.ensemble import MAX_MEMBERS, Ensemble
@@ -354,18 +364,25 @@ def test(model, test_loader, g, test_index, dev_, first_index, decode, n_bleu, o
 
 
 def ensemble_settings(mode):
+    """`test`'s FIRA_ENSEMBLE / FIRA_ENSEMBLE_WEIGHTS -> (checkpoint paths, weights or None for uniform), or None without
+    an ensemble; checked before any device work (SystemExit on an error)."""
+    if os.environ.get("FIRA_ENSEMBLE", ""):
+        if mode == "beam":
+            raise SystemExit("FIRA_ENSEMBLE applies to FIRA_DECODE=sample, nbest and mbr; the reference beam search "
+                             "decodes one model")
+        if "FIRA_CHECKPOINT" in os.environ:
+            raise SystemExit("FIRA_ENSEMBLE names the checkpoints itself: unset FIRA_CHECKPOINT")
+    return ensemble_checkpoints()
+
+
+def ensemble_checkpoints():
     """FIRA_ENSEMBLE / FIRA_ENSEMBLE_WEIGHTS -> (checkpoint paths, weights or None for uniform), or None without an
-    ensemble; checked before any device work (SystemExit on an error)."""
+    ensemble (SystemExit on an error)."""
     spec, wspec = os.environ.get("FIRA_ENSEMBLE", ""), os.environ.get("FIRA_ENSEMBLE_WEIGHTS", "")
     if not spec:
         if wspec:
             raise SystemExit("FIRA_ENSEMBLE_WEIGHTS needs FIRA_ENSEMBLE")
         return None
-    if mode == "beam":
-        raise SystemExit("FIRA_ENSEMBLE applies to FIRA_DECODE=sample, nbest and mbr; the reference beam search decodes "
-                         "one model")
-    if "FIRA_CHECKPOINT" in os.environ:
-        raise SystemExit("FIRA_ENSEMBLE names the checkpoints itself: unset FIRA_CHECKPOINT")
     paths = [p.strip() for p in spec.split(",")]
     if not all(paths) or not 1 <= len(paths) <= MAX_MEMBERS:
         raise SystemExit(f"FIRA_ENSEMBLE must list 1 to {MAX_MEMBERS} checkpoints separated by commas, got {spec!r}")
@@ -479,6 +496,71 @@ def main_finetune():
     print("best dev bleu: %f" % best_bleu)
 
 
+KD_CHECKPOINT = "best_model_kd.pt"
+
+
+def distill_settings():
+    """The distill stage's settings from the environment, checked before any device work (SystemExit on an error) ->
+    (settings, student checkpoint, (teacher checkpoints, weights or None))."""
+    if WORLD > 1:
+        raise SystemExit("run_model.py distill runs on one GPU: launch it without torchrun (WORLD_SIZE=1)")
+    try:
+        s = dict(alpha=float(os.environ.get("FIRA_KD_ALPHA", 0.5)), epochs=int(os.environ.get("FIRA_KD_EPOCHS", 1)),
+                 lr=float(os.environ.get("FIRA_KD_LR", 1e-4)))
+    except ValueError as e:
+        raise SystemExit(f"run_model.py distill: {e}")
+    if not 0.0 <= s["alpha"] <= 1.0:
+        raise SystemExit(f"FIRA_KD_ALPHA must be a number in [0, 1], got {s['alpha']}")
+    if s["epochs"] < 1:
+        raise SystemExit(f"FIRA_KD_EPOCHS must be >= 1, got {s['epochs']}")
+    if not 0.0 < s["lr"] < float("inf"):
+        raise SystemExit(f"FIRA_KD_LR must be a positive finite number, got {s['lr']}")
+    teacher = ensemble_checkpoints()
+    if teacher is None:
+        raise SystemExit("run_model.py distill needs the teacher: FIRA_ENSEMBLE=a.pt[,b.pt,...]")
+    student = os.environ.get("FIRA_CHECKPOINT", "best_model.pt")
+    if not os.path.isfile(student):
+        raise SystemExit(f"FIRA_CHECKPOINT: student checkpoint {student} not found")
+    out = os.path.realpath(KD_CHECKPOINT)
+    if any(os.path.realpath(p) == out for p in teacher[0]):
+        raise SystemExit(f"FIRA_ENSEMBLE names {KD_CHECKPOINT}, which distill writes: copy the teacher elsewhere")
+    return s, student, teacher
+
+
+def main_distill():
+    s, student, (paths, weights) = distill_settings()
+    dev_ = device()
+    g = load_globals()
+    train_set = TransDataset(args, 'train')
+    dev_set = TransDataset(args, 'valid')
+    all_index = json.load(open('all_index'))
+    model = load_model(student, dev_)
+    teacher = Ensemble([load_model(p, dev_) for p in paths], weights)
+    from fira_icse_b200 import optim
+    opt = optim.FlatAdam(model.live_parameters(), lr=s["lr"], groups=model.flat_groups())
+    optim.attach(model, [opt])
+    train_loader = loader(train_set, args.batch_size, True)
+    dev_loader = loader(dev_set, args.batch_size, False)
+    max_batches = int(os.environ.get("FIRA_MAX_BATCHES", 0))
+    best_bleu = -1.0
+    for epoch in range(s["epochs"]):
+        for idx, batch in enumerate(train_loader):
+            if max_batches and idx >= max_batches:
+                break
+            step = distill_step(model, opt, batch_to_device(batch, dev_), teacher, alpha=s["alpha"])
+            if idx % 10 == 0:
+                print("kd epoch: %d batch: %d/%d loss: %.4f nll: %.4f kd: %.4f tokens: %d" % (
+                    epoch, idx, len(train_loader), step.loss, step.nll, step.kd, step.tokens))
+        cur_bleu, output_str = dev(model, dev_loader, g, all_index['valid'], epoch, dev_)
+        open('OUTPUT/train_process', 'a').write(
+            'kd epoch: {} dev bleu: {} is better: {}\n'.format(epoch, cur_bleu, cur_bleu > best_bleu))
+        if cur_bleu > best_bleu:
+            best_bleu = cur_bleu
+            torch.save(model.state_dict(), KD_CHECKPOINT)
+            open('OUTPUT/dev_output_kd', 'w').write(output_str)
+    print("best dev bleu: %f" % best_bleu)
+
+
 if __name__ == '__main__':
     stage = str(sys.argv[1])
     seed_everything()
@@ -489,5 +571,7 @@ if __name__ == '__main__':
         main_test()
     elif stage == 'finetune':
         main_finetune()
+    elif stage == 'distill':
+        main_distill()
     else:
-        raise SystemExit("usage: python run_model.py train|test|finetune")
+        raise SystemExit("usage: python run_model.py train|test|finetune|distill")
