@@ -54,6 +54,18 @@ candidate whose word would complete an n-gram already in that history, or is <eo
 words, is never offered to the row stage's top K.  The select stage is unchanged, lp and score stay the model's, and a
 slot with fewer than K allowed entries proposes fewer.  A hypothesis can still end unfinished at tar_len.
 
+Lexically constrained n-best (`constraints`; dynamic beam allocation, Post & Vilar, 2018; DESIGN.md §9): each commit
+requires up to 4 phrases of up to 4 vocabulary ids (Tc words in all).  A phrase's progress on a slot's words (its
+history after <start>, copies as their words, prefix words included) is its length when it occurs contiguously, else
+the longest start of it the words end with; a slot meets its constraints when the progress summed over the phrases is
+Tc, and <eos> is banned until it does.  Besides its K best allowed labels, a live slot proposes, per phrase it has not
+met, the best label spelling that phrase's next word (the vocabulary entry or a copy of it).  Each candidate's bank is
+the progress with its word appended.  With Tc > 0 the carried finished slots are kept first, then the other slots are
+filled by striping over the banks: within each bank the candidates are ranked by (score, index), and the ranks are
+taken in order, higher banks first on a tie.  Tc = 0 is plain n-best.  Every finished hypothesis meets its
+constraints; one that reaches tar_len unfinished may not.  Each commit's K hypotheses are returned stably sorted by
+(meets its constraints, score), best first (`constraints_met`).
+
 The loop is decode_loop.PositionLoop (described there); a position ends with fira_pointer_mix_beam_step (per live slot
 row its top K, then per commit the merge, writing the new slots, their parents and the next tokens), the KV-cache
 reorder to the parents and the pad mask of the next tokens.  Slot state is double-buffered by the parity of the
@@ -68,8 +80,8 @@ import torch
 
 from . import ops
 from ._lib import call
-from .decode_loop import (PositionLoop, _f32, check_prefix, check_rules, check_tar_len, encode, encode_members, is_int,
-                          loop_for)
+from .decode_loop import (MAX_PHRASE_LEN, MAX_PHRASES, PositionLoop, _f32, check_constraints, check_prefix, check_rules,
+                          check_tar_len, encode, encode_members, is_int, loop_for)
 from .ensemble import refuse
 from .incremental import IncrementalDecoder
 
@@ -228,6 +240,48 @@ class _NBest(PositionLoop):
         inc.tok_mask[:, t + 1].copy_(inc.tok[:self.R] != pad_id)
 
 
+class _LexicalNBest(_NBest):
+    """_NBest with lexical constraints: the commits' phrases in a static buffer (written at start, read by every captured
+    position) and a row-stage workspace of K + 4 keys per row (the K best labels, then one per unmet phrase)."""
+
+    def __init__(self, model, B, K, T, S):
+        super().__init__(model, B, K, T, S)
+        self.work = torch.empty(self.R * (K + MAX_PHRASES), dtype=torch.int64, device=self.dev)
+        self.constraints = torch.zeros((B, MAX_PHRASES, MAX_PHRASE_LEN), dtype=torch.int32, device=self.dev)
+
+    def start(self, memory, mem_mask, copy_src, start_id, pad_id, constraints, prefix=None):
+        super().start(memory, mem_mask, copy_src, start_id, pad_id, prefix)
+        self.constraints.copy_(constraints)
+
+    def position(self, t, length_penalty, eos_id, pad_id, no_repeat_ngram, min_length):
+        self.head(t)
+        p = ops._ptr
+        inc = self.inc
+        call("fira_pointer_mix_beam_step_lexical", p(self.logits), self.ldl, p(self.sc), p(self.gl), p(self.mem_mask),
+             p(self.copy_src), float(length_penalty), int(eos_id), int(pad_id), p(self.work), p(self.seq), p(self.raw),
+             p(self.tlp), p(self.length), p(self.lp), p(self.score), p(self.status), p(self.parent), p(inc.tok),
+             self.T, t, self.B, self.N, self.V, self.S, self.code, ops._stream(), p(self.prefix), self.T,
+             p(self.prefix_len), int(no_repeat_ngram), int(min_length), p(self.constraints))
+        self.reorder(self.parent)
+        inc.tok_mask[:, t + 1].copy_(inc.tok[:self.R] != pad_id)
+
+
+def constraints_met(seq, length, constraints):
+    """bool [B, K] on seq's device: hypothesis (b, k) contains every phrase of commit b contiguously among its words
+    seq[b, k, 1:length[b, k]].  seq [B, K, T] vocabulary ids (Hypotheses.seq), length [B, K], constraints [B, P, L]
+    vocabulary ids with 0 = padding (check_constraints); a commit without phrases meets them."""
+    dev = seq.device
+    con = constraints.to(dev, torch.long)
+    B, K, T = seq.shape
+    P, Lc = con.shape[1:]
+    col = torch.arange(T, device=dev)
+    words = torch.where((col >= 1) & (col < length.to(dev).unsqueeze(-1)), seq.long(), -1)       # -1: no word
+    win = torch.cat((words, words.new_full((B, K, Lc - 1), -1)), 2).unfold(2, Lc, 1)          # [B, K, T, Lc]
+    care = con != 0                                                                             # [B, P, Lc]
+    hit = (win.unsqueeze(2) == con[:, None, :, None, :]) | ~care[:, None, :, None, :]           # [B, K, P, T, Lc]
+    return (hit.all(-1).any(-1) | ~care.any(-1).unsqueeze(1)).all(-1)
+
+
 class _DiverseNBest(_NBest):
     """_NBest with beam groups: the token every slot grew with at the current position (`chosen`, read by the later
     groups' penalty) and the true lp of every row winner next to its rank key."""
@@ -260,16 +314,21 @@ class _DiverseNBest(_NBest):
 
 @torch.no_grad()
 def nbest(model, sou, mark, ast_change, edge, sub_token, *, beam_size=3, length_penalty=0.0, tar_len=30, start_id,
-          eos_id, pad_id=0, groups=1, diversity=0.0, prefix=None, no_repeat_ngram=0, min_length=0):
+          eos_id, pad_id=0, groups=1, diversity=0.0, prefix=None, no_repeat_ngram=0, min_length=0, constraints=None):
     """Log-space beam search with length normalisation -> Hypotheses, each commit's K best first (module docstring).
     model: a TransModel, or an ensemble.Ensemble (ranked by its averaged distribution).
     groups > 1 splits the K slots into diverse beam groups penalised by `diversity` per earlier-group repeat.
     prefix: None, or labels [B, P] every hypothesis of a commit starts with (decode_loop.check_prefix: the tar_label
     encoding without <start>, a 0 ends a commit's prefix, no <eos>, at most tar_len - 2 labels).
     no_repeat_ngram = n >= 1 / min_length = m >= 1: a slot never extends with a word that completes an n-gram already
-    in its hypothesis, nor with <eos> before m words (0 = off; module docstring)."""
+    in its hypothesis, nor with <eos> before m words (0 = off; module docstring).
+    constraints: None, or vocabulary ids [B, P <= 4, L <= 4] (0 = padding), phrases every finished hypothesis of a
+    commit contains (decode_loop.check_constraints; plain n-best only); the hypotheses come sorted by (meets its
+    constraints, score), best first (module docstring)."""
     check_nbest_args(beam_size, length_penalty, tar_len, groups, diversity)
     check_rules(no_repeat_ngram, min_length, tar_len)
+    con = check_constraints(constraints, sou.shape[0], V=model.vocab_size, tar_len=tar_len, start_id=start_id,
+                            eos_id=eos_id, pad_id=pad_id, groups=groups)
     if beam_size > model.vocab_size:
         raise ValueError(f"beam_size {beam_size} exceeds the vocabulary ({model.vocab_size})")
     check_tar_len(model, tar_len)
@@ -277,6 +336,20 @@ def nbest(model, sou, mark, ast_change, edge, sub_token, *, beam_size=3, length_
                        eos_last=False)
     memory, mem_mask, copy_src = encode_members(model, sou, mark, ast_change, edge, sub_token, pad_id)
     B, S = memory[0].shape[:2]
+    if con is not None:
+        st = loop_for(_LexicalNBest, model, B, beam_size, tar_len, S)
+        st.start(memory, mem_mask, copy_src, start_id, pad_id, con, pre)
+        t = st.run((float(length_penalty), int(eos_id), int(pad_id), no_repeat_ngram, min_length))
+        seq, raw, length, lp, tlp, status = st.slots(t)
+        score = st.score[t & 1].view(B, beam_size)
+        met = constraints_met(seq, length, st.constraints)
+        # (meets descending, score descending), stable: score first, then a stable sort on met
+        score, order = torch.sort(score, dim=1, descending=True, stable=True)
+        _, o2 = torch.sort(met.gather(1, order).to(torch.int8), dim=1, descending=True, stable=True)
+        order, score = order.gather(1, o2), score.gather(1, o2)
+        o2, o3 = order, order.unsqueeze(-1).expand_as(seq)
+        return Hypotheses(seq.gather(1, o3), raw.gather(1, o3), length.gather(1, o2), lp.gather(1, o2), score,
+                          tlp.gather(1, o3), (status == 1).gather(1, o2))
     if groups == 1:
         st = loop_for(_NBest, model, B, beam_size, tar_len, S)
         st.start(memory, mem_mask, copy_src, start_id, pad_id, pre)

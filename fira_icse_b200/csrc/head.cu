@@ -760,12 +760,72 @@ __device__ __forceinline__ uint64_t topk_insert(uint64_t (&top)[kMaxBeam], uint6
   return last;
 }
 
-template <typename T>
+// Lexically constrained n-best (LEX = true, fira_pointer_mix_beam_step_lexical; dynamic beam allocation, Post & Vilar,
+// 2018).  Commit b has up to kPhrases phrases of up to kPhraseLen words, constraints[b][p][m] (0 = padding, no gaps),
+// Tc words in all.  The words of a row are its history hist[1..pos] (copies as their words, prefix words included).
+// Per phrase c of length L: prog_c(h) = L when c occurs contiguously in h, else the largest m < L with h ending in
+// c_1..c_m (0 if none).  A row's progress is the sum over its phrases; it meets its constraints when progress = Tc.
+// A live, non-forced row bans <eos> while its progress is below Tc and proposes
+//   (a) its K best allowed labels (the plain row stage), and
+//   (b) per unmet phrase, in phrase order, the best label by rank_key among j = w and the unmasked copies of w, where
+//       w = c_{prog_c + 1}; skipped when w is banned, when an earlier phrase proposed w, or when the label is in (a).
+// Every proposal (a forced row's one label too) carries its bank, the progress of the history with its word appended,
+// in key bits kBankShift.. (rank_key uses bits 0..46; key_lp and key_index ignore the bank).  Phrase state from the
+// history: occ (c occurs) and ends (bit m: h ends with c_1..c_m; bit 0 always); appending w gives L when occ, else the
+// largest m <= L with ends bit m - 1 and c_m == w (0 if none).
+constexpr int kPhrases = 4, kPhraseLen = 4, kMaxConstraintWords = kPhrases * kPhraseLen;
+constexpr int kBankShift = 48;
+
+struct Phrases { int con[kMaxConstraintWords], len[kPhrases], occ[kPhrases], ends[kPhrases], prog[kPhrases]; };
+
+__device__ __forceinline__ int constraint_words(const int* __restrict__ con) {     // Tc of one commit
+  int tc = 0;
+  for (int e = 0; e < kMaxConstraintWords; ++e) tc += con[e] != 0;
+  return tc;
+}
+// threads 0..kPhrases-1 fill phrase threadIdx.x's state from s_hist[1..pos]; a __syncthreads must follow
+__device__ __forceinline__ void phrase_state(const int* __restrict__ con, const int* s_hist, int pos, Phrases& ph) {
+  const int p = threadIdx.x;
+  if (p >= kPhrases) return;
+  const int* c = con + p * kPhraseLen;
+  int L = 0;
+  for (int m = 0; m < kPhraseLen; ++m) { ph.con[p * kPhraseLen + m] = c[m]; L += c[m] != 0; }
+  const int* h = s_hist + 1;                          // the pos words
+  bool occ = false;
+  for (int a = 0; L && a + L <= pos && !occ; ++a) {
+    bool same = true;
+    for (int m = 0; m < L; ++m) same &= h[a + m] == c[m];
+    occ = same;
+  }
+  int ends = 1, prog = 0;
+  for (int m = 1; m < L && m <= pos; ++m) {
+    bool same = true;
+    for (int e = 0; e < m; ++e) same &= h[pos - m + e] == c[e];
+    if (same) { ends |= 1 << m; prog = m; }
+  }
+  ph.len[p] = L; ph.occ[p] = occ; ph.ends[p] = ends; ph.prog[p] = occ ? L : prog;
+}
+// the progress of the row's words with w appended
+__device__ __forceinline__ int phrase_bank(const Phrases& ph, int w) {
+  int bank = 0;
+  for (int p = 0; p < kPhrases; ++p) {
+    const int L = ph.len[p];
+    int best = ph.occ[p] ? L : 0;
+    for (int m = 1; m <= L && !ph.occ[p]; ++m)
+      if (((ph.ends[p] >> (m - 1)) & 1) && ph.con[p * kPhraseLen + m - 1] == w) best = m;
+    bank += best;
+  }
+  return bank;
+}
+
+// LEX = false: the plain row stage (K entries per row); LEX = true: K + kPhrases entries per row, (a) then (b)
+template <typename T, bool LEX>
 __global__ void __launch_bounds__(kBeamThreads, 1) beam_row_kernel(
     const T* __restrict__ logits, long ldl, const float* __restrict__ sc, const float* __restrict__ gate_logit,
     const unsigned char* __restrict__ mem_mask, const int* __restrict__ copy_src, const unsigned char* __restrict__ status,
     const int* __restrict__ seq, int Tn, uint64_t* __restrict__ row_top, const int* __restrict__ prefix, int ld_prefix,
-    const int* __restrict__ prefix_len, int no_repeat, int min_len, int eos_id, int pos, int K, int V, int S) {
+    const int* __restrict__ prefix_len, int no_repeat, int min_len, int eos_id, int pos, int K, int V, int S,
+    const int* __restrict__ constraints) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
   __shared__ MaxSum sh_ms[8];
   __shared__ float bc[4];
@@ -774,21 +834,45 @@ __global__ void __launch_bounds__(kBeamThreads, 1) beam_row_kernel(
   const long row = blockIdx.x;
   if (status[row] != 0) return;                       // finished or inactive: the select stage reads nothing of it
   const int b = (int)(row / K);
+  const int W = LEX ? K + kPhrases : K;               // row_top entries per row
   const T* lrow = logits + row * ldl;
   const float* srow = sc + row * S;
   const unsigned char* mrow = mem_mask + (long)b * S;
   const int nb = ban_count(pos, no_repeat, min_len);
-  ban_load(seq + row * Tn, pos, nb, s_hist);
+  const int* con = LEX ? constraints + (long)b * kMaxConstraintWords : nullptr;
+  const int tc = LEX ? constraint_words(con) : 0;
+  ban_load(seq + row * Tn, pos, nb | tc, s_hist);
   const MixRow ms = mix_row_stats(lrow, srow, mrow, gate_logit + row * 2, V, S, sh_ms, bc);   // syncs s_hist too
+  __shared__ Phrases ph;
+  if constexpr (LEX) {
+    if (tc) {
+      phrase_state(con, s_hist, pos, ph);
+      __syncthreads();
+    }
+  }
+  auto with_bank = [&](uint64_t key) -> uint64_t {   // a proposal's key with its bank (LEX, Tc > 0)
+    if (!LEX || !tc || key == 0) return key;
+    const int j = key_index(key);
+    return key | ((uint64_t)phrase_bank(ph, j < V ? j : copy_src[(long)b * S + (j - V)]) << kBankShift);
+  };
   if (prefix && pos < prefix_len[b]) {                // inside the commit's prefix: its label is the row's one winner
     if (threadIdx.x == 0) {
       const int j = prefix[(long)b * ld_prefix + pos];
-      row_top[row * K] = rank_key(logf(fminf(fmaxf(mix_prob(ms, lrow, srow, mrow, V, j), 1e-10f), 1.f)), j);
-      for (int k = 1; k < K; ++k) row_top[row * K + k] = 0;
+      row_top[row * W] = with_bank(rank_key(logf(fminf(fmaxf(mix_prob(ms, lrow, srow, mrow, V, j), 1e-10f), 1.f)), j));
+      for (int k = 1; k < W; ++k) row_top[row * W + k] = 0;
     }
     return;
   }
-  if (nb) {
+  int nbx = nb;                                       // nb + the <eos> entry of the constraints (LEX, Tc > 0)
+  if constexpr (LEX) {
+    if (tc) {
+      int prog = 0;
+      for (int p = 0; p < kPhrases; ++p) prog += ph.prog[p];
+      if ((int)threadIdx.x == nb) s_ban[nb] = prog < tc ? eos_id : -1;
+      nbx = nb + 1;
+    }
+  }
+  if (nbx) {
     ban_build(s_hist, pos, no_repeat, min_len, eos_id, nb, s_ban);
     __syncthreads();
   }
@@ -801,7 +885,7 @@ __global__ void __launch_bounds__(kBeamThreads, 1) beam_row_kernel(
   auto offer = [&](float p, int j) {
     const uint64_t key = rank_key(logf(fminf(fmaxf(p, 1e-10f), 1.f)), j);   // lp = -nll of fira_pointer_mix_nll_fwd
     if (key <= thr) return;
-    if (nb && is_banned(s_ban, nb, j < V ? j : crow[j - V])) return;       // only entries that would enter the top K
+    if (nbx && is_banned(s_ban, nbx, j < V ? j : crow[j - V])) return;     // only entries that would enter the top K
     thr = topk_insert(top, key, K);
   };
   const int V8 = V >> 3;
@@ -823,7 +907,60 @@ __global__ void __launch_bounds__(kBeamThreads, 1) beam_row_kernel(
       for (int i = 0; i + 1 < kMaxBeam; ++i) top[i] = top[i + 1];
       top[kMaxBeam - 1] = 0;
     }
-    if (threadIdx.x == 0) row_top[row * K + k] = m;
+    if (threadIdx.x == 0) row_top[row * W + k] = with_bank(m);
+  }
+  if constexpr (LEX) {                                // (b): one block-wide best label per unmet phrase
+    int nx = K;                                       // thread 0: the next free entry
+    for (int p = 0; tc && p < kPhrases; ++p) {        // shared state only: uniform across the block
+      if (ph.prog[p] == ph.len[p]) continue;
+      const int w = ph.con[p * kPhraseLen + ph.prog[p]];
+      bool skip = is_banned(s_ban, nbx, w);
+      for (int q = 0; q < p; ++q) skip |= ph.prog[q] < ph.len[q] && ph.con[q * kPhraseLen + ph.prog[q]] == w;
+      if (skip) continue;
+      uint64_t best = threadIdx.x == 0 ? rank_key(logf(fminf(fmaxf(mix_prob(ms, lrow, srow, mrow, V, w), 1e-10f), 1.f)), w) : 0;
+      for (int s = threadIdx.x; s < S; s += blockDim.x)
+        if (mrow[s] && crow[s] == w)
+          best = key_max(best, rank_key(logf(fminf(fmaxf(ms.g1 * (expf(srow[s] - ms.cmax) / ms.csum), 1e-10f), 1.f)), V + s));
+      best = block_reduce(best, shk, key_max);
+      if (threadIdx.x == 0) {
+        bool in_a = false;                            // (a) as written above by this thread, without the banks
+        for (int k = 0; k < K; ++k) in_a |= (row_top[row * W + k] & (kKeyEnd - 1)) == best;
+        if (!in_a) row_top[row * W + nx++] = with_bank(best);
+      }
+    }
+    if (threadIdx.x == 0) for (; nx < W; ++nx) row_top[row * W + nx] = 0;
+  }
+}
+
+// Both select stages: new slot k continues slot s_from[k] (j = s_j[k], C: carried unchanged) -> the written half of the
+// slot state, parent, next_tok and the histories (a grown slot gets its new token at column pos + 1)
+__device__ __forceinline__ void beam_write_slots(const int* s_from, const int* s_j, const int* s_tok, const float* s_lp,
+                                                 const float* s_L, const float* s_score, int eos_id, int pad_id,
+                                                 int* __restrict__ seq, int* __restrict__ raw, float* __restrict__ tok_lp,
+                                                 int* __restrict__ length, float* __restrict__ lp_sum,
+                                                 float* __restrict__ score, unsigned char* __restrict__ status,
+                                                 long* __restrict__ parent, int* __restrict__ next_tok, int Tn, int pos,
+                                                 long in, long out, long base, int K, int C) {
+  if (threadIdx.x < K) {
+    const int k = threadIdx.x;
+    const long pr = in + base + s_from[k], nr = out + base + k;
+    parent[base + k] = base + s_from[k];
+    if (s_j[k] == C) {                                // a finished slot carried unchanged
+      length[nr] = length[pr]; lp_sum[nr] = lp_sum[pr]; score[nr] = score[pr]; status[nr] = status[pr];
+      next_tok[base + k] = pad_id;
+    } else {
+      length[nr] = length[pr] + 1; lp_sum[nr] = s_L[k]; score[nr] = s_score[k];
+      status[nr] = s_tok[k] == eos_id ? 1 : 0;
+      next_tok[base + k] = s_tok[k];
+    }
+  }
+  for (int e = threadIdx.x; e < K * Tn; e += blockDim.x) {
+    const int k = e / Tn, c = e % Tn;
+    const long src = (in + base + s_from[k]) * Tn + c, dst = (out + base + k) * Tn + c;
+    const bool grow = s_j[k] != C && c == pos + 1;
+    seq[dst] = grow ? s_tok[k] : seq[src];
+    raw[dst] = grow ? s_j[k] : raw[src];
+    tok_lp[dst] = grow ? s_lp[k] : tok_lp[src];
   }
 }
 
@@ -878,28 +1015,82 @@ __global__ void __launch_bounds__(kBeamThreads) beam_select_kernel(
     }
   }
   __syncthreads();
-  if (threadIdx.x < K) {
-    const int k = threadIdx.x;
-    const long pr = in + base + s_from[k], nr = out + base + k;
-    parent[base + k] = base + s_from[k];
-    if (s_j[k] == C) {                                // a finished slot carried unchanged
-      length[nr] = length[pr]; lp_sum[nr] = lp_sum[pr]; score[nr] = score[pr]; status[nr] = status[pr];
-      next_tok[base + k] = pad_id;
-    } else {
-      length[nr] = length[pr] + 1; lp_sum[nr] = s_L[k]; score[nr] = s_score[k];
-      status[nr] = s_tok[k] == eos_id ? 1 : 0;
-      next_tok[base + k] = s_tok[k];
+  beam_write_slots(s_from, s_j, s_tok, s_lp, s_L, s_score, eos_id, pad_id, seq, raw, tok_lp, length, lp_sum, score,
+                   status, parent, next_tok, Tn, pos, in, out, base, K, C);
+}
+
+// Lexical select stage: one CTA per commit, candidate threadIdx.x = i * W + q (W = K + kPhrases): the q-th row entry of
+// live slot i (its bank in key bits kBankShift..), or (q = 0) finished slot i itself; L, n and score as in the plain
+// select stage.  Tc = 0: the plain rule (one bank, every candidate by (score descending, i * (C + 1) + j ascending)).
+// Tc > 0: the carried finished slots first, best score first; then the live candidates striped over the banks: rank r
+// within the candidate's bank by (score, index) as above, then the order (r ascending, bank descending), which is
+// total since two candidates of one bank never share r.  Both orders count the larger keys, like the plain stage.
+constexpr int kLexSelectThreads = kMaxBeam * (kMaxBeam + kPhrases);     // 320 candidates at K = 16
+__global__ void __launch_bounds__(kLexSelectThreads) beam_select_lexical_kernel(
+    const uint64_t* __restrict__ row_top, const int* __restrict__ constraints, const int* __restrict__ copy_src,
+    float alpha, int eos_id, int pad_id, int* __restrict__ seq, int* __restrict__ raw, float* __restrict__ tok_lp,
+    int* __restrict__ length, float* __restrict__ lp_sum, float* __restrict__ score, unsigned char* __restrict__ status,
+    long* __restrict__ parent, int* __restrict__ next_tok, int Tn, int pos, int B, int K, int V, int S) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  __shared__ uint64_t sh_key[kLexSelectThreads];
+  __shared__ int sh_cls[kLexSelectThreads], sh_bank[kLexSelectThreads], sh_r[kLexSelectThreads];
+  __shared__ int s_from[kMaxBeam], s_j[kMaxBeam], s_tok[kMaxBeam];
+  __shared__ float s_lp[kMaxBeam], s_L[kMaxBeam], s_score[kMaxBeam];
+  const int b = blockIdx.x, C = V + S, W = K + kPhrases, n_cand = K * W;
+  const long R = (long)B * K;
+  const long in = (pos & 1) ? R : 0, out = (pos & 1) ? 0 : R;     // row offsets of the read and the written half
+  const long base = (long)b * K;
+  const int tc = constraint_words(constraints + (long)b * kMaxConstraintWords);
+  if (threadIdx.x < K) { s_from[threadIdx.x] = threadIdx.x; s_j[threadIdx.x] = C; }   // unfilled slot: keeps itself
+
+  uint64_t mine = 0;
+  int i = 0, j = C, bank = 0, cls = 0;                // cls: 0 none, 1 live candidate, 2 carried finished slot
+  float lp = 0.f, L = 0.f, sco = 0.f;
+  if ((int)threadIdx.x < n_cand) {
+    i = threadIdx.x / W;
+    const int q = threadIdx.x % W;
+    const long pr = in + base + i;
+    if (status[pr] == 0) {
+      const uint64_t c = row_top[(base + i) * W + q];
+      if (c != 0) {
+        lp = key_lp(c);
+        j = key_index(c);
+        bank = (int)(c >> kBankShift);
+        L = lp_sum[pr] + lp;
+        const int n = length[pr];                     // tokens generated with this one: (length - 1) + 1
+        sco = L / powf((5.f + (float)n) / 6.f, alpha) + 0.f;           // + 0: -0 and +0 rank as one value
+        cls = 1;
+      }
+    } else if (status[pr] == 1 && q == 0) {
+      L = lp_sum[pr];
+      sco = score[pr] + 0.f;
+      cls = 2;
     }
+    if (cls) mine = ((uint64_t)order_bits(sco) << 32) | (0xFFFFFFFFu - (uint32_t)(i * (C + 1) + j));
   }
-  // histories follow their parents; a grown slot gets its new token at column pos + 1
-  for (int e = threadIdx.x; e < K * Tn; e += blockDim.x) {
-    const int k = e / Tn, c = e % Tn;
-    const long src = (in + base + s_from[k]) * Tn + c, dst = (out + base + k) * Tn + c;
-    const bool grow = s_j[k] != C && c == pos + 1;
-    seq[dst] = grow ? s_tok[k] : seq[src];
-    raw[dst] = grow ? s_j[k] : raw[src];
-    tok_lp[dst] = grow ? s_lp[k] : tok_lp[src];
+  if ((int)threadIdx.x < n_cand) { sh_key[threadIdx.x] = mine; sh_cls[threadIdx.x] = cls; sh_bank[threadIdx.x] = bank; }
+  __syncthreads();
+  int rank = 0, r = 0;
+  if (cls && tc == 0) {
+    for (int u = 0; u < n_cand; ++u) rank += sh_key[u] > mine ? 1 : 0;
+  } else if (cls == 2) {
+    for (int u = 0; u < n_cand; ++u) rank += sh_cls[u] == 2 && sh_key[u] > mine ? 1 : 0;
+  } else if (cls == 1) {
+    for (int u = 0; u < n_cand; ++u) r += sh_cls[u] == 1 && sh_bank[u] == bank && sh_key[u] > mine ? 1 : 0;
   }
+  if ((int)threadIdx.x < n_cand) sh_r[threadIdx.x] = r;
+  __syncthreads();
+  if (cls == 1 && tc) {
+    for (int u = 0; u < n_cand; ++u)
+      rank += sh_cls[u] == 2 || (sh_cls[u] == 1 && (sh_r[u] < r || (sh_r[u] == r && sh_bank[u] > bank))) ? 1 : 0;
+  }
+  if (cls && rank < K) {
+    s_from[rank] = i; s_j[rank] = j; s_lp[rank] = lp; s_L[rank] = L; s_score[rank] = sco;
+    s_tok[rank] = j < V ? j : (j < C ? copy_src[(long)b * S + (j - V)] : pad_id);
+  }
+  __syncthreads();
+  beam_write_slots(s_from, s_j, s_tok, s_lp, s_L, s_score, eos_id, pad_id, seq, raw, tok_lp, length, lp_sum, score,
+                   status, parent, next_tok, Tn, pos, in, out, base, K, C);
 }
 
 // ------------------------------------------------------------------ one diverse n-best beam step (beam groups)
@@ -1709,9 +1900,11 @@ static int beam_step_impl(const void* logits, long ld_logits, const float* copy_
                           int pad_id, uint64_t* workspace, int* seq, int* raw, float* token_logprob, int* length,
                           float* logprob, float* score, unsigned char* status, long* parent, int* next_tok, int T_len,
                           int pos, int B, int K, int V, int S, const int* prefix, int ld_prefix, const int* prefix_len,
-                          int no_repeat, int min_len, int dtype, void* stream) {
+                          int no_repeat, int min_len, int dtype, void* stream, const int* constraints = nullptr) {
   FIRA_CHECK_ARG(!prefix || (prefix_len && ld_prefix > pos), FIRA_ERR_ARG,
                  "pointer_mix_beam_step_prefix: null prefix_len or ld_prefix %d <= pos %d", ld_prefix, pos);
+  FIRA_CHECK_ARG(!constraints || T_len <= TMAX, FIRA_ERR_SHAPE, "pointer_mix_beam_step_lexical: T_len %d > %d", T_len,
+                 TMAX);
   FIRA_CHECK_ARG(no_repeat >= 0 && min_len >= 0, FIRA_ERR_ARG,
                  "pointer_mix_beam_step_rules: no_repeat_ngram %d / min_length %d < 0", no_repeat, min_len);
   FIRA_CHECK_ARG((!no_repeat && !min_len) || T_len <= TMAX, FIRA_ERR_SHAPE,
@@ -1725,10 +1918,22 @@ static int beam_step_impl(const void* logits, long ld_logits, const float* copy_
   FIRA_CHECK_ARG(fira_aligned16(logits) && ld_logits % 8 == 0, FIRA_ERR_ALIGN,
                  "pointer_mix_beam_step: logits must be 16-byte aligned with a leading dimension that is a multiple of 8");
   if (B == 0) return FIRA_OK;
-  DISPATCH_T(dtype, launch_k(beam_row_kernel<T>, dim3((unsigned)(B * K)), dim3(kBeamThreads), 0, (cudaStream_t)stream,
-      (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src,
-      (const unsigned char*)status + (pos & 1) * (long)B * K, (const int*)seq + (pos & 1) * (long)B * K * T_len, T_len,
-      workspace, prefix, ld_prefix, prefix_len, no_repeat, min_len, eos_id, pos, K, V, S);)
+  const unsigned char* st_in = status + (pos & 1) * (long)B * K;
+  const int* seq_in = seq + (pos & 1) * (long)B * K * T_len;
+  if (constraints) {
+    DISPATCH_T(dtype, launch_k(beam_row_kernel<T, true>, dim3((unsigned)(B * K)), dim3(kBeamThreads), 0,
+        (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, st_in, seq_in,
+        T_len, workspace, prefix, ld_prefix, prefix_len, no_repeat, min_len, eos_id, pos, K, V, S, constraints);)
+    FIRA_CHECK_LAUNCH("fira_pointer_mix_beam_step_lexical (rows)");
+    launch_k(beam_select_lexical_kernel, dim3((unsigned)B), dim3(kLexSelectThreads), 0, (cudaStream_t)stream,
+             (const uint64_t*)workspace, constraints, copy_src, length_penalty, eos_id, pad_id, seq, raw, token_logprob,
+             length, logprob, score, status, parent, next_tok, T_len, pos, B, K, V, S);
+    FIRA_CHECK_LAUNCH("fira_pointer_mix_beam_step_lexical (select)");
+    return FIRA_OK;
+  }
+  DISPATCH_T(dtype, launch_k(beam_row_kernel<T, false>, dim3((unsigned)(B * K)), dim3(kBeamThreads), 0,
+      (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, st_in, seq_in,
+      T_len, workspace, prefix, ld_prefix, prefix_len, no_repeat, min_len, eos_id, pos, K, V, S, nullptr);)
   FIRA_CHECK_LAUNCH("fira_pointer_mix_beam_step (rows)");
   launch_k(beam_select_kernel, dim3((unsigned)B), dim3(kBeamThreads), 0, (cudaStream_t)stream, (const uint64_t*)workspace,
            copy_src, length_penalty, eos_id, pad_id, seq, raw, token_logprob, length, logprob, score, status, parent,
@@ -1769,6 +1974,21 @@ int fira_pointer_mix_beam_step_rules(const void* logits, long ld_logits, const f
   return beam_step_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, length_penalty, eos_id, pad_id,
                         workspace, seq, raw, token_logprob, length, logprob, score, status, parent, next_tok, T_len, pos,
                         B, K, V, S, prefix, ld_prefix, prefix_len, no_repeat_ngram, min_length, dtype, stream);
+}
+
+int fira_pointer_mix_beam_step_lexical(const void* logits, long ld_logits, const float* copy_scores,
+                                       const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
+                                       float length_penalty, int eos_id, int pad_id, uint64_t* workspace, int* seq,
+                                       int* raw, float* token_logprob, int* length, float* logprob, float* score,
+                                       unsigned char* status, long* parent, int* next_tok, int T_len, int pos, int B,
+                                       int K, int V, int S, int dtype, void* stream, const int* prefix, int ld_prefix,
+                                       const int* prefix_len, int no_repeat_ngram, int min_length,
+                                       const int* constraints) {
+  FIRA_CHECK_ARG(constraints && workspace, FIRA_ERR_ARG, "pointer_mix_beam_step_lexical: null constraints / workspace");
+  return beam_step_impl(logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, length_penalty, eos_id, pad_id,
+                        workspace, seq, raw, token_logprob, length, logprob, score, status, parent, next_tok, T_len, pos,
+                        B, K, V, S, prefix, ld_prefix, prefix_len, no_repeat_ngram, min_length, dtype, stream,
+                        constraints);
 }
 
 static int diverse_beam_step_impl(const void* logits, long ld_logits, const float* copy_scores,

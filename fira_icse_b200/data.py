@@ -120,6 +120,23 @@ def prefix_labels(raw, i, words, vocab, upper, diff_len=210):
     return _dual_copy_labels(msg, _to_ids(msg, vocab, upper), diff, sub_tokens, len(vocab), diff_len)
 
 
+def constraint_words(raw, i, phrases, vocab, upper):
+    """Words a user requires in commit i's message -> their vocabulary ids, for nbest's `constraints`: phrases is a list
+    of phrases, each a string of words separated by spaces or a list of words, normalised as build_commit normalises
+    message words (variable map, case, lemmatisation) -> a list of id lists.  ValueError for a word that maps to
+    <unkm>: it has no id a hypothesis could contain."""
+    var_map = raw["variable"][i]
+    out = []
+    for ph in phrases:
+        words = ph.split() if isinstance(ph, str) else list(ph)
+        ids = _to_ids(_msg_words(words, var_map, upper), vocab, upper)
+        for w, wid in zip(words, ids):
+            if wid == vocab["<unkm>"]:
+                raise ValueError(f"constraint word {w!r} of commit {i} is not in the vocabulary (<unkm>)")
+        out.append(ids)
+    return out
+
+
 def build_commit(raw, i, vocab, ast_vocab, upper, diff_len=210, msg_len=30, att_len=25, ast_change_len=280,
                  sub_len=160):
     """One commit -> padded id arrays + CSR pieces of its normalised adjacency.

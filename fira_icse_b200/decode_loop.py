@@ -61,6 +61,48 @@ def check_rules(no_repeat_ngram, min_length, tar_len):
         raise ValueError(f"no_repeat_ngram / min_length need tar_len <= {MAX_RULES_TAR_LEN}, got {tar_len}")
 
 
+MAX_PHRASES = MAX_PHRASE_LEN = 4    # head.cu kPhrases / kPhraseLen
+
+
+def check_constraints(constraints, B, *, V, tar_len, start_id, eos_id, pad_id, groups=1):
+    """Validates lexical constraints (called before any device work) -> int32 [B, 4, 4] on the host (zero-padded), or
+    None for constraints=None.
+
+    constraints: an integer tensor [B, P <= 4, L <= 4] of vocabulary ids, commit b's phrases; 0 ends a phrase (an
+    all-zero phrase is none).  ValueError for a wrong dtype or shape, a nonzero id after a 0 inside a phrase, an id
+    outside [0, V), <start>, <eos> or pad_id, more than tar_len - 2 words in one commit (every word needs a position
+    before <eos>), tar_len > 32 (the step keeps a row's history in shared memory) and groups > 1 (diverse groups take no
+    constraints)."""
+    if constraints is None:
+        return None
+    if not is_int(groups) or groups != 1:
+        raise ValueError(f"constraints apply to plain n-best only (groups = 1), got groups={groups!r}")
+    if tar_len > MAX_RULES_TAR_LEN:
+        raise ValueError(f"constraints need tar_len <= {MAX_RULES_TAR_LEN}, got {tar_len}")
+    if not torch.is_tensor(constraints) or constraints.dtype == torch.bool or constraints.is_floating_point() or \
+            constraints.is_complex():
+        raise ValueError(f"constraints must be an integer tensor, got {getattr(constraints, 'dtype', type(constraints))}")
+    if constraints.dim() != 3 or constraints.shape[0] != B or not 1 <= constraints.shape[1] <= MAX_PHRASES or \
+            not 1 <= constraints.shape[2] <= MAX_PHRASE_LEN:
+        raise ValueError(f"constraints must have shape [B={B}, P <= {MAX_PHRASES}, L <= {MAX_PHRASE_LEN}], got "
+                         f"{tuple(constraints.shape)}")
+    c = constraints.detach().to("cpu", torch.int64)
+    nz = c != 0
+    if (nz[:, :, 1:] & ~nz[:, :, :-1]).any():
+        raise ValueError("constraints: a nonzero id follows a 0 inside a phrase (a 0 ends a phrase)")
+    if ((c < 0) | (c >= V)).any():
+        raise ValueError(f"constraints: ids must be in [0, V = {V})")
+    for name, i in (("<start>", start_id), ("<eos>", eos_id), ("pad_id", pad_id)):
+        if i != 0 and (c == i).any():
+            raise ValueError(f"constraints: {name} ({i}) cannot be required")
+    tc = nz.sum((1, 2))
+    if (tc > tar_len - 2).any():
+        raise ValueError(f"constraints: at most tar_len - 2 = {tar_len - 2} words per commit, got {int(tc.max())}")
+    out = torch.zeros((B, MAX_PHRASES, MAX_PHRASE_LEN), dtype=torch.int32)
+    out[:, :c.shape[1], :c.shape[2]] = c.to(torch.int32)
+    return out
+
+
 def check_prefix(prefix, sou, sub_token, *, V, tar_len, eos_id, pad_id, eos_last):
     """Validates a prefix (called before any device work) -> (prefix int32 [B, tar_len], prefix_len int32 [B]) on the
     host, or None for prefix=None.

@@ -485,6 +485,30 @@ int fira_pointer_mix_diverse_beam_step_rules(const void* logits, long ld_logits,
                                              int dtype, void* stream, const int* prefix, int ld_prefix,
                                              const int* prefix_len, int no_repeat_ngram, int min_length);
 
+/* ---- lexically constrained n-best (fira_icse_b200.beam.nbest `constraints=`; dynamic beam allocation, Post & Vilar,
+ *      2018).  Arguments as the n-best _rules step, with workspace [B*K, K+4] keys (not [B*K, K]), plus constraints
+ *      int32 [B, 4, 4] on the device: commit b's phrases of up to 4 vocabulary ids, 0 = padding after a phrase's last
+ *      word; Tc = commit b's nonzero entries (<= 16; 0 = no constraints).  The words of a row are its seq ids in columns
+ *      1..pos, as for the rules.  Progress of phrase c (length L) on words h: L if c occurs contiguously in h, else the
+ *      largest m < L with h ending in c_1..c_m (0 if none); a row meets its constraints when the sum over its phrases
+ *      is Tc.  Row stage per live, non-forced row: <eos> is banned while its progress is below Tc (next to the rules);
+ *      it proposes (a) its K best allowed labels as the _rules step, and (b) per phrase it has not met, in phrase
+ *      order, the best label by (lp, then smaller j) among j = w and the unmasked copies of w, w = the phrase's next
+ *      word c_{prog+1}, unless w is banned, an earlier phrase proposed w or the label is in (a).  A forced row proposes
+ *      its one label.  Each proposal's bank = the progress of the row's words with its word appended.  Select stage,
+ *      L, n and score as the n-best step: with Tc = 0, the K best by (score descending, i * (C + 1) + j ascending),
+ *      bit for bit the _rules step; with Tc > 0, the carried finished slots first (best score first), then the live
+ *      candidates by (r ascending, bank descending), r = the candidate's rank by (score, index) within its bank.  The
+ *      chosen slots become slots 0..K-1 in that order.  Bounds: K <= 16 and T_len <= 32. */
+int fira_pointer_mix_beam_step_lexical(const void* logits, long ld_logits, const float* copy_scores,
+                                       const float* gate_logits, const unsigned char* mem_mask, const int* copy_src,
+                                       float length_penalty, int eos_id, int pad_id, uint64_t* workspace, int* seq,
+                                       int* raw, float* token_logprob, int* length, float* logprob, float* score,
+                                       unsigned char* status, long* parent, int* next_tok, int T_len, int pos, int B,
+                                       int K, int V, int S, int dtype, void* stream, const int* prefix, int ld_prefix,
+                                       const int* prefix_len, int no_repeat_ngram, int min_length,
+                                       const int* constraints);
+
 /* ---- ensemble decoding (fira_icse_b200/ensemble.py): M <= 8 models' mixtures (Model.py:54-86) averaged into one fp32
  *      triple the three step kernels above read with dtype FIRA_F32.  Member m: logits[m] (`dtype`, [B*N, ld_logits],
  *      16-byte aligned), copy_scores[m] [B, N, S] fp32, gate_logits[m] [B*N, 2] fp32 (host arrays of M device

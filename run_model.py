@@ -42,6 +42,12 @@ beam search ranking.  Differences, all below the module surface:
     §9).  A nonzero value appends _norepeat<n> / _minlen<m> to the output name, after any _prefix<k>
     (output_fira_nbest_norepeat2_minlen3, ...), so the outputs without them stay.  FIRA_DECODE=beam with either set
     exits with an error.
+    FIRA_CONSTRAINT_WORDS=k (default 0 = off, at most 4; FIRA_DECODE=nbest with FIRA_BEAM_GROUPS=1 only): lexically
+    constrained n-best (DESIGN.md §9), every test commit's message must contain the first k distinct words of its
+    reference that also occur among its diff ids (sou or sub_token, never <unkm>), each a one-word phrase: the
+    oracle-constraint evaluation of the constrained-decoding papers.  Appends _lex<k> to the output name after the other
+    tags (output_fira_nbest_lex1, ...) and prints, after the mean BLEU, the share of commits whose top hypothesis meets
+    its constraints.  Any other decoding mode, or FIRA_BEAM_GROUPS > 1, with k > 0 exits with an error.
     FIRA_CHECKPOINT (default best_model.pt): the state_dict `test` decodes with (best_model_scst.pt after finetune).
     FIRA_ENSEMBLE=a.pt,b.pt[,...] (FIRA_DECODE=sample, nbest or mbr; up to 8 state_dicts, not with FIRA_CHECKPOINT):
     decode with the ensemble of those checkpoints (fira_icse_b200.ensemble: the weighted average of their
@@ -78,8 +84,9 @@ from torch.optim import Adam
 from torch.utils.data import DataLoader
 
 from fira_icse_b200 import TransModel
-from fira_icse_b200.beam import beam_search, best_sequences, nbest
+from fira_icse_b200.beam import beam_search, best_sequences, constraints_met, nbest
 from fira_icse_b200.bleu import sentence_bleu_method2
+from fira_icse_b200.decode_loop import MAX_PHRASES
 from fira_icse_b200.distill import distill_step
 from fira_icse_b200.data import PackedBatchLoader, TransDataset, batch_to_device, collate_packed
 from fira_icse_b200.engine import GraphedTrainStep
@@ -161,6 +168,23 @@ def reference_prefix(b, k, eos_id, pad_id):
     V = args.vocab_size
     gone = (lab >= V) & ~mem_mask.gather(1, (lab - V).clamp(0, mem_mask.shape[1] - 1))
     return lab.masked_fill(((lab == eos_id) | gone).long().cumsum(1) > 0, 0)
+
+
+def oracle_constraints(b, k, vocab):
+    """Each commit's first k distinct reference words (b[1] after <start>, up to <eos>) that also occur among its diff ids
+    (sou b[0] or sub_token b[7]), never <unkm> or a special id, as one-word phrases -> [B, k, 1] (zeros where a commit
+    has fewer), nbest's `constraints`."""
+    special = {vocab[w] for w in ("<start>", "<eos>", "<pad>", "<unkm>") if w in vocab} | {0}
+    tar, sou, sub = b[1].tolist(), b[0].tolist(), b[7].tolist()
+    out = torch.zeros((len(tar), k, 1), dtype=torch.long)
+    for i, ref in enumerate(tar):
+        ref = ref[1:ref.index(vocab['<eos>'])] if vocab['<eos>'] in ref else ref[1:]
+        diff, words = set(sou[i]) | set(sub[i]), []
+        for w in ref:
+            if w in diff and w not in special and w not in words and len(words) < k:
+                words.append(w)
+        out[i, :len(words), 0] = torch.tensor(words, dtype=torch.long)
+    return out
 
 
 def loader(ds, batch_size, shuffle, indices=None):
@@ -293,8 +317,14 @@ def decoder(mode, vocab):
                          "reference beam search takes no rules")
     rules = dict(no_repeat_ngram=no_repeat, min_length=min_len)
     ens = ensemble_settings(mode)
+    n_lex = int(os.environ.get("FIRA_CONSTRAINT_WORDS", 0))
+    if n_lex and (mode != "nbest" or int(os.environ.get("FIRA_BEAM_GROUPS", 1)) != 1):
+        raise SystemExit("FIRA_CONSTRAINT_WORDS applies to FIRA_DECODE=nbest with FIRA_BEAM_GROUPS=1 only")
+    if not 0 <= n_lex <= MAX_PHRASES:
+        raise SystemExit(f"FIRA_CONSTRAINT_WORDS must be in [0, {MAX_PHRASES}], got {n_lex}")
     tag = (f"_prefix{k}" if k else "") + (f"_norepeat{no_repeat}" if no_repeat else "") + \
-        (f"_minlen{min_len}" if min_len else "") + (f"_ens{len(ens[0])}" if ens else "")
+        (f"_minlen{min_len}" if min_len else "") + (f"_ens{len(ens[0])}" if ens else "") + \
+        (f"_lex{n_lex}" if n_lex else "")
 
     def pre(b):                         # each commit's own first k reference labels, or no prefix
         return reference_prefix(b, k, vocab['<eos>'], vocab['<pad>']) if k else None
@@ -328,9 +358,15 @@ def decoder(mode, vocab):
         diverse = dict(groups=groups, diversity=float(os.environ.get("FIRA_DIVERSITY", 0.5))) if groups != 1 else {}
 
         def decode(model, b, first_index):
+            con = oracle_constraints(b, n_lex, vocab) if n_lex else None
             out = nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=args.beam_size, length_penalty=alpha, **diverse,
-                        prefix=pre(b), **rules, **ids)
+                        prefix=pre(b), **rules, constraints=con, **ids)
+            if n_lex:                   # commits whose top hypothesis meets its constraints, commits
+                decode.met[0] += int(constraints_met(out.seq[:, :1], out.length[:, :1], con).sum())
+                decode.met[1] += out.seq.shape[0]
             return out.seq, out.length, (out.score, out.logprob)
+        if n_lex:
+            decode.met = [0, 0]
         return "output_fira_nbest" + tag, decode, 1
     raise SystemExit("FIRA_DECODE must be 'beam', 'sample', 'nbest' or 'mbr'")
 
@@ -426,6 +462,8 @@ def main_test():
     out = f"OUTPUT/{name}" if WORLD == 1 else f"OUTPUT/{name}.part{RANK:02d}"
     bleu = test(model, test_loader, g, all_index['test'][lo:hi], dev_, lo, decode, n_bleu, out)
     print("mean sentence bleu: %f" % bleu)
+    if hasattr(decode, "met"):
+        print("constraints met by the top hypothesis: %f" % (decode.met[0] / max(1, decode.met[1])))
 
 
 def finetune_settings():

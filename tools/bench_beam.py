@@ -31,6 +31,14 @@ reference's own loop was timed on in BASELINE.md (72 s for 32 commits on CPU).  
                                M * 2 * (V * s + S * 4) + (V + S) * 4 (s = 2 bytes in bf16, 4 in fp32: each member row is
                                read twice, the fp32 triple written once) and the share of HBM peak that implies)
 
+    python tools/bench_beam.py --constraint-words k [--batches ...] [--beams ...] [--precision ...] [--reps ...]
+                               (lexically constrained n-best instead of the modes above: nbest per batch and beam
+                               width without and with each commit's first k distinct reference words that occur in
+                               its diff as one-word phrases (run_model.oracle_constraints), in the same run, each line
+                               with met_share, the share of commits whose top hypothesis meets the constraints; then
+                               one step call, fira_pointer_mix_beam_step_lexical against fira_pointer_mix_beam_step_rules,
+                               at B = 128, pos = 20 with every slot live)
+
 nbest and diverse lines also carry `self_bleu`: the mean pairwise id-level sentence BLEU among each commit's K
 hypotheses (one fira_mbr_select launch with pair_bleu, off-diagonal entries averaged over the batch); lower means a
 more diverse list.
@@ -66,6 +74,7 @@ def main():
     ap.add_argument("--no-repeat-ngram", type=int, default=0, help="also time the decoders with n-gram repeat blocking")
     ap.add_argument("--min-length", type=int, default=0, help="also time the decoders with a minimum message length")
     ap.add_argument("--ensemble", default="", help="member counts M to time ensemble decoding at (e.g. 1,2,4)")
+    ap.add_argument("--constraint-words", type=int, default=0, help="time nbest with k oracle constraint words")
     a = ap.parse_args()
     rules = (a.no_repeat_ngram, a.min_length)
     import torch
@@ -84,6 +93,8 @@ def main():
     model.eval()
     if a.ensemble:
         return bench_ensemble(a, model, dev)
+    if a.constraint_words:
+        return bench_lexical(a, model, dev)
     for B in (int(x) for x in a.batches.split(",")):
         hb = bench.host_batch(10_000, B, pin=False, trim=a.trim)
         b = bench.device_batch(hb, dev, B)
@@ -249,6 +260,86 @@ def bench_ensemble(a, model, dev):
                                       "CUDA events; bytes count each member row twice (the second read is meant to "
                                       "come from L2)"}), flush=True)
             del sets
+
+
+def bench_lexical(a, model, dev):
+    """--constraint-words: nbest without and with oracle constraints, then one step call of each kernel (module
+    docstring)."""
+    import torch
+    import bench
+    import run_model
+    from fira_icse_b200 import ops
+    from fira_icse_b200._lib import FIRA_BF16, FIRA_F32, call
+    from fira_icse_b200.beam import constraints_met, nbest
+    card, watts = torch.cuda.get_device_name(dev), power_limit()
+    ids = dict(tar_len=30, start_id=1, eos_id=2, pad_id=0)
+    vocab = {"<start>": 1, "<eos>": 2, "<pad>": 0}
+    for B in (int(x) for x in a.batches.split(",")):
+        b = bench.device_batch(bench.host_batch(10_000, B, pin=False, trim=a.trim), dev, B)
+        con = run_model.oracle_constraints(b, a.constraint_words, vocab)
+        for K in (int(x) for x in a.beams.split(",")):
+            for c in (None, con):
+                def run():
+                    return nbest(model, b[0], b[3], b[4], b[5], b[7], beam_size=K, constraints=c, **ids)
+                out = run()                                              # warm-up (graph capture)
+                torch.cuda.synchronize()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                for _ in range(a.reps):
+                    out = run()
+                e1.record()
+                torch.cuda.synchronize()
+                ms = e0.elapsed_time(e1) / a.reps
+                met = constraints_met(out.seq[:, :1], out.length[:, :1], con)
+                print(json.dumps({"metric": "lexically constrained n-best throughput", "unit": "commits/s",
+                                  "value": B / ms * 1e3, "ms_per_batch": ms, "batch": B, "beam": K,
+                                  "constraint_words": a.constraint_words if c is not None else 0,
+                                  "commits_with_constraints": int((con != 0).any(-1).any(-1).sum()),
+                                  "met_share": met.float().mean().item(), "mean_length": out.length.double().mean().item(),
+                                  "decoded_steps": int(out.length.max().item()) - 1, "precision": a.precision,
+                                  "card": card, "power_limit_w": watts,
+                                  "data": "synthetic (DataSet distribution), random weights"}), flush=True)
+    # one step call at B = 128, pos = 20: every slot live, random histories, the bench model's V and S = 370
+    gen = torch.Generator(device=dev).manual_seed(5)
+    B, K, T, pos, S, V = 128, int(a.beams.split(",")[0]), 30, 20, 370, model.vocab_size
+    R = B * K
+    ldl = ops._ld_logits(V)
+    tdt = torch.bfloat16 if a.precision == "bf16" else torch.float32
+    logits = (torch.randn((R, ldl), generator=gen, device=dev) * 3).to(tdt)
+    sc = torch.randn((B, K, S), generator=gen, device=dev) * 2
+    gl = torch.randn((R, 2), generator=gen, device=dev)
+    mask = torch.ones((B, S), dtype=torch.uint8, device=dev)
+    src = torch.randint(3, V, (B, S), generator=gen, device=dev, dtype=torch.int32)
+    seq = torch.randint(3, V, (2, R, T), generator=gen, device=dev, dtype=torch.int32)
+    raw, tlp = seq.clone(), torch.zeros((2, R, T), device=dev)
+    length = torch.full((2, R), pos + 1, dtype=torch.int32, device=dev)
+    lp, score = -torch.rand((2, R), generator=gen, device=dev), torch.zeros((2, R), device=dev)
+    status = torch.zeros((2, R), dtype=torch.uint8, device=dev)
+    parent = torch.empty(R, dtype=torch.int64, device=dev)
+    nxt = torch.empty(R, dtype=torch.int32, device=dev)
+    work = torch.empty(R * (K + 4), dtype=torch.int64, device=dev)
+    cons = torch.zeros((B, 4, 4), dtype=torch.int32, device=dev)
+    k = a.constraint_words
+    cons[:, :k, 0] = src[:, :k]                                      # one-word phrases the copies can spell
+    pre = torch.zeros((B, T), dtype=torch.int32, device=dev)
+    pre_len = torch.zeros(B, dtype=torch.int32, device=dev)
+    P = ops._ptr
+    args = [P(logits), ldl, P(sc), P(gl), P(mask), P(src), 0.0, 2, 0, P(work), P(seq), P(raw), P(tlp), P(length),
+            P(lp), P(score), P(status), P(parent), P(nxt), T, pos, B, K, V, S,
+            FIRA_BF16 if a.precision == "bf16" else FIRA_F32]
+    tail = [P(pre), T, P(pre_len), 0, 0]
+    times = {}
+    for name, extra in (("fira_pointer_mix_beam_step_rules", []), ("fira_pointer_mix_beam_step_lexical", [P(cons)]),
+                        ("fira_pointer_mix_beam_step_rules", []), ("fira_pointer_mix_beam_step_lexical", [P(cons)])):
+        # the stream is read per launch: time_launches captures on its own stream
+        _, med_ms, launches = bench.time_launches(lambda i: call(name, *args, ops._stream(), *tail, *extra), 1, reps=20)
+        times.setdefault(name, []).append(med_ms)                    # alternated: two measurements each
+    for name, t in times.items():
+        print(json.dumps({"metric": name + " time", "unit": "us", "value": min(t) * 1e3, "runs_us": [x * 1e3 for x in t],
+                          "batch": B, "beam": K, "pos": pos, "V": V, "S": S, "constraint_words": k,
+                          "precision": a.precision, "card": card, "power_limit_w": watts,
+                          "note": "median device time per call (row + select launches), calls replayed from one CUDA "
+                                  "graph between CUDA events, the two kernels alternated"}), flush=True)
 
 
 def self_bleu(h, B, K):
