@@ -1405,6 +1405,88 @@ __global__ void __launch_bounds__(kEnsThreads) pointer_mix_ensemble_kernel(
   if (threadIdx.x == 0) { gl_out[row * 2] = s_gate[0]; gl_out[row * 2 + 1] = s_gate[1]; }
 }
 
+// ------------------------------------------------------------------ nearest-neighbour combine
+// One row's (logits, copy scores, gate logits) and its k neighbours from fira_knn_search -> one fp32 triple whose
+// mixture is P'_j = (1 - lam) P_j + lam q_j (j < V), P'_{V+s} = (1 - lam) P_{V+s}.  P's row statistics come from
+// mix_row_stats (bit for bit the step kernels'); q_w = sum over neighbours i with word w of e_i / Z, e_i =
+// exp(-(d_i - d_1) / tau), Z = sum_i e_i in neighbour order.  With a0 = (1 - lam) g0, a1 = (1 - lam) g1, G0 = a0 + lam:
+//   gl'  = (log G0, log a1)                                           (a1 == 0: -inf, the copy side is exactly 0)
+//   x'_j = o + x_j,  o = log a0 - log G0 - vmax - log vsum            (a0 == 0: kMaskFill)
+//   x'_w = LSE(o + x_w, log(lam q_w) - log G0)                       for each neighbour word w
+//   c'_s = c_s                                                        (masked s: kMaskFill)
+// exp(gl'_0) + exp(gl'_1) = 1 and sum_j exp(x'_j) = 1 up to rounding, so the step kernels' g0' softmax(x')_j is P'_j.
+constexpr int kKnnMaxK = 64;
+
+__device__ __forceinline__ float lse2(float a, float b) {
+  const float mx = fmaxf(a, b), mn = fminf(a, b);
+  return mn == -INFINITY ? mx : mx + log1pf(expf(mn - mx));
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kEnsThreads) pointer_mix_knn_kernel(
+    const T* __restrict__ logits, long ldl, const float* __restrict__ sc, const float* __restrict__ gl,
+    const unsigned char* __restrict__ mem_mask, const int* __restrict__ nb_idx, const float* __restrict__ nb_dist,
+    const int* __restrict__ words, int k, const float* __restrict__ params, float* __restrict__ logits_out,
+    long ld_out, float* __restrict__ sc_out, float* __restrict__ gl_out, int N, int V, int S) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  __shared__ MaxSum sh_ms[8];
+  __shared__ float bc[4];
+  __shared__ int s_w[kKnnMaxK];
+  __shared__ float s_e[kKnnMaxK];
+  __shared__ float s_o[3];                            // o, log G0, Z
+  const long row = blockIdx.x;
+  const int b = (int)(row / N);
+  const T* lrow = logits + row * ldl;
+  const float* srow = sc + row * S;
+  const unsigned char* mrow = mem_mask + (long)b * S;
+  const MixRow ms = mix_row_stats(lrow, srow, mrow, gl + row * 2, V, S, sh_ms, bc);
+  const float lam = params[0], tau = params[1];
+  if ((int)threadIdx.x < k) {
+    const long i = row * k + threadIdx.x;
+    s_w[threadIdx.x] = words[nb_idx[i]];
+    s_e[threadIdx.x] = expf(-(nb_dist[i] - nb_dist[row * k]) / tau);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float Z = 0.f;
+    for (int i = 0; i < k; ++i) Z += s_e[i];
+    const float a0 = (1.f - lam) * ms.g0, a1 = (1.f - lam) * ms.g1, lG0 = logf(a0 + lam);
+    s_o[0] = a0 > 0.f ? logf(a0) - lG0 - ms.vmax - logf(ms.vsum) : -INFINITY;
+    s_o[1] = lG0;
+    s_o[2] = Z;
+    gl_out[row * 2] = lG0;
+    gl_out[row * 2 + 1] = a1 > 0.f ? logf(a1) : -INFINITY;
+  }
+  __syncthreads();
+  const float o = s_o[0];
+  float* orow = logits_out + row * ld_out;
+  const int V8 = V >> 3;
+  for (int g = threadIdx.x; g < V8; g += blockDim.x) {
+    float x[8];
+    Act<T>::load8(lrow + (long)g * 8, x);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) x[i] = o == -INFINITY ? kMaskFill : o + x[i];
+    Act<float>::store8(orow + (long)g * 8, x);
+  }
+  for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x)
+    orow[j] = o == -INFINITY ? kMaskFill : o + Act<T>::ld(lrow + j);
+  float* crow = sc_out + row * S;
+  for (int j = threadIdx.x; j < S; j += blockDim.x) crow[j] = mrow[j] ? srow[j] : kMaskFill;
+  __syncthreads();                                    // the plain entries are written; the neighbour words follow
+  if ((int)threadIdx.x < k) {
+    const int i = threadIdx.x, w = s_w[i];
+    bool first = w >= 0 && w < V;                     // the datastore holds vocabulary ids only
+    for (int j = 0; j < i && first; ++j) first = s_w[j] != w;
+    if (first) {                                      // the first neighbour with word w writes x'_w
+      float e = 0.f;
+      for (int j = i; j < k; ++j) e += s_w[j] == w ? s_e[j] : 0.f;
+      const float nb = logf(lam * (e / s_o[2])) - s_o[1];
+      const float x = o == -INFINITY ? nb : lse2(o + Act<T>::ld(lrow + w), nb);
+      orow[w] = x == -INFINITY ? kMaskFill : x;       // lam q_w underflowed with a0 == 0: P'_w is 0, as masked
+    }
+  }
+}
+
 // ------------------------------------------------------------------ knowledge distillation loss
 // Row r with shifted label y != 0: the student's mixture P (head_fwd_kernel's expressions) against the teacher's t (the
 // same expressions on the teacher's fp32 triple, fira_pointer_mix_ensemble's output):
@@ -2108,6 +2190,27 @@ int fira_pointer_mix_ensemble(const void* const* logits, long ld_logits, const f
   DISPATCH_T(dtype, launch_k(pointer_mix_ensemble_kernel<T>, dim3((unsigned)(B * N)), dim3(kEnsThreads), 0,
       (cudaStream_t)stream, mem, M, ld_logits, log_weights, mem_mask, logits_out, ld_out, copy_out, gate_out, N, V, S);)
   FIRA_CHECK_LAUNCH("fira_pointer_mix_ensemble");
+  return FIRA_OK;
+}
+
+int fira_pointer_mix_knn(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                         const unsigned char* mem_mask, const int* nb_idx, const float* nb_dist, const int* words,
+                         int k, const float* params, float* logits_out, long ld_out, float* copy_out, float* gate_out,
+                         int B, int N, int V, int S, int dtype, void* stream) {
+  FIRA_CHECK_ARG(k >= 1 && k <= kKnnMaxK, FIRA_ERR_ARG, "pointer_mix_knn: k %d not in [1, %d]", k, kKnnMaxK);
+  FIRA_CHECK_ARG(logits && copy_scores && gate_logits && mem_mask && nb_idx && nb_dist && words && params &&
+                 logits_out && copy_out && gate_out, FIRA_ERR_ARG, "pointer_mix_knn: null pointer");
+  FIRA_CHECK_ARG(fira_aligned16(logits) && fira_aligned16(logits_out) && ld_logits % 8 == 0 && ld_out % 8 == 0,
+                 FIRA_ERR_ALIGN, "pointer_mix_knn: logits / logits_out must be 16-byte aligned, ld_logits %ld and "
+                 "ld_out %ld multiples of 8", ld_logits, ld_out);
+  FIRA_CHECK_ARG(B >= 0 && N > 0 && V > 0 && S > 0 && V + S <= 0x7FFF && ld_logits >= V && ld_out >= V, FIRA_ERR_SHAPE,
+                 "pointer_mix_knn: shape (B %d, N %d, V %d, S %d, ld_logits %ld, ld_out %ld; V + S must be <= 32767)",
+                 B, N, V, S, ld_logits, ld_out);
+  if (B == 0) return FIRA_OK;
+  DISPATCH_T(dtype, launch_k(pointer_mix_knn_kernel<T>, dim3((unsigned)(B * N)), dim3(kEnsThreads), 0,
+      (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, nb_idx, nb_dist, words, k,
+      params, logits_out, ld_out, copy_out, gate_out, N, V, S);)
+  FIRA_CHECK_LAUNCH("fira_pointer_mix_knn");
   return FIRA_OK;
 }
 

@@ -21,6 +21,7 @@ from . import optim as _optim
 from ._lib import FIRA_F32, call
 from .ensemble import Ensemble, members
 from .incremental import IncrementalDecoder, replay_or_capture, weights_key
+from .knn import KNNModel, base_model, search_into, workspace_bytes
 
 D = ops.D
 POLL_EVERY = 8            # positions between two reads of the all-finished flag
@@ -37,7 +38,7 @@ def is_int(v):
 def check_tar_len(model, tar_len):
     """ValueError when the decoder (of any member of an ensemble) has fewer than tar_len positions (called before any
     device work)."""
-    for m in members(model):
+    for m in members(base_model(model)):
         if tar_len > m.decoder.pos_encode.shape[0]:
             raise ValueError(f"tar_len {tar_len} exceeds the decoder's {m.decoder.pos_encode.shape[0]} positions")
 
@@ -167,7 +168,7 @@ def encode(model, sou, mark, ast_change, edge, sub_token, pad_id):
 
 def encode_members(model, sou, mark, ast_change, edge, sub_token, pad_id):
     """encode() with every member of an ensemble (one model: itself) -> ([memory per member], mem_mask, copy_src)."""
-    out = [encode(m, sou, mark, ast_change, edge, sub_token, pad_id) for m in members(model)]
+    out = [encode(m, sou, mark, ast_change, edge, sub_token, pad_id) for m in members(base_model(model))]
     return [o[0] for o in out], out[0][1], out[0][2]
 
 
@@ -196,7 +197,7 @@ class _Head:
         """logits, copy scores and gate logits of decoder row t (every launch on the current stream: capturable)."""
         m, pr = self.model, self.pr
         cn = m.copy_net
-        x = self.inc.advance(t)                                                  # [R, D]
+        x = self.x = self.inc.advance(t)                                         # [R, D]; a kNN loop's queries
         pr.linear(x, m.out_fc.weight, m.out_fc.bias, out=self.logits, ld_out=self.logits.shape[1])
         pr.linear(x, cn.LinearTarget.weight, out=self.tgt)
         ops.linear(x.float() if pr.bf16 else x, cn.LinearProb.weight, cn.LinearProb.bias, out=self.gl)   # fp32 gate
@@ -222,13 +223,14 @@ class PositionLoop:
     first one's token buffer and pad mask (`inc`, which the step kernels write); reorder() moves every member's KV
     cache and the shared mask once.  head(t) runs the members one after another, then fira_pointer_mix_ensemble writes
     the averaged triple into the loop's own fp32 logits / sc / gl.  One model is one _Head whose buffers are the
-    loop's, with no combine."""
+    loop's, with no combine.  A knn.KNNModel is its model's _Head, then fira_knn_search of the decoder row and
+    fira_pointer_mix_knn into the loop's own fp32 triple, with lam / tau in a device buffer written at start()."""
 
     halves = 1
 
     def __init__(self, model, B, N, T, S):
         self.model, self.B, self.N, self.T, self.S = model, B, N, T, S
-        ms = members(model)
+        ms = members(base_model(model))
         self.heads = [_Head(ms[0], B, N, T, S)]
         self.heads += [_Head(m, B, N, T, S, share=self.heads[0].inc) for m in ms[1:]]
         h0 = self.heads[0]
@@ -240,7 +242,20 @@ class PositionLoop:
         self.mem_mask = torch.zeros((B, S), dtype=torch.uint8, device=dev)
         self.copy_src = torch.zeros((B, S), dtype=torch.int32, device=dev)
         self.ensemble = isinstance(model, Ensemble)
-        if self.ensemble:
+        self.knn = isinstance(model, KNNModel)
+        if self.knn:
+            f32 = dict(dtype=torch.float32, device=dev)
+            self.logits = torch.empty((R, self.ldl), **f32)
+            self.gl = torch.empty((R, 2), **f32)
+            self.sc = torch.empty((B, N, S), **f32)
+            self.code = FIRA_F32
+            self.store, self.k = model.datastore, model.k      # the loop holds the datastore its graphs read
+            self.knn_idx = torch.empty((R, self.k), dtype=torch.int32, device=dev)
+            self.knn_dist = torch.empty((R, self.k), **f32)
+            self.knn_ws = torch.empty(workspace_bytes(R, self.k, dev), dtype=torch.uint8, device=dev)
+            self.knn_params = torch.zeros(2, **f32)           # (lam, tau), read by the captured combine
+            self.knn_settings = (model.lam, model.temperature)  # loop_for sets the calling KNNModel's
+        elif self.ensemble:
             f32 = dict(dtype=torch.float32, device=dev)
             self.logits = torch.empty((R, self.ldl), **f32)
             self.gl = torch.empty((R, 2), **f32)
@@ -280,6 +295,8 @@ class PositionLoop:
             self.prefix_len.copy_(prefix[1])
         for h, mem in zip(self.heads, memory):
             h.start(mem, mem_mask)
+        if self.knn:
+            self.knn_params.copy_(torch.tensor(self.knn_settings, dtype=torch.float32))
         if self.ensemble:
             self.log_w.copy_(torch.tensor(self.log_weights, dtype=torch.float32))
         self.mem_mask.copy_(mem_mask)
@@ -324,6 +341,12 @@ class PositionLoop:
             call("fira_pointer_mix_ensemble", ctypes.addressof(lg), self.heads[0].logits.shape[1], ctypes.addressof(sc),
                  ctypes.addressof(gl), len(self.heads), p(self.log_w), p(self.mem_mask), p(self.logits), self.ldl,
                  p(self.sc), p(self.gl), B, N, self.V, S, self.pr.code, ops._stream())
+        elif self.knn:
+            h, p = self.heads[0], ops._ptr
+            search_into(self.store, h.x, self.k, self.knn_ws, self.knn_idx, self.knn_dist)
+            call("fira_pointer_mix_knn", p(h.logits), h.logits.shape[1], p(h.sc), p(h.gl), p(self.mem_mask),
+                 p(self.knn_idx), p(self.knn_dist), p(self.store.words), self.k, p(self.knn_params), p(self.logits),
+                 self.ldl, p(self.sc), p(self.gl), B, N, self.V, S, self.pr.code, ops._stream())
 
     def reorder(self, parent):
         """Row r of every member's KV cache and of the shared pad mask continues row parent[r] (n-best)."""
@@ -342,6 +365,21 @@ class PositionLoop:
         return t
 
 
+def drop_loops(model):
+    """Forget the cached loops (buffers and captured graphs) of `model`: a TransModel or an Ensemble drops every loop
+    of its first member, a KNNModel only the loops over its datastore, which releases the datastore and the search
+    workspace those loops hold.  The next decode captures its graphs again."""
+    ms = members(base_model(model))
+    store = _LOOPS.get(ms[0])
+    if store is None:
+        return
+    if isinstance(model, KNNModel):
+        for key in [k for k in store if "knn" in k and k[k.index("knn") + 1] == id(model.datastore)]:
+            del store[key]
+    else:
+        del _LOOPS[ms[0]]
+
+
 _LOOPS = weakref.WeakKeyDictionary()   # model (an ensemble's first member) -> {key: (weights keys, addresses, loop)}
 
 
@@ -350,12 +388,19 @@ def loop_for(cls, model, B, N, T, S):
     address the graphs captured) are refreshed inside the loop, whose position graphs keep replaying: a training loop
     that samples after every optimizer step (scst.py) does not recapture them.  A parameter that moved rebuilds the
     loop (fresh operand copies and graphs).  An ensemble is keyed by its members, not by the Ensemble object: a new
-    Ensemble of the same models replays the same graphs, with its own weights written at start()."""
-    ms = members(model)
+    Ensemble of the same models replays the same graphs, with its own weights written at start().  A KNNModel is keyed
+    by its model, its Datastore object (with the addresses of the keys, norms and words its graphs read) and k: a new
+    KNNModel over the same model and datastore replays the same graphs, with its own lam / tau written at start().
+    A cached kNN loop holds its datastore and search workspace for as long as the model lives; drop_loops releases
+    them."""
+    ms = members(base_model(model))
     store = _LOOPS.setdefault(ms[0], {})
     key = (cls, B, N, T, S, ms[0].precision)
     if isinstance(model, Ensemble):        # the loop holds its members, so their ids stay theirs while it is cached
         key += (tuple(id(m) for m in ms),)
+    if isinstance(model, KNNModel):        # the loop holds the datastore, so its id stays its own while cached
+        st = model.datastore
+        key += ("knn", id(st), st.keys.data_ptr(), st.norms.data_ptr(), st.words.data_ptr(), st.N, model.k)
     wkey = tuple(weights_key(m, m.decoder) for m in ms)
     addr = tuple(p.data_ptr() for m in ms for p in m.parameters())
     cur = store.get(key)
@@ -367,4 +412,6 @@ def loop_for(cls, model, B, N, T, S):
     loop = store[key][2]
     if isinstance(model, Ensemble):
         loop.log_weights = model.log_weights
+    if isinstance(model, KNNModel):
+        loop.knn_settings = (model.lam, model.temperature)
     return loop

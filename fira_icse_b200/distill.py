@@ -28,7 +28,7 @@ import torch
 from . import ops
 from . import optim as _optim
 from ._lib import FIRA_BF16, FIRA_F32, call
-from .ensemble import Ensemble
+from .ensemble import Ensemble, refuse
 from .model import TransModel
 from .modules import _i32, _u8
 from .scst import bump_weights
@@ -141,6 +141,7 @@ def distill_step(model, optimizer, batch, teacher, *, alpha):
     loss, nll and kd, tokens).  The student runs in training mode (the kernels' dropout) and stays in it; the
     teacher's members are left in eval mode.  Settings and teacher are checked on the host before any device work."""
     check_alpha(alpha)
+    refuse(model, "distill_step")
     teacher_members(teacher, model)
     dev = model.out_fc.weight.device
     label = model.shifted_label(batch[6].to(dev))

@@ -91,6 +91,9 @@ def members(model):
 
 
 def refuse(model, what):
-    """TypeError for an Ensemble passed where only one model is supported."""
+    """TypeError for an Ensemble or a knn.KNNModel passed where only one model is supported."""
+    from .knn import KNNModel
     if isinstance(model, Ensemble):
         raise TypeError(f"{what} takes a single model; ensembles decode through sample, score, nbest and mbr")
+    if isinstance(model, KNNModel):
+        raise TypeError(f"{what} takes a single model; a KNNModel decodes through sample, score, nbest and mbr")

@@ -528,6 +528,37 @@ int fira_pointer_mix_ensemble(const void* const* logits, long ld_logits, const f
                               const unsigned char* mem_mask, float* logits_out, long ld_out, float* copy_out,
                               float* gate_out, int B, int N, int V, int S, int dtype, void* stream);
 
+/* ---- nearest-neighbour decoding (fira_icse_b200/knn.py, knn.cu): exact k-nearest search of a datastore of N 256-wide
+ *      bf16 keys, then the mixture of a row's P with its neighbours' words.
+ *   knn_search: queries [R, ld_q] (`dtype`, rounded to bf16), keys [N, 256] bf16, norms [N] fp32 (sum of key^2 over
+ *      the bf16 values), all 16-byte aligned, ld_q a multiple of 8 and >= 256 -> idx [R, k] int32 and dist [R, k] fp32:
+ *      the k entries with the smallest (d_i, i), ascending, d_i = fma(-2, q . key_i, |q|^2 + norm_i) with the bf16
+ *      products accumulated in fp32 in a fixed order and |q|^2 in fp32.  Ties in d go to the smaller index.  A row's
+ *      output depends only on its query and the datastore (not on R, the other rows or the tiling): graph replays and
+ *      repeated runs agree bit for bit.  workspace: 16-byte aligned device memory of workspace_bytes >= 8 k R.  The
+ *      keys are split P ways, P = min(SMs / ceil(R / 128), workspace_bytes / (8 k R), ceil(N / 64), 256) (at least
+ *      1), one sorted candidate list per (split, row); so 8 k max(R, 128 SMs) bytes always give the full split
+ *      (8.7 MB at k = 64 on 132 SMs, for any R up to 16,896).  1 <= k <= 64, k <= N < 2^31.  Two launches: the
+ *      mma.sync distance product with the candidate lists in its epilogue, and a merge of the P lists per row.
+ *   pointer_mix_knn: the model's triple (logits `dtype` [B*N, ld_logits], copy_scores [B, N, S] fp32, gate_logits
+ *      [B*N, 2] fp32), mem_mask [B, S], nb_idx / nb_dist [B*N, k] from knn_search, words [N_store] int32 (the
+ *      entries' vocabulary ids), params [2] fp32 device = (lam, tau) (read at run time, so a captured launch follows
+ *      new values) -> the fp32 triple (logits_out [B*N, ld_out], copy_out [B, N, S], gate_out [B*N, 2]) whose step
+ *      kernel mixture is P'_j = (1 - lam) P_j + lam q_j (j < V), P'_{V+s} = (1 - lam) P_{V+s}, up to fp32 rounding;
+ *      q_w = sum over the neighbours with word w of exp(-(d_i - d_1) / tau) / Z.  With P's row statistics from the step
+ *      kernels' own expressions, a0 = (1 - lam) g0, a1 = (1 - lam) g1, G0 = a0 + lam:
+ *        gl' = (log G0, log a1),  x'_j = log a0 - log G0 + x_j - vmax - log vsum,  c'_s = c_s (masked s: -1e9),
+ *        x'_w = LSE(that, log(lam q_w) - log G0) for each neighbour word w.
+ *      a0 == 0 in fp32 gives x'_j = -1e9 for every word whose P' is 0 (no neighbour mass, or lam q_w underflowed
+ *      to 0); a1 == 0 gives gl'_1 = -inf.  One CTA of 256 threads per row.  1 <= k <= 64, ld_logits / ld_out
+ *      multiples of 8 and >= V, V + S <= 32767, 0 < lam < 1, tau > 0 (the caller checks lam and tau). */
+int fira_knn_search(const void* queries, long ld_q, int dtype, const void* keys, const float* norms, long N, int R,
+                    int k, void* workspace, long workspace_bytes, int* idx, float* dist, void* stream);
+int fira_pointer_mix_knn(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
+                         const unsigned char* mem_mask, const int* nb_idx, const float* nb_dist, const int* words,
+                         int k, const float* params, float* logits_out, long ld_out, float* copy_out, float* gate_out,
+                         int B, int N, int V, int S, int dtype, void* stream);
+
 /* ---- knowledge distillation (fira_icse_b200/distill.py): the student's mixture P against a teacher's fp32 triple
  *      (t_logits [rows, ld_t], t_copy_scores [B, T_len, S], t_gate_logits [rows, 2]; fira_pointer_mix_ensemble's output
  *      with N = T_len), whose mixture t is formed by the same expressions.  Student operands as

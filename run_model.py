@@ -54,6 +54,17 @@ beam search ranking.  Differences, all below the module surface:
     distributions at every position), weighted by FIRA_ENSEMBLE_WEIGHTS=w1,w2,... (positive, one per checkpoint;
     default uniform).  Appends _ens<M> to the output name after the other tags (output_fira_nbest_norepeat2_ens2, ...),
     so single-model outputs stay.  FIRA_DECODE=beam with an ensemble exits with an error.
+    FIRA_KNN=datastore.pt (FIRA_DECODE=sample, nbest or mbr; not with FIRA_ENSEMBLE): nearest-neighbour decoding
+    (fira_icse_b200.knn, DESIGN.md §9) with the datastore `datastore` built from this checkpoint: each position mixes the
+    model's distribution with the next words of the FIRA_KNN_K (default 8) nearest training positions, at temperature
+    FIRA_KNN_TEMPERATURE (default 10) and weight FIRA_KNN_LAMBDA (default 0.25).  The defaults are common starting
+    points of the kNN-MT papers, not tuned on this data.  Appends _knn<k> to the output name after the other tags.
+    FIRA_DECODE=beam, an ensemble, bad settings and a datastore built by another checkpoint exit with an error before
+    any device work.
+  * `datastore`: builds the kNN datastore of `test`'s FIRA_KNN from the train split with FIRA_CHECKPOINT (default
+    best_model.pt) in padded batches of FIRA_BATCH commits (FIRA_PRECISION: the precision it is built and used in) and
+    writes FIRA_DATASTORE (default datastore.pt): one entry per target position (decoder state -> next word).  Prints
+    the entry count and bytes.  One GPU.
   * `finetune`: self-critical fine-tuning on sentence BLEU (fira_icse_b200.scst, DESIGN.md §9), one GPU.  Loads
     best_model.pt and runs FIRA_SCST_EPOCHS (default 1) epochs of scst_step with optim.FlatAdam at FIRA_SCST_LR
     (default 1e-5) over padded batches of FIRA_BATCH commits (FIRA_MAX_BATCHES bounds an epoch): FIRA_SAMPLES (default
@@ -91,6 +102,7 @@ from fira_icse_b200.distill import distill_step
 from fira_icse_b200.data import PackedBatchLoader, TransDataset, batch_to_device, collate_packed
 from fira_icse_b200.engine import GraphedTrainStep
 from fira_icse_b200.ensemble import MAX_MEMBERS, Ensemble
+from fira_icse_b200.knn import Datastore, KNNModel, build_datastore, check_settings, state_fingerprint
 from fira_icse_b200.mbr import mbr
 from fira_icse_b200.parallel import DataParallelStep, shard_range
 from fira_icse_b200.sample import sample
@@ -301,10 +313,13 @@ def main_train():
         dist.destroy_process_group()
 
 
-def decoder(mode, vocab):
+_UNCHECKED = object()
+
+
+def decoder(mode, vocab, knn=_UNCHECKED):
     """FIRA_DECODE -> (output file, decode(model, batch, dataset position of its first commit) -> seq [B, N, T],
     length [B, N] and the numeric columns [B, N] written before each message, how many leading hypotheses of a commit
-    count towards the BLEU)."""
+    count towards the BLEU).  knn: knn_settings' result when the caller has already checked it."""
     ids = dict(tar_len=args.tar_len, start_id=vocab['<start>'], eos_id=vocab['<eos>'], pad_id=vocab['<pad>'])
     k = int(os.environ.get("FIRA_PREFIX_WORDS", 0))
     if k and mode == "beam":
@@ -322,9 +337,11 @@ def decoder(mode, vocab):
         raise SystemExit("FIRA_CONSTRAINT_WORDS applies to FIRA_DECODE=nbest with FIRA_BEAM_GROUPS=1 only")
     if not 0 <= n_lex <= MAX_PHRASES:
         raise SystemExit(f"FIRA_CONSTRAINT_WORDS must be in [0, {MAX_PHRASES}], got {n_lex}")
+    if knn is _UNCHECKED:
+        knn = knn_settings(mode, ens)
     tag = (f"_prefix{k}" if k else "") + (f"_norepeat{no_repeat}" if no_repeat else "") + \
         (f"_minlen{min_len}" if min_len else "") + (f"_ens{len(ens[0])}" if ens else "") + \
-        (f"_lex{n_lex}" if n_lex else "")
+        (f"_lex{n_lex}" if n_lex else "") + (f"_knn{knn['k']}" if knn else "")
 
     def pre(b):                         # each commit's own first k reference labels, or no prefix
         return reference_prefix(b, k, vocab['<eos>'], vocab['<pad>']) if k else None
@@ -438,6 +455,40 @@ def ensemble_checkpoints():
     return paths, weights
 
 
+def knn_settings(mode, ens):
+    """`test`'s FIRA_KNN / FIRA_KNN_K / FIRA_KNN_TEMPERATURE / FIRA_KNN_LAMBDA -> dict(path, k, temperature, lam, store),
+    or None without FIRA_KNN; store is the datastore on the host, loaded once.  Checked before any device work, the
+    datastore against the checkpoint on the host (SystemExit on an error)."""
+    path = os.environ.get("FIRA_KNN", "")
+    if not path:
+        return None
+    if mode == "beam":
+        raise SystemExit("FIRA_KNN applies to FIRA_DECODE=sample, nbest and mbr; the reference beam search decodes the "
+                         "model alone")
+    if ens:
+        raise SystemExit("FIRA_KNN decodes one checkpoint: unset FIRA_ENSEMBLE")
+    try:
+        s = dict(path=path, k=int(os.environ.get("FIRA_KNN_K", 8)),
+                 temperature=float(os.environ.get("FIRA_KNN_TEMPERATURE", 10.0)),
+                 lam=float(os.environ.get("FIRA_KNN_LAMBDA", 0.25)))
+        check_settings(s["k"], s["temperature"], s["lam"])
+    except ValueError as e:
+        raise SystemExit(f"FIRA_KNN settings: {e}")
+    ckpt = os.environ.get("FIRA_CHECKPOINT", "best_model.pt")
+    for p in (path, ckpt):
+        if not os.path.isfile(p):
+            raise SystemExit(f"FIRA_KNN: {p} not found")
+    try:
+        store = Datastore.load(path, "cpu", precision=os.environ.get("FIRA_PRECISION", "fp32"))
+        check_settings(s["k"], s["temperature"], s["lam"], store.N)
+    except ValueError as e:
+        raise SystemExit(f"FIRA_KNN: {e}")
+    if store.fingerprint != state_fingerprint(torch.load(ckpt, map_location="cpu")):
+        raise SystemExit(f"FIRA_KNN: {path} was built by other weights than {ckpt} (fingerprint mismatch)")
+    s["store"] = store
+    return s
+
+
 def load_model(path, dev_):
     model = TransModel(args)
     model.load_state_dict(torch.load(path, map_location="cpu"))
@@ -447,18 +498,22 @@ def load_model(path, dev_):
 def main_test():
     mode = os.environ.get("FIRA_DECODE", "beam")
     ens = ensemble_settings(mode)
+    knn = knn_settings(mode, ens)                                   # the datastore is read once, on the host
     dev_ = device()
     g = load_globals()
     test_set = TransDataset(args, 'test')
     all_index = json.load(open('all_index'))
+    name, decode, n_bleu = decoder(mode, g["vocab"], knn)           # every setting is checked before the models load
     if ens:
         model = Ensemble([load_model(p, dev_) for p in ens[0]], ens[1])
     else:
         model = load_model(os.environ.get("FIRA_CHECKPOINT", "best_model.pt"), dev_)
+    if knn:
+        model = KNNModel(model, knn.pop("store").to(dev_), k=knn["k"], temperature=knn["temperature"],
+                         lam=knn["lam"])
     lo, hi = shard_range(len(test_set), RANK, WORLD)                # replicas only: index ranges, files concatenated
     idx = list(range(lo, hi)) if WORLD > 1 else None
     test_loader = loader(test_set, args.test_batch_size, False, idx)
-    name, decode, n_bleu = decoder(mode, g["vocab"])
     out = f"OUTPUT/{name}" if WORLD == 1 else f"OUTPUT/{name}.part{RANK:02d}"
     bleu = test(model, test_loader, g, all_index['test'][lo:hi], dev_, lo, decode, n_bleu, out)
     print("mean sentence bleu: %f" % bleu)
@@ -599,6 +654,25 @@ def main_distill():
     print("best dev bleu: %f" % best_bleu)
 
 
+def main_datastore():
+    if WORLD > 1:
+        raise SystemExit("run_model.py datastore runs on one GPU: launch it without torchrun (WORLD_SIZE=1)")
+    ckpt = os.environ.get("FIRA_CHECKPOINT", "best_model.pt")
+    out = os.environ.get("FIRA_DATASTORE", "datastore.pt")
+    if not os.path.isfile(ckpt):
+        raise SystemExit(f"FIRA_CHECKPOINT: {ckpt} not found")
+    dev_ = device()
+    g = load_globals()
+    vocab = g["vocab"]
+    train_set = TransDataset(args, 'train')
+    model = load_model(ckpt, dev_)
+    batches = (batch_to_device(b, dev_) for b in loader(train_set, args.batch_size, False))
+    store = build_datastore(model, batches, first_index=0, start_id=vocab['<start>'], eos_id=vocab['<eos>'],
+                            pad_id=vocab['<pad>'], unk_id=vocab['<unkm>'])
+    store.save(out)
+    print("datastore: %d entries, %d bytes -> %s" % (store.N, store.nbytes, out))
+
+
 if __name__ == '__main__':
     stage = str(sys.argv[1])
     seed_everything()
@@ -611,5 +685,7 @@ if __name__ == '__main__':
         main_finetune()
     elif stage == 'distill':
         main_distill()
+    elif stage == 'datastore':
+        main_datastore()
     else:
-        raise SystemExit("usage: python run_model.py train|test|finetune|distill")
+        raise SystemExit("usage: python run_model.py train|test|finetune|distill|datastore")
