@@ -627,7 +627,10 @@ class DecoderFn(torch.autograd.Function):
     cfg["label"] (the shifted labels [B, T] of a packed bf16 training batch, else absent): the backward runs on the live
     target rows alone, the rows before each commit's last label (fira_target_rows, at most pk.Rt).  No later row carries
     a loss, and causal self-attention never lets a live row read one, so they change neither the loss nor a gradient;
-    their output rows are zero."""
+    their output rows are zero.  Precondition: tar_mask[b, 0] = 1 for every commit with a label.  A row whose causal
+    keys are all padding attends uniformly over all T rows (attn_mma.cuh), dead rows included, and the slot backward
+    would drop the gradient those rows receive; row 0 as a valid key rules such a live row out.  The loader never breaks
+    it: every target starts with the <start> token."""
 
     @staticmethod
     def forward(ctx, cfg, tar, memory, mem_mask, tar_mask, pos_table, dec_emb, *lp):

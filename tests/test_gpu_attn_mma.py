@@ -4,7 +4,8 @@ incremental-decoding form (few query rows, no statistics), causal rows without a
 any fixed chunk budget.  Tolerances as in test_gpu_ops_bf16.py: P is rounded to bf16 before P.V (2^-8 of the
 largest output), the backward consumes bf16 P / dS and the bf16 forward output (2^-6).  The packed form also runs on
 the FFMA kernels (fp32 parity mode at the fp32 bounds of test_gpu_ops.py, bf16 with FIRA_ATTN_TC=0), and all three
-kernels must reproduce the padded entry points bit for bit on the same keys."""
+kernels must reproduce the padded entry points bit for bit on the same keys.  fira_attn_bwd_rows, the backward on the
+training step's live-row slots, is checked against float64 over the live query rows alone."""
 import math
 
 import pytest
@@ -42,9 +43,8 @@ PACKED_SPEC = [(150, 27, "rand"), (100, 0, "rand"), (40, 12, "none"), (7, 3, "al
 SENTINEL = 3.0
 
 
-def _packed_layout():
+def _packed_layout(spec=PACKED_SPEC):
     """-> ranges [B][4], mask [B, pitch] bool, pitch, kv_rows; rows outside every range lie between and after them"""
-    spec = PACKED_SPEC
     B = len(spec)
     pitch = max(a + b for a, b, _ in spec) + 5
     gm = torch.Generator().manual_seed(7)
@@ -227,3 +227,122 @@ def test_attention_padded_shapes(Lq, Lk, causal):
     ref.backward(go.double())
     close16(dq, qd.grad, glob=2.0 ** -6, what="attention dq")
     close16(dkv, kvd.grad, glob=2.0 ** -6, what="attention dkv")
+
+
+# ------------------------------------------------------------------ the backward on live-row slots (fira_attn_bwd_rows)
+# layout -> (T, key ranges, live query rows per commit): counts at the m16 edge (1, 15, 16, 17) and the LQ_MAX edge
+# (a fully live 32-row commit), a commit without live rows inside the batch and one last (its CTAs zero the pad rows)
+SLOT_LAYOUTS = {
+    "T30": (30, PACKED_SPEC + [(33, 64, "rand")], [17, 30, 1, 0, 15, 16]),
+    "T32_empty_last": (32, PACKED_SPEC, [32, 16, 1, 17, 0]),
+}
+
+
+def _slots(counts, T, pad):
+    """-> qoff [B+1], trows [R] (row b*T + t of each slot, -1 for the pad slots) for live rows t < counts[b]"""
+    qoff = [0]
+    for n in counts:
+        qoff.append(qoff[-1] + n)
+    trows = [b * T + t for b, n in enumerate(counts) for t in range(n)] + [-1] * pad
+    return qoff, torch.tensor(trows, device=DEV)
+
+
+@pytest.mark.parametrize("pad", [0, 21], ids=["R_exact", "R_pad"])
+@pytest.mark.parametrize("layout", list(SLOT_LAYOUTS))
+@pytest.mark.parametrize("causal", [1, 0], ids=["self", "cross"])
+def test_attention_backward_on_slots_against_float64(causal, layout, pad):
+    """forward on every row (fira_attn_fwd causal over tar_mask / fira_attn_packed_fwd), then the live rows gathered into
+    slots qoff[b] + t and fira_attn_bwd_rows against float64 autograd over those rows alone.  Causal keys are the commit's
+    slots, cross keys its packed ranges.  dq and the causal dk / dv start as NaN, the cross dk / dv as SENTINEL: every key
+    row of every range is written (a commit without live rows: exactly zero), masked keys get exactly zero, rows outside
+    the ranges stay SENTINEL, pad slots come back zero"""
+    from fira_icse_b200 import _lib
+    T, spec, counts = SLOT_LAYOUTS[layout]
+    B = len(counts)
+    qoff, trows = _slots(counts, T, pad)
+    qoff_d = torch.tensor(qoff, dtype=torch.int32, device=DEV)
+    nl, R = qoff[B], qoff[B] + pad
+    tm = torch.ones(B, T, dtype=torch.uint8, device=DEV)
+    tm[0, 5] = 0                                              # a masked key among commit 0's live rows
+    for b, n in enumerate(counts):
+        tm[b, n + 2:] = 0                                     # padding past the message (never a live row's key)
+    ranges, mask, pitch, kv_rows = _packed_layout(spec)
+    stats = torch.empty(B, H, T, 2, device=DEV)
+    ctx = torch.empty(B * T, D, device=DEV, dtype=BF)
+    if causal:
+        qkv = rnd16(B * T, 3 * D, seed=21)
+        _lib.call("fira_attn_fwd", qkv.data_ptr(), 3 * D, qkv[:, D:].data_ptr(), 3 * D, qkv[:, 2 * D:].data_ptr(),
+                  3 * D, tm.data_ptr(), 1, ctx.data_ptr(), D, stats.data_ptr(), B, H, T, T, DH, 1, st())
+        q = qkv[:, :D]
+    else:
+        q, kv = rnd16(B * T, D, seed=22), rnd16(kv_rows, 2 * D, seed=23)
+        rg = torch.tensor(ranges, dtype=torch.int32, device=DEV)
+        mask_u8 = mask.to(torch.uint8).to(DEV)
+        _lib.call("fira_attn_packed_fwd", q.data_ptr(), D, kv.data_ptr(), 2 * D, kv[:, D:].data_ptr(), 2 * D,
+                  rg.data_ptr(), kv_rows, mask_u8.data_ptr(), pitch, 1, ctx.data_ptr(), D, stats.data_ptr(), B, H, T,
+                  DH, 1, st())
+    idx, padm = trows.clamp(min=0), (trows < 0)[:, None]
+
+    def gather(x):
+        return x[idx].masked_fill(padm, 0).contiguous()
+    q_s, ctx_s = gather(q), gather(ctx)
+    go_s = rnd16(R, D, seed=24).masked_fill(padm, 0).contiguous()
+    nan = float("nan")
+    dq_s = torch.full((R, D), nan, device=DEV, dtype=BF)
+    if causal:
+        qkv_s = gather(qkv)
+        dqkv_s = torch.full((R, 3 * D), nan, device=DEV, dtype=BF)
+        _lib.call("fira_attn_bwd_rows", qkv_s.data_ptr(), 3 * D, qkv_s[:, D:].data_ptr(), 3 * D,
+                  qkv_s[:, 2 * D:].data_ptr(), 3 * D, None, tm.data_ptr(), T, 1, qoff_d.data_ptr(), R,
+                  ctx_s.data_ptr(), go_s.data_ptr(), D, stats.data_ptr(), dqkv_s.data_ptr(), 3 * D,
+                  dqkv_s[:, D:].data_ptr(), 3 * D, dqkv_s[:, 2 * D:].data_ptr(), 3 * D, B, H, T, DH, 1, st())
+        dq_s = dqkv_s[:, :D]
+    else:
+        dkv = torch.full_like(kv, SENTINEL)
+        _lib.call("fira_attn_bwd_rows", q_s.data_ptr(), D, kv.data_ptr(), 2 * D, kv[:, D:].data_ptr(), 2 * D,
+                  rg.data_ptr(), mask_u8.data_ptr(), pitch, 0, qoff_d.data_ptr(), R, ctx_s.data_ptr(), go_s.data_ptr(),
+                  D, stats.data_ptr(), dq_s.data_ptr(), D, dkv.data_ptr(), 2 * D, dkv[:, D:].data_ptr(), 2 * D,
+                  B, H, T, DH, 1, st())
+    torch.cuda.synchronize()
+
+    # float64 autograd over the live query rows only
+    qd = q_s.double().requires_grad_(True)
+    outs = []
+    if causal:
+        kvd = qkv_s[:, D:].double().requires_grad_(True)
+        for b in range(B):
+            s = slice(qoff[b], qoff[b + 1])
+            if qoff[b + 1] > qoff[b]:
+                outs.append(_ref(qd[s], kvd[s, :D], kvd[s, D:], tm[b, :qoff[b + 1] - qoff[b]].bool(), True))
+    else:
+        kvd = kv.double().requires_grad_(True)
+        for b in range(B):
+            keys = kvd[_key_rows(ranges[b]).to(DEV)]
+            s0, n0, s1, n1 = ranges[b]
+            if qoff[b + 1] > qoff[b]:
+                outs.append(_ref(qd[qoff[b]:qoff[b + 1]], keys[:, :D], keys[:, D:], mask[b, :n0 + n1].to(DEV), False))
+    torch.cat(outs).backward(go_s[:nl].double())
+
+    assert not dq_s.isnan().any(), "dq: a slot was not written"
+    close16(dq_s[:nl], qd.grad[:nl], glob=2.0 ** -6, what="slot attention dq")
+    assert (dq_s[nl:] == 0).all(), "dq: a pad slot is not zero"
+    if causal:
+        dkv_s = dqkv_s[:, D:]
+        assert not dkv_s.isnan().any(), "dk / dv: a slot was not written"
+        close16(dkv_s[:nl], kvd.grad[:nl], glob=2.0 ** -6, what="slot attention causal dk / dv")
+        assert (dkv_s[nl:] == 0).all(), "dk / dv: a pad slot is not zero"
+        dead = [qoff[b] + t for b in range(B) for t in range(qoff[b + 1] - qoff[b]) if not tm[b, t]]
+        assert dead and (dkv_s[dead] == 0).all(), "masked keys must get exactly zero gradient"
+        return
+    touched = torch.zeros(kv_rows, dtype=torch.bool)
+    for b in range(B):
+        rows = _key_rows(ranges[b])
+        touched[rows] = True
+        n0, n1 = ranges[b][1], ranges[b][3]
+        if qoff[b + 1] == qoff[b]:
+            assert (dkv[rows.to(DEV)] == 0).all(), f"commit {b} has no live row: its keys must get exactly zero"
+        elif spec[b][2] != "none":
+            assert (dkv[rows[~mask[b, :n0 + n1]].to(DEV)] == 0).all(), "masked keys must get exactly zero gradient"
+    td = touched.to(DEV)
+    close16(dkv[td], kvd.grad[td], glob=2.0 ** -6, what="slot attention cross dk / dv")
+    assert (dkv[~td] == SENTINEL).all(), "rows outside every range were written"

@@ -7,7 +7,11 @@ kernel's own z and residuals must reproduce every LayerNorm output: a wrong mask
 
 Layouts: padded batches (T = 30 and 32; a commit without a valid memory key, a target row without a valid key) and
 packed batches of golden commits and of a hand-made ragged layout (an empty sub-token range, a commit without a valid
-key).  Outputs start as NaN, so an element the kernel does not write fails the comparison."""
+key).  Outputs start as NaN, so an element the kernel does not write fails the comparison.
+
+fira_decoder_fwd_rows (the live-row slot layout of the training step) runs on the same batches with maps from
+fira_target_rows: every slot must be bit-equal to its row of the map-less run above, pad slots zero, the output zero
+past each commit's last label and NaN for a live row without a slot, and nothing written past any buffer."""
 import ctypes
 
 import pytest
@@ -221,6 +225,152 @@ def test_layouts_have_the_edge_cases():
     assert 0 in [n1 for *_, n1 in lay.ranges] and not bool(lay.mask[1].any())
     bt = Batch(7, 30, 1)
     assert not bool(bt.mem_mask[2].any()) and int(bt.tar_mask[1, 0]) == 0
+
+
+# ------------------------------------------------------------------ the live-row slot layout (fira_decoder_fwd_rows)
+SLOT_NAMES = ("qkv", "ctx1", "z1", "x1", "q", "ctx2", "z2", "x2", "hh", "z3")      # with X: the 11 bf16 tensors
+GUARD = 64                      # elements after each buffer that no call may write
+FILL = 3.0                      # their value (exact in bf16)
+
+
+def target_map(label, R):
+    """fira_target_rows on labels [B, T] -> device tlen [B], toff [B+1], trows [R] (-1: a pad slot)"""
+    from fira_icse_b200 import _lib
+    B, T = label.shape
+    lab = torch.as_tensor(label, dtype=torch.int32).to(DEV)
+    m = torch.full((2 * B + 1 + R,), 7, dtype=torch.int32, device=DEV)
+    p = m.data_ptr()
+    _lib.call("fira_target_rows", lab.data_ptr(), B, T, p, p + 4 * B, p + 4 * (2 * B + 1), R, st())
+    torch.cuda.synchronize()
+    return m[:B], m[B:2 * B + 1], m[2 * B + 1:]
+
+
+def live_labels(bt, counts):
+    """labels [B, T] whose commit b has counts[b] live rows, a zero label inside the longest message"""
+    lab = torch.zeros(bt.B, bt.T, dtype=torch.int32)
+    for b, n in enumerate(counts):
+        lab[b, :n] = 5 + b
+        assert n == 0 or int(bt.tar_mask[b, 0]) == 1, "a labelled commit's row 0 must be a valid key (DecoderFn)"
+    lab[max(range(bt.B), key=lambda b: counts[b]), 2] = 0
+    return lab
+
+
+def run_rows(bt, tlen, toff, R, p=0.0, seed=0, sid=64):
+    """fira_decoder_fwd_rows with the map (tlen, toff) and R slots: every buffer starts as NaN, followed by GUARD
+    elements of FILL -> (outputs, guards)"""
+    from fira_icse_b200 import _lib
+    B, T = bt.B, bt.T
+    o, guards = {}, {}
+
+    def e(name, *shape, dtype=BF):
+        n = 1
+        for s in shape:
+            n *= s
+        buf = torch.full((n + GUARD,), float("nan"), dtype=dtype, device=DEV)
+        buf[n:] = FILL
+        o[name], guards[name] = buf[:n].view(*shape), buf[n:]
+    e("X", L, R, D)
+    e("out", B * T, D)
+    e("qkv", L, R, 3 * D)
+    e("hh", L, R, F)
+    for n in ("ctx1", "z1", "x1", "q", "ctx2", "z2", "x2", "z3"):
+        e(n, L, R, D)
+    for n in ("st1", "st2"):
+        e(n, L, B, H, T, 2, dtype=torch.float32)
+    for n in ("ls1", "ls2", "ls3"):
+        e(n, L, 2, R, dtype=torch.float32)
+    ptr = {k: v.data_ptr() for k, v in o.items()}
+    _lib.call("fira_decoder_fwd_rows", bt.tar.data_ptr(), bt.emb.data_ptr(), bt.pe.data_ptr(), bt.tar_mask.data_ptr(),
+              bt.kv.data_ptr(), bt.kv.shape[1], bt.mem_mask.data_ptr(),
+              bt.ranges.data_ptr() if bt.ranges is not None else None, bt.S, ctypes.addressof(bt.table), L,
+              ptr["X"], ptr["out"], ptr["qkv"], ptr["ctx1"], ptr["st1"], ptr["z1"], ptr["ls1"], ptr["x1"], ptr["q"],
+              ptr["ctx2"], ptr["st2"], ptr["z2"], ptr["ls2"], ptr["x2"], ptr["hh"], ptr["z3"], ptr["ls3"],
+              tlen.data_ptr(), toff.data_ptr(), R, B, T, float(p), seed, None, sid, st())
+    torch.cuda.synchronize()
+    return o, guards
+
+
+def check_slots(bt, full, o, guards, tlen, toff, trows):
+    """the slot layout against the map-less run `full` (checked against float64 by test_decoder_fwd_matches_float64):
+    slots bit-equal to their rows, pad slots zero, out = the last layer's rows / zero past tlen / NaN for a live row
+    without a slot, st1 / st2 unchanged, nothing written past any buffer"""
+    B, T = bt.B, bt.T
+    R = trows.numel()
+    nl = int(toff[B])
+    rows = trows[:nl].long()
+    assert bool((rows >= 0).all()) and bool((trows[nl:] == -1).all())
+    saved = dict((n, full[n]) for n in SLOT_NAMES)
+    saved["X"] = full["X"][:L]
+    for n, t in saved.items():
+        assert torch.equal(o[n][:, :nl], t[:, rows]), f"{n}: a slot differs from its row"
+        assert bool((o[n][:, nl:] == 0).all()), f"{n}: a pad slot is not zero"
+    for n in ("ls1", "ls2", "ls3"):
+        assert torch.equal(o[n][:, :, :nl], full[n][:, :, rows]), f"{n}: a slot differs from its row"
+    for n in ("st1", "st2"):
+        assert torch.equal(o[n], full[n]), f"{n}: the [L, B, H, T, 2] statistics changed"
+    tl, to = tlen.long().cpu(), toff.long().cpu()
+    t_idx = torch.arange(T)
+    slotted = (t_idx[None, :] < (to[1:] - to[:-1])[:, None]).view(-1).to(DEV)
+    alive = (t_idx[None, :] < tl[:, None]).view(-1).to(DEV)
+    last = full["X"][L]
+    assert torch.equal(o["out"][slotted], last[slotted]), "out: a live row differs from the map-less output"
+    assert bool((o["out"][~alive] == 0).all()), "out: a row past tlen is not zero"
+    assert bool(o["out"][alive & ~slotted].isnan().all()), "out: a live row without a slot is not NaN"
+    for n, g in guards.items():
+        assert bool((g == FILL).all()), f"{n}: written past the end of the buffer"
+    return R - nl
+
+
+# case -> (live rows per commit, p): every case has empty, 1-row, 16 / 17-row and full-length commits
+SLOT_CASES = {
+    "padded T=30": ([30, 0, 1, 16, 17, 9, 29], 0.0),
+    "padded T=30 dropout": ([30, 0, 1, 16, 17, 9, 29], 0.2),
+    "padded T=32": ([32, 0, 17, 1, 16, 31, 3], 0.0),
+    "packed hand T=30": ([30, 0, 17, 1, 16], 0.0),
+}
+
+
+@pytest.mark.parametrize("slots", ["exact", "pad", "short"])
+@pytest.mark.parametrize("case", list(SLOT_CASES))
+def test_decoder_fwd_rows_slot_layout(case, slots):
+    """fira_decoder_fwd_rows on the same batch as fira_decoder_fwd: R = the live count, R with pad slots, and R below
+    the live count (the commits past the last slot come up short)"""
+    counts, p = SLOT_CASES[case]
+    bt = CASES[case.replace(" dropout", "")]()
+    full = run(bt, p=p, seed=77, sid=64)
+    lab = live_labels(bt, counts)
+    n = sum(counts)
+    R = {"exact": n, "pad": min(n + 37, bt.B * bt.T), "short": n - 20}[slots]
+    tlen, toff, trows = target_map(lab, R)
+    assert tlen.tolist() == counts
+    o, guards = run_rows(bt, tlen, toff, R, p=p, seed=77, sid=64)
+    pad = check_slots(bt, full, o, guards, tlen, toff, trows)
+    assert pad == {"exact": 0, "pad": R - n, "short": 0}[slots]
+    if slots == "short":
+        assert bool(o["out"].isnan().any())
+
+
+def test_decoder_fwd_rows_bad_arguments():
+    """tlen without toff, R = 0 and R > B*T with a map are refused with an error code, before any launch"""
+    from fira_icse_b200 import _lib
+    bt = CASES["padded T=30"]()
+    B, T = bt.B, bt.T
+    tlen, toff, _ = target_map(live_labels(bt, SLOT_CASES["padded T=30"][0]), B * T)
+    X = torch.zeros(L, B * T, 4 * F, dtype=BF, device=DEV)
+    f = torch.zeros(L, B, H, T, 2, device=DEV)
+    x, s = X.data_ptr(), f.data_ptr()
+
+    def call(tl, to, R):
+        _lib.call("fira_decoder_fwd_rows", bt.tar.data_ptr(), bt.emb.data_ptr(), bt.pe.data_ptr(),
+                  bt.tar_mask.data_ptr(), bt.kv.data_ptr(), bt.kv.shape[1], bt.mem_mask.data_ptr(), None, bt.S,
+                  ctypes.addressof(bt.table), L, x, x, x, x, s, x, s, x, x, x, s, x, s, x, x, x, s, tl, to, R, B, T,
+                  0.0, 0, None, 64, st())
+    for tl, to, R in ((tlen.data_ptr(), None, B * T), (None, toff.data_ptr(), B * T),
+                      (tlen.data_ptr(), toff.data_ptr(), 0), (tlen.data_ptr(), toff.data_ptr(), B * T + 1)):
+        with pytest.raises(_lib.FiraLibraryError, match="tlen and toff"):
+            call(tl, to, R)
+    torch.cuda.synchronize()
+    assert bool((X == 0).all()) and bool((f == 0).all())
 
 
 @pytest.mark.parametrize("case", ["padded T=30", "packed hand T=30"])

@@ -1,6 +1,7 @@
 """The training step's decoder on the live target rows only, the rows before each commit's last label (ops.DecoderFn with
-cfg["label"]): fira_target_rows against numpy, the slot twins of the attention and LayerNorm backward against the
-row-layout kernels, and DecoderFn with the map against DecoderFn without it on a packed golden batch.  The map only
+cfg["label"]): fira_target_rows against numpy, the LayerNorm backward's slot twin against the row-layout kernel, the
+embedding backward through the map against float64, and DecoderFn with the map against DecoderFn without it on a
+packed golden batch (the attention backward on slots: tests/test_gpu_attn_mma.py).  The map only
 moves rows to other slots, so a live row's forward values are the same, and the gradients agree to the bf16 rounding of
 GEMM tiles that now hold other rows."""
 import copy
@@ -100,68 +101,49 @@ def _map(lab, cap):
     return m[B:2 * B + 1], m[2 * B + 1:]
 
 
-@pytest.mark.parametrize("causal", [True, False], ids=["self", "cross"])
-def test_attention_backward_on_slots_matches_rows(causal):
-    """fira_attn_bwd_rows on the slot layout == fira_attn_bwd on the row layout with zero d_ctx on the dead rows"""
+@pytest.mark.parametrize("dtype", [0, 1], ids=["fp32", "bf16"])
+def test_embedding_backward_through_the_map_against_float64(dtype):
+    """fira_embed_rows_bwd_rows: slot r adds its gradient row to the embedding row of token ids[rows_map[r]], against a
+    float64 index_add over the live slots.  Pad slots (-1), one token id in many slots (atomic adds onto one row), and a
+    slot whose gradient row is exactly zero (skipped: the only slot of its token, whose row must stay exactly zero).  The
+    adds happen in fp32 in any order: |g - r| <= 2^-20 sum |terms| per element"""
     _need_cuda()
     from fira_icse_b200 import _lib
-    rng = np.random.default_rng(3)
-    B, S = 12, 70
-    lab = _labels(B, rng)
-    lab[3, :21] = 9                                 # live rows across two m16 tiles
+    B, Vt = 24, 96
+    lab = _labels(B, np.random.default_rng(13))
     n = int(_target_rows_np(lab, B * T)[0].sum())
     R = -(-n // 128) * 128
-    toff, trows = _map(lab, R)
-    g = torch.Generator().manual_seed(5)
-    bf = dict(dtype=torch.bfloat16, device=DEV)
-
-    def rnd(*shape):
-        return (torch.randn(*shape, generator=g)).to(**bf)
-    tar_mask = torch.ones((B, T), dtype=torch.uint8, device=DEV)
-    tar_mask[5, 2] = 0
-    q = rnd(B * T, D)
-    Lk = T if causal else S
-    k, v = (rnd(B * T, D), rnd(B * T, D)) if causal else (rnd(B * S, D), rnd(B * S, D))
-    km = tar_mask if causal else (torch.rand((B, S), generator=g) < 0.7).to(torch.uint8).to(DEV)
-    ctx = torch.empty((B * T, D), **bf)
-    st = torch.empty((B, H, T, 2), dtype=torch.float32, device=DEV)
-    _lib.call("fira_attn_fwd", q.data_ptr(), D, k.data_ptr(), D, v.data_ptr(), D, km.data_ptr(), int(causal),
-              ctx.data_ptr(), D, st.data_ptr(), B, H, T, Lk, 32, 1, _st())
-    live = torch.zeros(B * T, dtype=torch.bool, device=DEV)
-    tr = trows[trows >= 0].long()
-    live[tr] = True
-    dctx = rnd(B * T, D) * live[:, None]
-    outs = [torch.zeros((B * T if i == 0 or causal else B * S, D), **bf) for i in range(3)]
-    _lib.call("fira_attn_bwd", q.data_ptr(), D, k.data_ptr(), D, v.data_ptr(), D, km.data_ptr(), int(causal),
-              ctx.data_ptr(), dctx.data_ptr(), D, st.data_ptr(), outs[0].data_ptr(), D, outs[1].data_ptr(), D,
-              outs[2].data_ptr(), D, B, H, T, Lk, 32, 1, _st())
-    idx = trows.clamp(min=0).long()
-    pad = (trows < 0)[:, None]
-
-    def slots(x):
-        return x[idx].masked_fill(pad, 0).contiguous()
-    q_s, ctx_s, dctx_s = slots(q), slots(ctx), slots(dctx)
-    dq_s = torch.full((R, D), float("nan"), **bf)                # pad slots must come back zero
-    if causal:
-        k_s, v_s = slots(k), slots(v)
-        dk_s, dv_s = torch.full((R, D), float("nan"), **bf), torch.full((R, D), float("nan"), **bf)
-        _lib.call("fira_attn_bwd_rows", q_s.data_ptr(), D, k_s.data_ptr(), D, v_s.data_ptr(), D, None, km.data_ptr(), T,
-                  1, toff.data_ptr(), R, ctx_s.data_ptr(), dctx_s.data_ptr(), D, st.data_ptr(), dq_s.data_ptr(), D,
-                  dk_s.data_ptr(), D, dv_s.data_ptr(), D, B, H, T, 32, 1, _st())
-        want = [slots(o) for o in outs]
-        got = [dq_s, dk_s, dv_s]
-    else:
-        dk, dv = torch.zeros((B * S, D), **bf), torch.zeros((B * S, D), **bf)
-        ranges = torch.tensor([[b * S, S, 0, 0] for b in range(B)], dtype=torch.int32, device=DEV)
-        _lib.call("fira_attn_bwd_rows", q_s.data_ptr(), D, k.data_ptr(), D, v.data_ptr(), D, ranges.data_ptr(),
-                  km.data_ptr(), S, 0, toff.data_ptr(), R, ctx_s.data_ptr(), dctx_s.data_ptr(), D, st.data_ptr(),
-                  dq_s.data_ptr(), D, dk.data_ptr(), D, dv.data_ptr(), D, B, H, T, 32, 1, _st())
-        want = [slots(outs[0]), outs[1], outs[2]]
-        got = [dq_s, dk, dv]
+    assert R > n, "the map needs pad slots"
+    _, trows = _map(lab, R)
+    g = torch.Generator().manual_seed(17)
+    ids = torch.randint(1, Vt - 1, (B * T,), generator=g, dtype=torch.int32)       # Vt - 1: only the zero slot
+    ids[::3] = 7                                              # one token in a third of the rows
+    tr = trows.cpu().long()
+    live = tr[tr >= 0]
+    zero_slot = int(torch.nonzero(tr >= 0)[len(live) // 2])
+    ids[tr[zero_slot]] = Vt - 1                               # the zero-gradient slot's token appears nowhere else
+    d_out = torch.randn(R, D, generator=g)
+    d_out[zero_slot] = 0.0
+    d_out = d_out.to(torch.bfloat16 if dtype else torch.float32)
+    d_emb = torch.zeros(Vt, D, device=DEV)
+    ids_d, d_out_d = ids.to(DEV), d_out.to(DEV)
+    _lib.call("fira_embed_rows_bwd_rows", ids_d.data_ptr(), trows.data_ptr(), d_out_d.data_ptr(), d_emb.data_ptr(), R,
+              D, dtype, _st())
     torch.cuda.synchronize()
-    for what, a, b in zip(("dq", "dk", "dv"), got, want):
-        assert torch.isfinite(a.float()).all(), what
-        close(f"attention {'self' if causal else 'cross'} {what}", a.float(), b.float(), 2 ** -8, rows=True)
+    slots = torch.nonzero(tr >= 0).view(-1)
+    terms = d_out.double()[slots]
+    tok = ids[tr[slots]].long()
+    ref = torch.zeros(Vt, D, dtype=torch.float64).index_add_(0, tok, terms)
+    mag = torch.zeros(Vt, D, dtype=torch.float64).index_add_(0, tok, terms.abs())
+    got = d_emb.cpu().double()
+    err = (got - ref).abs()
+    bound = 2.0 ** -20 * mag
+    assert bool((err <= bound).all()), f"{int((err > bound).sum())} elements off, worst {(err - bound).max():.3e}"
+    assert int((tok == 7).sum()) > 64, "one row takes many atomic adds"
+    assert bool((got[Vt - 1] == 0).all()), "the zero-gradient slot's row"
+    untouched = torch.ones(Vt, dtype=torch.bool)
+    untouched[tok] = False
+    assert bool((got[untouched] == 0).all()), "a row no live slot names was written"
 
 
 @pytest.mark.parametrize("p", [0.0, 0.1])
