@@ -195,6 +195,66 @@ __device__ __forceinline__ ArgMax am_better(ArgMax a, ArgMax b) {   // larger va
   return (b.v > a.v || (b.v == a.v && b.i < a.i)) ? b : a;
 }
 
+// The mixture of one row, defined once: every kernel that forms P_j or log clamp(P_j) goes through these, so the
+// log-probability a decoding step emits for label j is bit for bit -nll of fira_pointer_mix_nll_fwd for that label.
+// Row statistics: vocab max / sum-exp (online, 8 logits per 16-byte (bf16) / 32-byte (fp32) load, the running (max, sum)
+// rescaled once per group), copy max / sum-exp with the -1e9 fill (Model.py:61), gates.  Block-wide: every thread of
+// the 256 calls it.  vocab == false skips the vocabulary pass without reading lrow and records vmax = 0, vsum = 1.
+struct MixRow {
+  float vmax, vsum, cmax, csum, g0, g1;
+  __device__ __forceinline__ float pv(float x) const { return g0 * (expf(x - vmax) / vsum); }   // P of logit x
+  __device__ __forceinline__ float pc(float c) const { return g1 * (expf(c - cmax) / csum); }   // P of copy score c
+};
+template <typename T>
+__device__ __forceinline__ MixRow mix_row_stats(const T* __restrict__ lrow, const float* __restrict__ srow,
+                                                const unsigned char* __restrict__ mrow, const float* __restrict__ gl,
+                                                int V, int S, MaxSum* sh_ms, float* bc, bool vocab = true) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  MaxSum v{-INFINITY, 0.f};
+  if (vocab) {
+    const int V8 = V >> 3;
+    for (int g = threadIdx.x; g < V8; g += blockDim.x) {
+      float x[8];
+      Act<T>::load8(lrow + (long)g * 8, x);
+      float m8 = x[0];
+#pragma unroll
+      for (int i = 1; i < 8; ++i) m8 = fmaxf(m8, x[i]);
+      if (m8 > v.m) { v.s *= expf(v.m - m8); v.m = m8; }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) v.s += expf(x[i] - v.m);
+    }
+    for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) { MaxSum u{Act<T>::ld(lrow + j), 1.f}; v = ms_merge(v, u); }
+  } else if (threadIdx.x == 0) v = MaxSum{0.f, 1.f};
+  v = ms_warp(v);
+  if (lane == 0) sh_ms[warp] = v;
+  __syncthreads();
+  if (warp == 0) { MaxSum u = lane < 8 ? sh_ms[lane] : MaxSum{-INFINITY, 0.f}; u = ms_warp(u); if (lane == 0) { bc[0] = u.m; bc[1] = u.s; } }
+  __syncthreads();
+  MaxSum c{-INFINITY, 0.f};
+  for (int j = threadIdx.x; j < S; j += blockDim.x) { MaxSum u{mrow[j] ? srow[j] : kMaskFill, 1.f}; c = ms_merge(c, u); }
+  c = ms_warp(c);
+  if (lane == 0) sh_ms[warp] = c;
+  __syncthreads();
+  if (warp == 0) { MaxSum u = lane < 8 ? sh_ms[lane] : MaxSum{-INFINITY, 0.f}; u = ms_warp(u); if (lane == 0) { bc[2] = u.m; bc[3] = u.s; } }
+  __syncthreads();
+  const float vmax = bc[0], vsum = bc[1], cmax = bc[2], csum = bc[3];
+  const float gl0 = gl[0], gl1 = gl[1];
+  const float gm = fmaxf(gl0, gl1);
+  const float e0 = expf(gl0 - gm), e1 = expf(gl1 - gm);
+  const float g0 = e0 / (e0 + e1), g1 = e1 / (e0 + e1);
+  return MixRow{vmax, vsum, cmax, csum, g0, g1};
+}
+// P_j, the probability of label j < V + S
+template <typename T>
+__device__ __forceinline__ float mix_prob(const MixRow& ms, const T* __restrict__ lrow, const float* __restrict__ srow,
+                                          const unsigned char* __restrict__ mrow, int V, int j) {
+  if (j < V) return ms.pv(Act<T>::ld(lrow + j));
+  const int s = j - V;
+  return ms.pc(mrow[s] ? srow[s] : kMaskFill);
+}
+// log(clamp(p, 1e-10, 1)): the label's log-probability, -nll (Model.py:69,81-82)
+__device__ __forceinline__ float mix_lp(float p) { return logf(fminf(fmaxf(p, 1e-10f), 1.f)); }
+
 // Vocabulary-label rows of a training batch (label in (0, V)) in row order: vslot[row] = the row's compact slot or -1,
 // vrows[slot] = its row, -1 in the slots [count, cap).  One CTA; each thread takes a contiguous run of rows.
 constexpr int kRowsThreads = 1024;
@@ -293,75 +353,39 @@ __global__ void __launch_bounds__(256) head_fwd_kernel(const T* __restrict__ log
   const float* srow = sc + row * S;
   const unsigned char* mrow = mem_mask + (long)b * S;
 
-  // pass 1: vocab max / sum-exp (online), copy max / sum-exp with the -1e9 fill (Model.py:61).
-  // Training (no argmax wanted): a row's loss only needs the softmax its label lives in, so rows whose label is
-  // padding or a copy label skip the 24,650-wide pass (and copy-label rows are the only ones that need `sc`).
-  const int lab_row = label[row];
-  const bool need_vocab = argmax_out != nullptr || (lab_row != 0 && lab_row < V && lslot >= 0);
-  MaxSum v{-INFINITY, 0.f};
-  if (need_vocab) {
-    // 8 logits per 16-byte (bf16) / 32-byte (fp32) load; the running (max, sum) is rescaled once per group instead of
-    // once per element (instead of one 2-byte load and two expf per element)
-    const int V8 = V >> 3;
-    for (int g = threadIdx.x; g < V8; g += blockDim.x) {
-      float x[8];
-      Act<T>::load8(lrow + (long)g * 8, x);
-      float m8 = x[0];
-#pragma unroll
-      for (int i = 1; i < 8; ++i) m8 = fmaxf(m8, x[i]);
-      if (m8 > v.m) { v.s *= expf(v.m - m8); v.m = m8; }
-#pragma unroll
-      for (int i = 0; i < 8; ++i) v.s += expf(x[i] - v.m);
-    }
-    for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) { MaxSum u{Act<T>::ld(lrow + j), 1.f}; v = ms_merge(v, u); }
-  } else if (threadIdx.x == 0) v = MaxSum{0.f, 1.f};
-  v = ms_warp(v);
-  if (lane == 0) sh_ms[warp] = v;
-  __syncthreads();
-  if (warp == 0) { MaxSum u = lane < 8 ? sh_ms[lane] : MaxSum{-INFINITY, 0.f}; u = ms_warp(u); if (lane == 0) { bc[0] = u.m; bc[1] = u.s; } }
-  __syncthreads();
-  MaxSum c{-INFINITY, 0.f};
-  for (int j = threadIdx.x; j < S; j += blockDim.x) { MaxSum u{mrow[j] ? srow[j] : kMaskFill, 1.f}; c = ms_merge(c, u); }
-  c = ms_warp(c);
-  if (lane == 0) sh_ms[warp] = c;
-  __syncthreads();
-  if (warp == 0) { MaxSum u = lane < 8 ? sh_ms[lane] : MaxSum{-INFINITY, 0.f}; u = ms_warp(u); if (lane == 0) { bc[2] = u.m; bc[3] = u.s; } }
-  __syncthreads();
-  const float vmax = bc[0], vsum = bc[1], cmax = bc[2], csum = bc[3];
-  const float gl0 = gate_logit[row * 2], gl1 = gate_logit[row * 2 + 1];
-  const float gm = fmaxf(gl0, gl1);
-  const float e0 = expf(gl0 - gm), e1 = expf(gl1 - gm);
-  const float g0 = e0 / (e0 + e1), g1 = e1 / (e0 + e1);
+  // pass 1: the row statistics.  Training (no argmax wanted): a row's loss only needs the softmax its label lives in,
+  // so rows whose label is padding or a copy label skip the 24,650-wide pass (and copy-label rows are the only ones
+  // that need `sc`).
+  const int lab = label[row];
+  const bool need_vocab = argmax_out != nullptr || (lab != 0 && lab < V && lslot >= 0);
+  const MixRow ms = mix_row_stats(lrow, srow, mrow, gate_logit + row * 2, V, S, sh_ms, bc, need_vocab);
 
   if (threadIdx.x == 0) {
-    const int lab = label[row];
     float p = 1.f;
     // a vocabulary-label row left without a slot (a caller's cap below the row count) reports NaN, not a plausible loss
     const bool no_slot = lab != 0 && lab < V && lslot < 0;
     if (lab != 0) {
-      if (lab < V) p = no_slot ? NAN : g0 * (expf(Act<T>::ld(lrow + lab) - vmax) / vsum);
-      else {
-        // a copy label beyond the (possibly loader-trimmed) source is never read out of bounds: it gets p = 0 -> the
-        // clamp floor, no gradient -- what the reference computes for a label on a padded (masked) source position
-        // (Model.py:61,69); beyond V+370 the reference's nll_loss raises instead (Model.py:81)
-        const int s = lab - V;
-        p = s < S ? g1 * (expf((mrow[s] ? srow[s] : kMaskFill) - cmax) / csum) : 0.f;
-      }
+      // a copy label beyond the (possibly loader-trimmed) source is never read out of bounds: it gets p = 0 -> the
+      // clamp floor, no gradient -- what the reference computes for a label on a padded (masked) source position
+      // (Model.py:61,69); beyond V+370 the reference's nll_loss raises instead (Model.py:81)
+      if (no_slot) p = NAN;
+      else p = lab - V < S ? mix_prob(ms, lrow, srow, mrow, V, lab) : 0.f;
     }
     float* st = stats + row * 8;
-    st[0] = vmax; st[1] = vsum; st[2] = cmax; st[3] = csum; st[4] = g0; st[5] = g1; st[6] = p; st[7] = 0.f;
-    // loss = -log(clamp(p, 1e-10, 1)), zeroed where label == 0 (Model.py:69,81-82)
-    nll[row] = no_slot ? NAN : (lab != 0 ? -logf(fminf(fmaxf(p, 1e-10f), 1.f)) : 0.f);
+    st[0] = ms.vmax; st[1] = ms.vsum; st[2] = ms.cmax; st[3] = ms.csum; st[4] = ms.g0; st[5] = ms.g1; st[6] = p;
+    st[7] = 0.f;
+    // loss = -log(clamp(p, 1e-10, 1)), zeroed where label == 0
+    nll[row] = no_slot ? NAN : (lab != 0 ? -mix_lp(p) : 0.f);
   }
   if (argmax_out) {
     // argmax over log(clamp(p)) of the concatenation, first index wins ties (Model.py:86)
     ArgMax best{-INFINITY, 0x7fffffff};
-    const float iv = 1.f / vsum, ic = 1.f / csum;
+    const float iv = 1.f / ms.vsum, ic = 1.f / ms.csum;
     for (int j = threadIdx.x; j < V + S; j += blockDim.x) {
       float p;
-      if (j < V) p = g0 * (expf(Act<T>::ld(lrow + j) - vmax) * iv);
-      else { const int s = j - V; p = g1 * (expf((mrow[s] ? srow[s] : kMaskFill) - cmax) * ic); }
-      ArgMax cand{logf(fminf(fmaxf(p, 1e-10f), 1.f)), j};
+      if (j < V) p = ms.g0 * (expf(Act<T>::ld(lrow + j) - ms.vmax) * iv);
+      else { const int s = j - V; p = ms.g1 * (expf((mrow[s] ? srow[s] : kMaskFill) - ms.cmax) * ic); }
+      ArgMax cand{mix_lp(p), j};
       best = am_better(best, cand);
     }
 #pragma unroll
@@ -492,56 +516,6 @@ __device__ __forceinline__ V block_reduce(V v, V* sh, Op op) {
   return r;
 }
 
-// Row statistics of the mixture exactly as head_fwd_kernel forms them when the vocabulary pass runs (same loops, same
-// reduction order): with them, g0 * (expf(x_j - vmax) / vsum) and g1 * (expf(c_s - cmax) / csum) are bit for bit the
-// probabilities fira_pointer_mix_nll_fwd gives labels j and V + s.  Block-wide: every thread of the 256 calls it.
-struct MixRow { float vmax, vsum, cmax, csum, g0, g1; };
-template <typename T>
-__device__ __forceinline__ MixRow mix_row_stats(const T* __restrict__ lrow, const float* __restrict__ srow,
-                                                const unsigned char* __restrict__ mrow, const float* __restrict__ gl,
-                                                int V, int S, MaxSum* sh_ms, float* bc) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  MaxSum v{-INFINITY, 0.f};
-  const int V8 = V >> 3;
-  for (int g = threadIdx.x; g < V8; g += blockDim.x) {
-    float x[8];
-    Act<T>::load8(lrow + (long)g * 8, x);
-    float m8 = x[0];
-#pragma unroll
-    for (int i = 1; i < 8; ++i) m8 = fmaxf(m8, x[i]);
-    if (m8 > v.m) { v.s *= expf(v.m - m8); v.m = m8; }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v.s += expf(x[i] - v.m);
-  }
-  for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) { MaxSum u{Act<T>::ld(lrow + j), 1.f}; v = ms_merge(v, u); }
-  v = ms_warp(v);
-  if (lane == 0) sh_ms[warp] = v;
-  __syncthreads();
-  if (warp == 0) { MaxSum u = lane < 8 ? sh_ms[lane] : MaxSum{-INFINITY, 0.f}; u = ms_warp(u); if (lane == 0) { bc[0] = u.m; bc[1] = u.s; } }
-  __syncthreads();
-  MaxSum c{-INFINITY, 0.f};
-  for (int j = threadIdx.x; j < S; j += blockDim.x) { MaxSum u{mrow[j] ? srow[j] : kMaskFill, 1.f}; c = ms_merge(c, u); }
-  c = ms_warp(c);
-  if (lane == 0) sh_ms[warp] = c;
-  __syncthreads();
-  if (warp == 0) { MaxSum u = lane < 8 ? sh_ms[lane] : MaxSum{-INFINITY, 0.f}; u = ms_warp(u); if (lane == 0) { bc[2] = u.m; bc[3] = u.s; } }
-  __syncthreads();
-  const float vmax = bc[0], vsum = bc[1], cmax = bc[2], csum = bc[3];
-  const float gl0 = gl[0], gl1 = gl[1];
-  const float gm = fmaxf(gl0, gl1);
-  const float e0 = expf(gl0 - gm), e1 = expf(gl1 - gm);
-  const float g0 = e0 / (e0 + e1), g1 = e1 / (e0 + e1);
-  return MixRow{vmax, vsum, cmax, csum, g0, g1};
-}
-// P_j as head_fwd_kernel forms the probability of label j (a forced label of a prefix may be any j < V + S)
-template <typename T>
-__device__ __forceinline__ float mix_prob(const MixRow& ms, const T* __restrict__ lrow, const float* __restrict__ srow,
-                                          const unsigned char* __restrict__ mrow, int V, int j) {
-  if (j < V) return ms.g0 * (expf(Act<T>::ld(lrow + j) - ms.vmax) / ms.vsum);
-  const int s = j - V;
-  return ms.g1 * (expf((mrow[s] ? srow[s] : kMaskFill) - ms.cmax) / ms.csum);
-}
-
 // n-gram repeat blocking and minimum length (the _rules entry points).  The words of a live row at position `pos` are
 // its history hist[1..pos] (hist[0] is <start>; a copy's word is already copy_src there).  Label j with word w is banned
 // at column pos + 1 when appending w repeats an n-gram of the history (n = no_repeat >= 1) or when w is eos_id and the
@@ -609,19 +583,10 @@ __global__ void __launch_bounds__(kSampleThreads) pointer_mix_sample_kernel(
   const float* srow = sc + row * S;
   const unsigned char* mrow = mem_mask + (long)b * S;
 
-  // row statistics exactly as head_fwd_kernel forms them (same loop, same reduction order), so the emitted
-  // log-probability is the one fira_pointer_mix_nll_fwd gives the same label
   const MixRow ms = mix_row_stats(lrow, srow, mrow, gate_logit + row * 2, V, S, sh_ms, bc);
-  const float vmax = ms.vmax, vsum = ms.vsum, cmax = ms.cmax, csum = ms.csum, g0 = ms.g0, g1 = ms.g1;
-  // P_j as head_fwd_kernel forms the probability of label j
-  auto prob = [&](int j) {
-    if (j < V) return g0 * (expf(Act<T>::ld(lrow + j) - vmax) / vsum);
-    const int s = j - V;
-    return g1 * (expf((mrow[s] ? srow[s] : kMaskFill) - cmax) / csum);
-  };
   // thread 0: label j becomes the row's token at column pos + 1, with the loop bookkeeping
   auto emit = [&](int j) {
-    const float lp = logf(fminf(fmaxf(prob(j), 1e-10f), 1.f));        // = -nll of fira_pointer_mix_nll_fwd for label j
+    const float lp = mix_lp(mix_prob(ms, lrow, srow, mrow, V, j));
     const int tok = j < V ? j : copy_src[(long)b * S + (j - V)];
     next_tok[row] = tok; seq[o] = tok; raw[o] = j; tok_lp[o] = lp; tok_mask[o] = tok != pad_id;
     length[row] += 1;
@@ -637,7 +602,7 @@ __global__ void __launch_bounds__(kSampleThreads) pointer_mix_sample_kernel(
   ban_load(seq + row * ld_out, pos, nb, s_hist);
   const int C = V + S;
   for (int j = threadIdx.x; j < C; j += blockDim.x) {
-    const float p = prob(j);
+    const float p = mix_prob(ms, lrow, srow, mrow, V, j);
     s_sc[j] = ((j < V || mrow[j - V]) && p > 0.f) ? logf(fminf(p, 1.f)) / temp : __int_as_float(0x7fffffff);
   }
   __syncthreads();
@@ -759,6 +724,36 @@ __device__ __forceinline__ uint64_t topk_insert(uint64_t (&top)[kMaxBeam], uint6
     if (i < K) { const uint64_t hi = key_max(top[i], x); x = key_min(top[i], x); top[i] = hi; last = key_min(last, hi); }
   return last;
 }
+// offer(P_j, j) for every vocabulary entry and unmasked copy position j of the row, this thread's strided share:
+// 8 logits per vector load, the scalar tail, then the copy positions
+template <typename T, typename Offer>
+__device__ __forceinline__ void mix_scan(const MixRow& ms, const T* __restrict__ lrow, const float* __restrict__ srow,
+                                         const unsigned char* __restrict__ mrow, int V, int S, Offer&& offer) {
+  const int V8 = V >> 3;
+  for (int g = threadIdx.x; g < V8; g += blockDim.x) {
+    float x[8];
+    Act<T>::load8(lrow + (long)g * 8, x);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) offer(ms.pv(x[i]), g * 8 + i);
+  }
+  for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) offer(ms.pv(Act<T>::ld(lrow + j)), j);
+  for (int s = threadIdx.x; s < S; s += blockDim.x)
+    if (mrow[s]) offer(ms.pc(srow[s]), V + s);
+}
+// block top K of the threads' descending lists: K fixed-order maxima over the list heads; keys are distinct, so exactly
+// one thread owns each maximum and pops it.  Every thread calls emit(k, m) with the k-th best key m (0 = none left).
+template <typename Emit>
+__device__ __forceinline__ void topk_pop(uint64_t (&top)[kMaxBeam], int K, uint64_t* shk, Emit&& emit) {
+  for (int k = 0; k < K; ++k) {
+    const uint64_t m = block_reduce(top[0], shk, key_max);
+    if (m != 0 && top[0] == m) {
+#pragma unroll
+      for (int i = 0; i + 1 < kMaxBeam; ++i) top[i] = top[i + 1];
+      top[kMaxBeam - 1] = 0;
+    }
+    emit(k, m);
+  }
+}
 
 // Lexically constrained n-best (LEX = true, fira_pointer_mix_beam_step_lexical; dynamic beam allocation, Post & Vilar,
 // 2018).  Commit b has up to kPhrases phrases of up to kPhraseLen words, constraints[b][p][m] (0 = padding, no gaps),
@@ -858,7 +853,7 @@ __global__ void __launch_bounds__(kBeamThreads, 1) beam_row_kernel(
   if (prefix && pos < prefix_len[b]) {                // inside the commit's prefix: its label is the row's one winner
     if (threadIdx.x == 0) {
       const int j = prefix[(long)b * ld_prefix + pos];
-      row_top[row * W] = with_bank(rank_key(logf(fminf(fmaxf(mix_prob(ms, lrow, srow, mrow, V, j), 1e-10f), 1.f)), j));
+      row_top[row * W] = with_bank(rank_key(mix_lp(mix_prob(ms, lrow, srow, mrow, V, j)), j));
       for (int k = 1; k < W; ++k) row_top[row * W + k] = 0;
     }
     return;
@@ -882,33 +877,13 @@ __global__ void __launch_bounds__(kBeamThreads, 1) beam_row_kernel(
 #pragma unroll
   for (int i = 0; i < kMaxBeam; ++i) top[i] = 0;
   uint64_t thr = 0;                                   // top[K - 1]: the key a candidate has to beat
-  auto offer = [&](float p, int j) {
-    const uint64_t key = rank_key(logf(fminf(fmaxf(p, 1e-10f), 1.f)), j);   // lp = -nll of fira_pointer_mix_nll_fwd
+  mix_scan(ms, lrow, srow, mrow, V, S, [&](float p, int j) {
+    const uint64_t key = rank_key(mix_lp(p), j);
     if (key <= thr) return;
     if (nbx && is_banned(s_ban, nbx, j < V ? j : crow[j - V])) return;     // only entries that would enter the top K
     thr = topk_insert(top, key, K);
-  };
-  const int V8 = V >> 3;
-  for (int g = threadIdx.x; g < V8; g += blockDim.x) {
-    float x[8];
-    Act<T>::load8(lrow + (long)g * 8, x);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) offer(ms.g0 * (expf(x[i] - ms.vmax) / ms.vsum), g * 8 + i);
-  }
-  for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) offer(ms.g0 * (expf(Act<T>::ld(lrow + j) - ms.vmax) / ms.vsum), j);
-  for (int s = threadIdx.x; s < S; s += blockDim.x)
-    if (mrow[s]) offer(ms.g1 * (expf(srow[s] - ms.cmax) / ms.csum), V + s);
-
-  // block top K: K fixed-order maxima over the list heads; keys are distinct, so exactly one thread owns each maximum
-  for (int k = 0; k < K; ++k) {
-    const uint64_t m = block_reduce(top[0], shk, key_max);
-    if (m != 0 && top[0] == m) {
-#pragma unroll
-      for (int i = 0; i + 1 < kMaxBeam; ++i) top[i] = top[i + 1];
-      top[kMaxBeam - 1] = 0;
-    }
-    if (threadIdx.x == 0) row_top[row * W + k] = with_bank(m);
-  }
+  });
+  topk_pop(top, K, shk, [&](int k, uint64_t m) { if (threadIdx.x == 0) row_top[row * W + k] = with_bank(m); });
   if constexpr (LEX) {                                // (b): one block-wide best label per unmet phrase
     int nx = K;                                       // thread 0: the next free entry
     for (int p = 0; tc && p < kPhrases; ++p) {        // shared state only: uniform across the block
@@ -917,10 +892,9 @@ __global__ void __launch_bounds__(kBeamThreads, 1) beam_row_kernel(
       bool skip = is_banned(s_ban, nbx, w);
       for (int q = 0; q < p; ++q) skip |= ph.prog[q] < ph.len[q] && ph.con[q * kPhraseLen + ph.prog[q]] == w;
       if (skip) continue;
-      uint64_t best = threadIdx.x == 0 ? rank_key(logf(fminf(fmaxf(mix_prob(ms, lrow, srow, mrow, V, w), 1e-10f), 1.f)), w) : 0;
+      uint64_t best = threadIdx.x == 0 ? rank_key(mix_lp(mix_prob(ms, lrow, srow, mrow, V, w)), w) : 0;
       for (int s = threadIdx.x; s < S; s += blockDim.x)
-        if (mrow[s] && crow[s] == w)
-          best = key_max(best, rank_key(logf(fminf(fmaxf(ms.g1 * (expf(srow[s] - ms.cmax) / ms.csum), 1e-10f), 1.f)), V + s));
+        if (mrow[s] && crow[s] == w) best = key_max(best, rank_key(mix_lp(ms.pc(srow[s])), V + s));
       best = block_reduce(best, shk, key_max);
       if (threadIdx.x == 0) {
         bool in_a = false;                            // (a) as written above by this thread, without the banks
@@ -932,31 +906,35 @@ __global__ void __launch_bounds__(kBeamThreads, 1) beam_row_kernel(
   }
 }
 
-// Both select stages: new slot k continues slot s_from[k] (j = s_j[k], C: carried unchanged) -> the written half of the
-// slot state, parent, next_tok and the histories (a grown slot gets its new token at column pos + 1)
+// Every select stage: new slot k0 + k (k < n) continues slot s_from[k] (j = s_j[k], C: carried unchanged) -> the written
+// half of the slot state, parent, next_tok, chosen (may be NULL: the token it grew with, -1 when carried) and the
+// histories (a grown slot gets its new token at column pos + 1)
 __device__ __forceinline__ void beam_write_slots(const int* s_from, const int* s_j, const int* s_tok, const float* s_lp,
                                                  const float* s_L, const float* s_score, int eos_id, int pad_id,
                                                  int* __restrict__ seq, int* __restrict__ raw, float* __restrict__ tok_lp,
                                                  int* __restrict__ length, float* __restrict__ lp_sum,
                                                  float* __restrict__ score, unsigned char* __restrict__ status,
-                                                 long* __restrict__ parent, int* __restrict__ next_tok, int Tn, int pos,
-                                                 long in, long out, long base, int K, int C) {
-  if (threadIdx.x < K) {
+                                                 long* __restrict__ parent, int* __restrict__ next_tok,
+                                                 int* __restrict__ chosen, int Tn, int pos, long in, long out, long base,
+                                                 int k0, int n, int C) {
+  if (threadIdx.x < n) {
     const int k = threadIdx.x;
-    const long pr = in + base + s_from[k], nr = out + base + k;
-    parent[base + k] = base + s_from[k];
-    if (s_j[k] == C) {                                // a finished slot carried unchanged
+    const long pr = in + base + s_from[k], slot = base + k0 + k, nr = out + slot;
+    parent[slot] = base + s_from[k];
+    if (s_j[k] == C) {                                // a finished (or inactive) slot carried unchanged
       length[nr] = length[pr]; lp_sum[nr] = lp_sum[pr]; score[nr] = score[pr]; status[nr] = status[pr];
-      next_tok[base + k] = pad_id;
+      next_tok[slot] = pad_id;
+      if (chosen) chosen[slot] = -1;
     } else {
       length[nr] = length[pr] + 1; lp_sum[nr] = s_L[k]; score[nr] = s_score[k];
       status[nr] = s_tok[k] == eos_id ? 1 : 0;
-      next_tok[base + k] = s_tok[k];
+      next_tok[slot] = s_tok[k];
+      if (chosen) chosen[slot] = s_tok[k];
     }
   }
-  for (int e = threadIdx.x; e < K * Tn; e += blockDim.x) {
+  for (int e = threadIdx.x; e < n * Tn; e += blockDim.x) {
     const int k = e / Tn, c = e % Tn;
-    const long src = (in + base + s_from[k]) * Tn + c, dst = (out + base + k) * Tn + c;
+    const long src = (in + base + s_from[k]) * Tn + c, dst = (out + base + k0 + k) * Tn + c;
     const bool grow = s_j[k] != C && c == pos + 1;
     seq[dst] = grow ? s_tok[k] : seq[src];
     raw[dst] = grow ? s_j[k] : raw[src];
@@ -964,83 +942,29 @@ __device__ __forceinline__ void beam_write_slots(const int* s_from, const int* s
   }
 }
 
-__global__ void __launch_bounds__(kBeamThreads) beam_select_kernel(
-    const uint64_t* __restrict__ row_top, const int* __restrict__ copy_src, float alpha, int eos_id, int pad_id,
-    int* __restrict__ seq, int* __restrict__ raw, float* __restrict__ tok_lp, int* __restrict__ length,
-    float* __restrict__ lp_sum, float* __restrict__ score, unsigned char* __restrict__ status,
-    long* __restrict__ parent, int* __restrict__ next_tok, int Tn, int pos, int B, int K, int V, int S) {
-  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
-  __shared__ uint64_t sh_key[kBeamThreads];
-  __shared__ int s_from[kMaxBeam], s_j[kMaxBeam], s_tok[kMaxBeam];
-  __shared__ float s_lp[kMaxBeam], s_L[kMaxBeam], s_score[kMaxBeam];
-  const int b = blockIdx.x, C = V + S;
-  const long R = (long)B * K;
-  const long in = (pos & 1) ? R : 0, out = (pos & 1) ? 0 : R;     // row offsets of the read and the written half
-  const long base = (long)b * K;
-  if (threadIdx.x < K) { s_from[threadIdx.x] = threadIdx.x; s_j[threadIdx.x] = C; }   // unfilled slot: keeps itself
-
-  // candidate threadIdx.x = i * K + q: the q-th row winner of live slot i, or (q = 0) finished slot i itself
-  uint64_t mine = 0;
-  int i = 0, j = C;
-  float lp = 0.f, L = 0.f, sco = 0.f;
-  if (threadIdx.x < K * K) {
-    i = threadIdx.x / K;
-    const int q = threadIdx.x % K;
-    const long pr = in + base + i;
-    if (status[pr] == 0) {
-      const uint64_t c = row_top[(base + i) * K + q];
-      if (c != 0) {
-        lp = key_lp(c);
-        j = key_index(c);
-        L = lp_sum[pr] + lp;
-        const int n = length[pr];                     // tokens generated with this one: (length - 1) + 1
-        sco = L / powf((5.f + (float)n) / 6.f, alpha) + 0.f;           // + 0: -0 and +0 rank as one value
-        mine = 1;
-      }
-    } else if (status[pr] == 1 && q == 0) {
-      L = lp_sum[pr];
-      sco = score[pr] + 0.f;
-      mine = 1;
-    }
-    if (mine) mine = ((uint64_t)order_bits(sco) << 32) | (0xFFFFFFFFu - (uint32_t)(i * (C + 1) + j));
-  }
-  sh_key[threadIdx.x] = mine;
-  __syncthreads();
-  if (mine) {
-    int rank = 0;
-    for (int u = 0; u < K * K; ++u) rank += sh_key[u] > mine ? 1 : 0;
-    if (rank < K) {
-      s_from[rank] = i; s_j[rank] = j; s_lp[rank] = lp; s_L[rank] = L; s_score[rank] = sco;
-      s_tok[rank] = j < V ? j : (j < C ? copy_src[(long)b * S + (j - V)] : pad_id);
-    }
-  }
-  __syncthreads();
-  beam_write_slots(s_from, s_j, s_tok, s_lp, s_L, s_score, eos_id, pad_id, seq, raw, tok_lp, length, lp_sum, score,
-                   status, parent, next_tok, Tn, pos, in, out, base, K, C);
-}
-
-// Lexical select stage: one CTA per commit, candidate threadIdx.x = i * W + q (W = K + kPhrases): the q-th row entry of
-// live slot i (its bank in key bits kBankShift..), or (q = 0) finished slot i itself; L, n and score as in the plain
-// select stage.  Tc = 0: the plain rule (one bank, every candidate by (score descending, i * (C + 1) + j ascending)).
+// Select stage, plain and lexical: one CTA per commit, candidate threadIdx.x = i * W + q (W = K plain, K + kPhrases
+// lexical: the row stage's entries per row): the q-th row entry of live slot i (lexical: its bank in key bits
+// kBankShift..), or (q = 0) finished slot i itself; L = L_i + lp, n = n_i + 1, score = L / powf((5 + n) / 6, alpha).
+// Tc = 0 (always without constraints): one bank, the K best by (score descending, i * (C + 1) + j ascending).
 // Tc > 0: the carried finished slots first, best score first; then the live candidates striped over the banks: rank r
 // within the candidate's bank by (score, index) as above, then the order (r ascending, bank descending), which is
-// total since two candidates of one bank never share r.  Both orders count the larger keys, like the plain stage.
-constexpr int kLexSelectThreads = kMaxBeam * (kMaxBeam + kPhrases);     // 320 candidates at K = 16
-__global__ void __launch_bounds__(kLexSelectThreads) beam_select_lexical_kernel(
-    const uint64_t* __restrict__ row_top, const int* __restrict__ constraints, const int* __restrict__ copy_src,
+// total since two candidates of one bank never share r.  Every order counts the larger keys.
+constexpr int kSelectThreads = kMaxBeam * (kMaxBeam + kPhrases);     // 320 candidates at K = 16
+__global__ void __launch_bounds__(kSelectThreads) beam_select_kernel(
+    const uint64_t* __restrict__ row_top, int W, const int* __restrict__ constraints, const int* __restrict__ copy_src,
     float alpha, int eos_id, int pad_id, int* __restrict__ seq, int* __restrict__ raw, float* __restrict__ tok_lp,
     int* __restrict__ length, float* __restrict__ lp_sum, float* __restrict__ score, unsigned char* __restrict__ status,
     long* __restrict__ parent, int* __restrict__ next_tok, int Tn, int pos, int B, int K, int V, int S) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
-  __shared__ uint64_t sh_key[kLexSelectThreads];
-  __shared__ int sh_cls[kLexSelectThreads], sh_bank[kLexSelectThreads], sh_r[kLexSelectThreads];
+  __shared__ uint64_t sh_key[kSelectThreads];
+  __shared__ int sh_cls[kSelectThreads], sh_bank[kSelectThreads], sh_r[kSelectThreads];
   __shared__ int s_from[kMaxBeam], s_j[kMaxBeam], s_tok[kMaxBeam];
   __shared__ float s_lp[kMaxBeam], s_L[kMaxBeam], s_score[kMaxBeam];
-  const int b = blockIdx.x, C = V + S, W = K + kPhrases, n_cand = K * W;
+  const int b = blockIdx.x, C = V + S, n_cand = K * W;
   const long R = (long)B * K;
   const long in = (pos & 1) ? R : 0, out = (pos & 1) ? 0 : R;     // row offsets of the read and the written half
   const long base = (long)b * K;
-  const int tc = constraint_words(constraints + (long)b * kMaxConstraintWords);
+  const int tc = constraints ? constraint_words(constraints + (long)b * kMaxConstraintWords) : 0;
   if (threadIdx.x < K) { s_from[threadIdx.x] = threadIdx.x; s_j[threadIdx.x] = C; }   // unfilled slot: keeps itself
 
   uint64_t mine = 0;
@@ -1090,7 +1014,7 @@ __global__ void __launch_bounds__(kLexSelectThreads) beam_select_lexical_kernel(
   }
   __syncthreads();
   beam_write_slots(s_from, s_j, s_tok, s_lp, s_L, s_score, eos_id, pad_id, seq, raw, tok_lp, length, lp_sum, score,
-                   status, parent, next_tok, Tn, pos, in, out, base, K, C);
+                   status, parent, next_tok, nullptr, Tn, pos, in, out, base, 0, K, C);
 }
 
 // ------------------------------------------------------------------ one diverse n-best beam step (beam groups)
@@ -1144,11 +1068,10 @@ __global__ void __launch_bounds__(kBeamThreads, 1) diverse_row_kernel(
   const int* crow = copy_src + (long)b * S;
   const MixRow ms = mix_row_stats(lrow, srow, mrow, gate_logit + row * 2, V, S, sh_ms, bc);   // syncs s_prev, s_hist
   const float L_i = lp_sum[row], norm = beam_norm(length[row], alpha);
-  auto lp_of = [&](float p) { return logf(fminf(fmaxf(p, 1e-10f), 1.f)); };   // = -nll of fira_pointer_mix_nll_fwd
   if (prefix && pos < prefix_len[b]) {                // inside the commit's prefix: its label is the row's one winner
     if (threadIdx.x == 0) {
       const int j = prefix[(long)b * ld_prefix + pos];
-      const float lp = lp_of(mix_prob(ms, lrow, srow, mrow, V, j));
+      const float lp = mix_lp(mix_prob(ms, lrow, srow, mrow, V, j));
       const int h = n_prev ? count_token(s_prev, n_prev, j < V ? j : crow[j - V]) : 0;
       float score;
       row_top[row * Kg] = rank_key(diverse_value(L_i, lp, norm, diversity, h, &score), j);
@@ -1166,47 +1089,24 @@ __global__ void __launch_bounds__(kBeamThreads, 1) diverse_row_kernel(
 #pragma unroll
   for (int i = 0; i < kMaxBeam; ++i) top[i] = 0;
   uint64_t thr = 0;                                   // top[Kg - 1]: the key a candidate has to beat
-  auto offer = [&](float p, int j) {
+  mix_scan(ms, lrow, srow, mrow, V, S, [&](float p, int j) {
+    const float lp = mix_lp(p);
     float score;
-    const float v0 = diverse_value(L_i, lp_of(p), norm, diversity, 0, &score);
+    const float v0 = diverse_value(L_i, lp, norm, diversity, 0, &score);
     if (rank_key(v0, j) <= thr) return;               // the penalty only lowers the value
     const int w = j < V ? j : crow[j - V];
     if (nb && is_banned(s_ban, nb, w)) return;        // only entries that would enter the top Kg
     const int h = n_prev ? count_token(s_prev, n_prev, w) : 0;
-    const uint64_t key = h ? rank_key(diverse_value(L_i, lp_of(p), norm, diversity, h, &score), j) : rank_key(v0, j);
+    const uint64_t key = h ? rank_key(diverse_value(L_i, lp, norm, diversity, h, &score), j) : rank_key(v0, j);
     if (key > thr) thr = topk_insert(top, key, Kg);
-  };
-  const int V8 = V >> 3;
-  for (int gi = threadIdx.x; gi < V8; gi += blockDim.x) {
-    float x[8];
-    Act<T>::load8(lrow + (long)gi * 8, x);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) offer(ms.g0 * (expf(x[i] - ms.vmax) / ms.vsum), gi * 8 + i);
-  }
-  for (int j = V8 * 8 + threadIdx.x; j < V; j += blockDim.x) offer(ms.g0 * (expf(Act<T>::ld(lrow + j) - ms.vmax) / ms.vsum), j);
-  for (int s = threadIdx.x; s < S; s += blockDim.x)
-    if (mrow[s]) offer(ms.g1 * (expf(srow[s] - ms.cmax) / ms.csum), V + s);
-
-  // block top Kg: fixed-order maxima over the list heads (keys are distinct); the winner's lp is formed again from
-  // its index with the same expression, so it is the lp its value was ranked with
-  for (int k = 0; k < Kg; ++k) {
-    const uint64_t m = block_reduce(top[0], shk, key_max);
-    if (m != 0 && top[0] == m) {
-#pragma unroll
-      for (int i = 0; i + 1 < kMaxBeam; ++i) top[i] = top[i + 1];
-      top[kMaxBeam - 1] = 0;
-    }
+  });
+  // the winner's lp is formed again from its index, so it is the lp its value was ranked with
+  topk_pop(top, Kg, shk, [&](int k, uint64_t m) {
     if (threadIdx.x == 0) {
-      float lp = 0.f;
-      if (m != 0) {
-        const int j = key_index(m);
-        lp = lp_of(j < V ? ms.g0 * (expf(Act<T>::ld(lrow + j) - ms.vmax) / ms.vsum)
-                         : ms.g1 * (expf(srow[j - V] - ms.cmax) / ms.csum));
-      }
       row_top[row * Kg + k] = m;
-      row_lp[row * Kg + k] = lp;
+      row_lp[row * Kg + k] = m != 0 ? mix_lp(mix_prob(ms, lrow, srow, mrow, V, key_index(m))) : 0.f;
     }
-  }
+  });
 }
 
 __global__ void __launch_bounds__(kBeamThreads) diverse_select_kernel(
@@ -1265,31 +1165,8 @@ __global__ void __launch_bounds__(kBeamThreads) diverse_select_kernel(
     if (rank < Kg) { s_from[rank] = i; s_j[rank] = j; s_lp[rank] = lp; s_L[rank] = L; s_score[rank] = sco; s_tok[rank] = tok; }
   }
   __syncthreads();
-  if (threadIdx.x < Kg) {
-    const int k = g0 + threadIdx.x, f = s_from[threadIdx.x];
-    const long pr = in + base + f, nr = out + base + k;
-    parent[base + k] = base + f;
-    if (s_j[threadIdx.x] == C) {                      // a finished (or inactive) slot carried unchanged
-      length[nr] = length[pr]; lp_sum[nr] = lp_sum[pr]; score[nr] = score[pr]; status[nr] = status[pr];
-      next_tok[base + k] = pad_id;
-      chosen[base + k] = -1;
-    } else {
-      const int t = s_tok[threadIdx.x];
-      length[nr] = length[pr] + 1; lp_sum[nr] = s_L[threadIdx.x]; score[nr] = s_score[threadIdx.x];
-      status[nr] = t == eos_id ? 1 : 0;
-      next_tok[base + k] = t;
-      chosen[base + k] = t;
-    }
-  }
-  // histories follow their parents; a grown slot gets its new token at column pos + 1
-  for (int e = threadIdx.x; e < Kg * Tn; e += blockDim.x) {
-    const int k = e / Tn, c = e % Tn;
-    const long src = (in + base + s_from[k]) * Tn + c, dst = (out + base + g0 + k) * Tn + c;
-    const bool grow = s_j[k] != C && c == pos + 1;
-    seq[dst] = grow ? s_tok[k] : seq[src];
-    raw[dst] = grow ? s_j[k] : raw[src];
-    tok_lp[dst] = grow ? s_lp[k] : tok_lp[src];
-  }
+  beam_write_slots(s_from, s_j, s_tok, s_lp, s_L, s_score, eos_id, pad_id, seq, raw, tok_lp, length, lp_sum, score,
+                   status, parent, next_tok, chosen, Tn, pos, in, out, base, g0, Kg, C);
 }
 
 // ------------------------------------------------------------------ ensemble combine
@@ -1510,7 +1387,7 @@ __device__ __forceinline__ KdRow kd_row(const float* st, float alpha, int y) {
   k.vmax = st[0]; k.iv = 1.f / st[1]; k.g0 = st[4]; k.lv = logf(st[4]) - st[0] - logf(st[1]);
   k.cmax = st[2]; k.ic = 1.f / st[3]; k.g1 = st[5]; k.lc = logf(st[5]) - st[2] - logf(st[3]);
   k.tvmax = st[8]; k.tiv = 1.f / st[9]; k.tcmax = st[10]; k.tic = 1.f / st[11]; k.tg0 = st[12]; k.tg1 = st[13];
-  k.p_lab = st[6]; k.lp_lab = logf(fminf(fmaxf(st[6], 1e-10f), 1.f));
+  k.p_lab = st[6]; k.lp_lab = mix_lp(st[6]);
   k.hard = 1.f - alpha; k.alpha = alpha; k.y = y;
   return k;
 }
@@ -1609,15 +1486,10 @@ __global__ void __launch_bounds__(kKdThreads) pointer_mix_kd_fwd_kernel(
     o[3] = bc[4 * threadIdx.x + 3]; o[4] = e0 / (e0 + e1); o[5] = e1 / (e0 + e1);
   }
   __syncthreads();
-  if (threadIdx.x == 0) {                             // P_y exactly as head_fwd_kernel forms it
-    const float vmax = s_st[0], vsum = s_st[1], cmax = s_st[2], csum = s_st[3], g0 = s_st[4], g1 = s_st[5];
-    float p;
-    if (y < V) p = g0 * (expf(Act<T>::ld(lrow + y) - vmax) / vsum);
-    else {
-      const int s = y - V;                            // a copy label beyond S: p = 0, the clamp floor, no gradient
-      p = s < S ? g1 * (expf((mrow[s] ? srow[s] : kMaskFill) - cmax) / csum) : 0.f;
-    }
-    s_st[6] = p; s_st[7] = 0.f;
+  if (threadIdx.x == 0) {                             // P_y; a copy label beyond S: p = 0, the clamp floor, no gradient
+    const MixRow ms{s_st[0], s_st[1], s_st[2], s_st[3], s_st[4], s_st[5]};
+    s_st[6] = y - V < S ? mix_prob(ms, lrow, srow, mrow, V, y) : 0.f;
+    s_st[7] = 0.f;
   }
   __syncthreads();
 
@@ -1902,6 +1774,22 @@ int fira_pointer_mix_nll_bwd(const void* logits, long ld_logits, const float* co
                                        dtype, stream);
 }
 
+// The checks every decoding step makes; `who` is the entry point's name without its _prefix / _rules suffix, `hist` the
+// width of the token histories (its name in the messages: `hist_name`)
+static int step_check(const char* who, const void* logits, long ld_logits, long hist, const char* hist_name, int pos,
+                      const int* prefix, int ld_prefix, const int* prefix_len, int no_repeat, int min_len) {
+  FIRA_CHECK_ARG(!prefix || (prefix_len && ld_prefix > pos), FIRA_ERR_ARG,
+                 "%s_prefix: null prefix_len or ld_prefix %d <= pos %d", who, ld_prefix, pos);
+  FIRA_CHECK_ARG(no_repeat >= 0 && min_len >= 0, FIRA_ERR_ARG,
+                 "%s_rules: no_repeat_ngram %d / min_length %d < 0", who, no_repeat, min_len);
+  FIRA_CHECK_ARG((!no_repeat && !min_len) || hist <= TMAX, FIRA_ERR_SHAPE, "%s_rules: %s %ld > %d", who, hist_name,
+                 hist, TMAX);
+  FIRA_CHECK_ARG(pos >= 0 && hist >= pos + 2, FIRA_ERR_SHAPE, "%s: pos %d, %s %ld", who, pos, hist_name, hist);
+  FIRA_CHECK_ARG(fira_aligned16(logits) && ld_logits % 8 == 0, FIRA_ERR_ALIGN,
+                 "%s: logits must be 16-byte aligned with a leading dimension that is a multiple of 8", who);
+  return FIRA_OK;
+}
+
 static int sample_impl(const void* logits, long ld_logits, const float* copy_scores, const float* gate_logits,
                        const unsigned char* mem_mask, const int* copy_src, const uint64_t* seed, const int* first_index,
                        const float* uniforms, float temperature, int top_k, float top_p, int eos_id, int pad_id,
@@ -1909,22 +1797,16 @@ static int sample_impl(const void* logits, long ld_logits, const float* copy_sco
                        int pos, unsigned char* finished, int* length, float* logprob, int B, int N, int V, int S,
                        const int* prefix, int ld_prefix, const int* prefix_len, int no_repeat, int min_len, int dtype,
                        void* stream) {
-  FIRA_CHECK_ARG(!prefix || (prefix_len && ld_prefix > pos), FIRA_ERR_ARG,
-                 "pointer_mix_sample_prefix: null prefix_len or ld_prefix %d <= pos %d", ld_prefix, pos);
-  FIRA_CHECK_ARG(no_repeat >= 0 && min_len >= 0, FIRA_ERR_ARG,
-                 "pointer_mix_sample_rules: no_repeat_ngram %d / min_length %d < 0", no_repeat, min_len);
-  FIRA_CHECK_ARG((!no_repeat && !min_len) || ld_out <= TMAX, FIRA_ERR_SHAPE,
-                 "pointer_mix_sample_rules: ld_out %ld > %d", ld_out, TMAX);
+  const int rc = step_check("pointer_mix_sample", logits, ld_logits, ld_out, "ld_out", pos, prefix, ld_prefix,
+                            prefix_len, no_repeat, min_len);
+  if (rc != FIRA_OK) return rc;
   FIRA_CHECK_ARG(B >= 0 && N > 0 && V > 0 && S > 0 && V + S <= 0x7FFF, FIRA_ERR_SHAPE,
                  "pointer_mix_sample: shape (B %d, N %d, V %d, S %d; V + S must be <= 32767)", B, N, V, S);
-  FIRA_CHECK_ARG(pos >= 0 && ld_out >= pos + 2, FIRA_ERR_SHAPE, "pointer_mix_sample: pos %d, ld_out %ld", pos, ld_out);
   FIRA_CHECK_ARG(temperature > 0.f && temperature <= 3.4e38f, FIRA_ERR_ARG, "pointer_mix_sample: temperature %g",
                  (double)temperature);
   FIRA_CHECK_ARG(top_k >= 0, FIRA_ERR_ARG, "pointer_mix_sample: top_k %d < 0", top_k);
   FIRA_CHECK_ARG(top_p > 0.f && top_p <= 1.f, FIRA_ERR_ARG, "pointer_mix_sample: top_p %g not in (0, 1]", (double)top_p);
   FIRA_CHECK_ARG(uniforms || (seed && first_index), FIRA_ERR_ARG, "pointer_mix_sample: seed / first_index missing");
-  FIRA_CHECK_ARG(fira_aligned16(logits) && ld_logits % 8 == 0, FIRA_ERR_ALIGN,
-                 "pointer_mix_sample: logits must be 16-byte aligned with a leading dimension that is a multiple of 8");
   if (B == 0) return FIRA_OK;
   const int smem = (int)sizeof(float) * (V + S);
   cudaError_t e = dtype == FIRA_F32
@@ -1983,22 +1865,16 @@ static int beam_step_impl(const void* logits, long ld_logits, const float* copy_
                           float* logprob, float* score, unsigned char* status, long* parent, int* next_tok, int T_len,
                           int pos, int B, int K, int V, int S, const int* prefix, int ld_prefix, const int* prefix_len,
                           int no_repeat, int min_len, int dtype, void* stream, const int* constraints = nullptr) {
-  FIRA_CHECK_ARG(!prefix || (prefix_len && ld_prefix > pos), FIRA_ERR_ARG,
-                 "pointer_mix_beam_step_prefix: null prefix_len or ld_prefix %d <= pos %d", ld_prefix, pos);
+  const int rc = step_check("pointer_mix_beam_step", logits, ld_logits, T_len, "T_len", pos, prefix, ld_prefix,
+                            prefix_len, no_repeat, min_len);
+  if (rc != FIRA_OK) return rc;
   FIRA_CHECK_ARG(!constraints || T_len <= TMAX, FIRA_ERR_SHAPE, "pointer_mix_beam_step_lexical: T_len %d > %d", T_len,
                  TMAX);
-  FIRA_CHECK_ARG(no_repeat >= 0 && min_len >= 0, FIRA_ERR_ARG,
-                 "pointer_mix_beam_step_rules: no_repeat_ngram %d / min_length %d < 0", no_repeat, min_len);
-  FIRA_CHECK_ARG((!no_repeat && !min_len) || T_len <= TMAX, FIRA_ERR_SHAPE,
-                 "pointer_mix_beam_step_rules: T_len %d > %d", T_len, TMAX);
   FIRA_CHECK_ARG(B >= 0 && K >= 1 && K <= kMaxBeam && V >= K && S > 0 && V + S <= 0x7FFF, FIRA_ERR_SHAPE,
                  "pointer_mix_beam_step: shape (B %d, K %d, V %d, S %d; 1 <= K <= 16, K <= V, V + S <= 32767)",
                  B, K, V, S);
-  FIRA_CHECK_ARG(pos >= 0 && pos + 2 <= T_len, FIRA_ERR_SHAPE, "pointer_mix_beam_step: pos %d, T_len %d", pos, T_len);
   FIRA_CHECK_ARG(length_penalty >= 0.f && length_penalty <= 3.4e38f, FIRA_ERR_ARG,
                  "pointer_mix_beam_step: length_penalty %g", (double)length_penalty);
-  FIRA_CHECK_ARG(fira_aligned16(logits) && ld_logits % 8 == 0, FIRA_ERR_ALIGN,
-                 "pointer_mix_beam_step: logits must be 16-byte aligned with a leading dimension that is a multiple of 8");
   if (B == 0) return FIRA_OK;
   const unsigned char* st_in = status + (pos & 1) * (long)B * K;
   const int* seq_in = seq + (pos & 1) * (long)B * K * T_len;
@@ -2007,20 +1883,17 @@ static int beam_step_impl(const void* logits, long ld_logits, const float* copy_
         (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, st_in, seq_in,
         T_len, workspace, prefix, ld_prefix, prefix_len, no_repeat, min_len, eos_id, pos, K, V, S, constraints);)
     FIRA_CHECK_LAUNCH("fira_pointer_mix_beam_step_lexical (rows)");
-    launch_k(beam_select_lexical_kernel, dim3((unsigned)B), dim3(kLexSelectThreads), 0, (cudaStream_t)stream,
-             (const uint64_t*)workspace, constraints, copy_src, length_penalty, eos_id, pad_id, seq, raw, token_logprob,
-             length, logprob, score, status, parent, next_tok, T_len, pos, B, K, V, S);
-    FIRA_CHECK_LAUNCH("fira_pointer_mix_beam_step_lexical (select)");
-    return FIRA_OK;
+  } else {
+    DISPATCH_T(dtype, launch_k(beam_row_kernel<T, false>, dim3((unsigned)(B * K)), dim3(kBeamThreads), 0,
+        (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, st_in, seq_in,
+        T_len, workspace, prefix, ld_prefix, prefix_len, no_repeat, min_len, eos_id, pos, K, V, S, nullptr);)
+    FIRA_CHECK_LAUNCH("fira_pointer_mix_beam_step (rows)");
   }
-  DISPATCH_T(dtype, launch_k(beam_row_kernel<T, false>, dim3((unsigned)(B * K)), dim3(kBeamThreads), 0,
-      (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, copy_src, st_in, seq_in,
-      T_len, workspace, prefix, ld_prefix, prefix_len, no_repeat, min_len, eos_id, pos, K, V, S, nullptr);)
-  FIRA_CHECK_LAUNCH("fira_pointer_mix_beam_step (rows)");
-  launch_k(beam_select_kernel, dim3((unsigned)B), dim3(kBeamThreads), 0, (cudaStream_t)stream, (const uint64_t*)workspace,
-           copy_src, length_penalty, eos_id, pad_id, seq, raw, token_logprob, length, logprob, score, status, parent,
-           next_tok, T_len, pos, B, K, V, S);
-  FIRA_CHECK_LAUNCH("fira_pointer_mix_beam_step (select)");
+  const int W = constraints ? K + kPhrases : K;       // row_top entries per row (beam_row_kernel)
+  launch_k(beam_select_kernel, dim3((unsigned)B), dim3(kSelectThreads), 0, (cudaStream_t)stream,
+           (const uint64_t*)workspace, W, constraints, copy_src, length_penalty, eos_id, pad_id, seq, raw, token_logprob,
+           length, logprob, score, status, parent, next_tok, T_len, pos, B, K, V, S);
+  FIRA_CHECK_LAUNCH(constraints ? "fira_pointer_mix_beam_step_lexical (select)" : "fira_pointer_mix_beam_step (select)");
   return FIRA_OK;
 }
 
@@ -2081,17 +1954,12 @@ static int diverse_beam_step_impl(const void* logits, long ld_logits, const floa
                                   int V, int S, int groups, float diversity, int* chosen, float* lp_workspace,
                                   const int* prefix, int ld_prefix, const int* prefix_len, int no_repeat, int min_len,
                                   int dtype, void* stream) {
-  FIRA_CHECK_ARG(!prefix || (prefix_len && ld_prefix > pos), FIRA_ERR_ARG,
-                 "pointer_mix_diverse_beam_step_prefix: null prefix_len or ld_prefix %d <= pos %d", ld_prefix, pos);
-  FIRA_CHECK_ARG(no_repeat >= 0 && min_len >= 0, FIRA_ERR_ARG,
-                 "pointer_mix_diverse_beam_step_rules: no_repeat_ngram %d / min_length %d < 0", no_repeat, min_len);
-  FIRA_CHECK_ARG((!no_repeat && !min_len) || T_len <= TMAX, FIRA_ERR_SHAPE,
-                 "pointer_mix_diverse_beam_step_rules: T_len %d > %d", T_len, TMAX);
+  const int rc = step_check("pointer_mix_diverse_beam_step", logits, ld_logits, T_len, "T_len", pos, prefix, ld_prefix,
+                            prefix_len, no_repeat, min_len);
+  if (rc != FIRA_OK) return rc;
   FIRA_CHECK_ARG(B >= 0 && K >= 1 && K <= kMaxBeam && V >= K && S > 0 && V + S <= 0x7FFF, FIRA_ERR_SHAPE,
                  "pointer_mix_diverse_beam_step: shape (B %d, K %d, V %d, S %d; 1 <= K <= 16, K <= V, V + S <= 32767)",
                  B, K, V, S);
-  FIRA_CHECK_ARG(pos >= 0 && pos + 2 <= T_len, FIRA_ERR_SHAPE, "pointer_mix_diverse_beam_step: pos %d, T_len %d",
-                 pos, T_len);
   FIRA_CHECK_ARG(groups >= 1 && groups <= K && K % groups == 0, FIRA_ERR_ARG,
                  "pointer_mix_diverse_beam_step: groups %d must divide K %d", groups, K);
   FIRA_CHECK_ARG(length_penalty >= 0.f && length_penalty <= 3.4e38f, FIRA_ERR_ARG,
@@ -2100,9 +1968,6 @@ static int diverse_beam_step_impl(const void* logits, long ld_logits, const floa
                  "pointer_mix_diverse_beam_step: diversity %g", (double)diversity);
   FIRA_CHECK_ARG(workspace && lp_workspace && chosen, FIRA_ERR_ARG,
                  "pointer_mix_diverse_beam_step: null workspace / lp_workspace / chosen");
-  FIRA_CHECK_ARG(fira_aligned16(logits) && ld_logits % 8 == 0, FIRA_ERR_ALIGN,
-                 "pointer_mix_diverse_beam_step: logits must be 16-byte aligned with a leading dimension that is a "
-                 "multiple of 8");
   if (B == 0) return FIRA_OK;
   const int Kg = K / groups;
   const long in = (pos & 1) * (long)B * K;            // the read half of the slot state
