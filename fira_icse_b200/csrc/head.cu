@@ -515,6 +515,20 @@ __device__ __forceinline__ V block_reduce(V v, V* sh, Op op) {
   for (int w = 1; w < kSampleThreads / 32; ++w) r = op(r, sh[w]);
   return r;
 }
+// the candidates among this thread's staged scores s[j0, j1) with rank_key(s_j, j) >= th, counted over the block
+__device__ __forceinline__ unsigned count_key_ge(const float* s, int j0, int j1, uint64_t th, unsigned* shu) {
+  unsigned k = 0;
+  for (int j = j0; j < j1; ++j) { const float v = s[j]; k += (is_cand(v) && rank_key(v, j) >= th) ? 1u : 0u; }
+  return block_reduce(k, shu, [](unsigned a, unsigned x) { return a + x; });
+}
+// for k below the candidate count: the largest cut with count_ge(cut) >= k.  Keys are distinct, so the candidates with
+// rank_key >= cut are exactly the k best.
+template <typename Count>
+__device__ __forceinline__ uint64_t key_cut(unsigned k, Count&& count_ge) {
+  uint64_t lo = 1, hi = kKeyEnd;                      // count_ge(lo) >= k, count_ge(hi) < k
+  while (hi - lo > 1) { const uint64_t mid = lo + (hi - lo) / 2; if (count_ge(mid) >= k) lo = mid; else hi = mid; }
+  return lo;
+}
 
 // n-gram repeat blocking and minimum length (the _rules entry points).  The words of a live row at position `pos` are
 // its history hist[1..pos] (hist[0] is <start>; a copy's word is already copy_src there).  Label j with word w is banned
@@ -627,22 +641,14 @@ __global__ void __launch_bounds__(kSampleThreads) pointer_mix_sample_kernel(
   smax = block_reduce(smax, shf, [](float a, float x) { return fmaxf(a, x); });
   const unsigned n_cand = block_reduce(cnt, shu, add_u);
   auto weight = [&](float s) { return s == smax ? 1.f : expf(s - smax); };
-  auto count_ge = [&](uint64_t th) {
-    unsigned k = 0;
-    for (int j = j0; j < j1; ++j) { const float s = s_sc[j]; k += (is_cand(s) && rank_key(s, j) >= th) ? 1u : 0u; }
-    return block_reduce(k, shu, add_u);
-  };
+  auto count_ge = [&](uint64_t th) { return count_key_ge(s_sc, j0, j1, th, shu); };
   auto weight_ge = [&](uint64_t th) {
     float a = 0.f;
     for (int j = j0; j < j1; ++j) { const float s = s_sc[j]; if (is_cand(s) && rank_key(s, j) >= th) a += weight(s); }
     return block_reduce(a, shf, add_f);
   };
   uint64_t cut = 1;                                   // kept <=> candidate with rank_key >= cut
-  if (top_k > 0 && (unsigned)top_k < n_cand) {
-    uint64_t lo = cut, hi = kKeyEnd;                  // count_ge(lo) >= k, count_ge(hi) < k
-    while (hi - lo > 1) { const uint64_t mid = lo + (hi - lo) / 2; if (count_ge(mid) >= (unsigned)top_k) lo = mid; else hi = mid; }
-    cut = lo;
-  }
+  if (top_k > 0 && (unsigned)top_k < n_cand) cut = key_cut((unsigned)top_k, count_ge);
   if (top_p < 1.f && n_cand > 1) {
     const float target = top_p * weight_ge(cut);
     uint64_t lo = cut, hi = kKeyEnd;                  // the top candidate alone has weight 1 > 0: lo stays at or below it
@@ -1382,13 +1388,19 @@ struct KdRow {
   float p_lab, lp_lab, hard, alpha;  // P_y as head_fwd_kernel forms it, log clamp(P_y), 1 - alpha, alpha
   int y;
 };
-__device__ __forceinline__ KdRow kd_row(const float* st, float alpha, int y) {
+// the student's fields from st[0..6] (both stats layouts start with them); kd_row adds the teacher's
+__device__ __forceinline__ KdRow kd_student(const float* st, float alpha, int y) {
   KdRow k;
   k.vmax = st[0]; k.iv = 1.f / st[1]; k.g0 = st[4]; k.lv = logf(st[4]) - st[0] - logf(st[1]);
   k.cmax = st[2]; k.ic = 1.f / st[3]; k.g1 = st[5]; k.lc = logf(st[5]) - st[2] - logf(st[3]);
-  k.tvmax = st[8]; k.tiv = 1.f / st[9]; k.tcmax = st[10]; k.tic = 1.f / st[11]; k.tg0 = st[12]; k.tg1 = st[13];
+  k.tvmax = k.tiv = k.tg0 = k.tcmax = k.tic = k.tg1 = 0.f;
   k.p_lab = st[6]; k.lp_lab = mix_lp(st[6]);
   k.hard = 1.f - alpha; k.alpha = alpha; k.y = y;
+  return k;
+}
+__device__ __forceinline__ KdRow kd_row(const float* st, float alpha, int y) {
+  KdRow k = kd_student(st, alpha, y);
+  k.tvmax = st[8]; k.tiv = 1.f / st[9]; k.tcmax = st[10]; k.tic = 1.f / st[11]; k.tg0 = st[12]; k.tg1 = st[13];
   return k;
 }
 // a_j of entry j from the student's P_j and the teacher's t_j (forward and backward form it the same way)
@@ -1596,6 +1608,231 @@ __global__ void __launch_bounds__(kKdThreads) pointer_mix_kd_bwd_kernel(
     }
   } else {
     for (int s = threadIdx.x; s < S; s += blockDim.x) dsrow[s] = 0.f;
+  }
+  if (threadIdx.x == 0) {
+    const float A = A_V + A_C;
+    d_gate_logit[row * 2] = y ? up * (k.g0 * A - A_V) : 0.f;
+    d_gate_logit[row * 2 + 1] = y ? up * (k.g1 * A - A_C) : 0.f;
+    row_active[row] = A_C != 0.f ? 1 : 0;
+  }
+}
+
+// ------------------------------------------------------------------ offline distillation: top-k teacher targets
+// fira_pointer_mix_topk keeps, per loss row, the teacher's k candidates (every vocabulary entry and unmasked copy
+// position with P_j > 0 in fp32, P from mix_row_stats / mix_prob) with the largest rank_key(P_j, j): P descending, then
+// j ascending, the sampler's key taken on P itself.  mass = the kept P summed in key order; stored t~_i = P_i / mass.
+// The sparse loss kernels then read the student row as fira_pointer_mix_kd_fwd / _bwd do against the dense vector that
+// holds t~ at the kept labels and 0 elsewhere:
+//   forward   mix_row_stats once, then the <= k + 1 weighted entries (the kept labels and y), one per thread, summed by
+//             block_reduce in entry order
+//   backward  one dense write pass of u (softmax A - a) without the a term, then, after a __syncthreads, the <= k + 1
+//             columns with a != 0 rewritten from the whole expression (one rounding, as the dense kernel's)
+// stats row (kKdSparseStats floats): student vmax vsum cmax csum g0 g1, p_label, 0, A_V, A_C
+constexpr int kKdMaxTopk = 64;
+constexpr int kKdSparseStats = 10;
+
+// P_j (P_y: the forward's p_label) and log P_j of entry j < V + S; log P_j is what kd_term reads for a live P_j
+template <typename T>
+__device__ __forceinline__ float kd_entry(const MixRow& ms, const KdRow& k, const T* __restrict__ lrow,
+                                          const float* __restrict__ srow, const unsigned char* __restrict__ mrow, int V,
+                                          int j, float& lp) {
+  if (j < V) lp = Act<T>::ld(lrow + j) + k.lv;
+  else lp = (mrow[j - V] ? srow[j - V] : kMaskFill) + k.lc;
+  return j == k.y ? k.p_lab : mix_prob(ms, lrow, srow, mrow, V, j);
+}
+// thread i's entry: the kept label i < K with its t~, or y (t = 0) at i == K unless y is a kept label; -1: none.
+// Block-wide (a __syncthreads_or).
+__device__ __forceinline__ int kd_sparse_entry(const int* __restrict__ lab, const float* __restrict__ prob, int K, int y,
+                                               int V, int S, float& t) {
+  const int i = threadIdx.x;
+  int j = i < K ? lab[i] : (i == K ? y : -1);
+  t = i < K ? prob[i] : 0.f;
+  const bool y_kept = __syncthreads_or(i < K && j == y);
+  if (j < 0 || j >= V + S || (i == K && y_kept)) j = -1;
+  return j;
+}
+
+__global__ void __launch_bounds__(kSampleThreads) pointer_mix_topk_kernel(
+    const float* __restrict__ t_logits, long ldt, const float* __restrict__ t_sc, const float* __restrict__ t_gl,
+    const unsigned char* __restrict__ mem_mask, const int* __restrict__ label, int K, int* __restrict__ t_label,
+    float* __restrict__ t_prob, float* __restrict__ mass, int Tn, int V, int S) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  extern __shared__ float s_p[];                      // [V + S] P_j, NaN = not a candidate
+  __shared__ MaxSum sh_ms[8];
+  __shared__ float bc[4];
+  __shared__ unsigned shu[8];
+  __shared__ unsigned s_n;
+  __shared__ uint64_t s_key[kKdMaxTopk], s_sorted[kKdMaxTopk];
+  __shared__ float s_mass;
+  const long row = blockIdx.x;
+  int* lo = t_label + row * K;
+  float* po = t_prob + row * K;
+  if (label[row] == 0) {                              // no loss: nothing is read
+    if ((int)threadIdx.x < K) { lo[threadIdx.x] = -1; po[threadIdx.x] = 0.f; }
+    if (threadIdx.x == 0) mass[row] = 0.f;
+    return;
+  }
+  const int b = (int)(row / Tn);
+  const float* lrow = t_logits + row * ldt;
+  const float* srow = t_sc + row * S;
+  const unsigned char* mrow = mem_mask + (long)b * S;
+  const MixRow ms = mix_row_stats(lrow, srow, mrow, t_gl + row * 2, V, S, sh_ms, bc);
+  const float nan = __int_as_float(0x7fffffff);
+  for (int s = threadIdx.x; s < S; s += blockDim.x)
+    if (!mrow[s]) s_p[V + s] = nan;                   // mix_scan does not offer masked copies
+  mix_scan(ms, lrow, srow, mrow, V, S, [&](float p, int j) { s_p[j] = p > 0.f ? p : nan; });
+  if (threadIdx.x == 0) s_n = 0;
+  __syncthreads();
+
+  const int C = V + S;
+  const int chunk = (C + kSampleThreads - 1) / kSampleThreads;
+  const int j0 = min(C, (int)threadIdx.x * chunk), j1 = min(C, j0 + chunk);
+  unsigned cnt = 0;
+  for (int j = j0; j < j1; ++j) cnt += is_cand(s_p[j]) ? 1u : 0u;
+  const unsigned n_cand = block_reduce(cnt, shu, [](unsigned a, unsigned x) { return a + x; });
+  uint64_t cut = 1;
+  if ((unsigned)K < n_cand) cut = key_cut((unsigned)K, [&](uint64_t th) { return count_key_ge(s_p, j0, j1, th, shu); });
+  // the kept keys (min(K, n_cand) of them) in arrival order, then each placed at its rank: keys are distinct
+  for (int j = j0; j < j1; ++j) {
+    const float p = s_p[j];
+    if (is_cand(p)) { const uint64_t key = rank_key(p, j); if (key >= cut) s_key[atomicAdd(&s_n, 1u)] = key; }
+  }
+  __syncthreads();
+  const int n = (int)s_n;
+  if ((int)threadIdx.x < n) {
+    const uint64_t key = s_key[threadIdx.x];
+    int r = 0;
+    for (int q = 0; q < n; ++q) r += s_key[q] > key;
+    s_sorted[r] = key;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float m = 0.f;
+    for (int i = 0; i < n; ++i) m += s_p[key_index(s_sorted[i])];
+    s_mass = m;
+    mass[row] = m;
+  }
+  __syncthreads();
+  if ((int)threadIdx.x < K) {
+    const int i = threadIdx.x;
+    const int j = i < n ? key_index(s_sorted[i]) : -1;
+    lo[i] = j;
+    po[i] = i < n ? s_p[j] / s_mass : 0.f;
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kKdThreads) pointer_mix_kd_sparse_fwd_kernel(
+    const T* __restrict__ logits, long ldl, const float* __restrict__ sc, const float* __restrict__ gate_logit,
+    const unsigned char* __restrict__ mem_mask, const int* __restrict__ label, const int* __restrict__ t_label,
+    const float* __restrict__ t_prob, int K, float alpha, float* __restrict__ stats, float* __restrict__ nll,
+    float* __restrict__ kd, float* __restrict__ loss, int Tn, int V, int S) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  __shared__ MaxSum sh_ms[8];
+  __shared__ float bc[4];
+  __shared__ float shf[8];
+  __shared__ float s_st[8];
+  const long row = blockIdx.x;
+  const int y = label[row];
+  float* st = stats + row * kKdSparseStats;
+  if (y == 0) {                                       // no loss: neither the row nor its targets are read
+    if (threadIdx.x < kKdSparseStats) st[threadIdx.x] = 0.f;
+    if (threadIdx.x == 0) { nll[row] = 0.f; kd[row] = 0.f; loss[row] = 0.f; }
+    return;
+  }
+  const int b = (int)(row / Tn);
+  const T* lrow = logits + row * ldl;
+  const float* srow = sc + row * S;
+  const unsigned char* mrow = mem_mask + (long)b * S;
+  // the student's statistics and P_y: fira_pointer_mix_nll_fwd's, bit for bit
+  const MixRow ms = mix_row_stats(lrow, srow, mrow, gate_logit + row * 2, V, S, sh_ms, bc);
+  if (threadIdx.x == 0) {                             // a copy label beyond S: p = 0, the clamp floor, no gradient
+    s_st[0] = ms.vmax; s_st[1] = ms.vsum; s_st[2] = ms.cmax; s_st[3] = ms.csum; s_st[4] = ms.g0; s_st[5] = ms.g1;
+    s_st[6] = y - V < S ? mix_prob(ms, lrow, srow, mrow, V, y) : 0.f;
+    s_st[7] = 0.f;
+  }
+  __syncthreads();
+  const KdRow k = kd_student(s_st, alpha, y);
+  float t;
+  const int j = kd_sparse_entry(t_label + row * K, t_prob + row * K, K, y, V, S, t);
+  float kdp = 0.f, acc = 0.f;
+  if (j >= 0) {
+    float lp;
+    const float p = kd_entry(ms, k, lrow, srow, mrow, V, j, lp);
+    kd_term(k, j, p, t, lp, kdp, acc);
+  }
+  float av = j < V ? acc : 0.f, ac = j < V ? 0.f : acc;
+  auto add = [](float a, float x) { return a + x; };
+  kdp = block_reduce(kdp, shf, add);
+  av = block_reduce(av, shf, add);
+  ac = block_reduce(ac, shf, add);
+  if (threadIdx.x < kKdSparseStats) st[threadIdx.x] = threadIdx.x == 8 ? av : threadIdx.x == 9 ? ac : s_st[threadIdx.x];
+  if (threadIdx.x == 0) {
+    const float h = -k.lp_lab;                        // = fira_pointer_mix_nll_fwd's nll
+    nll[row] = h;
+    kd[row] = kdp;
+    loss[row] = fmaf(alpha, kdp, k.hard * h);
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kKdThreads) pointer_mix_kd_sparse_bwd_kernel(
+    const T* __restrict__ logits, long ldl, const float* __restrict__ sc, const unsigned char* __restrict__ mem_mask,
+    const int* __restrict__ label, const int* __restrict__ t_label, const float* __restrict__ t_prob, int K,
+    float alpha, const float* __restrict__ stats, const float* __restrict__ upstream, T* __restrict__ d_logits,
+    float* __restrict__ d_sc, float* __restrict__ d_gate_logit, unsigned char* __restrict__ row_active, int Tn, int V,
+    int S) {
+  pdl_wait(); pdl_trigger();       // PDL (common.cuh)
+  const long row = blockIdx.x;
+  const int b = (int)(row / Tn);
+  const int y = label[row];
+  const float* st = stats + row * kKdSparseStats;
+  const float A_V = y ? st[8] : 0.f, A_C = y ? st[9] : 0.f;
+  const float up = *upstream;
+  const KdRow k = kd_student(st, alpha, y);
+  const T* lrow = logits + row * ldl;
+  const float* srow = sc + row * S;
+  const unsigned char* mrow = mem_mask + (long)b * S;
+  T* drow = d_logits + row * ldl;
+  float* dsrow = d_sc + row * S;
+  // this thread's entry and its a_j, as the forward formed them (a != 0 implies its side's A != 0)
+  float t, a = 0.f;
+  const int j = y ? kd_sparse_entry(t_label + row * K, t_prob + row * K, K, y, V, S, t) : -1;
+  if (j >= 0) {
+    const MixRow ms{st[0], st[1], st[2], st[3], st[4], st[5]};
+    float lp;
+    a = kd_weight(k, j, kd_entry(ms, k, lrow, srow, mrow, V, j, lp), t);
+  }
+  const int V8 = V >> 3;                              // 8 logits per vector load / store, scalar tail
+  const float sv = k.iv * A_V, scc = k.ic * A_C;
+  if (A_V != 0.f) {
+    for (int g = threadIdx.x; g < V8; g += blockDim.x) {
+      float x[8];
+      Act<T>::load8(lrow + (long)g * 8, x);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) x[i] = up * (expf(x[i] - k.vmax) * sv);
+      Act<T>::store8(drow + (long)g * 8, x);
+    }
+    for (int q = V8 * 8 + threadIdx.x; q < V; q += blockDim.x)
+      Act<T>::st(drow + q, up * (expf(Act<T>::ld(lrow + q) - k.vmax) * sv));
+  } else {
+    const float z[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int g = threadIdx.x; g < V8; g += blockDim.x) Act<T>::store8(drow + (long)g * 8, z);
+    for (int q = V8 * 8 + threadIdx.x; q < V; q += blockDim.x) Act<T>::st(drow + q, 0.f);
+  }
+  if (A_C != 0.f) {
+    for (int s = threadIdx.x; s < S; s += blockDim.x)   // a masked position takes no gradient (masked_fill)
+      dsrow[s] = mrow[s] ? up * (expf(srow[s] - k.cmax) * scc) : 0.f;
+  } else {
+    for (int s = threadIdx.x; s < S; s += blockDim.x) dsrow[s] = 0.f;
+  }
+  __syncthreads();                                    // the dense pass is written; the weighted columns follow
+  if (a != 0.f) {
+    if (j < V) {
+      Act<T>::st(drow + j, up * (expf(Act<T>::ld(lrow + j) - k.vmax) * sv - a));
+    } else if (mrow[j - V]) {
+      dsrow[j - V] = up * (expf(srow[j - V] - k.cmax) * scc - a);
+    }
   }
   if (threadIdx.x == 0) {
     const float A = A_V + A_C;
@@ -2123,6 +2360,76 @@ int fira_pointer_mix_kd_bwd(const void* logits, long ld_logits, const float* cop
       (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, mem_mask, label, t_logits, ld_t, t_copy_scores,
       alpha, stats, upstream, (T*)d_logits, d_copy_scores, d_gate_logits, row_active, T_len, V, S);)
   FIRA_CHECK_LAUNCH("fira_pointer_mix_kd_bwd");
+  return FIRA_OK;
+}
+
+int fira_pointer_mix_topk(const float* t_logits, long ld_t, const float* t_copy_scores, const float* t_gate_logits,
+                          const unsigned char* mem_mask, const int* label, int k, int* t_label, float* t_prob,
+                          float* mass, long rows, int T_len, int V, int S, void* stream) {
+  FIRA_CHECK_ARG(k >= 1 && k <= kKdMaxTopk, FIRA_ERR_ARG, "pointer_mix_topk: k %d not in [1, %d]", k, kKdMaxTopk);
+  FIRA_CHECK_ARG(t_logits && t_copy_scores && t_gate_logits && mem_mask && label && t_label && t_prob && mass,
+                 FIRA_ERR_ARG, "pointer_mix_topk: null pointer");
+  FIRA_CHECK_ARG(rows >= 0 && T_len > 0 && V > 0 && S > 0 && V + S <= 0x7FFF && ld_t >= V, FIRA_ERR_SHAPE,
+                 "pointer_mix_topk: shape (rows %ld, T_len %d, V %d, S %d, ld_t %ld; V + S must be <= 32767)", rows,
+                 T_len, V, S, ld_t);
+  FIRA_CHECK_ARG(fira_aligned16(t_logits) && ld_t % 8 == 0, FIRA_ERR_ALIGN,
+                 "pointer_mix_topk: t_logits must be 16-byte aligned, ld_t %ld a multiple of 8", ld_t);
+  if (rows == 0) return FIRA_OK;
+  const size_t smem = (size_t)(V + S) * sizeof(float);
+  const cudaError_t e = cudaFuncSetAttribute(pointer_mix_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)smem);
+  if (e != cudaSuccess) { fira_set_error(FIRA_ERR_CUDA, "pointer_mix_topk attr: %s", cudaGetErrorString(e)); return FIRA_ERR_CUDA; }
+  launch_k(pointer_mix_topk_kernel, dim3((unsigned)rows), dim3(kSampleThreads), smem, (cudaStream_t)stream, t_logits,
+           ld_t, t_copy_scores, t_gate_logits, mem_mask, label, k, t_label, t_prob, mass, T_len, V, S);
+  FIRA_CHECK_LAUNCH("fira_pointer_mix_topk");
+  return FIRA_OK;
+}
+
+static int kd_sparse_check(const char* who, const void* logits, long ld_logits, int k, float alpha, long rows,
+                           int T_len, int V, int S) {
+  FIRA_CHECK_ARG(alpha >= 0.f && alpha <= 1.f, FIRA_ERR_ARG, "%s: alpha %g not in [0, 1]", who, (double)alpha);
+  FIRA_CHECK_ARG(k >= 1 && k <= kKdMaxTopk, FIRA_ERR_ARG, "%s: k %d not in [1, %d]", who, k, kKdMaxTopk);
+  FIRA_CHECK_ARG(rows >= 0 && T_len > 0 && V > 0 && S > 0 && V + S <= 0x7FFF && ld_logits >= V, FIRA_ERR_SHAPE,
+                 "%s: shape (rows %ld, T_len %d, V %d, S %d, ld_logits %ld; V + S must be <= 32767)", who, rows, T_len,
+                 V, S, ld_logits);
+  FIRA_CHECK_ARG(fira_aligned16(logits) && ld_logits % 8 == 0, FIRA_ERR_ALIGN,
+                 "%s: logits must be 16-byte aligned with a leading dimension that is a multiple of 8", who);
+  return FIRA_OK;
+}
+
+int fira_pointer_mix_kd_sparse_fwd(const void* logits, long ld_logits, const float* copy_scores,
+                                   const float* gate_logits, const unsigned char* mem_mask, const int* label,
+                                   const int* t_label, const float* t_prob, int k, float alpha, float* stats,
+                                   float* nll, float* kd, float* loss, long rows, int T_len, int V, int S, int dtype,
+                                   void* stream) {
+  FIRA_CHECK_ARG(logits && copy_scores && gate_logits && mem_mask && label && t_label && t_prob && stats && nll && kd
+                 && loss, FIRA_ERR_ARG, "pointer_mix_kd_sparse_fwd: null pointer");
+  const int rc = kd_sparse_check("pointer_mix_kd_sparse_fwd", logits, ld_logits, k, alpha, rows, T_len, V, S);
+  if (rc != FIRA_OK) return rc;
+  if (rows == 0) return FIRA_OK;
+  DISPATCH_T(dtype, launch_k(pointer_mix_kd_sparse_fwd_kernel<T>, dim3((unsigned)rows), dim3(kKdThreads), 0,
+      (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, gate_logits, mem_mask, label, t_label, t_prob, k,
+      alpha, stats, nll, kd, loss, T_len, V, S);)
+  FIRA_CHECK_LAUNCH("fira_pointer_mix_kd_sparse_fwd");
+  return FIRA_OK;
+}
+
+int fira_pointer_mix_kd_sparse_bwd(const void* logits, long ld_logits, const float* copy_scores,
+                                   const unsigned char* mem_mask, const int* label, const int* t_label,
+                                   const float* t_prob, int k, float alpha, const float* stats, const float* upstream,
+                                   void* d_logits, float* d_copy_scores, float* d_gate_logits,
+                                   unsigned char* row_active, long rows, int T_len, int V, int S, int dtype,
+                                   void* stream) {
+  FIRA_CHECK_ARG(logits && copy_scores && mem_mask && label && t_label && t_prob && stats && upstream && d_logits &&
+                 d_copy_scores && d_gate_logits && row_active, FIRA_ERR_ARG, "pointer_mix_kd_sparse_bwd: null pointer");
+  const int rc = kd_sparse_check("pointer_mix_kd_sparse_bwd", logits, ld_logits, k, alpha, rows, T_len, V, S);
+  if (rc != FIRA_OK) return rc;
+  FIRA_CHECK_ARG(fira_aligned16(d_logits), FIRA_ERR_ALIGN, "pointer_mix_kd_sparse_bwd: d_logits must be 16-byte aligned");
+  if (rows == 0) return FIRA_OK;
+  DISPATCH_T(dtype, launch_k(pointer_mix_kd_sparse_bwd_kernel<T>, dim3((unsigned)rows), dim3(kKdThreads), 0,
+      (cudaStream_t)stream, (const T*)logits, ld_logits, copy_scores, mem_mask, label, t_label, t_prob, k, alpha, stats,
+      upstream, (T*)d_logits, d_copy_scores, d_gate_logits, row_active, T_len, V, S);)
+  FIRA_CHECK_LAUNCH("fira_pointer_mix_kd_sparse_bwd");
   return FIRA_OK;
 }
 

@@ -17,11 +17,20 @@ and its gradient through both softmaxes, the gate and the clamp in fira_pointer_
 so the 25,020-wide distributions are never stored.  distill_step is the eager padded-batch path, as scst.scst_step:
 the kernels' dropout in the student, an eager optim.FlatAdam step and scst.bump_weights.  The teacher keeps M member
 triples and their fp32 average on the device, about (M s + 4) B T ld_logits bytes (s = 4 fp32, 2 bf16).
+
+Offline distillation: the teacher is frozen and teacher-forced, so its distributions are the same every epoch.
+build_targets runs it once over a split and keeps, per loss row, its k most probable labels (fira_pointer_mix_topk:
+P descending, then label ascending; Tan et al., ICLR 2019 keep 8) renormalised to t~_i = P_i / mass, mass = the kept
+P summed in key order.  A KDTargets holds them; KDTargets.batch gathers a batch's [B*T, k] labels and probabilities,
+and distill_step trains against them with fira_pointer_mix_kd_sparse_fwd / _bwd: the loss above with t = t~ at the
+kept labels and 0 elsewhere, no teacher run and no teacher memory.
 """
 import ctypes
 import math
 import numbers
 from typing import NamedTuple
+
+import numpy as np
 
 import torch
 
@@ -29,6 +38,7 @@ from . import ops
 from . import optim as _optim
 from ._lib import FIRA_BF16, FIRA_F32, call
 from .ensemble import Ensemble, refuse
+from .knn import fingerprint
 from .model import TransModel
 from .modules import _i32, _u8
 from .scst import bump_weights
@@ -114,9 +124,170 @@ def teacher_targets(teacher, batch, label):
     return out, sc_out, gl_out
 
 
+MAX_TOPK = 64             # fira_pointer_mix_topk / fira_pointer_mix_kd_sparse_*
+FORMAT = "fira-kd-targets-1"
+
+
+class SparseTargets(NamedTuple):
+    """One padded batch's stored teacher targets (KDTargets.batch), on the student's device."""
+    t_label: torch.Tensor     # int32 [B*T, k]: vocabulary id j < V or V + copy position; -1 = no entry
+    t_prob: torch.Tensor      # fp32 [B*T, k]: t~ of each label (0 for -1)
+
+
+def check_topk(k):
+    """ValueError unless k is an integer in [1, MAX_TOPK] (host only)."""
+    if isinstance(k, bool) or not isinstance(k, numbers.Integral) or not 1 <= int(k) <= MAX_TOPK:
+        raise ValueError(f"k must be an integer in [1, {MAX_TOPK}], got {k!r}")
+
+
+def topk_targets(targets, mem_mask, label, V, k):
+    """fira_pointer_mix_topk of the teacher's triple (teacher_targets) -> (t_label int32 [B*T, k], t_prob fp32
+    [B*T, k], mass fp32 [B*T]) on its device; mem_mask [B, S] uint8, label the shifted labels [B, T]."""
+    check_topk(k)
+    logits, sc, gl = targets
+    B, T, S = sc.shape
+    dev = logits.device
+    t_label = torch.empty((B * T, k), dtype=torch.int32, device=dev)
+    t_prob = torch.empty((B * T, k), dtype=torch.float32, device=dev)
+    mass = torch.empty((B * T,), dtype=torch.float32, device=dev)
+    lab = _i32(label).reshape(-1).contiguous()
+    call("fira_pointer_mix_topk", ops._ptr(logits), logits.stride(0), ops._ptr(sc), ops._ptr(gl), ops._ptr(mem_mask),
+         ops._ptr(lab), int(k), ops._ptr(t_label), ops._ptr(t_prob), ops._ptr(mass), B * T, T, V, S, ops._stream())
+    return t_label, t_prob, mass
+
+
+class KDTargets:
+    """A split's stored top-k teacher targets (build_targets).  Commit i of the split (dataset position first + i)
+    owns rows row_off[i] .. row_off[i + 1] - 1, its loss rows (shifted label y != 0) in position order; per row: pos
+    (the target position t) and y, kept to check that a batch is the one the rows were built from, and the kept labels
+    t_label [R, k] int32 (-1: none), their renormalised probabilities t_prob [R, k] fp32 and the kept teacher mass
+    [R] fp32.  All on the host.  provenance: the teacher members' knn.state_fingerprint, their weights, the precision
+    the teacher ran in and the split size.  ValueError for inconsistent shapes or dtypes."""
+
+    def __init__(self, row_off, pos, y, t_label, t_prob, mass, *, vocab_size, k, first, provenance):
+        check_topk(k)
+        for name, t, dt in (("row_off", row_off, torch.int64), ("pos", pos, torch.int16), ("y", y, torch.int32),
+                            ("t_label", t_label, torch.int32), ("t_prob", t_prob, torch.float32),
+                            ("mass", mass, torch.float32)):
+            if not torch.is_tensor(t) or t.dtype != dt or t.device.type != "cpu":
+                raise ValueError(f"KDTargets {name} must be a host {dt} tensor, got {getattr(t, 'dtype', type(t))}")
+        R = pos.numel()
+        if row_off.dim() != 1 or row_off.numel() < 1 or int(row_off[0]) != 0 or int(row_off[-1]) != R or \
+                bool((row_off[1:] < row_off[:-1]).any()):
+            raise ValueError("KDTargets row_off must rise from 0 to the row count")
+        if tuple(y.shape) != (R,) or tuple(mass.shape) != (R,) or tuple(t_label.shape) != (R, k) or \
+                tuple(t_prob.shape) != (R, k):
+            raise ValueError(f"KDTargets rows: pos / y / mass [{R}], t_label / t_prob [{R}, {k}], got "
+                             f"{tuple(y.shape)}, {tuple(mass.shape)}, {tuple(t_label.shape)}, {tuple(t_prob.shape)}")
+        if isinstance(vocab_size, bool) or not isinstance(vocab_size, int) or vocab_size < 1:
+            raise ValueError(f"vocab_size must be a positive integer, got {vocab_size!r}")
+        self.row_off, self.pos, self.y = row_off.contiguous(), pos.contiguous(), y.contiguous()
+        self.t_label, self.t_prob, self.mass = t_label.contiguous(), t_prob.contiguous(), mass.contiguous()
+        self.vocab_size, self.k, self.first = vocab_size, int(k), int(first)
+        self.provenance = dict(provenance)
+
+    @property
+    def n(self):
+        """number of commits"""
+        return self.row_off.numel() - 1
+
+    @property
+    def rows(self):
+        return self.pos.numel()
+
+    @property
+    def nbytes(self):
+        return sum(t.numel() * t.element_size() for t in (self.row_off, self.pos, self.y, self.t_label, self.t_prob,
+                                                          self.mass))
+
+    def save(self, path):
+        torch.save({"format": FORMAT, "vocab_size": self.vocab_size, "k": self.k, "first": self.first,
+                    "provenance": self.provenance, "row_off": self.row_off, "pos": self.pos, "y": self.y,
+                    "t_label": self.t_label, "t_prob": self.t_prob, "mass": self.mass}, path)
+
+    @classmethod
+    def load(cls, path, *, vocab_size=None, k=None, commits=None):
+        """The targets saved at `path`.  ValueError for another file format and a vocabulary size, k or commit count
+        other than the given ones (None: not checked)."""
+        s = torch.load(path, map_location="cpu", weights_only=True)
+        if not isinstance(s, dict) or s.get("format") != FORMAT:
+            raise ValueError(f"{path} is not a distillation target file ({FORMAT})")
+        n = s["row_off"].numel() - 1
+        for name, want, got in (("vocab_size", vocab_size, s["vocab_size"]), ("k", k, s["k"]), ("commits", commits, n)):
+            if want is not None and want != got:
+                raise ValueError(f"{path}: {name} {got}, expected {want}")
+        return cls(*(s[f] for f in ("row_off", "pos", "y", "t_label", "t_prob", "mass")), vocab_size=s["vocab_size"],
+                   k=s["k"], first=s["first"], provenance=s["provenance"])
+
+    def batch(self, indices, label, device=None):
+        """SparseTargets of the padded batch holding the commits at dataset positions `indices` (in batch order) with
+        shifted labels `label` [B, T] (TransModel.shifted_label of its tar_label; host tensors avoid a device
+        read-back) -> [B*T, k] labels and probabilities on `device` (default: label's).  ValueError, before anything is
+        sent to the device, for a position outside the stored commits or stored rows other than the batch's loss rows
+        (another split, order or label encoding)."""
+        idx = torch.as_tensor(np.asarray(indices, dtype=np.int64)).view(-1) - self.first
+        lab = label.detach().to("cpu")
+        B, T = lab.shape
+        if idx.numel() != B:
+            raise ValueError(f"KDTargets.batch: {idx.numel()} positions for a batch of {B} commits")
+        if idx.numel() and (int(idx.min()) < 0 or int(idx.max()) >= self.n):
+            raise ValueError(f"KDTargets.batch: a position outside the stored commits {self.first}.."
+                             f"{self.first + self.n - 1}")
+        live = lab != 0
+        lo, hi = self.row_off[idx], self.row_off[idx + 1]
+        if not torch.equal(hi - lo, live.sum(1)):
+            raise ValueError("KDTargets.batch: the stored row counts differ from the batch's loss rows (a file built "
+                             "for another split or order?)")
+        src = torch.cat([torch.arange(int(a), int(z)) for a, z in zip(lo, hi)] + [torch.zeros(0, dtype=torch.int64)])
+        b, t = live.nonzero(as_tuple=True)
+        if not torch.equal(self.pos[src].long(), t) or not torch.equal(self.y[src], lab[b, t].to(torch.int32)):
+            raise ValueError("KDTargets.batch: the stored positions or labels differ from the batch's (a file built "
+                             "for another split or order?)")
+        t_label = torch.full((B * T, self.k), -1, dtype=torch.int32)
+        t_prob = torch.zeros((B * T, self.k), dtype=torch.float32)
+        dst = b * T + t
+        t_label[dst] = self.t_label[src]
+        t_prob[dst] = self.t_prob[src]
+        dev = label.device if device is None else device
+        return SparseTargets(t_label.to(dev), t_prob.to(dev))
+
+
+@torch.no_grad()
+def build_targets(teacher, batches, *, k, first_index):
+    """KDTargets from padded batches (the 8-tuples of run_model.py on the teacher's device) that follow one another
+    from dataset position first_index: teacher_targets, then fira_pointer_mix_topk, per batch.  Only rows with y != 0
+    are stored."""
+    check_topk(k)
+    models, _ = teacher_members(teacher)
+    weights = teacher.weights if isinstance(teacher, Ensemble) else (1.0,)
+    V = models[0].vocab_size
+    dev = models[0].out_fc.weight.device
+    parts, counts = [], []
+    for batch in batches:
+        label = TransModel.shifted_label(batch[6].to(dev))
+        targets = teacher_targets(teacher, batch, label)
+        mem_mask = _u8(torch.cat((batch[0] != 0, batch[7] != 0), dim=1).to(dev))
+        t_label, t_prob, mass = topk_targets(targets, mem_mask, label, V, k)
+        live = (label != 0).view(-1)
+        t = torch.arange(label.shape[1], device=dev).expand_as(label).reshape(-1)
+        parts.append(tuple(a[live].cpu() for a in (t.to(torch.int16), _i32(label).view(-1), t_label, t_prob, mass)))
+        counts.append((label != 0).sum(1).cpu())
+    if not parts:
+        raise ValueError("build_targets: no batches")
+    pos, y, t_label, t_prob, mass = (torch.cat(x) for x in zip(*parts))
+    counts = torch.cat(counts)
+    row_off = torch.zeros(counts.numel() + 1, dtype=torch.int64)
+    row_off[1:] = torch.cumsum(counts, 0)
+    provenance = dict(fingerprints=[fingerprint(m) for m in models], weights=[float(w) for w in weights],
+                      precision=models[0].precision, commits=counts.numel())
+    return KDTargets(row_off, pos, y, t_label, t_prob, mass, vocab_size=V, k=k, first=first_index,
+                     provenance=provenance)
+
+
 def distill_loss(model, batch, targets, label, alpha):
     """sum_r loss_r under autograd in the model's current mode -> (loss_sum, nll [B, T], kd [B*T]).  targets: the
-    teacher's triple of teacher_targets; label: the shifted labels [B, T] on the model's device."""
+    teacher's triple of teacher_targets, or the batch's SparseTargets; label: the shifted labels [B, T] on the model's
+    device."""
     m = model
     dev = m.out_fc.weight.device
     sou, tar, _, mark, ast_change, edge, _, sub_token = batch
@@ -130,22 +301,45 @@ def distill_loss(model, batch, targets, label, alpha):
     mem_mask = torch.cat((sou != 0, sub_token != 0), dim=1)
     dec = m.decoder(tar, memory, mem_mask, tar != 0)
     kd = torch.empty(label.numel(), dtype=torch.float32, device=dev)
+    if isinstance(targets, SparseTargets):
+        dense, sparse = None, (targets.t_label, targets.t_prob, float(alpha), kd)
+    else:
+        dense, sparse = (*targets, float(alpha), kd), None
     loss, nll, _ = ops.HeadFn.apply(False, bf16, pf_head, memory, dec, _u8(mem_mask), _i32(label).view(-1),
-                                    m.out_fc.weight, m.out_fc.bias, *m.copy_net.flat_params(), None, None,
-                                    (*targets, float(alpha), kd))
+                                    m.out_fc.weight, m.out_fc.bias, *m.copy_net.flat_params(), None, None, dense,
+                                    sparse)
     return loss, nll, kd
+
+
+def check_sparse(targets, model, rows):
+    """ValueError unless targets are SparseTargets of `rows` rows and 1..MAX_TOPK labels on the model's device (host
+    only)."""
+    dev = model.out_fc.weight.device
+    a, p = targets
+    ok = torch.is_tensor(a) and torch.is_tensor(p) and a.dtype == torch.int32 and p.dtype == torch.float32 and \
+        a.dim() == 2 and p.shape == a.shape and a.shape[0] == rows and 1 <= a.shape[1] <= MAX_TOPK
+    if not ok:
+        raise ValueError(f"sparse targets must be int32 labels and fp32 probabilities [{rows}, k], 1 <= k <= "
+                         f"{MAX_TOPK}")
+    if a.device != dev or p.device != dev:
+        raise ValueError(f"the sparse targets are on {a.device}, the student on {dev}")
 
 
 def distill_step(model, optimizer, batch, teacher, *, alpha):
     """One distillation step on the padded batch (the 8-tuple of run_model.py on the model's device) -> Step(per-token
-    loss, nll and kd, tokens).  The student runs in training mode (the kernels' dropout) and stays in it; the
-    teacher's members are left in eval mode.  Settings and teacher are checked on the host before any device work."""
+    loss, nll and kd, tokens).  teacher: a TransModel or an Ensemble, run on the batch (its members are left in eval
+    mode), or the batch's SparseTargets (KDTargets.batch): then no teacher runs.  The student runs in training mode
+    (the kernels' dropout) and stays in it.  Settings and teacher are checked on the host before any device work."""
     check_alpha(alpha)
     refuse(model, "distill_step")
-    teacher_members(teacher, model)
+    sparse = isinstance(teacher, SparseTargets)
+    if sparse:
+        check_sparse(teacher, model, batch[6].shape[0] * batch[6].shape[1])
+    else:
+        teacher_members(teacher, model)
     dev = model.out_fc.weight.device
     label = model.shifted_label(batch[6].to(dev))
-    targets = teacher_targets(teacher, batch, label)
+    targets = teacher if sparse else teacher_targets(teacher, batch, label)
     model.train()
     optimizer.zero_grad()
     loss_sum, nll, kd = distill_loss(model, batch, targets, label, alpha)

@@ -877,11 +877,14 @@ class HeadFn(torch.autograd.Function):
     teacher (padded training batches only, not with seq_weight): (t_logits fp32 [B*T, >= V], t_copy_scores fp32
     [B, T, S], t_gate_logits fp32 [B*T, 2], alpha, kd fp32 [B*T]), a teacher's triple (distill.teacher_targets):
     loss_sum = sum_r (1 - alpha) nll_r + alpha kd_r with kd_r = -sum_j t_j log clamp(P_j, 1e-10, 1), written to `kd`
-    (fira_pointer_mix_kd_fwd / _bwd; distill.py)."""
+    (fira_pointer_mix_kd_fwd / _bwd; distill.py).
+    sparse (instead of teacher, on the same path): (t_label int32 [B*T, k], t_prob fp32 [B*T, k], alpha, kd fp32
+    [B*T]), a batch's stored top-k targets (distill.KDTargets.batch): the same loss with t_j = t_prob at the labels
+    t_label and 0 elsewhere (fira_pointer_mix_kd_sparse_fwd / _bwd)."""
 
     @staticmethod
     def forward(ctx, want_argmax, bf16, pf, memory, dec, mem_mask, label, Wout, bout, Ws, Wt, Wres, bres, Wp, bp,
-                pk=None, seq_weight=None, teacher=None):
+                pk=None, seq_weight=None, teacher=None, sparse=None):
         _require_cuda(memory, dec, Wout)
         B, T = dec.shape[0], dec.shape[1]
         S = pk.S if pk is not None else memory.shape[1]      # packed batch: memory is [1, Rc + Rs, D]
@@ -904,6 +907,17 @@ class HeadFn(torch.autograd.Function):
                     not kd.is_contiguous():
                 raise ValueError(f"HeadFn: the teacher needs CUDA fp32 logits [{Mt}, >= {V}], copy scores "
                                  f"[{B}, {T}, {S}], gate logits [{Mt}, 2] and a kd buffer of {Mt}")
+        if sparse is not None:
+            if pk is not None or want_argmax or seq_weight is not None or teacher is not None:
+                raise ValueError("HeadFn: sparse targets apply to the padded training path without seq_weight or a "
+                                 "teacher")
+            t_label, t_prob, _, kd = sparse
+            ok = all(t is not None and t.is_cuda and t.is_contiguous() for t in (t_label, t_prob, kd)) and \
+                t_label.dtype == torch.int32 and t_prob.dtype == torch.float32 and kd.dtype == torch.float32
+            if not ok or t_label.dim() != 2 or t_label.shape[0] != Mt or not 1 <= t_label.shape[1] <= 64 or \
+                    t_prob.shape != t_label.shape or kd.numel() != Mt:
+                raise ValueError(f"HeadFn: sparse targets need contiguous CUDA int32 labels and fp32 probabilities "
+                                 f"[{Mt}, k] with 1 <= k <= 64 and an fp32 kd buffer of {Mt}")
         pr = Prec(bf16)
         if pf is not None and pf.event is not None:
             torch.cuda.current_stream().wait_event(pf.event)
@@ -916,7 +930,8 @@ class HeadFn(torch.autograd.Function):
         dec2 = dec.contiguous().to(pr.tdt).view(Mt, D)
         dec32 = dec2 if not pr.bf16 else dec2.float()            # the 2-wide gate stays on the fp32 path
         ldl = _ld_logits(V)
-        if want_argmax or teacher is not None:        # every loss row of a teacher's batch reads its logits
+        kdt = teacher is not None or sparse is not None
+        if want_argmax or kdt:                        # every loss row of a teacher's batch reads its logits
             cap, vslot, vrows, dec_v = Mt, None, None, dec2
         else:
             # training: out_fc runs on the vocabulary-label rows alone, compacted into `cap` slots (a packed batch
@@ -931,14 +946,19 @@ class HeadFn(torch.autograd.Function):
         # training only needs pointer scores of real source positions at target rows whose label is a COPY
         # label (vocabulary-label rows take their loss from the vocabulary softmax alone, Model.py:64-81); with a
         # teacher every loss row spreads over the copy positions too
-        row_mask = None if want_argmax else ((label != 0) if teacher is not None else (label >= V)).to(torch.uint8)
+        row_mask = None if want_argmax else ((label != 0) if kdt else (label >= V)).to(torch.uint8)
         logits, src, tgt, sc, gl = head_products(pr, memory2, dec2, dec32, dec_v, cap, Wout, bout, Ws, Wt, Wres, bres,
                                                  Wp, bp, B, T, S, mem_mask, row_mask,
                                                  ranges=pk.ranges if pk is not None else None)
-        stats = torch.empty((Mt, 8 if teacher is None else 16), **f32)
+        stats = torch.empty((Mt, 16 if teacher is not None else 10 if sparse is not None else 8), **f32)
         nll = torch.empty((Mt,), **f32)
         amax = torch.empty((Mt,), dtype=torch.int32, device=dev) if want_argmax else None
-        if teacher is None:
+        if sparse is not None:
+            loss_rows = torch.empty((Mt,), **f32)
+            call("fira_pointer_mix_kd_sparse_fwd", _ptr(logits), ldl, _ptr(sc), _ptr(gl), _ptr(mem_mask), _ptr(label),
+                 _ptr(t_label), _ptr(t_prob), t_label.shape[1], float(sparse[2]), _ptr(stats), _ptr(nll), _ptr(kd),
+                 _ptr(loss_rows), Mt, T, V, S, pr.code, st)
+        elif teacher is None:
             call("fira_pointer_mix_nll_fwd_rows", _ptr(logits), ldl, _ptr(sc), _ptr(gl), _ptr(mem_mask), _ptr(label),
                  _ptr(vslot), _ptr(stats), _ptr(nll), _ptr(amax), Mt, T, V, S, pr.code, st)
         else:
@@ -947,9 +967,9 @@ class HeadFn(torch.autograd.Function):
                  _ptr(t_logits), t_logits.stride(0), _ptr(t_sc), _ptr(t_gl), float(alpha), _ptr(stats), _ptr(nll),
                  _ptr(kd), _ptr(loss_rows), Mt, T, V, S, pr.code, st)
         ctx.misc = (pr, memory2, dec2, dec32, mem_mask, label, logits, ldl, src, tgt, sc, stats, B, T, S, V,
-                    memory.dtype, dec.dtype, pk, memory.shape, cap, vslot, vrows, dec_v, seq_weight, teacher)
+                    memory.dtype, dec.dtype, pk, memory.shape, cap, vslot, vrows, dec_v, seq_weight, teacher, sparse)
         ctx.save_for_backward(Wout, Ws, Wt, Wres, Wp, bout, bres, bp)
-        if teacher is not None:
+        if kdt:
             loss_sum = colsum(loss_rows, 1, Mt, 1).view(())
         elif seq_weight is None:
             loss_sum = colsum(nll, 1, Mt, 1).view(())
@@ -963,7 +983,7 @@ class HeadFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_loss, g_nll, g_ids):
         (pr, memory2, dec2, dec32, mem_mask, label, logits, ldl, src, tgt, sc, stats, B, T, S, V,
-         mem_dt, dec_dt, pk, mem_shape, cap, vslot, vrows, dec_v, seq_weight, teacher) = ctx.misc
+         mem_dt, dec_dt, pk, mem_shape, cap, vslot, vrows, dec_v, seq_weight, teacher, sparse) = ctx.misc
         Wout, Ws, Wt, Wres, Wp, bout, bres, bp = ctx.saved_tensors
         Mt, Ms = B * T, memory2.shape[0]
         dev = dec2.device
@@ -976,7 +996,12 @@ class HeadFn(torch.autograd.Function):
         active = torch.empty((Mt,), dtype=torch.uint8, device=dev)
         args = (_ptr(logits), ldl, _ptr(sc), _ptr(mem_mask), _ptr(label), _ptr(vslot), _ptr(vrows), cap, _ptr(stats),
                 _ptr(up), _ptr(dlogits), _ptr(dsc), _ptr(dgl), _ptr(active), Mt, T, V, S, pr.code, st)
-        if teacher is not None:
+        if sparse is not None:
+            t_label, t_prob, alpha, _ = sparse
+            call("fira_pointer_mix_kd_sparse_bwd", _ptr(logits), ldl, _ptr(sc), _ptr(mem_mask), _ptr(label),
+                 _ptr(t_label), _ptr(t_prob), t_label.shape[1], float(alpha), _ptr(stats), _ptr(up), _ptr(dlogits),
+                 _ptr(dsc), _ptr(dgl), _ptr(active), Mt, T, V, S, pr.code, st)
+        elif teacher is not None:
             t_logits, t_sc, _, alpha, _ = teacher
             call("fira_pointer_mix_kd_bwd", _ptr(logits), ldl, _ptr(sc), _ptr(mem_mask), _ptr(label), _ptr(t_logits),
                  t_logits.stride(0), _ptr(t_sc), float(alpha), _ptr(stats), _ptr(up), _ptr(dlogits), _ptr(dsc),
@@ -1022,7 +1047,7 @@ class HeadFn(torch.autograd.Function):
         linear_dx(d_tgt, D, Wt, Mt, out=d_dec, accumulate=True)
         fork.join()
         return (None, None, None, d_mem.view(mem_shape).to(mem_dt), d_dec.view(B, T, D).to(dec_dt), None, None, d_Wout,
-                d_bout, d_Ws, d_Wt, d_wres, d_bres, d_Wp, d_bp, None, None, None)
+                d_bout, d_Ws, d_Wt, d_wres, d_bres, d_Wp, d_bp, None, None, None, None)
 
 
 # ============================================================================= module-surface pieces

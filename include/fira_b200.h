@@ -587,6 +587,38 @@ int fira_pointer_mix_kd_bwd(const void* logits, long ld_logits, const float* cop
                             void* d_logits, float* d_copy_scores, float* d_gate_logits, unsigned char* row_active,
                             long rows, int T_len, int V, int S, int dtype, void* stream);
 
+/* ---- offline distillation (fira_icse_b200/distill.py KDTargets): the teacher's top-k labels, stored once, and the
+ *      loss against them.
+ * fira_pointer_mix_topk: the teacher's fp32 triple as fira_pointer_mix_kd_fwd reads it, mem_mask and the shifted labels.
+ *      Row r with label[r] != 0: P = the triple's mixture (the step kernels' expressions); the candidates are every
+ *      vocabulary entry and every unmasked copy position with P_j > 0 in fp32; the kept labels are the k candidates with
+ *      the largest key (P_j descending, then j ascending; the sampler's 47-bit key taken on P), in key order, in
+ *      t_label [rows, k] int32 (j < V a vocabulary id, V + s copy position s).  mass[r] = the kept P_j summed in key
+ *      order in fp32, t_prob [rows, k] = P_j / mass.  A row with fewer than k candidates fills the rest with label -1
+ *      and probability 0; a label-0 row reads nothing and writes labels -1, probabilities 0 and mass 0.  One CTA of 256
+ *      threads per row, (V + S) * 4 bytes of dynamic shared memory; a row's result depends on that row alone.
+ *      1 <= k <= 64, t_logits 16-byte aligned, ld_t a multiple of 8 and >= V, V + S <= 32767.
+ * fira_pointer_mix_kd_sparse_fwd / _bwd: fira_pointer_mix_kd_fwd / _bwd with the teacher's t replaced by the dense
+ *      vector that holds t_prob[r, i] at label t_label[r, i] and 0 elsewhere (entries with label -1 or probability 0
+ *      add nothing); the student operands, the outputs, the rule and the argument checks are theirs, plus
+ *      1 <= k <= 64.  With alpha = 0 every output equals fira_pointer_mix_nll_fwd / _bwd's bit for bit.  stats: 10
+ *      floats per row (the student's vmax, vsum, cmax, csum, g0, g1, p_label, 0, A_V, A_C).  The forward reads the
+ *      student row once; the backward writes it once and then rewrites the <= k + 1 columns with a_j != 0. */
+int fira_pointer_mix_topk(const float* t_logits, long ld_t, const float* t_copy_scores, const float* t_gate_logits,
+                          const unsigned char* mem_mask, const int* label, int k, int* t_label, float* t_prob,
+                          float* mass, long rows, int T_len, int V, int S, void* stream);
+int fira_pointer_mix_kd_sparse_fwd(const void* logits, long ld_logits, const float* copy_scores,
+                                   const float* gate_logits, const unsigned char* mem_mask, const int* label,
+                                   const int* t_label, const float* t_prob, int k, float alpha, float* stats,
+                                   float* nll, float* kd, float* loss, long rows, int T_len, int V, int S, int dtype,
+                                   void* stream);
+int fira_pointer_mix_kd_sparse_bwd(const void* logits, long ld_logits, const float* copy_scores,
+                                   const unsigned char* mem_mask, const int* label, const int* t_label,
+                                   const float* t_prob, int k, float alpha, const float* stats, const float* upstream,
+                                   void* d_logits, float* d_copy_scores, float* d_gate_logits,
+                                   unsigned char* row_active, long rows, int T_len, int V, int S, int dtype,
+                                   void* stream);
+
 /* ---- minimum-Bayes-risk selection among each commit's N samples (fira_icse_b200/mbr.py).  seq [B, N, ld_seq] int32
  *      (row (b, n) at (b*N + n) * ld_seq, columns 0..T_len-1), length [B, N] int32 (counts <start>; clamped to
  *      [1, T_len]).  Rule:

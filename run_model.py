@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""`python run_model.py train|test|finetune|distill` -- the reference's CLI (run_model.py:417-425) on the CUDA path.
+"""`python run_model.py train|test|finetune|distill|kd-targets` -- the reference's CLI (run_model.py:417-425) on the CUDA path.
 
 Same CWD-relative files (DataSet/*.json, all_index, VOCAB_UPPER_CASE, best_model.pt,
 OUTPUT/{output_fira,train_process,dev_output}), same hyper-parameters (run_model.py:27-46), same
@@ -81,12 +81,20 @@ beam search ranking.  Differences, all below the module surface:
     cross-entropy against the teacher's distribution (FIRA_KD_ALPHA in [0, 1], default 0.5).  Prints loss / nll / kd
     every 10 batches, runs dev() after every epoch and saves the state_dict of the best dev BLEU to best_model_kd.pt
     (dev output: OUTPUT/dev_output_kd); best_model.pt and the teacher checkpoints are never overwritten.  WORLD_SIZE > 1
-    exits with an error.
+    exits with an error.  With FIRA_KD_TARGETS=path (not with FIRA_ENSEMBLE) the teacher is the file `kd-targets`
+    wrote: no teacher is loaded or run, and each epoch e visits the train split in the seeded permutation FIRA_SEED + e
+    (the file's rows are found by dataset position).  The file's vocabulary size and commit count are checked against
+    the data before any device work.
+  * `kd-targets`: runs the teacher of FIRA_ENSEMBLE / FIRA_ENSEMBLE_WEIGHTS (one checkpoint is allowed) once over the
+    train split in dataset order, in padded batches of FIRA_BATCH commits and FIRA_PRECISION, and writes its
+    FIRA_KD_TOPK (default 8, 1..64) most probable labels per target position, renormalised, to FIRA_KD_TARGETS (default
+    kd_targets.pt) for `distill`.  Prints the rows, the bytes and the mean kept teacher mass.  One GPU.
 """
 import json
 import os
 import random
 import sys
+import time
 
 import numpy as np
 import torch
@@ -98,7 +106,7 @@ from fira_icse_b200 import TransModel
 from fira_icse_b200.beam import beam_search, best_sequences, constraints_met, nbest
 from fira_icse_b200.bleu import sentence_bleu_method2
 from fira_icse_b200.decode_loop import MAX_PHRASES
-from fira_icse_b200.distill import distill_step
+from fira_icse_b200.distill import MAX_TOPK, KDTargets, build_targets, distill_step
 from fira_icse_b200.data import PackedBatchLoader, TransDataset, batch_to_device, collate_packed
 from fira_icse_b200.engine import GraphedTrainStep
 from fira_icse_b200.ensemble import MAX_MEMBERS, Ensemble
@@ -608,38 +616,70 @@ def distill_settings():
         raise SystemExit(f"FIRA_KD_EPOCHS must be >= 1, got {s['epochs']}")
     if not 0.0 < s["lr"] < float("inf"):
         raise SystemExit(f"FIRA_KD_LR must be a positive finite number, got {s['lr']}")
-    teacher = ensemble_checkpoints()
-    if teacher is None:
-        raise SystemExit("run_model.py distill needs the teacher: FIRA_ENSEMBLE=a.pt[,b.pt,...]")
+    targets = os.environ.get("FIRA_KD_TARGETS", "")
+    if targets:
+        if os.environ.get("FIRA_ENSEMBLE", ""):
+            raise SystemExit("FIRA_KD_TARGETS is the teacher: unset FIRA_ENSEMBLE")
+        if not os.path.isfile(targets):
+            raise SystemExit(f"FIRA_KD_TARGETS: {targets} not found")
+        teacher = targets
+    else:
+        teacher = ensemble_checkpoints()
+        if teacher is None:
+            raise SystemExit("run_model.py distill needs the teacher: FIRA_ENSEMBLE=a.pt[,b.pt,...] or "
+                             "FIRA_KD_TARGETS=kd_targets.pt")
     student = os.environ.get("FIRA_CHECKPOINT", "best_model.pt")
     if not os.path.isfile(student):
         raise SystemExit(f"FIRA_CHECKPOINT: student checkpoint {student} not found")
     out = os.path.realpath(KD_CHECKPOINT)
-    if any(os.path.realpath(p) == out for p in teacher[0]):
+    if not targets and any(os.path.realpath(p) == out for p in teacher[0]):
         raise SystemExit(f"FIRA_ENSEMBLE names {KD_CHECKPOINT}, which distill writes: copy the teacher elsewhere")
     return s, student, teacher
 
 
+def load_targets(path, train_set):
+    """The KDTargets file of FIRA_KD_TARGETS, checked against the vocabulary and the train split on the host
+    (SystemExit on an error)."""
+    try:
+        return KDTargets.load(path, vocab_size=args.vocab_size, commits=len(train_set))
+    except (ValueError, RuntimeError, OSError, KeyError) as e:
+        raise SystemExit(f"FIRA_KD_TARGETS: {e}")
+
+
 def main_distill():
-    s, student, (paths, weights) = distill_settings()
-    dev_ = device()
-    g = load_globals()
-    train_set = TransDataset(args, 'train')
+    s, student, teacher_spec = distill_settings()
+    if isinstance(teacher_spec, str):
+        g = load_globals()
+        train_set = TransDataset(args, 'train')
+        targets = load_targets(teacher_spec, train_set)       # before any device work
+        seed = int(os.environ.get("FIRA_SEED", 0))
+        dev_ = device()
+    else:
+        targets = None
+        dev_ = device()
+        g = load_globals()
+        train_set = TransDataset(args, 'train')
     dev_set = TransDataset(args, 'valid')
     all_index = json.load(open('all_index'))
     model = load_model(student, dev_)
-    teacher = Ensemble([load_model(p, dev_) for p in paths], weights)
+    teacher = Ensemble([load_model(p, dev_) for p in teacher_spec[0]], teacher_spec[1]) if targets is None else None
     from fira_icse_b200 import optim
     opt = optim.FlatAdam(model.live_parameters(), lr=s["lr"], groups=model.flat_groups())
     optim.attach(model, [opt])
-    train_loader = loader(train_set, args.batch_size, True)
+    train_loader = loader(train_set, args.batch_size, True) if targets is None else None
     dev_loader = loader(dev_set, args.batch_size, False)
     max_batches = int(os.environ.get("FIRA_MAX_BATCHES", 0))
     best_bleu = -1.0
     for epoch in range(s["epochs"]):
+        if targets is not None:                 # a seeded permutation: each batch's dataset positions are known
+            perm = torch.randperm(len(train_set), generator=torch.Generator().manual_seed(seed + epoch)).tolist()
+            train_loader = loader(train_set, args.batch_size, False, indices=perm)
         for idx, batch in enumerate(train_loader):
             if max_batches and idx >= max_batches:
                 break
+            if targets is not None:
+                pos = perm[idx * args.batch_size: idx * args.batch_size + batch[6].shape[0]]
+                teacher = targets.batch(pos, TransModel.shifted_label(batch[6]), device=dev_)
             step = distill_step(model, opt, batch_to_device(batch, dev_), teacher, alpha=s["alpha"])
             if idx % 10 == 0:
                 print("kd epoch: %d batch: %d/%d loss: %.4f nll: %.4f kd: %.4f tokens: %d" % (
@@ -652,6 +692,39 @@ def main_distill():
             torch.save(model.state_dict(), KD_CHECKPOINT)
             open('OUTPUT/dev_output_kd', 'w').write(output_str)
     print("best dev bleu: %f" % best_bleu)
+
+
+def kd_targets_settings():
+    """`kd-targets`' settings, checked before any device work (SystemExit on an error) -> (k, (teacher checkpoints,
+    weights or None), output path)."""
+    if WORLD > 1:
+        raise SystemExit("run_model.py kd-targets runs on one GPU: launch it without torchrun (WORLD_SIZE=1)")
+    try:
+        k = int(os.environ.get("FIRA_KD_TOPK", 8))
+    except ValueError as e:
+        raise SystemExit(f"FIRA_KD_TOPK: {e}")
+    if not 1 <= k <= MAX_TOPK:
+        raise SystemExit(f"FIRA_KD_TOPK must be in [1, {MAX_TOPK}], got {k}")
+    teacher = ensemble_checkpoints()
+    if teacher is None:
+        raise SystemExit("run_model.py kd-targets needs the teacher: FIRA_ENSEMBLE=a.pt[,b.pt,...]")
+    return k, teacher, os.environ.get("FIRA_KD_TARGETS", "kd_targets.pt")
+
+
+def main_kd_targets():
+    k, (paths, weights), out = kd_targets_settings()
+    dev_ = device()
+    load_globals()
+    train_set = TransDataset(args, 'train')
+    teacher = Ensemble([load_model(p, dev_) for p in paths], weights)
+    batches = (batch_to_device(b, dev_) for b in loader(train_set, args.batch_size, False))
+    t0 = time.perf_counter()
+    targets = build_targets(teacher, batches, k=k, first_index=0)
+    dt = time.perf_counter() - t0
+    targets.save(out)
+    print("kd-targets: %d commits, %d rows, k = %d, %d bytes, mean kept mass %.4f, %.1f commits/s -> %s" % (
+        targets.n, targets.rows, k, targets.nbytes, float(targets.mass.double().mean()) if targets.rows else 0.0,
+        targets.n / dt, out))
 
 
 def main_datastore():
@@ -687,5 +760,7 @@ if __name__ == '__main__':
         main_distill()
     elif stage == 'datastore':
         main_datastore()
+    elif stage == 'kd-targets':
+        main_kd_targets()
     else:
-        raise SystemExit("usage: python run_model.py train|test|finetune|distill|datastore")
+        raise SystemExit("usage: python run_model.py train|test|finetune|distill|datastore|kd-targets")

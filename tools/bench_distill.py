@@ -2,7 +2,8 @@
 """Knowledge distillation (fira_icse_b200.distill) on one GPU: time per step split into its parts, next to the plain
 eager MLE step, and the two loss kernels against the NLL kernels on the same rows.
 
-    python tools/bench_distill.py [--batch 64] [--members 1 2 4] [--steps 10] [--warmup 3] [--json out.json]
+    python tools/bench_distill.py [--batch 64] [--members 1 2 4] [--steps 10] [--warmup 3] [--topk 8 32]
+                                  [--json out.json]
 
 Step: synthetic commits (fira_icse_b200.synth), B = --batch, fp32 and bf16; the teacher is M copies of the seeded model,
 each but the first with the seeded perturbation of tools/bench_beam.py --ensemble.  CUDA events around the teacher's
@@ -15,6 +16,11 @@ same rows (the batch's shifted labels), replayed from a CUDA graph over buffer s
 the teacher row (V 4 + S 4) twice; the kd backward reads each once and writes V s + S 4 + 8; the NLL forward reads the
 one softmax the label lives in, the NLL backward reads it and writes both gradient rows; both backward kernels also
 write zero gradient rows for the rows without a loss.  Share of the 3,350 GB/s data-sheet peak.
+--topk K...: offline distillation with stored top-K targets (distill.KDTargets), per precision and K: the step with
+SparseTargets (student forward + backward, FlatAdam; no teacher), fira_pointer_mix_topk per launch on the M = 1 teacher's
+triple, the sparse kernels next to the dense kd and NLL kernels on the same rows (the sparse forward reads the student
+row once and the targets, 8 K bytes per row; the backward reads it once and writes the gradient rows), the targets'
+production rate (teacher forward + combine + top-K, commits/s), stored bytes per commit and the mean kept teacher mass.
 One JSON object on stdout, with the card name and power limit read in the same run."""
 import argparse
 import copy
@@ -198,12 +204,121 @@ def kernel_times(m, batch, targets):
     return out
 
 
+def sparse_times(m, opt, batch, targets, k, steps, warmup):
+    """offline distillation at top-k: step parts, kernel µs per launch, rate and bytes of the stored targets"""
+    import bench
+    from fira_icse_b200 import distill, ops
+    from fira_icse_b200._lib import call
+    label = m.shifted_label(batch[6])
+    B, T = label.shape
+    sou, _, _, _, _, _, _, sub_token = batch
+    mm = torch.cat((sou != 0, sub_token != 0), 1).to(torch.uint8).contiguous()
+    S, V, R = mm.shape[1], m.vocab_size, B * T
+    lab = label.to(torch.int32).contiguous().view(-1)
+    tl, tp, mass = distill.topk_targets(targets, mm, label, V, k)
+    sparse = distill.SparseTargets(tl, tp)
+    parts = []
+    for i in range(warmup + steps):
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+        ev[0].record()
+        m.train()
+        opt.zero_grad()
+        loss, _, _ = distill.distill_loss(m, batch, sparse, label, 0.5)
+        (loss / (label != 0).sum()).backward()
+        ev[1].record()
+        opt.step()
+        distill.bump_weights(m)
+        ev[2].record()
+        torch.cuda.synchronize()
+        if i >= warmup:
+            parts.append([ev[0].elapsed_time(ev[1]), ev[1].elapsed_time(ev[2])])
+    med = [statistics.median(x[j] for x in parts) for j in range(2)]
+    # the kernels on the student's head products of this batch
+    bf16 = m.precision == "bf16"
+    with torch.no_grad():
+        m.eval()
+        memory = m.encoder.encode_memory(*(batch[i] for i in (0, 3, 4, 5, 7)))
+        mem_mask = mm != 0
+        dec = m.decoder(batch[1], memory, mem_mask, batch[1] != 0)
+        pr = ops.Prec(bf16)
+        dec2 = dec.contiguous().to(pr.tdt).view(R, ops.D)
+        lg, _, _, sc, gl = ops.head_products(pr, memory.contiguous().to(pr.tdt).view(-1, ops.D), dec2,
+                                             dec2.float() if bf16 else dec2, dec2, R, m.out_fc.weight, m.out_fc.bias,
+                                             *m.copy_net.flat_params(), B, T, S, mm, (lab != 0).to(torch.uint8))
+    s = 2 if bf16 else 4
+    ld = lg.shape[1]
+    n_rot = max(2, -(-2 * L2_BYTES // (R * ld * 2 * s + R * S * 8)))
+    f32 = dict(dtype=torch.float32, device=lg.device)
+    sets = [dict(lg=lg.clone(), dl=torch.empty_like(lg), dsc=torch.empty((B, T, S), **f32),
+                 st=torch.empty((R, 10), **f32), o=torch.empty((R, 3), **f32)) for _ in range(n_rot)]
+    u = torch.ones(1, **f32)
+    p, code = ops._ptr, pr.code
+    dgl, act = torch.empty((R, 2), **f32), torch.empty(R, dtype=torch.uint8, device=lg.device)
+
+    def fwd(i):
+        z = sets[i % n_rot]
+        call("fira_pointer_mix_kd_sparse_fwd", p(z["lg"]), ld, p(sc), p(gl), p(mm), p(lab), p(tl), p(tp), k, 0.5,
+             p(z["st"]), p(z["o"]), p(z["o"], R), p(z["o"], 2 * R), R, T, V, S, code, ops._stream())
+
+    def bwd(i):
+        z = sets[i % n_rot]
+        call("fira_pointer_mix_kd_sparse_bwd", p(z["lg"]), ld, p(sc), p(mm), p(lab), p(tl), p(tp), k, 0.5, p(z["st"]),
+             p(u), p(z["dl"]), p(z["dsc"]), p(dgl), p(act), R, T, V, S, code, ops._stream())
+
+    tx, tsc, tgl = targets
+    outs = [(torch.empty((R, k), dtype=torch.int32, device=lg.device), torch.empty((R, k), **f32),
+             torch.empty(R, **f32), tx.clone()) for _ in range(max(2, -(-2 * L2_BYTES // (R * ld * 4))))]
+
+    def topk(i):
+        a, b, c, x = outs[i % len(outs)]
+        call("fira_pointer_mix_topk", p(x), ld, p(tsc), p(tgl), p(mm), p(lab), k, p(a), p(b), p(c), R, T, V, S,
+             ops._stream())
+
+    y = lab.long()
+    n_loss = int((y != 0).sum())
+    zero = (R - n_loss) * (V * s + S * 4 + 8)
+    row = V * s + S * 4
+    bytes_ = {"sparse_fwd": (row + 8 * k) * n_loss, "sparse_bwd": (2 * row + 8 + 8 * k) * n_loss + zero,
+              "topk": (V * 4 + S * 4 + 8 * k) * n_loss}
+    kern = {}
+    for i in range(n_rot):
+        fwd(i)
+    for name, fn, n in (("sparse_fwd", fwd, n_rot), ("sparse_bwd", bwd, n_rot), ("topk", topk, len(outs))):
+        _, med_ms, _ = bench.time_launches(fn, n)
+        kern[name] = {"us": med_ms * 1e3, "bytes": bytes_[name], "GB_s": bytes_[name] / (med_ms * 1e-3) / 1e9,
+                      "share_of_peak": bytes_[name] / (med_ms * 1e-3) / 1e9 / PEAK_GBS}
+    live = y != 0
+    per_commit = (n_loss * (2 + 4 + 8 * k + 4) + 8 * B) / B
+    return {"ms": {"student_forward_backward": med[0], "adam": med[1]}, "ms_step": statistics.median(sum(x) for x in
+            parts), "kernels": kern, "bytes_per_commit": per_commit,
+            "mean_kept_mass": float(mass[live].double().mean())}
+
+
+def targets_rate(ens, batch, k, steps):
+    """commits/s of teacher_targets + fira_pointer_mix_topk (what `run_model.py kd-targets` runs per batch)"""
+    from fira_icse_b200 import distill
+    m = ens.models[0]
+    label = m.shifted_label(batch[6])
+    mm = torch.cat((batch[0] != 0, batch[7] != 0), 1).to(torch.uint8).contiguous()
+    times = []
+    for i in range(steps + 1):
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+        ev[0].record()
+        distill.topk_targets(distill.teacher_targets(ens, batch, label), mm, label, m.vocab_size, k)
+        ev[1].record()
+        torch.cuda.synchronize()
+        if i:
+            times.append(ev[0].elapsed_time(ev[1]))
+    return batch[0].shape[0] / (statistics.median(times) * 1e-3)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=64)
     ap.add_argument("--members", type=int, nargs="+", default=[1, 2, 4])
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--topk", type=int, nargs="*", default=[], help="stored top-k targets at these k")
     ap.add_argument("--json", default=None, help="also write the result here")
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -230,6 +345,12 @@ def main():
                    "ms_step": statistics.median(steps), "ms_mle_step": statistics.median(mle)}
             if M == args.members[0]:
                 row["kernels"] = kernel_times(m, batch, targets)
+            if M == 1:
+                row["topk"] = {}
+                for k in args.topk:
+                    r = sparse_times(m, opt, batch, targets, k, args.steps, args.warmup)
+                    r["kd_targets_commits_s"] = targets_rate(ens, batch, k, args.steps)
+                    row["topk"][k] = r
             rows.append(row)
             print(json.dumps(row), file=sys.stderr, flush=True)
             del m, opt, ens, targets
