@@ -6,18 +6,24 @@
 //   m  = b1 m + (1 - b1) g' ;  v = b2 v + (1 - b2) g'^2
 //   p -= lr / (1 - b1^t) * m / (sqrt(v) / sqrt(1 - b2^t) + eps)          t = *step (device scalar, already incremented)
 //   p16 = bf16(p)                              (the GEMM-operand mirror of the throughput mode; may be NULL)
+//   e   = fma(d, e, fl(c * p))                 (ema: exponential moving average of the stored p, may be NULL;
+//                                               c = fl(1 - d), fl() = fp32 rounding, fma = one rounding)
 //
-// Memory-bound: 16 B read + 12 B written per parameter (+ 2 B mirror); 8 parameters per thread, 16-byte accesses.
+// Memory-bound: 16 B read + 12 B written per parameter + 2 B mirror = 30 B; with ema 20 B read + 16 B written + 2 B = 38 B.
+// 8 parameters per thread, 16-byte accesses.  The EMA is a second instantiation of the kernel: the Adam arithmetic of
+// both is the same source, so p, m, v and the mirror do not depend on whether ema is set.
 #include "common.cuh"
 #include "fira_b200.h"
 
 namespace {
 
+template <bool EMA>
 __global__ void __launch_bounds__(256) adam_flat_kernel(float* __restrict__ p, const float* __restrict__ g,
                                                         float* __restrict__ m, float* __restrict__ v,
-                                                        __nv_bfloat16* __restrict__ p16, long n8, float lr, float b1,
-                                                        float b2, float eps, const float* __restrict__ step,
-                                                        const float* __restrict__ grad_scale) {
+                                                        __nv_bfloat16* __restrict__ p16, float* __restrict__ ema,
+                                                        long n8, float lr, float b1, float b2, float eps,
+                                                        const float* __restrict__ step,
+                                                        const float* __restrict__ grad_scale, float ema_decay) {
   pdl_wait(); pdl_trigger();       // PDL (common.cuh)
   const float t = *step;
   const float bc1 = 1.f - powf(b1, t), bc2 = 1.f - powf(b2, t);
@@ -41,6 +47,14 @@ __global__ void __launch_bounds__(256) adam_flat_kernel(float* __restrict__ p, c
     Act<float>::store8(m + i * 8, mv);
     Act<float>::store8(v + i * 8, vv);
     if (p16) Act<__nv_bfloat16>::store8(p16 + i * 8, pv);
+    if constexpr (EMA) {
+      const float c = 1.f - ema_decay;
+      float ev[8];
+      Act<float>::load8(ema + i * 8, ev);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) ev[j] = __fmaf_rn(ema_decay, ev[j], __fmul_rn(c, pv[j]));
+      Act<float>::store8(ema + i * 8, ev);
+    }
   }
 }
 
@@ -64,13 +78,20 @@ int grid_for(long n8) {
 extern "C" {
 
 int fira_adam_flat(float* p, const float* g, float* m, float* v, void* p_bf16, long n, float lr, float beta1, float beta2,
-                   float eps, const float* step, const float* grad_scale, void* stream) {
+                   float eps, const float* step, const float* grad_scale, float* ema, float ema_decay, void* stream) {
   FIRA_CHECK_ARG(p && g && m && v && step, FIRA_ERR_ARG, "adam_flat: null argument");
   FIRA_CHECK_ARG(n > 0 && n % 8 == 0, FIRA_ERR_SHAPE, "adam_flat: n %ld must be a positive multiple of 8", n);
-  FIRA_CHECK_ARG(fira_aligned16(p) && fira_aligned16(g) && fira_aligned16(m) && fira_aligned16(v) && fira_aligned16(p_bf16),
-                 FIRA_ERR_ALIGN, "adam_flat: 16-B alignment");
-  launch_k(adam_flat_kernel, dim3(grid_for(n / 8)), dim3(256), 0, (cudaStream_t)stream, p, g, m, v, (__nv_bfloat16*)p_bf16,
-           n / 8, lr, beta1, beta2, eps, step, grad_scale);
+  FIRA_CHECK_ARG(fira_aligned16(p) && fira_aligned16(g) && fira_aligned16(m) && fira_aligned16(v) && fira_aligned16(p_bf16) &&
+                 fira_aligned16(ema), FIRA_ERR_ALIGN, "adam_flat: 16-B alignment");
+  if (ema) {
+    FIRA_CHECK_ARG(ema_decay > 0.f && ema_decay < 1.f, FIRA_ERR_ARG,       // NaN fails both comparisons
+                   "adam_flat: ema_decay %g must be a finite number in (0, 1)", (double)ema_decay);
+    launch_k(adam_flat_kernel<true>, dim3(grid_for(n / 8)), dim3(256), 0, (cudaStream_t)stream, p, g, m, v,
+             (__nv_bfloat16*)p_bf16, ema, n / 8, lr, beta1, beta2, eps, step, grad_scale, ema_decay);
+  } else {
+    launch_k(adam_flat_kernel<false>, dim3(grid_for(n / 8)), dim3(256), 0, (cudaStream_t)stream, p, g, m, v,
+             (__nv_bfloat16*)p_bf16, (float*)nullptr, n / 8, lr, beta1, beta2, eps, step, grad_scale, 0.f);
+  }
   FIRA_CHECK_LAUNCH("fira_adam_flat");
   return FIRA_OK;
 }

@@ -20,6 +20,9 @@ optimizer inside the graph or right after the replay), so all of them capture in
 memory is the maximum over the shapes, not the sum (FIRA_GRAPH_PRIVATE_POOLS=1 gives each graph its own).
 N > 1: forward/backward graph, eager NCCL all-reduce of ONE flat gradient buffer, optimizer graph
 (same numerics as parallel.DataParallelStep).
+An optimizer factory that builds optim.FlatAdam(..., ema_decay=d) gets the weights' moving average in every mode: each
+captured optimizer step is a fira_adam_flat launch, which updates the EMA too.  `ema_model()` is the EMA as a model;
+every replay marks it stale.  Under data parallelism every rank updates the same EMA from the same parameters.
 """
 import os
 
@@ -128,6 +131,7 @@ class GraphedTrainStep:
         self.graph_opt = None
         self.static_flat = None
         self.pool = None                     # graph memory pool shared by every captured shape
+        self._ema = None                     # optim.ema_model of the optimizers, built by ema_model()
 
     def _note_optimizers(self):
         """optim.FlatAdam instances own the parameters' storage, their flat gradient buffers and the bf16 mirror"""
@@ -135,6 +139,22 @@ class GraphedTrainStep:
         self.flat_optims = [o for o in opts if isinstance(o, FlatAdam)]
         if self.flat_optims:
             _optim.attach(self.model, self.flat_optims)
+
+    def ema_model(self):
+        """The moving average of the weights kept by the optimizers (FlatAdam with ema_decay) as a TransModel in eval mode
+        (optim.ema_model), built once: its parameters are views of the EMA buffers, so it follows every step.  The
+        optimizers exist after the first step(), not before."""
+        if self._ema is None:
+            if not self.opt_ready:
+                raise RuntimeError("GraphedTrainStep.ema_model: the optimizers exist after the first step()")
+            self._ema = _optim.ema_model(self.model, self.flat_optims)
+        return self._ema
+
+    def _ema_moved(self):
+        """a replay moved the EMA behind Python's back: the shadow model's bf16 mirror and weight caches are stale"""
+        for o in self.flat_optims:
+            if o.ema is not None:
+                o.ema_moved()
 
     def _cap_stream(self):
         """Capture stream of the step graphs: HIGH priority, so that the kernels of the main chain (the critical path:
@@ -439,6 +459,7 @@ class GraphedTrainStep:
         if self.split:
             self._replay_split(c)
             self.model.decoder.weights_epoch = getattr(self.model.decoder, "weights_epoch", 0) + 1
+            self._ema_moved()
             return self.loss_sum, self.n_local
         c.graph.replay()
         # graph replays update the parameters without touching their autograd version counters: tell weight caches
@@ -448,4 +469,5 @@ class GraphedTrainStep:
             torch.cat([g.reshape(-1) for g in c.grads], out=self.static_flat)
             dist.all_reduce(self.static_flat, group=self.group)
             self.graph_opt.replay()
+        self._ema_moved()
         return self.loss_sum, self.n_local

@@ -10,6 +10,7 @@ fira_icse_b200.graph.PackedEdges (what the packed loader emits).  Sub-modules `e
 requires (run_model.py:204,256,257,259).
 """
 import os
+from types import SimpleNamespace
 
 import torch
 import torch.nn as nn
@@ -54,6 +55,12 @@ class TransModel(nn.Module):
 
     def __init__(self, args):
         super().__init__()
+        # the constructor arguments as a plain attribute (no state_dict entry; a namespace, so deepcopy and pickle work
+        # whatever type the caller used): optim.ema_model builds a twin from them.  Attributes win over mapping keys:
+        # run_model.py's DotDict gets vocab_size by attribute assignment after it was built
+        fields = dict(args) if isinstance(args, dict) else {}
+        fields.update(getattr(args, "__dict__", {}))
+        self.args = SimpleNamespace(**fields)
         self.embedding_dim = args.embedding_dim
         self.vocab_size = args.vocab_size
         self.sou_len = args.sou_len

@@ -115,10 +115,44 @@ def plan_layout(params, groups=()):
     return [offs[id(p)] for p in params], (off + ALIGN - 1) // ALIGN * ALIGN
 
 
-class FlatAdam:
-    """torch.optim.Adam(params, lr, betas, eps) on flat buffers; `step()` is one kernel launch (capturable)."""
+def check_ema_decay(d):
+    """d as a float; ValueError unless 0 < d < 1 (finite)"""
+    try:
+        d = float(d)
+    except (TypeError, ValueError):
+        raise ValueError(f"ema_decay must be a number in (0, 1), got {d!r}")
+    if not 0.0 < d < 1.0:
+        raise ValueError(f"ema_decay must be a number in (0, 1), got {d!r}")
+    return d
 
-    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, groups=()):
+
+class _EmaMirror:
+    """The EMA buffer of one FlatAdam as the owner of a shadow model's parameters (ema_model): `p` is the EMA, `p16` its
+    own bf16 mirror, refreshed on demand by ensure_fresh -- what mirror_of / cat_rows look up.  `moved()` marks the mirror
+    stale and bumps `decoder.weights_epoch` of every shadow model, so weight caches keyed on weights_key re-read."""
+
+    def __init__(self, opt):
+        self.p, self.n = opt.ema, opt.n
+        self.p16 = torch.zeros(self.n, dtype=torch.bfloat16, device=opt.ema.device)
+        self.fresh = False
+        self.direct = False                                   # never a gradient destination (grad_dest)
+        self.models = weakref.WeakSet()
+
+    def sync_mirror(self):
+        _lib.call("fira_cast_bf16", self.p.data_ptr(), self.p16.data_ptr(), self.n, torch.cuda.current_stream().cuda_stream)
+        self.fresh = True
+
+    def moved(self):
+        self.fresh = False
+        for m in self.models:
+            m.decoder.weights_epoch = getattr(m.decoder, "weights_epoch", 0) + 1
+
+
+class FlatAdam:
+    """torch.optim.Adam(params, lr, betas, eps) on flat buffers; `step()` is one kernel launch (capturable).
+    ema_decay: keep `ema`, the exponential moving average of the parameters, updated in the same launch (None = off)."""
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, groups=(), ema_decay=None):
         self.params = [p for p in params if p.requires_grad]
         if not self.params:
             raise ValueError("FlatAdam: no parameters")
@@ -146,6 +180,28 @@ class FlatAdam:
                 _SLOTS[(view.data_ptr(), p.numel())] = _Slot(self, o, p.numel())
         self.gviews = [self.g[o:o + p.numel()].view(p.shape) for p, o in zip(self.params, self.offsets)]
         self.sync_mirror()
+        self.ema_decay = None if ema_decay is None else check_ema_decay(ema_decay)
+        self.ema = None if ema_decay is None else torch.empty_like(self.p)
+        self._ema_mirror = None                               # created by ema_model
+        if self.ema is not None:
+            self.reset_ema()
+
+    def reset_ema(self):
+        """ema <- the parameters"""
+        self.ema.copy_(self.p)
+        self.ema_moved()
+
+    def ema_moved(self):
+        """The EMA moved (step(), a graph replay of a captured step(), load_state_dict): shadow models re-read it."""
+        if self._ema_mirror is not None:
+            self._ema_mirror.moved()
+
+    def ema_mirror(self):
+        if self.ema is None:
+            raise ValueError("FlatAdam: no EMA (built without ema_decay)")
+        if self._ema_mirror is None:
+            self._ema_mirror = _EmaMirror(self)
+        return self._ema_mirror
 
     def sync_mirror(self):
         """bf16 mirror <- parameters (after load_state_dict / any update that did not go through step())"""
@@ -187,16 +243,23 @@ class FlatAdam:
         _lib.call("fira_adam_flat", self.p.data_ptr(), self.g.data_ptr(), self.m.data_ptr(), self.v.data_ptr(),
                   self.p16.data_ptr(), self.n, self.lr, self.betas[0], self.betas[1], self.eps, self.step_t.data_ptr(),
                   self.grad_scale.data_ptr() if self.grad_scale is not None else None,
-                  torch.cuda.current_stream().cuda_stream)
+                  self.ema.data_ptr() if self.ema is not None else None,
+                  self.ema_decay if self.ema is not None else 0.0, torch.cuda.current_stream().cuda_stream)
         self.fresh = True
+        if self.ema is not None:
+            self.ema_moved()
 
     def _state_views(self, buf):
         return [buf[o:o + p.numel()].view(p.shape) for p, o in zip(self.params, self.offsets)]
 
     def state_dict(self):
-        return {"step": float(self.step_t.item()), "lr": self.lr, "betas": self.betas, "eps": self.eps,
-                "exp_avg": [t.clone() for t in self._state_views(self.m)],
-                "exp_avg_sq": [t.clone() for t in self._state_views(self.v)]}
+        sd = {"step": float(self.step_t.item()), "lr": self.lr, "betas": self.betas, "eps": self.eps,
+              "exp_avg": [t.clone() for t in self._state_views(self.m)],
+              "exp_avg_sq": [t.clone() for t in self._state_views(self.v)]}
+        if self.ema is not None:
+            sd["ema"] = [t.clone() for t in self._state_views(self.ema)]
+            sd["ema_decay"] = self.ema_decay
+        return sd
 
     def load_state_dict(self, sd):
         self.step_t.fill_(float(sd["step"]))
@@ -204,6 +267,11 @@ class FlatAdam:
             dst.copy_(src)
         for dst, src in zip(self._state_views(self.v), sd["exp_avg_sq"]):
             dst.copy_(src)
+        if self.ema is not None and "ema" in sd:
+            self.ema_decay = check_ema_decay(sd["ema_decay"])
+            for dst, src in zip(self._state_views(self.ema), sd["ema"]):
+                dst.copy_(src)
+            self.ema_moved()
 
 
 def attach(model, optims):
@@ -223,3 +291,46 @@ def ensure_fresh(model):
     for o in getattr(model, "_flat_optims", ()):
         if not o.fresh:
             o.sync_mirror()
+
+
+def ema_model(model, optims):
+    """The EMA weights of `optims` (FlatAdam instances built with ema_decay that own `model`'s live parameters: one, or
+    both halves of engine.GraphedTrainStep's pair) as a TransModel: built from `model.args`, in eval mode, no parameter
+    requires grad.  Its live parameters are zero-copy views of the EMA buffers -- they follow every step -- and its dead
+    parameters (and buffers) are copies of `model`'s.  state_dict() gives the reference's 338 keys, so torch.save of it
+    is a checkpoint like best_model.pt.  ValueError if a live parameter is owned by no optimizer with an EMA."""
+    from .model import TransModel
+    owned = [o for o in optims if isinstance(o, FlatAdam) and o.ema is not None]
+    dead = {id(p) for p in model.dead_parameters()}
+    homes = []                                                # per parameter: None (dead) or (optimizer, slot)
+    for name, p in model.named_parameters():
+        if id(p) in dead:
+            homes.append(None)
+            continue
+        o, s = _lookup(p)
+        if o is None or not any(o is x for x in owned):
+            raise ValueError(f"ema_model: live parameter {name} is owned by no optimizer with an EMA")
+        homes.append((o, s))
+    shadow = TransModel(model.args).to(model.out_fc.weight.device)
+    shadow.set_precision(model.precision)
+    mirrors = []
+    with torch.no_grad():
+        for home, p, q in zip(homes, model.parameters(), shadow.parameters()):
+            if home is None:
+                q.copy_(p)
+                continue
+            o, s = home
+            mirror = o.ema_mirror()
+            view = o.ema[s.off:s.off + s.numel].view(p.shape)
+            q.data = view
+            _SLOTS[(view.data_ptr(), s.numel)] = _Slot(mirror, s.off, s.numel)
+            if not any(mirror is x for x in mirrors):
+                mirrors.append(mirror)
+        for b, c in zip(model.buffers(), shadow.buffers()):
+            c.copy_(b)
+    shadow.eval()
+    shadow.requires_grad_(False)
+    for mirror in mirrors:
+        mirror.models.add(shadow)
+    attach(shadow, mirrors)
+    return shadow

@@ -157,9 +157,13 @@ int fira_colsum(const void* x, long ld, long M, int N, const float* row_weight, 
  *        g' = g / *grad_scale (grad_scale NULL -> 1);  m = b1 m + (1-b1) g';  v = b2 v + (1-b2) g'^2;
  *        p -= lr / (1 - b1^t) * m / (sqrt(v) / sqrt(1 - b2^t) + eps),  t = *step (device fp32 scalar, the caller has
  *        already incremented it);  p_bf16 (may be NULL) receives the bf16 copy of the updated parameters (the GEMM
- *        operands of the throughput mode).  n: multiple of 8; all buffers 16-byte aligned. */
+ *        operands of the throughput mode).  ema (may be NULL = off): an exponential moving average of the parameters,
+ *        updated from the fp32 p just stored, in this fp32 order:  c = fl(1 - ema_decay);  e = fma(ema_decay, e, fl(c p))
+ *        (fl = one fp32 rounding, fma = one rounding), 0 < ema_decay < 1.  p, m, v and p_bf16 are the same bits with
+ *        and without ema.  Bytes per parameter: 16 read + 12 written + 2 (p_bf16) = 30; with ema 20 + 16 + 2 = 38.
+ *        n: multiple of 8; all buffers 16-byte aligned. */
 int fira_adam_flat(float* p, const float* g, float* m, float* v, void* p_bf16, long n, float lr, float beta1, float beta2,
-                   float eps, const float* step, const float* grad_scale, void* stream);
+                   float eps, const float* step, const float* grad_scale, float* ema, float ema_decay, void* stream);
 /* y = bf16(x), n a multiple of 8 (refresh of the bf16 parameter mirror after parameters were set from outside). */
 int fira_cast_bf16(const float* x, void* y, long n, void* stream);
 

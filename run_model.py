@@ -16,6 +16,13 @@ beam search ranking.  Differences, all below the module surface:
     FIRA_MAX_BATCHES (smoke runs), FIRA_WORKERS, FIRA_PRECISION (fp32 parity mode | bf16 throughput mode),
     FIRA_MAX_SHAPES (bound on distinct trimmed batch shapes = captured graphs, default 24), FIRA_BUCKET (0 = the
     reference's uniform batching; K > 1 = size-bucketed batches within windows of K batches, see PackedBatchLoader).
+  * FIRA_EMA=d (`train`, default unset = off; 0 < d < 1, e.g. 0.999): keep an exponential moving average of the weights,
+    e = d e + (1 - d) p after every Adam step, updated inside the optimizer kernel (optim.FlatAdam, DESIGN.md §9).  Every
+    dev gate first scores and saves the trained weights as without it, then scores the EMA weights with the same dev()
+    and keeps their own best: best_model_ema.pt, OUTPUT/dev_output_ema and `ema epoch: ...` lines in
+    OUTPUT/train_process.  This doubles the time spent at dev gates.  `test`, `datastore`, `finetune` and `distill` read
+    the EMA checkpoint with FIRA_CHECKPOINT=best_model_ema.pt, a teacher or ensemble with FIRA_ENSEMBLE=best_model_ema.pt.
+    FIRA_ENGINE=eager (torch's fused Adam) with FIRA_EMA exits with an error.
   * `test` decoding: FIRA_DECODE=beam (default, the reference's beam search -> OUTPUT/output_fira) or sample (seeded
     sampling, fira_icse_b200.sample -> OUTPUT/output_fira_samples: FIRA_SAMPLES consecutive lines per commit in test
     order, `<log-probability>\\t<message>`; prints the mean sentence BLEU over all samples).  Sampling parameters:
@@ -246,7 +253,8 @@ def dev(model, dev_loader, g, valid_index, epoch, dev):
     return bleus / max(1, len(dev_loader.dataset)), out_str
 
 
-def train_epoch(dp, model, train_loader, epoch, best_bleu, dev_loader, g, valid_index, dev_):
+def train_epoch(dp, model, train_loader, epoch, best_bleu, dev_loader, g, valid_index, dev_, ema=None):
+    """ema: None, or {"best": best dev BLEU of the EMA weights so far} when FIRA_EMA is set (updated in place)"""
     model.train()
     graphed = isinstance(dp, GraphedTrainStep)
     total_data, total_loss = 0, (torch.zeros((), device=dev_) if graphed else 0.0)
@@ -263,6 +271,19 @@ def train_epoch(dp, model, train_loader, epoch, best_bleu, dev_loader, g, valid_
                     best_bleu = cur_bleu
                     torch.save(model.state_dict(), "best_model.pt")
                     open('OUTPUT/dev_output', 'w').write(output_str)
+                if ema is not None and dp.opt_ready:
+                    # the EMA weights, scored and kept on their own; building the shadow model and the dev loader's
+                    # iterator draw from torch's CPU generator, which also shuffles and seeds dropout: fork it, so
+                    # training goes on exactly as without FIRA_EMA
+                    with torch.random.fork_rng(devices=[]):
+                        shadow = dp.ema_model()
+                        ema_bleu, output_str = dev(shadow, dev_loader, g, valid_index, epoch, dev_)
+                    open('OUTPUT/train_process', 'a').write('ema epoch: {} batch: {} dev bleu: {} is better: {}\n'.format(
+                        epoch, idx, ema_bleu, ema_bleu > ema["best"]))
+                    if ema_bleu > ema["best"]:
+                        ema["best"] = ema_bleu
+                        torch.save(shadow.state_dict(), EMA_CHECKPOINT)
+                        open('OUTPUT/dev_output_ema', 'w').write(output_str)
             if WORLD > 1:
                 dist.barrier()
             model.train()
@@ -284,7 +305,27 @@ def n_train_total(train_loader):
     return len(train_loader.indices) if isinstance(train_loader, PackedBatchLoader) else len(train_loader.dataset)
 
 
+EMA_CHECKPOINT = "best_model_ema.pt"
+
+
+def ema_settings():
+    """FIRA_EMA -> the EMA decay, or None when unset; checked before any device work (SystemExit on an error)."""
+    spec = os.environ.get("FIRA_EMA", "")
+    if not spec:
+        return None
+    try:
+        d = float(spec)
+    except ValueError:
+        raise SystemExit(f"FIRA_EMA must be a number in (0, 1), got {spec!r}")
+    if not 0.0 < d < 1.0:
+        raise SystemExit(f"FIRA_EMA must be a number in (0, 1), got {spec!r}")
+    if os.environ.get("FIRA_ENGINE", "graph") != "graph":
+        raise SystemExit("FIRA_EMA is kept by the graph engine's flat Adam kernel: unset FIRA_ENGINE=eager")
+    return d
+
+
 def main_train():
+    ema_decay = ema_settings()
     dev_ = device()
     if WORLD > 1:
         dist.init_process_group("nccl", device_id=dev_)
@@ -307,16 +348,21 @@ def main_train():
                                          # the padded batches cut to the batch maximum
                                          packed=os.environ.get("FIRA_LAYOUT", "packed") == "packed")
         from fira_icse_b200.optim import FlatAdam
-        dp = GraphedTrainStep(model, args.batch_size, lambda ps: FlatAdam(ps, lr=args.lr, groups=model.flat_groups()),
+        dp = GraphedTrainStep(model, args.batch_size,
+                              lambda ps: FlatAdam(ps, lr=args.lr, groups=model.flat_groups(), ema_decay=ema_decay),
                               edge_capacity=train_loader.edge_cap)
     else:
         train_loader = loader(train_set, args.batch_size, True, list(range(lo, hi)) if WORLD > 1 else None)
         dp = DataParallelStep(model, lambda ps: Adam(ps, args.lr, fused=True))
     best_bleu = -1
+    ema = None if ema_decay is None else {"best": -1}
     for epoch in range(args.epoches):
-        best_bleu = train_epoch(dp, model, train_loader, epoch, best_bleu, dev_loader, g, all_index['valid'], dev_)
+        best_bleu = train_epoch(dp, model, train_loader, epoch, best_bleu, dev_loader, g, all_index['valid'], dev_, ema)
     if RANK == 0 and not os.path.exists("best_model.pt"):
         torch.save(model.state_dict(), "best_model.pt")             # short runs never reach the epoch-15 dev gate
+    if RANK == 0 and ema is not None and not os.path.exists(EMA_CHECKPOINT):
+        # as for best_model.pt; before the first step the average is the initial weights
+        torch.save((dp.ema_model() if dp.opt_ready else model).state_dict(), EMA_CHECKPOINT)
     if WORLD > 1:
         dist.destroy_process_group()
 
