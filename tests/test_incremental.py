@@ -2,8 +2,10 @@
 
 The product backend launches CUDA kernels; here a torch backend (test infrastructure, below) is injected so
 that the incremental evaluation -- token feeding, pad masks, cache writes, beam reordering -- can be compared
-with the oracle's full 30-position decoder without a GPU.  The kernels themselves are covered by
-tests/test_gpu_ops.py and the end-to-end id parity by tests/test_gpu_cli.py."""
+with the oracle's full 30-position decoder without a GPU.  The same path on the CUDA backend -- its kernels at the
+decoding shapes, strides and row paddings, captured graphs, weight refreshes, shared buffers and the position loop's
+head -- is checked against float64 by tests/test_gpu_incremental.py, and the end-to-end id parity by
+tests/test_gpu_cli.py."""
 import math
 
 import torch
