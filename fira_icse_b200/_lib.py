@@ -14,7 +14,7 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "fira_b200.h")
 FIRA_F32, FIRA_BF16 = 0, 1
 EDGE_F32, EDGE_BF16, EDGE_F64 = 0, 1, 2
 
-_SCALARS = {"int": ctypes.c_int, "long": ctypes.c_long, "float": ctypes.c_float,
+_SCALARS = {"int": ctypes.c_int, "long": ctypes.c_long, "float": ctypes.c_float, "double": ctypes.c_double,
             "uint64_t": ctypes.c_uint64, "uint32_t": ctypes.c_uint32}
 
 

@@ -23,6 +23,17 @@ N > 1: forward/backward graph, eager NCCL all-reduce of ONE flat gradient buffer
 An optimizer factory that builds optim.FlatAdam(..., ema_decay=d) gets the weights' moving average in every mode: each
 captured optimizer step is a fira_adam_flat launch, which updates the EMA too.  `ema_model()` is the EMA as a model;
 every replay marks it stale.  Under data parallelism every rank updates the same EMA from the same parameters.
+An optimizer factory that builds optim.FlatAdam(..., max_grad_norm=c) clips the gradient's global norm over BOTH halves
+of the optimizer pair (one optim.ClipGroup) and skips steps whose gradient is not finite, inside the captured work:
+  * overlap: the head/decoder half's sum of squares runs on the side stream while the encoder backward runs; after the
+    join, the encoder half's sum of squares, the finalize and both Adam launches (Adam can no longer hide behind the
+    encoder backward: it needs the whole norm);
+  * one optimizer (FIRA_OPT_OVERLAP=0, or N > 1 without the split): sum of squares -> finalize -> Adam, at the end of the
+    graph or in the optimizer graph after the all-reduce;
+  * split: half A's all-reduce and sum of squares still run behind graph B; half B's all-reduce is followed by its sum
+    of squares, the finalize and both Adam launches.
+`grad_norm`, `clipped` and `skipped` are the group's device scalars.  A skipped step changes no buffer and captures
+nothing new.
 """
 import os
 
@@ -81,6 +92,10 @@ class _OptimizerPair:
         self.pair = pair
 
     def step(self):
+        clip = getattr(self.pair[0], "clip", None)
+        if clip is not None:                         # one norm over both halves
+            clip.step()
+            return
         for o in self.pair:
             o.step()
 
@@ -149,6 +164,29 @@ class GraphedTrainStep:
                 raise RuntimeError("GraphedTrainStep.ema_model: the optimizers exist after the first step()")
             self._ema = _optim.ema_model(self.model, self.flat_optims)
         return self._ema
+
+    @property
+    def clip(self):
+        """the optim.ClipGroup of the optimizers (FlatAdam with max_grad_norm), or None (no clipping, or before the first
+        step() in the modes that build their optimizers then)"""
+        for o in self.flat_optims:
+            if o.clip is not None:
+                return o.clip
+        return None
+
+    @property
+    def grad_norm(self):
+        """device float64 scalar: the last step's global gradient norm (non-finite on a skipped step); None without
+        clipping"""
+        return None if self.clip is None else self.clip.grad_norm
+
+    @property
+    def clipped(self):
+        return None if self.clip is None else self.clip.clipped
+
+    @property
+    def skipped(self):
+        return None if self.clip is None else self.clip.skipped
 
     def _ema_moved(self):
         """a replay moved the EMA behind Python's back: the shadow model's bf16 mirror and weight caches are stale"""
@@ -294,11 +332,17 @@ class GraphedTrainStep:
             self._bind_flat(c, "a", self.params_a)
             self._bind_flat(c, "b", self.params_b)
             if self.graph_opt is None:
+                clip = self.clip
                 self.graph_opt = []
-                for o in self.opt_pair:
+                for k, o in enumerate(self.opt_pair):
                     g = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(g):
-                        o.step()
+                        if clip is None:
+                            o.step()
+                        else:                             # A: its sum of squares; B: its sum of squares + both Adams
+                            clip.sumsq(o)
+                            if k == len(self.opt_pair) - 1:
+                                clip.finish()
                     self.graph_opt.append(g)
             return
         if self.flat_a is None:
@@ -360,6 +404,8 @@ class GraphedTrainStep:
         self._phase_b()
         self.params_a, self.params_b = pa, pb
         self.opt_pair = (self.opt_factory(pa), self.opt_factory(pb))
+        if any(getattr(o, "max_grad_norm", None) is not None for o in self.opt_pair):
+            _optim.ClipGroup(self.opt_pair)            # one norm over both halves (ValueError unless both clip alike)
         self.optimizer = _OptimizerPair(self.opt_pair)
         self._note_optimizers()
         if self.opt_overlap:
@@ -406,14 +452,22 @@ class GraphedTrainStep:
             if self.world == 1 and self.opt_overlap:
                 # ONE graph, two branches: Adam on the head/decoder parameters (3/4 of the bytes, memory-bound, nothing
                 # else could hide it at the end of the step) runs on a side stream WHILE the encoder backward runs
+                clip = self.clip
                 self._phase_a(c)
                 cur = torch.cuda.current_stream()
                 self.opt_stream.wait_stream(cur)
                 with torch.cuda.stream(self.opt_stream):
-                    self.opt_pair[0].step()
+                    if clip is None:
+                        self.opt_pair[0].step()
+                    else:                                  # clipping: only this half's share of the norm runs here
+                        clip.sumsq(self.opt_pair[0])
                 self._phase_b()
                 cur.wait_stream(self.opt_stream)
-                self.opt_pair[1].step()
+                if clip is None:
+                    self.opt_pair[1].step()
+                else:
+                    clip.sumsq(self.opt_pair[1])
+                    clip.finish()
             else:
                 self._forward_backward(c)
                 if self.world == 1:

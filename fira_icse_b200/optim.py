@@ -11,6 +11,11 @@ One `fira_adam_flat` launch updates everything (csrc/optim.cu) and refreshes the
     concatenated weights of the fused projections plain views (`cat_rows`): no per-step `torch.cat`;
   * backward passes write parameter gradients straight into views of `g` (`grad_dest`), so neither the optimizer nor
     the data-parallel all-reduce needs a packing pass: the all-reduce runs on `g` itself.
+
+`max_grad_norm=c` clips the gradient's global norm before Adam (torch.nn.utils.clip_grad_norm_) and skips steps whose
+gradient is not finite, on the device (csrc/optim.cu): a float64 sum of squares per buffer, one finalize kernel, then
+the Adam launch scaled by the coefficient.  `ClipGroup(optims)` takes one norm over several instances (the two halves
+of engine.GraphedTrainStep's pair); a FlatAdam alone is a group of one.
 """
 import weakref
 
@@ -126,6 +131,90 @@ def check_ema_decay(d):
     return d
 
 
+def check_max_grad_norm(c):
+    """c as a float; ValueError unless 0 < c <= inf (inf: the norm is monitored and non-finite steps are skipped, but
+    no step is clipped)"""
+    try:
+        c = float(c)
+    except (TypeError, ValueError):
+        raise ValueError(f"max_grad_norm must be a positive number or inf, got {c!r}")
+    if not c > 0.0:                                          # NaN fails the comparison
+        raise ValueError(f"max_grad_norm must be a positive number or inf, got {c!r}")
+    return c
+
+
+CLIP_NORM, CLIP_COEF, CLIP_TAKEN, CLIP_CLIPPED, CLIP_SKIPPED = range(5)       # FIRA_CLIP_* (include/fira_b200.h)
+
+
+class ClipGroup:
+    """One global gradient norm over the FlatAdam instances `optims` (all built with the same max_grad_norm c).  Per step:
+    `sumsq(o)` for every member once its gradients are final (any order, any stream), then `finish()`: the finalize
+    kernel (norm, coefficient, skip flag, counters, every member's step counter) and every member's clipped Adam launch.
+    `step()` does all of it in one go.  `grad_norm`, `clipped` and `skipped` are device scalars (float64 views of the
+    state), read without a synchronisation inside the step.  Members must share `grad_scale` (or have none)."""
+
+    def __init__(self, optims):
+        optims = list(optims)
+        if not optims or not all(isinstance(o, FlatAdam) for o in optims):
+            raise ValueError("ClipGroup: needs FlatAdam instances")
+        cs = {o.max_grad_norm for o in optims}
+        if None in cs or len(cs) != 1:
+            raise ValueError(f"ClipGroup: every member needs the same max_grad_norm, got {[o.max_grad_norm for o in optims]}")
+        self.members = optims
+        self.max_grad_norm = cs.pop()
+        dev = optims[0].p.device
+        counts = [_lib.lib().fira_grad_sumsq_blocks(o.n) for o in optims]
+        self.partials = torch.zeros(sum(counts), dtype=torch.float64, device=dev)
+        self._slot, off = {}, 0
+        for o, k in zip(optims, counts):
+            self._slot[id(o)] = self.partials[off:off + k]
+            off += k
+        self.state = torch.tensor([0.0, 1.0, 1.0, 0.0, 0.0], dtype=torch.float64, device=dev)
+        # the members' step counters, advanced by the finalize kernel on a taken step only
+        self.steps = torch.tensor([o.step_t.data_ptr() for o in optims], dtype=torch.int64, device=dev)
+        for o in optims:
+            o.clip = self
+
+    @property
+    def grad_norm(self):
+        """the last step's gradient norm sqrt(sum g^2) / grad_scale (non-finite on a skipped step)"""
+        return self.state[CLIP_NORM]
+
+    @property
+    def clipped(self):
+        """steps whose gradient was scaled down (coefficient < 1)"""
+        return self.state[CLIP_CLIPPED]
+
+    @property
+    def skipped(self):
+        """steps skipped because the gradient was not finite"""
+        return self.state[CLIP_SKIPPED]
+
+    def sumsq(self, o):
+        """member o's gradients are final: gather them into its flat buffer and launch its sum of squares"""
+        o.gather_grads()
+        o.direct = False                                      # g now holds this step's gradients
+        slot = self._slot[id(o)]
+        _lib.call("fira_grad_sumsq", o.g.data_ptr(), o.n, slot.data_ptr(), torch.cuda.current_stream().cuda_stream)
+
+    def finish(self):
+        """every member's sumsq() is done (on this stream or joined into it): finalize, then every clipped Adam launch"""
+        scale = self.members[0].grad_scale
+        if any(o.grad_scale is not scale for o in self.members):
+            raise RuntimeError("ClipGroup: the members must share grad_scale")
+        stream = torch.cuda.current_stream().cuda_stream
+        _lib.call("fira_grad_clip_finalize", self.partials.data_ptr(), self.partials.numel(),
+                  scale.data_ptr() if scale is not None else None, self.max_grad_norm, self.state.data_ptr(),
+                  self.steps.data_ptr(), len(self.members), stream)
+        for o in self.members:
+            o._adam_clip(self.state)
+
+    def step(self):
+        for o in self.members:
+            self.sumsq(o)
+        self.finish()
+
+
 class _EmaMirror:
     """The EMA buffer of one FlatAdam as the owner of a shadow model's parameters (ema_model): `p` is the EMA, `p16` its
     own bf16 mirror, refreshed on demand by ensure_fresh -- what mirror_of / cat_rows look up.  `moved()` marks the mirror
@@ -150,9 +239,11 @@ class _EmaMirror:
 
 class FlatAdam:
     """torch.optim.Adam(params, lr, betas, eps) on flat buffers; `step()` is one kernel launch (capturable).
-    ema_decay: keep `ema`, the exponential moving average of the parameters, updated in the same launch (None = off)."""
+    ema_decay: keep `ema`, the exponential moving average of the parameters, updated in the same launch (None = off).
+    max_grad_norm: clip the gradient's global norm to it and skip non-finite steps (None = off; see ClipGroup): `step()`
+    is then three launches, and `clip` the group this instance belongs to."""
 
-    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, groups=(), ema_decay=None):
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, groups=(), ema_decay=None, max_grad_norm=None):
         self.params = [p for p in params if p.requires_grad]
         if not self.params:
             raise ValueError("FlatAdam: no parameters")
@@ -185,6 +276,10 @@ class FlatAdam:
         self._ema_mirror = None                               # created by ema_model
         if self.ema is not None:
             self.reset_ema()
+        self.max_grad_norm = None if max_grad_norm is None else check_max_grad_norm(max_grad_norm)
+        self.clip = None
+        if self.max_grad_norm is not None:
+            ClipGroup([self])
 
     def reset_ema(self):
         """ema <- the parameters"""
@@ -236,7 +331,35 @@ class FlatAdam:
             torch._foreach_copy_(dst, src)
         return len(src)
 
+    @property
+    def grad_norm(self):
+        return None if self.clip is None else self.clip.grad_norm
+
+    @property
+    def clipped(self):
+        return None if self.clip is None else self.clip.clipped
+
+    @property
+    def skipped(self):
+        return None if self.clip is None else self.clip.skipped
+
+    def _adam_clip(self, state):
+        _lib.call("fira_adam_flat_clip", self.p.data_ptr(), self.g.data_ptr(), self.m.data_ptr(), self.v.data_ptr(),
+                  self.p16.data_ptr(), self.n, self.lr, self.betas[0], self.betas[1], self.eps, self.step_t.data_ptr(),
+                  self.grad_scale.data_ptr() if self.grad_scale is not None else None,
+                  self.ema.data_ptr() if self.ema is not None else None,
+                  self.ema_decay if self.ema is not None else 0.0, state.data_ptr(),
+                  torch.cuda.current_stream().cuda_stream)
+        self.fresh = True
+        if self.ema is not None:
+            self.ema_moved()
+
     def step(self):
+        if self.clip is not None:
+            if len(self.clip.members) > 1:
+                raise RuntimeError("FlatAdam.step: this optimizer shares a ClipGroup; step the group")
+            self.clip.step()
+            return
         self.gather_grads()
         self.direct = False                                   # g now holds this step's gradients
         self.step_t.add_(1.0)

@@ -164,6 +164,36 @@ int fira_colsum(const void* x, long ld, long M, int N, const float* row_weight, 
  *        n: multiple of 8; all buffers 16-byte aligned. */
 int fira_adam_flat(float* p, const float* g, float* m, float* v, void* p_bf16, long n, float lr, float beta1, float beta2,
                    float eps, const float* step, const float* grad_scale, float* ema, float ema_decay, void* stream);
+/* ---- global-norm gradient clipping (torch.nn.utils.clip_grad_norm_ before the Adam step) over a group of flat
+ *      buffers, with a non-finite guard, in three launches that need no host synchronisation:
+ *        fira_grad_sumsq (per member)  ->  fira_grad_clip_finalize (once)  ->  fira_adam_flat_clip (per member).
+ *      The state `clip` is 5 doubles, indexed by FIRA_CLIP_*: the last norm, the fp32 coefficient (held as a double),
+ *      the taken flag (1 taken, 0 skipped) and the clipped / skipped step counts (exact integers). */
+#define FIRA_CLIP_NORM 0
+#define FIRA_CLIP_COEF 1
+#define FIRA_CLIP_TAKEN 2
+#define FIRA_CLIP_CLIPPED 3
+#define FIRA_CLIP_SKIPPED 4
+/* The number of float64 partials fira_grad_sumsq writes for n elements (a function of n alone, at most 1024), or 0 if
+ * n is not a positive multiple of 8. */
+int fira_grad_sumsq_blocks(long n);
+/* partials[b] = sum of g[i]^2 over CTA b's grid-stride share of g, accumulated in float64 (the squares of fp32 values
+ * are exact in float64, so values above ~1.8e19 do not overflow).  The grid and the order of every sum depend on n
+ * alone.  4 B read per element.  n: multiple of 8; g 16-byte aligned. */
+int fira_grad_sumsq(const float* g, long n, double* partials, void* stream);
+/* One CTA: S = sum of partials[0 .. n_partials) in a fixed order (the members' partials back to back);
+ * clip[NORM] = sqrt(S) / s, s = *grad_scale (NULL -> 1).  S not finite: clip[TAKEN] = 0, clip[SKIPPED] += 1 and nothing
+ * else changes.  Otherwise clip[COEF] = fl32(min(1, max_norm / (norm + 1e-6))) (computed in float64), clip[TAKEN] = 1,
+ * clip[CLIPPED] += 1 if coef < 1, and *steps[k] += 1 for each of the n_steps step counters (a device array of device
+ * pointers: every member's Adam step count advances only on a taken step).  max_norm > 0; inf never clips. */
+int fira_grad_clip_finalize(const double* partials, long n_partials, const float* grad_scale, double max_norm,
+                            double* clip, float* const* steps, int n_steps, void* stream);
+/* fira_adam_flat with g' = fl(fl(g / s) * coef), coef = clip[COEF]; a skipped step (clip[TAKEN] == 0) writes nothing.
+ * With coef == 1 every output is the same bits as fira_adam_flat's.  Same arguments and bytes otherwise; clip 8-byte
+ * aligned. */
+int fira_adam_flat_clip(float* p, const float* g, float* m, float* v, void* p_bf16, long n, float lr, float beta1,
+                        float beta2, float eps, const float* step, const float* grad_scale, float* ema, float ema_decay,
+                        const double* clip, void* stream);
 /* y = bf16(x), n a multiple of 8 (refresh of the bf16 parameter mirror after parameters were set from outside). */
 int fira_cast_bf16(const float* x, void* y, long n, void* stream);
 

@@ -23,6 +23,11 @@ beam search ranking.  Differences, all below the module surface:
     OUTPUT/train_process.  This doubles the time spent at dev gates.  `test`, `datastore`, `finetune` and `distill` read
     the EMA checkpoint with FIRA_CHECKPOINT=best_model_ema.pt, a teacher or ensemble with FIRA_ENSEMBLE=best_model_ema.pt.
     FIRA_ENGINE=eager (torch's fused Adam) with FIRA_EMA exits with an error.
+  * FIRA_CLIP_NORM=c (`train`, `finetune` and `distill`; default unset = off; a positive number or inf): clip the
+    gradient's global norm to c before every Adam step (torch.nn.utils.clip_grad_norm_'s rule) and skip steps whose
+    gradient is not finite, on the device (optim.FlatAdam(max_grad_norm), DESIGN.md §9); inf only monitors the norm and
+    skips non-finite steps.  The 10-batch progress line then also prints the window's mean gradient norm and the
+    clipped / skipped step counts.  Bad values, and FIRA_ENGINE=eager in `train`, exit with an error.
   * `test` decoding: FIRA_DECODE=beam (default, the reference's beam search -> OUTPUT/output_fira) or sample (seeded
     sampling, fira_icse_b200.sample -> OUTPUT/output_fira_samples: FIRA_SAMPLES consecutive lines per commit in test
     order, `<log-probability>\\t<message>`; prints the mean sentence BLEU over all samples).  Sampling parameters:
@@ -253,8 +258,32 @@ def dev(model, dev_loader, g, valid_index, epoch, dev):
     return bleus / max(1, len(dev_loader.dataset)), out_str
 
 
-def train_epoch(dp, model, train_loader, epoch, best_bleu, dev_loader, g, valid_index, dev_, ema=None):
-    """ema: None, or {"best": best dev BLEU of the EMA weights so far} when FIRA_EMA is set (updated in place)"""
+class ClipLog:
+    """The gradient fields of the 10-batch progress line under FIRA_CLIP_NORM: the window's mean norm, summed on the
+    device after every step, and the clipped / skipped step counts, all read where the line reads the loss.
+    `group()` returns the optim.ClipGroup, or None before it exists."""
+
+    def __init__(self, group):
+        self.group, self.sum, self.n = group, None, 0
+
+    def add(self):
+        c = self.group()
+        if c is not None:
+            self.sum = c.grad_norm.clone() if self.sum is None else self.sum + c.grad_norm
+            self.n += 1
+
+    def text(self):
+        c = self.group()
+        if c is None:
+            return ""
+        mean = float(self.sum) / self.n if self.n else float("nan")
+        self.sum, self.n = None, 0
+        return " grad_norm: %.4f clipped: %d skipped: %d" % (mean, int(c.clipped.item()), int(c.skipped.item()))
+
+
+def train_epoch(dp, model, train_loader, epoch, best_bleu, dev_loader, g, valid_index, dev_, ema=None, clip_log=None):
+    """ema: None, or {"best": best dev BLEU of the EMA weights so far} when FIRA_EMA is set (updated in place);
+    clip_log: a ClipLog when FIRA_CLIP_NORM is set"""
     model.train()
     graphed = isinstance(dp, GraphedTrainStep)
     total_data, total_loss = 0, (torch.zeros((), device=dev_) if graphed else 0.0)
@@ -294,9 +323,12 @@ def train_epoch(dp, model, train_loader, epoch, best_bleu, dev_loader, g, valid_
             loss, _ = dp.step(batch_to_device(batch, dev_))
             total_loss += loss.item()
         total_data += (batch.B if hasattr(batch, "shape_key") else len(batch[0])) * WORLD
+        if clip_log is not None:
+            clip_log.add()
         if idx % 10 == 0 and RANK == 0:
             print("epoch: %d batch: %d/%d  data: %d/%d loss: %.4f" % (
-                epoch, idx, len(train_loader), total_data, n_train_total(train_loader) * WORLD, float(total_loss) / 10))
+                epoch, idx, len(train_loader), total_data, n_train_total(train_loader) * WORLD, float(total_loss) / 10)
+                + (clip_log.text() if clip_log is not None else ""))
             total_loss = torch.zeros((), device=dev_) if graphed else 0.0
     return best_bleu
 
@@ -324,7 +356,25 @@ def ema_settings():
     return d
 
 
+def clip_settings(engine_checked=False):
+    """FIRA_CLIP_NORM -> the clipping threshold (a positive float, inf allowed), or None when unset; checked before any
+    device work (SystemExit on an error).  engine_checked: `train`, where clipping needs the graph engine."""
+    spec = os.environ.get("FIRA_CLIP_NORM", "")
+    if not spec:
+        return None
+    try:
+        c = float(spec)
+    except ValueError:
+        raise SystemExit(f"FIRA_CLIP_NORM must be a positive number or inf, got {spec!r}")
+    if not c > 0.0:                                              # NaN fails the comparison
+        raise SystemExit(f"FIRA_CLIP_NORM must be a positive number or inf, got {spec!r}")
+    if engine_checked and os.environ.get("FIRA_ENGINE", "graph") != "graph":
+        raise SystemExit("FIRA_CLIP_NORM is applied by the graph engine's flat Adam kernels: unset FIRA_ENGINE=eager")
+    return c
+
+
 def main_train():
+    max_grad_norm = clip_settings(engine_checked=True)
     ema_decay = ema_settings()
     dev_ = device()
     if WORLD > 1:
@@ -349,15 +399,18 @@ def main_train():
                                          packed=os.environ.get("FIRA_LAYOUT", "packed") == "packed")
         from fira_icse_b200.optim import FlatAdam
         dp = GraphedTrainStep(model, args.batch_size,
-                              lambda ps: FlatAdam(ps, lr=args.lr, groups=model.flat_groups(), ema_decay=ema_decay),
+                              lambda ps: FlatAdam(ps, lr=args.lr, groups=model.flat_groups(), ema_decay=ema_decay,
+                                                  max_grad_norm=max_grad_norm),
                               edge_capacity=train_loader.edge_cap)
     else:
         train_loader = loader(train_set, args.batch_size, True, list(range(lo, hi)) if WORLD > 1 else None)
         dp = DataParallelStep(model, lambda ps: Adam(ps, args.lr, fused=True))
     best_bleu = -1
     ema = None if ema_decay is None else {"best": -1}
+    clip_log = None if max_grad_norm is None else ClipLog(lambda: dp.clip)
     for epoch in range(args.epoches):
-        best_bleu = train_epoch(dp, model, train_loader, epoch, best_bleu, dev_loader, g, all_index['valid'], dev_, ema)
+        best_bleu = train_epoch(dp, model, train_loader, epoch, best_bleu, dev_loader, g, all_index['valid'], dev_, ema,
+                                clip_log)
     if RANK == 0 and not os.path.exists("best_model.pt"):
         torch.save(model.state_dict(), "best_model.pt")             # short runs never reach the epoch-15 dev gate
     if RANK == 0 and ema is not None and not os.path.exists(EMA_CHECKPOINT):
@@ -602,6 +655,7 @@ def finetune_settings():
 
 
 def main_finetune():
+    max_grad_norm = clip_settings()
     s, sampling = finetune_settings()
     dev_ = device()
     g = load_globals()
@@ -614,8 +668,9 @@ def main_finetune():
     model.load_state_dict(torch.load("best_model.pt", map_location="cpu"))
     model = model.to(dev_)
     from fira_icse_b200 import optim
-    opt = optim.FlatAdam(model.live_parameters(), lr=s["lr"], groups=model.flat_groups())
+    opt = optim.FlatAdam(model.live_parameters(), lr=s["lr"], groups=model.flat_groups(), max_grad_norm=max_grad_norm)
     optim.attach(model, [opt])
+    clip_log = None if max_grad_norm is None else ClipLog(lambda: opt.clip)
     train_loader = loader(train_set, args.batch_size, True)
     dev_loader = loader(dev_set, args.batch_size, False)
     max_batches = int(os.environ.get("FIRA_MAX_BATCHES", 0))
@@ -629,9 +684,12 @@ def main_finetune():
             step = scst_step(model, opt, b, **dict(sampling, seed=sampling["seed"] + epoch), first_index=total, **ids)
             rewards.append(step.reward)
             total += len(b[0])
+            if clip_log is not None:
+                clip_log.add()
             if idx % 10 == 0:
                 print("scst epoch: %d batch: %d/%d reward: %.4f |advantage|: %.4f loss: %.6f" % (
-                    epoch, idx, len(train_loader), sum(rewards) / len(rewards), step.advantage, step.loss))
+                    epoch, idx, len(train_loader), sum(rewards) / len(rewards), step.advantage, step.loss)
+                    + (clip_log.text() if clip_log is not None else ""))
                 rewards = []
         cur_bleu, output_str = dev(model, dev_loader, g, all_index['valid'], epoch, dev_)
         open('OUTPUT/train_process', 'a').write(
@@ -693,6 +751,7 @@ def load_targets(path, train_set):
 
 
 def main_distill():
+    max_grad_norm = clip_settings()
     s, student, teacher_spec = distill_settings()
     if isinstance(teacher_spec, str):
         g = load_globals()
@@ -710,8 +769,9 @@ def main_distill():
     model = load_model(student, dev_)
     teacher = Ensemble([load_model(p, dev_) for p in teacher_spec[0]], teacher_spec[1]) if targets is None else None
     from fira_icse_b200 import optim
-    opt = optim.FlatAdam(model.live_parameters(), lr=s["lr"], groups=model.flat_groups())
+    opt = optim.FlatAdam(model.live_parameters(), lr=s["lr"], groups=model.flat_groups(), max_grad_norm=max_grad_norm)
     optim.attach(model, [opt])
+    clip_log = None if max_grad_norm is None else ClipLog(lambda: opt.clip)
     train_loader = loader(train_set, args.batch_size, True) if targets is None else None
     dev_loader = loader(dev_set, args.batch_size, False)
     max_batches = int(os.environ.get("FIRA_MAX_BATCHES", 0))
@@ -727,9 +787,12 @@ def main_distill():
                 pos = perm[idx * args.batch_size: idx * args.batch_size + batch[6].shape[0]]
                 teacher = targets.batch(pos, TransModel.shifted_label(batch[6]), device=dev_)
             step = distill_step(model, opt, batch_to_device(batch, dev_), teacher, alpha=s["alpha"])
+            if clip_log is not None:
+                clip_log.add()
             if idx % 10 == 0:
                 print("kd epoch: %d batch: %d/%d loss: %.4f nll: %.4f kd: %.4f tokens: %d" % (
-                    epoch, idx, len(train_loader), step.loss, step.nll, step.kd, step.tokens))
+                    epoch, idx, len(train_loader), step.loss, step.nll, step.kd, step.tokens)
+                    + (clip_log.text() if clip_log is not None else ""))
         cur_bleu, output_str = dev(model, dev_loader, g, all_index['valid'], epoch, dev_)
         open('OUTPUT/train_process', 'a').write(
             'kd epoch: {} dev bleu: {} is better: {}\n'.format(epoch, cur_bleu, cur_bleu > best_bleu))
