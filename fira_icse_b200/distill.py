@@ -11,12 +11,12 @@ over its members, or one model's own):
     loss_r = (1 - alpha) nll_r + alpha kd_r,   step loss = sum_r loss_r / sum_r [y != 0]
 
 Where it runs: teacher_targets runs every teacher member's teacher-forced forward (encoder, decoder, the head's three
-products, ops.head_products) under no_grad in eval mode, then one fira_pointer_mix_ensemble launch with N = T turns
-the M triples into one fp32 triple whose mixture is t.  The student's head (ops.HeadFn with a teacher) forms the loss
-and its gradient through both softmaxes, the gate and the clamp in fira_pointer_mix_kd_fwd / _bwd (include/fira_b200.h),
-so the 25,020-wide distributions are never stored.  distill_step is the eager padded-batch path, as scst.scst_step:
-the kernels' dropout in the student, an eager optim.FlatAdam step and scst.bump_weights.  The teacher keeps M member
-triples and their fp32 average on the device, about (M s + 4) B T ld_logits bytes (s = 4 fp32, 2 bf16).
+products, ops.head_products) under no_grad in eval mode (member_triples), then one fira_pointer_mix_ensemble launch
+with N = T turns the M triples into one fp32 triple whose mixture is t (combine).  The student's head (ops.HeadFn with a
+teacher) forms the loss and its gradient through both softmaxes, the gate and the clamp in fira_pointer_mix_kd_fwd /
+_bwd (include/fira_b200.h), so the 25,020-wide distributions are never stored.  distill_step is the eager
+padded-batch path, as scst.scst_step: the kernels' dropout in the student and optim.eager_step.  The teacher keeps M
+member triples and their fp32 average on the device, about (M s + 4) B T ld_logits bytes (s = 4 fp32, 2 bf16).
 
 Offline distillation: the teacher is frozen and teacher-forced, so its distributions are the same every epoch.
 build_targets runs it once over a split and keeps, per loss row, its k most probable labels (fira_pointer_mix_topk:
@@ -41,7 +41,7 @@ from .ensemble import Ensemble, refuse
 from .knn import fingerprint
 from .model import TransModel
 from .modules import _i32, _u8
-from .scst import bump_weights
+from .ops import MAX_TOPK
 
 
 class Step(NamedTuple):
@@ -81,50 +81,57 @@ def teacher_members(teacher, student=None):
     return models, log_w
 
 
+@torch.no_grad()
+def member_triples(models, batch, label):
+    """Each model's teacher-forced head products for the padded batch (the 8-tuple of run_model.py) and its shifted
+    labels [B, T], in eval mode without autograd -> ([(logits [B*T, ld_logits] in the model's precision, copy scores
+    [B, T, S], gate logits [B*T, 2])], copy mask [B, S] uint8).  Leaves the models in eval mode.  Rows with label 0 are
+    not meaningful: no loss reads them."""
+    sou, tar, _, mark, ast_change, edge, _, sub_token = batch
+    B, T = label.shape
+    row_mask = _u8(label.to(models[0].out_fc.weight.device) != 0).view(-1)     # the rows a loss reads
+    triples = []
+    for m in models:
+        m.eval()
+        pf_head, memory, mem_mask, dec = m.teacher_forced(sou, tar, mark, ast_change, edge, sub_token)
+        mm = _u8(mem_mask)
+        pr = ops.head_prec(m.precision == "bf16", pf_head)
+        dec2 = dec.contiguous().to(pr.tdt).view(B * T, ops.D)
+        logits, _, _, sc, gl = ops.head_products(
+            pr, memory.contiguous().to(pr.tdt).view(-1, ops.D), dec2, dec2.float() if pr.bf16 else dec2, dec2, B * T,
+            m.out_fc.weight, m.out_fc.bias, *m.copy_net.flat_params(), B, T, mm.shape[1], mm, row_mask)
+        triples.append((logits, sc, gl))
+    return triples, mm
+
+
+def combine(triples, log_w, mem_mask, vocab_size):
+    """One fira_pointer_mix_ensemble launch (N = T): the M member triples of member_triples and their log weights ->
+    one fp32 triple (logits [B*T, ld_logits], copy scores [B, T, S], gate logits [B*T, 2]) whose mixture is the
+    weighted average of the members' distributions."""
+    logits, sc, _ = triples[0]
+    B, T, S = sc.shape
+    M, Mt, ld = len(triples), B * T, logits.shape[1]
+    f32 = dict(dtype=torch.float32, device=logits.device)
+    out, sc_out, gl_out = torch.empty((Mt, ld), **f32), torch.empty((B, T, S), **f32), torch.empty((Mt, 2), **f32)
+    lw = torch.tensor(log_w, **f32)
+    arrs = [(ctypes.c_void_p * M)(*[ops._ptr(t[k]) for t in triples]) for k in range(3)]
+    call("fira_pointer_mix_ensemble", ctypes.addressof(arrs[0]), ld, ctypes.addressof(arrs[1]),
+         ctypes.addressof(arrs[2]), M, ops._ptr(lw), ops._ptr(mem_mask), ops._ptr(out), ld, ops._ptr(sc_out),
+         ops._ptr(gl_out), B, T, vocab_size, S, FIRA_BF16 if logits.dtype == torch.bfloat16 else FIRA_F32,
+         ops._stream())
+    return out, sc_out, gl_out
+
+
 def teacher_targets(teacher, batch, label):
     """The teacher's fp32 triple for the padded batch (the 8-tuple of run_model.py) and its shifted labels [B, T]:
     (logits [B*T, ld_logits], copy scores [B, T, S], gate logits [B*T, 2]) whose mixture is the teacher's distribution
     at every position (a single model is an ensemble of one).  Leaves the members in eval mode.  Rows with label 0 are
     not meaningful: the loss never reads them."""
     models, log_w = teacher_members(teacher)
-    first = models[0]
-    dev = first.out_fc.weight.device
-    sou, tar, _, mark, ast_change, edge, _, sub_token = batch
-    sou, tar, mark, ast_change, sub_token = (t.to(dev) for t in (sou, tar, mark, ast_change, sub_token))
-    label = label.to(dev)
-    B, T = label.shape
-    mem_mask = torch.cat((sou != 0, sub_token != 0), dim=1)
-    S, V, Mt = mem_mask.shape[1], first.vocab_size, B * T
-    mm = _u8(mem_mask)
-    row_mask = _u8(label != 0).view(-1)                   # the rows a loss reads
-    triples = []
-    with torch.no_grad():
-        for m in models:
-            m.eval()
-            bf16 = m.precision == "bf16"
-            if bf16:
-                _optim.ensure_fresh(m)
-            memory = m.encoder.encode_memory(sou, mark, ast_change, edge, sub_token)
-            dec = m.decoder(tar, memory, mem_mask, tar != 0)
-            pr = ops.Prec(bf16)
-            dec2 = dec.contiguous().to(pr.tdt).view(Mt, ops.D)
-            logits, _, _, sc, gl = ops.head_products(
-                pr, memory.contiguous().to(pr.tdt).view(-1, ops.D), dec2, dec2.float() if bf16 else dec2, dec2, Mt,
-                m.out_fc.weight, m.out_fc.bias, *m.copy_net.flat_params(), B, T, S, mm, row_mask)
-            triples.append((logits, sc, gl))
-    M = len(models)
-    ld = triples[0][0].shape[1]
-    f32 = dict(dtype=torch.float32, device=dev)
-    out, sc_out, gl_out = torch.empty((Mt, ld), **f32), torch.empty((B, T, S), **f32), torch.empty((Mt, 2), **f32)
-    lw = torch.tensor(log_w, **f32)
-    arrs = [(ctypes.c_void_p * M)(*[ops._ptr(t[k]) for t in triples]) for k in range(3)]
-    call("fira_pointer_mix_ensemble", ctypes.addressof(arrs[0]), ld, ctypes.addressof(arrs[1]),
-         ctypes.addressof(arrs[2]), M, ops._ptr(lw), ops._ptr(mm), ops._ptr(out), ld, ops._ptr(sc_out),
-         ops._ptr(gl_out), B, T, V, S, FIRA_BF16 if first.precision == "bf16" else FIRA_F32, ops._stream())
-    return out, sc_out, gl_out
+    triples, mm = member_triples(models, batch, label)
+    return combine(triples, log_w, mm, models[0].vocab_size)
 
 
-MAX_TOPK = 64             # fira_pointer_mix_topk / fira_pointer_mix_kd_sparse_*
 FORMAT = "fira-kd-targets-1"
 
 
@@ -288,41 +295,14 @@ def distill_loss(model, batch, targets, label, alpha):
     """sum_r loss_r under autograd in the model's current mode -> (loss_sum, nll [B, T], kd [B*T]).  targets: the
     teacher's triple of teacher_targets, or the batch's SparseTargets; label: the shifted labels [B, T] on the model's
     device."""
-    m = model
-    dev = m.out_fc.weight.device
     sou, tar, _, mark, ast_change, edge, _, sub_token = batch
-    sou, tar, mark, ast_change, sub_token = (t.to(dev) for t in (sou, tar, mark, ast_change, sub_token))
-    bf16 = m.precision == "bf16"
-    if bf16:
-        _optim.ensure_fresh(m)
-    m.decoder.prefetch_weights()
-    pf_head = ops.prefetch_head(bf16, m.out_fc.weight, m.copy_net.LinearSource.weight, m.copy_net.LinearTarget.weight)
-    memory = m.encoder.encode_memory(sou, mark, ast_change, edge, sub_token)
-    mem_mask = torch.cat((sou != 0, sub_token != 0), dim=1)
-    dec = m.decoder(tar, memory, mem_mask, tar != 0)
-    kd = torch.empty(label.numel(), dtype=torch.float32, device=dev)
+    head_in = model.teacher_forced(sou, tar, mark, ast_change, edge, sub_token)
+    kd = torch.empty(label.numel(), dtype=torch.float32, device=label.device)
     if isinstance(targets, SparseTargets):
-        dense, sparse = None, (targets.t_label, targets.t_prob, float(alpha), kd)
+        loss, nll, _ = model.head(*head_in, label, sparse=(targets.t_label, targets.t_prob, float(alpha), kd))
     else:
-        dense, sparse = (*targets, float(alpha), kd), None
-    loss, nll, _ = ops.HeadFn.apply(False, bf16, pf_head, memory, dec, _u8(mem_mask), _i32(label).view(-1),
-                                    m.out_fc.weight, m.out_fc.bias, *m.copy_net.flat_params(), None, None, dense,
-                                    sparse)
+        loss, nll, _ = model.head(*head_in, label, teacher=(*targets, float(alpha), kd))
     return loss, nll, kd
-
-
-def check_sparse(targets, model, rows):
-    """ValueError unless targets are SparseTargets of `rows` rows and 1..MAX_TOPK labels on the model's device (host
-    only)."""
-    dev = model.out_fc.weight.device
-    a, p = targets
-    ok = torch.is_tensor(a) and torch.is_tensor(p) and a.dtype == torch.int32 and p.dtype == torch.float32 and \
-        a.dim() == 2 and p.shape == a.shape and a.shape[0] == rows and 1 <= a.shape[1] <= MAX_TOPK
-    if not ok:
-        raise ValueError(f"sparse targets must be int32 labels and fp32 probabilities [{rows}, k], 1 <= k <= "
-                         f"{MAX_TOPK}")
-    if a.device != dev or p.device != dev:
-        raise ValueError(f"the sparse targets are on {a.device}, the student on {dev}")
 
 
 def distill_step(model, optimizer, batch, teacher, *, alpha):
@@ -333,20 +313,19 @@ def distill_step(model, optimizer, batch, teacher, *, alpha):
     check_alpha(alpha)
     refuse(model, "distill_step")
     sparse = isinstance(teacher, SparseTargets)
+    dev = model.out_fc.weight.device
     if sparse:
-        check_sparse(teacher, model, batch[6].shape[0] * batch[6].shape[1])
+        ops.check_sparse(*teacher, batch[6].shape[0] * batch[6].shape[1], dev)
     else:
         teacher_members(teacher, model)
-    dev = model.out_fc.weight.device
     label = model.shifted_label(batch[6].to(dev))
     targets = teacher if sparse else teacher_targets(teacher, batch, label)
-    model.train()
-    optimizer.zero_grad()
-    loss_sum, nll, kd = distill_loss(model, batch, targets, label, alpha)
     tokens = (label != 0).sum()
-    (loss_sum / tokens).backward()
-    optimizer.step()
-    bump_weights(model)                   # the decoding loops' cached weight operands follow the eager step
+
+    def loss():
+        loss_sum, nll, kd = distill_loss(model, batch, targets, label, alpha)
+        return loss_sum / tokens, loss_sum, nll, kd
+    _, loss_sum, nll, kd = _optim.eager_step(model, optimizer, loss)
     n = int(tokens.item())
     d = max(n, 1)
     return Step(loss_sum.item() / d, float(nll.sum().item()) / d, float(kd.sum().item()) / d, n)

@@ -112,52 +112,71 @@ class TransModel(nn.Module):
         pad = torch.zeros((tar_label.shape[0], 1), dtype=tar_label.dtype, device=tar_label.device)
         return torch.cat((tar_label[:, 1:], pad), dim=1)
 
-    def forward_packed(self, pb, stage="train"):
-        """The same computation on a per-commit PACKED batch (fira_icse_b200.packed.PackedBatch on this device, what
-        PackedBatchLoader(packed=True) emits): node rows = the real nodes of every commit, no 210/160/280 padding
-        (Dataset.py:80-94).  Loss, token count and gradients equal forward() on the padded batch; 'dev' ids number
-        copy positions by the commit's own memory rows (V + m, m < code rows + sub-token rows)."""
+    def _prefetch(self):
+        """Brings the bf16 mirror of parameters re-homed by optim.FlatAdam up to date, then starts the decoder's and the
+        head's weight preparation, which overlaps with the encoder -> the head's prefetch (None off CUDA)."""
         bf16 = self.precision == "bf16"
         if bf16:
             _optim.ensure_fresh(self)
         self.decoder.prefetch_weights()
-        pf_head = ops.prefetch_head(bf16, self.out_fc.weight, self.copy_net.LinearSource.weight,
-                                    self.copy_net.LinearTarget.weight)
-        memory = self.encoder.encode_memory_packed(pb)                       # [1, Rc + Rs, D]
-        if self._memory_hook is not None:
-            memory = self._memory_hook(memory)
-        want_ids = stage != "train"
-        dec = self.decoder(pb.tar, memory, pb.mem_mask, pb.tar_mask, packed=pb, label=None if want_ids else pb.label)
-        loss_sum, _, ids = ops.HeadFn.apply(want_ids, bf16, pf_head, memory, dec, pb.mem_mask, pb.label.view(-1),
-                                            self.out_fc.weight, self.out_fc.bias, *self.copy_net.flat_params(), pb)
-        if stage == "train":
-            return loss_sum, (pb.label != 0).sum()
-        elif stage == "dev" or stage == "test":
-            return ids.long()
-        raise ValueError(f"unknown stage {stage!r}")
+        if not self.out_fc.weight.is_cuda:
+            return None
+        return ops.prefetch_head(bf16, self.out_fc.weight, self.copy_net.LinearSource.weight,
+                                 self.copy_net.LinearTarget.weight)
 
-    def forward(self, sou, tar, attr, mark, ast_change, edge, tar_label, sub_token, stage="train"):
+    def teacher_forced(self, sou, tar, mark, ast_change, edge, sub_token, pad_id=0, repeat=1):
+        """The padded batch's teacher-forced pass up to the head, in the model's current mode and under autograd ->
+        (head prefetch, memory [B', S, D], copy mask [B', S] = cat(sou != pad_id, sub_token != 0), decoder output
+        [B', T, D] of tar masked by tar != pad_id), what head() takes.  The inputs are moved to the model's device.
+        repeat = N > 1 replicates memory and mask N-fold along the batch (commit b -> rows b*N .. b*N + N-1; the
+        encoder's gradient is the sum over the copies): tar then holds B' = B*N rows."""
         dev = self.out_fc.weight.device
-        sou, tar, mark, ast_change, tar_label, sub_token = (
-            t.to(dev, non_blocking=True) for t in (sou, tar, mark, ast_change, tar_label, sub_token))
-        mem_mask = torch.cat((sou != 0, sub_token != 0), dim=1)
-        bf16 = self.precision == "bf16"
-        if bf16:
-            _optim.ensure_fresh(self)            # parameters re-homed by optim.FlatAdam: bf16 mirror up to date
-        self.decoder.prefetch_weights()          # decoder / head weight preparation overlaps with the encoder
-        pf_head = ops.prefetch_head(bf16, self.out_fc.weight, self.copy_net.LinearSource.weight,
-                                    self.copy_net.LinearTarget.weight) if sou.is_cuda else None
+        sou, tar, mark, ast_change, sub_token = (
+            t.to(dev, non_blocking=True) for t in (sou, tar, mark, ast_change, sub_token))
+        mem_mask = torch.cat((sou != pad_id, sub_token != 0), dim=1)
+        pf_head = self._prefetch()
         memory = self.encoder.encode_memory(sou, mark, ast_change, edge, sub_token)
         if self._memory_hook is not None:
             memory = self._memory_hook(memory)
-        dec = self.decoder(tar, memory, mem_mask, tar != 0)
-        label = self.shifted_label(tar_label)
-        want_ids = stage != "train"
-        loss_sum, _, ids = ops.HeadFn.apply(want_ids, bf16, pf_head, memory, dec, _u8(mem_mask),
-                                            _i32(label).view(-1),
-                                            self.out_fc.weight, self.out_fc.bias, *self.copy_net.flat_params())
+        if repeat > 1:
+            def rep(x):
+                return x.unsqueeze(1).expand(x.shape[0], repeat, *x.shape[1:]).reshape(-1, *x.shape[1:])
+            memory, mem_mask = rep(memory), rep(mem_mask)
+        return pf_head, memory, mem_mask, self.decoder(tar, memory, mem_mask, tar != pad_id)
+
+    def head(self, pf_head, memory, mem_mask, dec, label, want_ids=False, pk=None, seq_weight=None, teacher=None,
+             sparse=None):
+        """ops.HeadFn on this model's head weights -> (loss_sum, per-position nll [B, T], argmax ids or None).  label:
+        the shifted labels [B, T]; the objectives as HeadFn documents them."""
+        return ops.HeadFn.apply(want_ids, self.precision == "bf16", pf_head, memory, dec, _u8(mem_mask),
+                                _i32(label).view(-1), self.out_fc.weight, self.out_fc.bias,
+                                *self.copy_net.flat_params(), pk, seq_weight, teacher, sparse)
+
+    @staticmethod
+    def _result(stage, loss_sum, ids, label):
         if stage == "train":
             return loss_sum, (label != 0).sum()
         elif stage == "dev" or stage == "test":
             return ids.long()
         raise ValueError(f"unknown stage {stage!r}")
+
+    def forward_packed(self, pb, stage="train"):
+        """The same computation on a per-commit PACKED batch (fira_icse_b200.packed.PackedBatch on this device, what
+        PackedBatchLoader(packed=True) emits): node rows = the real nodes of every commit, no 210/160/280 padding
+        (Dataset.py:80-94).  Loss, token count and gradients equal forward() on the padded batch; 'dev' ids number
+        copy positions by the commit's own memory rows (V + m, m < code rows + sub-token rows)."""
+        pf_head = self._prefetch()
+        memory = self.encoder.encode_memory_packed(pb)                       # [1, Rc + Rs, D]
+        if self._memory_hook is not None:
+            memory = self._memory_hook(memory)
+        want_ids = stage != "train"
+        dec = self.decoder(pb.tar, memory, pb.mem_mask, pb.tar_mask, packed=pb, label=None if want_ids else pb.label)
+        loss_sum, _, ids = self.head(pf_head, memory, pb.mem_mask, dec, pb.label, want_ids=want_ids, pk=pb)
+        return self._result(stage, loss_sum, ids, pb.label)
+
+    def forward(self, sou, tar, attr, mark, ast_change, edge, tar_label, sub_token, stage="train"):
+        tar_label = tar_label.to(self.out_fc.weight.device, non_blocking=True)
+        pf_head, memory, mem_mask, dec = self.teacher_forced(sou, tar, mark, ast_change, edge, sub_token)
+        label = self.shifted_label(tar_label)
+        loss_sum, _, ids = self.head(pf_head, memory, mem_mask, dec, label, want_ids=stage != "train")
+        return self._result(stage, loss_sum, ids, label)

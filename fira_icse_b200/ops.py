@@ -417,6 +417,16 @@ def prefetch_head(bf16, Wout, Ws, Wt):
     return pf
 
 
+def head_prec(bf16, pf):
+    """The head's precision context, holding the weight copies of prefetch_head's `pf` (None: none), joined here."""
+    pr = Prec(bf16)
+    if pf is not None and pf.event is not None:
+        torch.cuda.current_stream().wait_event(pf.event)
+        pf.fork.join()
+        pr.wcache.update(pf.wcache)
+    return pr
+
+
 def make_seed():
     """64-bit dropout seed drawn from torch's CPU generator (so torch.manual_seed controls it)."""
     return int(torch.randint(0, 2 ** 62, (1,)).item())
@@ -856,6 +866,23 @@ def copy_scores_fwd(pr, memory2, dec2, Ws, Wt, wres, bres, B, T, S, src_mask=Non
     return src, tgt, sc
 
 
+MAX_TOPK = 64             # labels per row of fira_pointer_mix_topk / fira_pointer_mix_kd_sparse_*
+
+
+def check_sparse(t_label, t_prob, rows, device):
+    """ValueError unless t_label / t_prob are contiguous int32 / fp32 [rows, k] with 1 <= k <= MAX_TOPK on `device`
+    (host only)."""
+    ok = torch.is_tensor(t_label) and torch.is_tensor(t_prob) and t_label.dtype == torch.int32 and \
+        t_prob.dtype == torch.float32 and t_label.dim() == 2 and t_prob.shape == t_label.shape and \
+        t_label.shape[0] == rows and 1 <= t_label.shape[1] <= MAX_TOPK and t_label.is_contiguous() and \
+        t_prob.is_contiguous()
+    if not ok:
+        raise ValueError(f"sparse targets must be contiguous int32 labels and fp32 probabilities [{rows}, k]: the "
+                         f"sparse targets need 1 <= k <= {MAX_TOPK} labels per row")
+    if t_label.device != device or t_prob.device != device:
+        raise ValueError(f"the sparse targets are on {t_label.device}, the model on {device}")
+
+
 def head_products(pr, memory2, dec2, dec32, dec_v, cap, Wout, bout, Ws, Wt, Wres, bres, Wp, bp, B, T, S, mem_mask,
                   row_mask, ranges=None):
     """The output head's three products (Model.py:54-60): out_fc logits of the `cap` rows dec_v ([cap, _ld_logits(V)],
@@ -912,17 +939,10 @@ class HeadFn(torch.autograd.Function):
                 raise ValueError("HeadFn: sparse targets apply to the padded training path without seq_weight or a "
                                  "teacher")
             t_label, t_prob, _, kd = sparse
-            ok = all(t is not None and t.is_cuda and t.is_contiguous() for t in (t_label, t_prob, kd)) and \
-                t_label.dtype == torch.int32 and t_prob.dtype == torch.float32 and kd.dtype == torch.float32
-            if not ok or t_label.dim() != 2 or t_label.shape[0] != Mt or not 1 <= t_label.shape[1] <= 64 or \
-                    t_prob.shape != t_label.shape or kd.numel() != Mt:
-                raise ValueError(f"HeadFn: sparse targets need contiguous CUDA int32 labels and fp32 probabilities "
-                                 f"[{Mt}, k] with 1 <= k <= 64 and an fp32 kd buffer of {Mt}")
-        pr = Prec(bf16)
-        if pf is not None and pf.event is not None:
-            torch.cuda.current_stream().wait_event(pf.event)
-            pf.fork.join()
-            pr.wcache.update(pf.wcache)
+            check_sparse(t_label, t_prob, Mt, dec.device)
+            if kd is None or not kd.is_cuda or kd.dtype != torch.float32 or not kd.is_contiguous() or kd.numel() != Mt:
+                raise ValueError(f"HeadFn: sparse targets need a contiguous CUDA fp32 kd buffer of {Mt}")
+        pr = head_prec(bf16, pf)
         dev = dec.device
         f32 = dict(dtype=torch.float32, device=dev)
         st = _stream()

@@ -416,6 +416,20 @@ def ensure_fresh(model):
             o.sync_mirror()
 
 
+def eager_step(model, optimizer, loss_fn):
+    """One eager training step: model.train(), optimizer.zero_grad(), loss_fn() -> (loss, ...), loss.backward(),
+    optimizer.step() -> what loss_fn returned.  Then the decoder's weights_epoch is bumped: a FlatAdam step writes the
+    parameters through a raw kernel that moves neither their version counters nor their addresses, and the decoding
+    loops' cached weight operands (decode_loop.loop_for) must re-read them."""
+    model.train()
+    optimizer.zero_grad()
+    out = loss_fn()
+    out[0].backward()
+    optimizer.step()
+    model.decoder.weights_epoch = getattr(model.decoder, "weights_epoch", 0) + 1
+    return out
+
+
 def ema_model(model, optims):
     """The EMA weights of `optims` (FlatAdam instances built with ema_decay that own `model`'s live parameters: one, or
     both halves of engine.GraphedTrainStep's pair) as a TransModel: built from `model.args`, in eval mode, no parameter

@@ -21,12 +21,9 @@ sample).  The gradient pass encodes the batch once, in training mode with the ke
 N-fold along the batch under autograd (the encoder's gradient is the sum over the copies); the decoder and the head then
 run on the B*N sampled targets with seq_weight = A / (B*N) (fira_pointer_mix_nll_bwd_rows_weighted; a sample whose
 advantage is exactly 0 costs the head's backward nothing).  The cross-attention K/V projection of the memory is paid N
-times.  This is the eager padded-batch path: no CUDA graph of the step, no packed layout.
-
-After the optimizer step the decoder's weights_epoch is bumped: an eager FlatAdam step writes the parameters through a raw
-kernel that moves neither their version counters nor their addresses, and the next sample() must decode with the new
-weights.  decode_loop.loop_for then refreshes the cached loop's weight operands in place and keeps replaying its
-captured position graphs.
+times.  This is the eager padded-batch path (optim.eager_step): no CUDA graph of the step, no packed layout.  The step
+bumps the decoder's weights_epoch, so the next sample() decodes with the new weights: decode_loop.loop_for then
+refreshes the cached loop's weight operands in place and keeps replaying its captured position graphs.
 """
 from typing import NamedTuple
 
@@ -37,7 +34,6 @@ from . import optim as _optim
 from ._lib import call
 from .decode_loop import check_rules, check_tar_len, is_int
 from .ensemble import refuse
-from .modules import _i32, _u8
 from .sample import MAX_SAMPLES, check_args, sample
 
 MAX_TAR_LEN = 32          # fira_bleu_reward: at most 31 words per message, one per lane of a warp
@@ -88,32 +84,12 @@ def policy_loss(model, batch, seq, raw, seq_weight, pad_id=0):
     """sum over the B*N sampled messages of seq_weight[b*N + n] * their NLL, under autograd, in the model's current
     mode -> (loss, per-position nll [B*N, T]).  batch: the padded 8-tuple; seq / raw [B, N, T] of sample()."""
     sou, _, _, mark, ast_change, edge, _, sub_token = batch
-    m = model
-    dev = m.out_fc.weight.device
-    sou, mark, ast_change, sub_token = (t.to(dev) for t in (sou, mark, ast_change, sub_token))
     B, N, T = seq.shape
-    bf16 = m.precision == "bf16"
-    if bf16:
-        _optim.ensure_fresh(m)
-    m.decoder.prefetch_weights()
-    pf_head = ops.prefetch_head(bf16, m.out_fc.weight, m.copy_net.LinearSource.weight, m.copy_net.LinearTarget.weight)
-    memory = m.encoder.encode_memory(sou, mark, ast_change, edge, sub_token)
-    mem_mask = torch.cat((sou != pad_id, sub_token != 0), dim=1)       # as decode_loop.encode forms it for the sampler
-
-    def rep(x):                                                         # commit b -> rows b*N .. b*N + N-1
-        return x.unsqueeze(1).expand(B, N, *x.shape[1:]).reshape(B * N, *x.shape[1:])
-    memory_r, mem_mask_r = rep(memory), rep(mem_mask)
-    tar = seq.reshape(B * N, T)
-    label = m.shifted_label(raw.reshape(B * N, T))
-    dec = m.decoder(tar, memory_r, mem_mask_r, tar != pad_id)
-    loss, nll, _ = ops.HeadFn.apply(False, bf16, pf_head, memory_r, dec, _u8(mem_mask_r), _i32(label).view(-1),
-                                    m.out_fc.weight, m.out_fc.bias, *m.copy_net.flat_params(), None, seq_weight)
+    # the copy mask with pad_id, as decode_loop.encode forms it for the sampler
+    head_in = model.teacher_forced(sou, seq.reshape(B * N, T), mark, ast_change, edge, sub_token, pad_id=pad_id,
+                                   repeat=N)
+    loss, nll, _ = model.head(*head_in, model.shifted_label(raw.reshape(B * N, T)), seq_weight=seq_weight)
     return loss, nll
-
-
-def bump_weights(model):
-    """Tell the decoding loops' weight caches that the parameters moved (decode_loop.loop_for)."""
-    model.decoder.weights_epoch = getattr(model.decoder, "weights_epoch", 0) + 1
 
 
 def scst_step(model, optimizer, batch, *, num_samples, temperature=1.0, top_k=0, top_p=1.0, seed=0, first_index=0,
@@ -132,10 +108,5 @@ def scst_step(model, optimizer, batch, *, num_samples, temperature=1.0, top_k=0,
     reward, advantage = rewards(s.seq, s.length, tar, start_id=start_id, eos_id=eos_id, pad_id=pad_id)
     B, N = reward.shape
     weight = (advantage / (B * N)).to(torch.float32).reshape(-1)
-    model.train()
-    optimizer.zero_grad()
-    loss, _ = policy_loss(model, batch, s.seq, s.raw, weight, pad_id)
-    loss.backward()
-    optimizer.step()
-    bump_weights(model)
+    loss, _ = _optim.eager_step(model, optimizer, lambda: policy_loss(model, batch, s.seq, s.raw, weight, pad_id))
     return Step(reward.mean().item(), advantage.abs().mean().item(), loss.item())

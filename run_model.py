@@ -281,6 +281,19 @@ class ClipLog:
         return " grad_norm: %.4f clipped: %d skipped: %d" % (mean, int(c.clipped.item()), int(c.skipped.item()))
 
 
+def keep_best(model, scored, best_bleu, progress, checkpoint, dev_output):
+    """Appends `<progress> dev bleu: <bleu> is better: <bool>` to OUTPUT/train_process for dev()'s (bleu, output); when
+    the BLEU beats best_bleu, saves the model's state_dict to `checkpoint` and the output to OUTPUT/<dev_output> -> the
+    best dev BLEU so far."""
+    bleu, output_str = scored
+    open('OUTPUT/train_process', 'a').write('{} dev bleu: {} is better: {}\n'.format(progress, bleu, bleu > best_bleu))
+    if not bleu > best_bleu:
+        return best_bleu
+    torch.save(model.state_dict(), checkpoint)
+    open('OUTPUT/' + dev_output, 'w').write(output_str)
+    return bleu
+
+
 def train_epoch(dp, model, train_loader, epoch, best_bleu, dev_loader, g, valid_index, dev_, ema=None, clip_log=None):
     """ema: None, or {"best": best dev BLEU of the EMA weights so far} when FIRA_EMA is set (updated in place);
     clip_log: a ClipLog when FIRA_CLIP_NORM is set"""
@@ -293,26 +306,17 @@ def train_epoch(dp, model, train_loader, epoch, best_bleu, dev_loader, g, valid_
             break
         if epoch >= 15 and idx % 10 == 0:
             if RANK == 0:
-                cur_bleu, output_str = dev(model, dev_loader, g, valid_index, epoch, dev_)
-                open('OUTPUT/train_process', 'a').write(
-                    'epoch: {} batch: {} dev bleu: {} is better: {}\n'.format(epoch, idx, cur_bleu, cur_bleu > best_bleu))
-                if cur_bleu > best_bleu:
-                    best_bleu = cur_bleu
-                    torch.save(model.state_dict(), "best_model.pt")
-                    open('OUTPUT/dev_output', 'w').write(output_str)
+                best_bleu = keep_best(model, dev(model, dev_loader, g, valid_index, epoch, dev_), best_bleu,
+                                      f"epoch: {epoch} batch: {idx}", "best_model.pt", "dev_output")
                 if ema is not None and dp.opt_ready:
                     # the EMA weights, scored and kept on their own; building the shadow model and the dev loader's
                     # iterator draw from torch's CPU generator, which also shuffles and seeds dropout: fork it, so
                     # training goes on exactly as without FIRA_EMA
                     with torch.random.fork_rng(devices=[]):
                         shadow = dp.ema_model()
-                        ema_bleu, output_str = dev(shadow, dev_loader, g, valid_index, epoch, dev_)
-                    open('OUTPUT/train_process', 'a').write('ema epoch: {} batch: {} dev bleu: {} is better: {}\n'.format(
-                        epoch, idx, ema_bleu, ema_bleu > ema["best"]))
-                    if ema_bleu > ema["best"]:
-                        ema["best"] = ema_bleu
-                        torch.save(shadow.state_dict(), EMA_CHECKPOINT)
-                        open('OUTPUT/dev_output_ema', 'w').write(output_str)
+                        scored = dev(shadow, dev_loader, g, valid_index, epoch, dev_)
+                    ema["best"] = keep_best(shadow, scored, ema["best"], f"ema epoch: {epoch} batch: {idx}",
+                                            EMA_CHECKPOINT, "dev_output_ema")
             if WORLD > 1:
                 dist.barrier()
             model.train()
@@ -628,10 +632,46 @@ def main_test():
         print("constraints met by the top hypothesis: %f" % (decode.met[0] / max(1, decode.met[1])))
 
 
+def one_gpu(stage):
+    """SystemExit when launched with torchrun: `stage` runs on one GPU."""
+    if WORLD > 1:
+        raise SystemExit(f"run_model.py {stage} runs on one GPU: launch it without torchrun (WORLD_SIZE=1)")
+
+
+def finetune_epochs(stage, model, lr, max_grad_norm, epochs, batches, step, progress, checkpoint, dev_output, g, dev_):
+    """The epoch loop of `finetune` and `distill`: optim.FlatAdam at `lr` over the model's live parameters, clipped at
+    max_grad_norm (FIRA_CLIP_NORM); per epoch e, step(optimizer, e, idx, batch) on every batch of batches(e)
+    (FIRA_MAX_BATCHES bounds an epoch), and every 10 batches a progress line ending in progress(the step results since
+    the last line); then dev(), keeping the best dev BLEU's weights in `checkpoint` and its output in
+    OUTPUT/<dev_output>."""
+    from fira_icse_b200 import optim
+    opt = optim.FlatAdam(model.live_parameters(), lr=lr, groups=model.flat_groups(), max_grad_norm=max_grad_norm)
+    optim.attach(model, [opt])
+    clip_log = None if max_grad_norm is None else ClipLog(lambda: opt.clip)
+    dev_loader = loader(TransDataset(args, 'valid'), args.batch_size, False)
+    valid_index = json.load(open('all_index'))['valid']
+    max_batches = int(os.environ.get("FIRA_MAX_BATCHES", 0))
+    best_bleu = -1.0
+    for epoch in range(epochs):
+        train_loader, steps = batches(epoch), []
+        for idx, batch in enumerate(train_loader):
+            if max_batches and idx >= max_batches:
+                break
+            steps.append(step(opt, epoch, idx, batch))
+            if clip_log is not None:
+                clip_log.add()
+            if idx % 10 == 0:
+                print("%s epoch: %d batch: %d/%d " % (stage, epoch, idx, len(train_loader)) + progress(steps)
+                      + (clip_log.text() if clip_log is not None else ""))
+                steps = []
+        best_bleu = keep_best(model, dev(model, dev_loader, g, valid_index, epoch, dev_), best_bleu,
+                              f"{stage} epoch: {epoch}", checkpoint, dev_output)
+    print("best dev bleu: %f" % best_bleu)
+
+
 def finetune_settings():
     """The finetune stage's settings from the environment, checked before any device work (SystemExit on an error)."""
-    if WORLD > 1:
-        raise SystemExit("run_model.py finetune runs on one GPU: launch it without torchrun (WORLD_SIZE=1)")
+    one_gpu("finetune")
     try:
         s = dict(epochs=int(os.environ.get("FIRA_SCST_EPOCHS", 1)), lr=float(os.environ.get("FIRA_SCST_LR", 1e-5)),
                  num_samples=int(os.environ.get("FIRA_SAMPLES", 5)),
@@ -661,44 +701,18 @@ def main_finetune():
     g = load_globals()
     vocab = g["vocab"]
     ids = dict(tar_len=args.tar_len, start_id=vocab['<start>'], eos_id=vocab['<eos>'], pad_id=vocab['<pad>'])
-    train_set = TransDataset(args, 'train')
-    dev_set = TransDataset(args, 'valid')
-    all_index = json.load(open('all_index'))
-    model = TransModel(args)
-    model.load_state_dict(torch.load("best_model.pt", map_location="cpu"))
-    model = model.to(dev_)
-    from fira_icse_b200 import optim
-    opt = optim.FlatAdam(model.live_parameters(), lr=s["lr"], groups=model.flat_groups(), max_grad_norm=max_grad_norm)
-    optim.attach(model, [opt])
-    clip_log = None if max_grad_norm is None else ClipLog(lambda: opt.clip)
-    train_loader = loader(train_set, args.batch_size, True)
-    dev_loader = loader(dev_set, args.batch_size, False)
-    max_batches = int(os.environ.get("FIRA_MAX_BATCHES", 0))
-    best_bleu = -1.0
-    for epoch in range(s["epochs"]):
-        total, rewards = 0, []
-        for idx, batch in enumerate(train_loader):
-            if max_batches and idx >= max_batches:
-                break
-            b = batch_to_device(batch, dev_)
-            step = scst_step(model, opt, b, **dict(sampling, seed=sampling["seed"] + epoch), first_index=total, **ids)
-            rewards.append(step.reward)
-            total += len(b[0])
-            if clip_log is not None:
-                clip_log.add()
-            if idx % 10 == 0:
-                print("scst epoch: %d batch: %d/%d reward: %.4f |advantage|: %.4f loss: %.6f" % (
-                    epoch, idx, len(train_loader), sum(rewards) / len(rewards), step.advantage, step.loss)
-                    + (clip_log.text() if clip_log is not None else ""))
-                rewards = []
-        cur_bleu, output_str = dev(model, dev_loader, g, all_index['valid'], epoch, dev_)
-        open('OUTPUT/train_process', 'a').write(
-            'scst epoch: {} dev bleu: {} is better: {}\n'.format(epoch, cur_bleu, cur_bleu > best_bleu))
-        if cur_bleu > best_bleu:
-            best_bleu = cur_bleu
-            torch.save(model.state_dict(), "best_model_scst.pt")
-            open('OUTPUT/dev_output_scst', 'w').write(output_str)
-    print("best dev bleu: %f" % best_bleu)
+    train_loader = loader(TransDataset(args, 'train'), args.batch_size, True)
+    model = load_model("best_model.pt", dev_)
+
+    def step(opt, epoch, idx, batch):          # every batch but an epoch's last holds batch_size commits
+        return scst_step(model, opt, batch_to_device(batch, dev_), **dict(sampling, seed=sampling["seed"] + epoch),
+                         first_index=idx * args.batch_size, **ids)
+
+    def progress(steps):
+        return "reward: %.4f |advantage|: %.4f loss: %.6f" % (
+            sum(x.reward for x in steps) / len(steps), steps[-1].advantage, steps[-1].loss)
+    finetune_epochs("scst", model, s["lr"], max_grad_norm, s["epochs"], lambda epoch: train_loader, step, progress,
+                    "best_model_scst.pt", "dev_output_scst", g, dev_)
 
 
 KD_CHECKPOINT = "best_model_kd.pt"
@@ -707,8 +721,7 @@ KD_CHECKPOINT = "best_model_kd.pt"
 def distill_settings():
     """The distill stage's settings from the environment, checked before any device work (SystemExit on an error) ->
     (settings, student checkpoint, (teacher checkpoints, weights or None))."""
-    if WORLD > 1:
-        raise SystemExit("run_model.py distill runs on one GPU: launch it without torchrun (WORLD_SIZE=1)")
+    one_gpu("distill")
     try:
         s = dict(alpha=float(os.environ.get("FIRA_KD_ALPHA", 0.5)), epochs=int(os.environ.get("FIRA_KD_EPOCHS", 1)),
                  lr=float(os.environ.get("FIRA_KD_LR", 1e-4)))
@@ -764,50 +777,37 @@ def main_distill():
         dev_ = device()
         g = load_globals()
         train_set = TransDataset(args, 'train')
-    dev_set = TransDataset(args, 'valid')
-    all_index = json.load(open('all_index'))
+        train_loader = loader(train_set, args.batch_size, True)
     model = load_model(student, dev_)
     teacher = Ensemble([load_model(p, dev_) for p in teacher_spec[0]], teacher_spec[1]) if targets is None else None
-    from fira_icse_b200 import optim
-    opt = optim.FlatAdam(model.live_parameters(), lr=s["lr"], groups=model.flat_groups(), max_grad_norm=max_grad_norm)
-    optim.attach(model, [opt])
-    clip_log = None if max_grad_norm is None else ClipLog(lambda: opt.clip)
-    train_loader = loader(train_set, args.batch_size, True) if targets is None else None
-    dev_loader = loader(dev_set, args.batch_size, False)
-    max_batches = int(os.environ.get("FIRA_MAX_BATCHES", 0))
-    best_bleu = -1.0
-    for epoch in range(s["epochs"]):
-        if targets is not None:                 # a seeded permutation: each batch's dataset positions are known
-            perm = torch.randperm(len(train_set), generator=torch.Generator().manual_seed(seed + epoch)).tolist()
-            train_loader = loader(train_set, args.batch_size, False, indices=perm)
-        for idx, batch in enumerate(train_loader):
-            if max_batches and idx >= max_batches:
-                break
-            if targets is not None:
-                pos = perm[idx * args.batch_size: idx * args.batch_size + batch[6].shape[0]]
-                teacher = targets.batch(pos, TransModel.shifted_label(batch[6]), device=dev_)
-            step = distill_step(model, opt, batch_to_device(batch, dev_), teacher, alpha=s["alpha"])
-            if clip_log is not None:
-                clip_log.add()
-            if idx % 10 == 0:
-                print("kd epoch: %d batch: %d/%d loss: %.4f nll: %.4f kd: %.4f tokens: %d" % (
-                    epoch, idx, len(train_loader), step.loss, step.nll, step.kd, step.tokens)
-                    + (clip_log.text() if clip_log is not None else ""))
-        cur_bleu, output_str = dev(model, dev_loader, g, all_index['valid'], epoch, dev_)
-        open('OUTPUT/train_process', 'a').write(
-            'kd epoch: {} dev bleu: {} is better: {}\n'.format(epoch, cur_bleu, cur_bleu > best_bleu))
-        if cur_bleu > best_bleu:
-            best_bleu = cur_bleu
-            torch.save(model.state_dict(), KD_CHECKPOINT)
-            open('OUTPUT/dev_output_kd', 'w').write(output_str)
-    print("best dev bleu: %f" % best_bleu)
+    perm = None
+
+    def batches(epoch):
+        nonlocal perm
+        if targets is None:
+            return train_loader
+        # a seeded permutation: each batch's dataset positions are known
+        perm = torch.randperm(len(train_set), generator=torch.Generator().manual_seed(seed + epoch)).tolist()
+        return loader(train_set, args.batch_size, False, indices=perm)
+
+    def step(opt, epoch, idx, batch):
+        t = teacher
+        if targets is not None:
+            pos = perm[idx * args.batch_size: idx * args.batch_size + batch[6].shape[0]]
+            t = targets.batch(pos, TransModel.shifted_label(batch[6]), device=dev_)
+        return distill_step(model, opt, batch_to_device(batch, dev_), t, alpha=s["alpha"])
+
+    def progress(steps):
+        return "loss: %.4f nll: %.4f kd: %.4f tokens: %d" % (steps[-1].loss, steps[-1].nll, steps[-1].kd,
+                                                             steps[-1].tokens)
+    finetune_epochs("kd", model, s["lr"], max_grad_norm, s["epochs"], batches, step, progress, KD_CHECKPOINT,
+                    "dev_output_kd", g, dev_)
 
 
 def kd_targets_settings():
     """`kd-targets`' settings, checked before any device work (SystemExit on an error) -> (k, (teacher checkpoints,
     weights or None), output path)."""
-    if WORLD > 1:
-        raise SystemExit("run_model.py kd-targets runs on one GPU: launch it without torchrun (WORLD_SIZE=1)")
+    one_gpu("kd-targets")
     try:
         k = int(os.environ.get("FIRA_KD_TOPK", 8))
     except ValueError as e:
@@ -837,8 +837,7 @@ def main_kd_targets():
 
 
 def main_datastore():
-    if WORLD > 1:
-        raise SystemExit("run_model.py datastore runs on one GPU: launch it without torchrun (WORLD_SIZE=1)")
+    one_gpu("datastore")
     ckpt = os.environ.get("FIRA_CHECKPOINT", "best_model.pt")
     out = os.environ.get("FIRA_DATASTORE", "datastore.pt")
     if not os.path.isfile(ckpt):

@@ -7,9 +7,9 @@ eager MLE step, and the two loss kernels against the NLL kernels on the same row
 
 Step: synthetic commits (fira_icse_b200.synth), B = --batch, fp32 and bf16; the teacher is M copies of the seeded model,
 each but the first with the seeded perturbation of tools/bench_beam.py --ensemble.  CUDA events around the teacher's
-forward (all members), the combine (fira_pointer_mix_ensemble), the student's forward + backward (training mode with
-dropout) and the FlatAdam step; the median of each over --steps after --warmup.  The MLE step is model(..., 'train'),
-backward and FlatAdam on the same batch, eager.
+forward (all members), the combine (fira_pointer_mix_ensemble) and the student's step (optim.eager_step: forward +
+backward in training mode with dropout, then FlatAdam); the median of each over --steps after --warmup.  The MLE step
+is model(..., 'train'), backward and FlatAdam on the same batch, eager.
 Kernels: microseconds per launch of fira_pointer_mix_kd_fwd / _bwd and fira_pointer_mix_nll_fwd_rows / _bwd_rows on the
 same rows (the batch's shifted labels), replayed from a CUDA graph over buffer sets larger than L2
 (bench.time_launches).  Algorithmic bytes per loss row (y != 0): the kd forward reads the student row (V s + S 4) and
@@ -36,7 +36,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import torch  # noqa: E402
 
-from bench_scst import card, new_model, synthetic_batch  # noqa: E402
+from bench_scst import card, mle_loss, new_model, synthetic_batch  # noqa: E402
 
 PEAK_GBS = 3350.0
 L2_BYTES = 50 * 2 ** 20
@@ -58,62 +58,27 @@ def teacher(precision, dev, M):
 
 def timed_step(m, opt, batch, ens, alpha=0.5):
     """one distill_step, its parts between CUDA events -> milliseconds per part"""
-    import ctypes
-    from fira_icse_b200 import distill, ops
-    from fira_icse_b200._lib import FIRA_BF16, FIRA_F32, call
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
+    from fira_icse_b200 import distill, optim
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
     label = m.shifted_label(batch[6])
     ev[0].record()
-    # teacher_targets, split at the combine: the members' forwards, then the one combine launch
     models, log_w = distill.teacher_members(ens, m)
-    sou, tar, _, mark, ast_change, edge, _, sub_token = batch
-    B, T = label.shape
-    mem_mask = torch.cat((sou != 0, sub_token != 0), 1)
-    mm = mem_mask.to(torch.uint8).contiguous()
-    row_mask = (label != 0).to(torch.uint8).contiguous().view(-1)
-    S, V = mem_mask.shape[1], m.vocab_size
-    triples = []
-    with torch.no_grad():
-        for t in models:
-            bf16 = t.precision == "bf16"
-            memory = t.encoder.encode_memory(sou, mark, ast_change, edge, sub_token)
-            dec = t.decoder(tar, memory, mem_mask, tar != 0)
-            pr = ops.Prec(bf16)
-            dec2 = dec.contiguous().to(pr.tdt).view(B * T, ops.D)
-            lg, _, _, sc, gl = ops.head_products(pr, memory.contiguous().to(pr.tdt).view(-1, ops.D), dec2,
-                                                 dec2.float() if bf16 else dec2, dec2, B * T, t.out_fc.weight,
-                                                 t.out_fc.bias, *t.copy_net.flat_params(), B, T, S, mm, row_mask)
-            triples.append((lg, sc, gl))
+    triples, mm = distill.member_triples(models, batch, label)
     ev[1].record()
-    ld = triples[0][0].shape[1]
-    f32 = dict(dtype=torch.float32, device=batch[0].device)
-    out, sc_out, gl_out = torch.empty((B * T, ld), **f32), torch.empty((B, T, S), **f32), torch.empty((B * T, 2), **f32)
-    lw = torch.tensor(log_w, **f32)
-    arrs = [(ctypes.c_void_p * len(models))(*[ops._ptr(x[k]) for x in triples]) for k in range(3)]
-    call("fira_pointer_mix_ensemble", ctypes.addressof(arrs[0]), ld, ctypes.addressof(arrs[1]),
-         ctypes.addressof(arrs[2]), len(models), ops._ptr(lw), ops._ptr(mm), ops._ptr(out), ld, ops._ptr(sc_out),
-         ops._ptr(gl_out), B, T, V, S, FIRA_BF16 if models[0].precision == "bf16" else FIRA_F32, ops._stream())
+    targets = distill.combine(triples, log_w, mm, m.vocab_size)
     ev[2].record()
-    m.train()
-    opt.zero_grad()
-    loss, _, _ = distill.distill_loss(m, batch, (out, sc_out, gl_out), label, alpha)
-    (loss / (label != 0).sum()).backward()
+    tokens = (label != 0).sum()
+    optim.eager_step(m, opt, lambda: (distill.distill_loss(m, batch, targets, label, alpha)[0] / tokens,))
     ev[3].record()
-    opt.step()
-    distill.bump_weights(m)
-    ev[4].record()
     torch.cuda.synchronize()
-    return [ev[i].elapsed_time(ev[i + 1]) for i in range(4)], (out, sc_out, gl_out)
+    return [ev[i].elapsed_time(ev[i + 1]) for i in range(3)], targets
 
 
 def mle_step(m, opt, batch):
+    from fira_icse_b200 import optim
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
     ev[0].record()
-    m.train()
-    opt.zero_grad()
-    ls, nt = m(*batch, "train")
-    (ls / nt).backward()
-    opt.step()
+    optim.eager_step(m, opt, lambda: mle_loss(m, batch))
     ev[1].record()
     torch.cuda.synchronize()
     return ev[0].elapsed_time(ev[1])
@@ -122,25 +87,15 @@ def mle_step(m, opt, batch):
 def kernel_times(m, batch, targets):
     """µs per launch of the kd and NLL kernels on this batch's rows, with the student's head products"""
     import bench
-    from fira_icse_b200 import ops
+    from fira_icse_b200 import distill, ops
     from fira_icse_b200._lib import call
     label = m.shifted_label(batch[6])
     B, T = label.shape
-    sou, tar, _, mark, ast_change, edge, _, sub_token = batch
-    mem_mask = torch.cat((sou != 0, sub_token != 0), 1)
-    mm = mem_mask.to(torch.uint8).contiguous()
+    [(lg, sc, gl)], mm = distill.member_triples([m], batch, label)
     lab = label.to(torch.int32).contiguous().view(-1)
-    S, V, R = mem_mask.shape[1], m.vocab_size, B * T
+    S, V, R = mm.shape[1], m.vocab_size, B * T
     bf16 = m.precision == "bf16"
-    with torch.no_grad():
-        m.eval()
-        memory = m.encoder.encode_memory(sou, mark, ast_change, edge, sub_token)
-        dec = m.decoder(tar, memory, mem_mask, tar != 0)
-        pr = ops.Prec(bf16)
-        dec2 = dec.contiguous().to(pr.tdt).view(R, ops.D)
-        lg, _, _, sc, gl = ops.head_products(pr, memory.contiguous().to(pr.tdt).view(-1, ops.D), dec2,
-                                             dec2.float() if bf16 else dec2, dec2, R, m.out_fc.weight, m.out_fc.bias,
-                                             *m.copy_net.flat_params(), B, T, S, mm, (lab != 0).to(torch.uint8))
+    pr = ops.Prec(bf16)
     tx, tsc, tgl = targets
     s = 2 if bf16 else 4
     ld = lg.shape[1]
@@ -205,9 +160,9 @@ def kernel_times(m, batch, targets):
 
 
 def sparse_times(m, opt, batch, targets, k, steps, warmup):
-    """offline distillation at top-k: step parts, kernel µs per launch, rate and bytes of the stored targets"""
+    """offline distillation at top-k: step time, kernel µs per launch, rate and bytes of the stored targets"""
     import bench
-    from fira_icse_b200 import distill, ops
+    from fira_icse_b200 import distill, ops, optim
     from fira_icse_b200._lib import call
     label = m.shifted_label(batch[6])
     B, T = label.shape
@@ -217,34 +172,20 @@ def sparse_times(m, opt, batch, targets, k, steps, warmup):
     lab = label.to(torch.int32).contiguous().view(-1)
     tl, tp, mass = distill.topk_targets(targets, mm, label, V, k)
     sparse = distill.SparseTargets(tl, tp)
-    parts = []
+    tokens = (label != 0).sum()
+    times = []
     for i in range(warmup + steps):
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
         ev[0].record()
-        m.train()
-        opt.zero_grad()
-        loss, _, _ = distill.distill_loss(m, batch, sparse, label, 0.5)
-        (loss / (label != 0).sum()).backward()
+        optim.eager_step(m, opt, lambda: (distill.distill_loss(m, batch, sparse, label, 0.5)[0] / tokens,))
         ev[1].record()
-        opt.step()
-        distill.bump_weights(m)
-        ev[2].record()
         torch.cuda.synchronize()
         if i >= warmup:
-            parts.append([ev[0].elapsed_time(ev[1]), ev[1].elapsed_time(ev[2])])
-    med = [statistics.median(x[j] for x in parts) for j in range(2)]
+            times.append(ev[0].elapsed_time(ev[1]))
     # the kernels on the student's head products of this batch
+    [(lg, sc, gl)], _ = distill.member_triples([m], batch, label)
     bf16 = m.precision == "bf16"
-    with torch.no_grad():
-        m.eval()
-        memory = m.encoder.encode_memory(*(batch[i] for i in (0, 3, 4, 5, 7)))
-        mem_mask = mm != 0
-        dec = m.decoder(batch[1], memory, mem_mask, batch[1] != 0)
-        pr = ops.Prec(bf16)
-        dec2 = dec.contiguous().to(pr.tdt).view(R, ops.D)
-        lg, _, _, sc, gl = ops.head_products(pr, memory.contiguous().to(pr.tdt).view(-1, ops.D), dec2,
-                                             dec2.float() if bf16 else dec2, dec2, R, m.out_fc.weight, m.out_fc.bias,
-                                             *m.copy_net.flat_params(), B, T, S, mm, (lab != 0).to(torch.uint8))
+    pr = ops.Prec(bf16)
     s = 2 if bf16 else 4
     ld = lg.shape[1]
     n_rot = max(2, -(-2 * L2_BYTES // (R * ld * 2 * s + R * S * 8)))
@@ -289,8 +230,7 @@ def sparse_times(m, opt, batch, targets, k, steps, warmup):
                       "share_of_peak": bytes_[name] / (med_ms * 1e-3) / 1e9 / PEAK_GBS}
     live = y != 0
     per_commit = (n_loss * (2 + 4 + 8 * k + 4) + 8 * B) / B
-    return {"ms": {"student_forward_backward": med[0], "adam": med[1]}, "ms_step": statistics.median(sum(x) for x in
-            parts), "kernels": kern, "bytes_per_commit": per_commit,
+    return {"ms_step": statistics.median(times), "kernels": kern, "bytes_per_commit": per_commit,
             "mean_kept_mass": float(mass[live].double().mean())}
 
 
@@ -338,10 +278,10 @@ def main():
                 t, targets = timed_step(m, opt, batch, ens)
                 if i >= args.warmup:
                     parts.append(t)
-            med = [statistics.median(x[k] for x in parts) for k in range(4)]
+            med = [statistics.median(x[k] for x in parts) for k in range(3)]
             steps = [sum(x) for x in parts]
             row = {"precision": precision, "B": args.batch, "M": M,
-                   "ms": dict(zip(("teacher_forward", "combine", "student_forward_backward", "adam"), med)),
+                   "ms": dict(zip(("teacher_forward", "combine", "student_step"), med)),
                    "ms_step": statistics.median(steps), "ms_mle_step": statistics.median(mle)}
             if M == args.members[0]:
                 row["kernels"] = kernel_times(m, batch, targets)

@@ -6,9 +6,10 @@ reward of a model first trained with the MLE loss.
                                [--reward-steps 50] [--json out.json]
 
 Timing: synthetic commits (fira_icse_b200.synth), B = --batch, each N of --samples, fp32 and bf16; per step, CUDA events
-around sampling (eval mode, sample()), the rewards (fira_bleu_reward), forward + backward (policy_loss, training mode
-with dropout) and the FlatAdam step; the median over --steps after --warmup.  The cross-attention K/V projection of
-the memory runs on the N replicas (scst.py): its forward product is timed on B and on B*N memory rows.
+around sampling (eval mode, sample()), the rewards (fira_bleu_reward) and the training step (optim.eager_step:
+policy_loss forward + backward in training mode with dropout, then FlatAdam); the median over --steps after --warmup.
+The cross-attention K/V projection of the memory runs on the N replicas (scst.py): its forward product is timed on B and
+on B*N memory rows.
 Reward: the seeded model trained for --mle-steps Adam steps (lr 1e-4, bf16, batches of 16 golden commits), then
 --reward-steps SCST steps (N = 4, lr 1e-5) on the same commits; the mean reward over those steps.
 One JSON object on stdout, with the card name and power limit read in the same run."""
@@ -59,11 +60,17 @@ def new_model(precision, dev, lr):
     return m, opt
 
 
+def mle_loss(m, batch):
+    """the training loss of model(..., 'train') per token, as optim.eager_step takes it"""
+    ls, nt = m(*batch, "train")
+    return (ls / nt,)
+
+
 def timed_step(m, opt, batch, N, ids, seed):
-    """one scst_step, its four parts between CUDA events -> milliseconds per part"""
-    from fira_icse_b200 import scst
+    """one scst_step, its three parts between CUDA events -> milliseconds per part"""
+    from fira_icse_b200 import optim, scst
     from fira_icse_b200.sample import sample
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
     sou, tar, _, mark, ast_change, edge, _, sub_token = batch
     ev[0].record()
     m.eval()
@@ -73,16 +80,10 @@ def timed_step(m, opt, batch, N, ids, seed):
     B = reward.shape[0]
     w = (adv / (B * N)).float().reshape(-1)
     ev[2].record()
-    m.train()
-    opt.zero_grad()
-    loss, _ = scst.policy_loss(m, batch, s.seq, s.raw, w, ids["pad_id"])
-    loss.backward()
+    optim.eager_step(m, opt, lambda: scst.policy_loss(m, batch, s.seq, s.raw, w, ids["pad_id"]))
     ev[3].record()
-    opt.step()
-    scst.bump_weights(m)
-    ev[4].record()
     torch.cuda.synchronize()
-    return [ev[i].elapsed_time(ev[i + 1]) for i in range(4)]
+    return [ev[i].elapsed_time(ev[i + 1]) for i in range(3)]
 
 
 def kv_projection_ms(m, memory, N, reps=20):
@@ -118,12 +119,12 @@ def timing(args, dev):
                 t = timed_step(m, opt, batch, N, ids, seed=i)
                 if i >= args.warmup:
                     parts.append(t)
-            med = [statistics.median(p[k] for p in parts) for k in range(4)]
+            med = [statistics.median(p[k] for p in parts) for k in range(3)]
             with torch.no_grad():
                 m.eval()
-                memory = m.encoder.encode_memory(batch[0], batch[3], batch[4], batch[5], batch[7])
+                memory = m.teacher_forced(*(batch[i] for i in (0, 1, 3, 4, 5, 7)))[1]
             rows.append({"precision": precision, "B": args.batch, "N": N,
-                         "ms": dict(zip(("sampling", "reward", "forward_backward", "adam"), med)),
+                         "ms": dict(zip(("sampling", "reward", "train_step"), med)),
                          "ms_step": sum(med), "kv_projection_fwd_ms": kv_projection_ms(m, memory, N)})
             print(json.dumps(rows[-1]), file=sys.stderr, flush=True)
             del m, opt
@@ -138,13 +139,8 @@ def reward_after_mle(args, dev):
     ids = dict(start_id=v["<start>"], eos_id=v["<eos>"], pad_id=v["<pad>"])
     batches = [[t.to(dev) for t in golden_batch(lo, lo + 16)] for lo in range(0, 128, 16)]
     m, opt = new_model("bf16", dev, 1e-4)
-    m.train()
     for i in range(args.mle_steps):
-        opt.zero_grad()
-        ls, nt = m(*batches[i % len(batches)], "train")
-        (ls / nt).backward()
-        opt.step()
-    scst.bump_weights(m)
+        optim.eager_step(m, opt, lambda: mle_loss(m, batches[i % len(batches)]))
     ft = optim.FlatAdam(m.live_parameters(), lr=1e-5, groups=m.flat_groups())
     optim.attach(m, [ft])
     steps = []
